@@ -156,6 +156,21 @@ int srgpt_rope_kv_append_bf16(void* qkv, int rows, int n_heads, int n_kv_heads, 
 int srgpt_rope_kv_append_varlen_bf16(void* qkv, int rows, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
                                      const void* sin_tab, const int* start_pos, void* kv_pages, const int* page_tables,
                                      int page_table_stride, int page_size, int n_seqs, const int* cu_seqlens, void* stream);
+/* Causal prefill attention of new prompt rows over the paged cache (attention_paged_wgmma.cu; chunked prefill).  Replaces
+ * flash_attn_varlen_func over the past_key_value concatenation (modeling_llama.py:451-456,540-566).  n_seqs chunks are packed
+ * back to back: chunk b owns rows [cu_seqlens[b], cu_seqlens[b+1]) of q / out, and its row r sits at position
+ * start_pos[b] + r - cu_seqlens[b] (device int32 arrays).  Row r attends to positions 0 .. its own position of sequence b, whose
+ * K/V are read from kv_pages [n_pages, 2, page_size, nkv, hd] (one layer) through page_tables + b * page_table_stride; the
+ * chunk's own K/V must already be in the cache (srgpt_rope_kv_append_varlen_bf16 first).  q: the rotated q columns of the fused
+ * qkv buffer, row stride q_ld.  max_rows = longest chunk, total_rows = cu_seqlens[n_seqs] (host values).  head_dim 128 and
+ * page_size 16 only; n_heads % n_kv_heads == 0 (the query heads of a kv head are served by one pass over its pages). */
+int srgpt_attention_prefill_paged_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages, int n_pages,
+                                       const int* page_tables, int page_table_stride, int page_size, const int* start_pos,
+                                       const int* cu_seqlens, int n_seqs, int max_rows, int total_rows, int n_heads, int n_kv_heads,
+                                       int head_dim, float scale, void* stream);
+/* flags[r] = 1 when rows r of a and b ([rows, row_bytes] bytes, rows contiguous) are bitwise equal, else 0 (rowops.cu).  The
+ * prompt-prefix cache of generate(prefix_cache=True) compares a request's images / depths / masks with the previous ones. */
+int srgpt_rows_equal(const void* a, const void* b, int rows, long long row_bytes, int* flags, void* stream);
 /* Decode attention for ONE new token over the paged cache (replaces torch.cat of the cache +
  * flash_attn_func with q_len 1, modeling_llama.py:451-456,564).  q: [nh*hd] bf16 (already rotated),
  * kv_len_minus1: device int = position of the new token (its k/v are already in the cache). */
@@ -289,6 +304,14 @@ int srgpt_llama_prefill_layers_bf16(void* x, const srgpt_llama_layer_weights* la
                                     float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
                                     const int* page_tables, int page_size, int n_seqs, const int* cu_seqlens, int max_seqlen,
                                     int page_table_stride, void* stream);
+/* Chunked prefill: the same layers over S new rows of n_seqs chunks packed back to back (cu_seqlens, start_pos [n_seqs] on the
+ * device, max_rows = longest chunk) that continue sequences whose earlier positions are already in the cache.  The sequencing of
+ * srgpt_llama_prefill_layers_bf16 with attention through srgpt_attention_prefill_paged_bf16 (n_pages = pages per layer). */
+int srgpt_llama_prefill_chunk_layers_bf16(void* x, const srgpt_llama_layer_weights* layers, int n_layers, void* ws_h, void* ws_qkv,
+                                          void* ws_attn, void* ws_act, int S, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                          float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
+                                          const int* page_tables, int page_table_stride, int page_size, int n_pages, int n_seqs,
+                                          const int* cu_seqlens, int max_rows, void* stream);
 /* One whole decode step (5 kernels per layer + lm_head + argmax), h [H] in/out = residual stream of the new token. */
 int srgpt_llama_decode_step_bf16(void* h, const srgpt_llama_layer_weights* layers, int n_layers, void* q_buf, void* attn_buf,
                                  void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,

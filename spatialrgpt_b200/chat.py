@@ -25,8 +25,12 @@ from .mm_utils import KeywordsStoppingCriteria, process_images, process_regions,
 
 
 class RegionChat:
-    def __init__(self, model, tokenizer, image_processor, conv_mode: str = "llama_3", temperature: float = 0.0, max_new_tokens: int = 512):
+    def __init__(self, model, tokenizer, image_processor, conv_mode: str = "llama_3", temperature: float = 0.0, max_new_tokens: int = 512,
+                 prefix_cache: bool = False):
+        """``prefix_cache``: a follow-up reuses the earlier turns' encoder outputs and prompt K/V and prefills only the new rows
+        (generate(prefix_cache=True)); answers match a full re-prefill up to bf16 rounding."""
         self.model, self.tokenizer, self.image_processor = model, tokenizer, image_processor
+        self.prefix_cache = prefix_cache
         self.conv_mode, self.temperature, self.max_new_tokens = conv_mode, temperature, max_new_tokens
         self.conv = conv_templates[conv_mode].copy()
         self.user_turns: List[str] = []
@@ -59,7 +63,8 @@ class RegionChat:
         stop = stop_string(self.conv_mode)
         out = model.generate(input_ids, images=[images], depths=None if depths is None else [depths], masks=[masks],
                              do_sample=self.temperature > 0, temperature=self.temperature, max_new_tokens=self.max_new_tokens, use_cache=True,
-                             stopping_criteria=[KeywordsStoppingCriteria([stop], self.tokenizer, input_ids)])
+                             stopping_criteria=[KeywordsStoppingCriteria([stop], self.tokenizer, input_ids)],
+                             **({"prefix_cache": True} if self.prefix_cache else {}))
         answer = clean_output(self.tokenizer.batch_decode(out, skip_special_tokens=True)[0], stop)
         turn_regions = re.findall(r"<region(\d+)>", text)
         mapping = {str(k): r for k, r in enumerate(turn_regions)}

@@ -547,3 +547,32 @@ extern "C" __attribute__((visibility("default"))) int srgpt_decode_batch_advance
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }
+
+// flags[r] = 1 when row r of a and row r of b ([rows, row_bytes], rows contiguous) hold the same bytes, else 0.  The prompt-prefix
+// cache compares a request's images / depths / masks with the ones it kept from the previous request on the device.
+__global__ void rows_equal_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, long long row_bytes, int* __restrict__ flags) {
+  const uint8_t* ra = a + (size_t)blockIdx.x * row_bytes;
+  const uint8_t* rb = b + (size_t)blockIdx.x * row_bytes;
+  int same = 1;
+  const bool vec = ((reinterpret_cast<uintptr_t>(ra) | reinterpret_cast<uintptr_t>(rb)) & 15) == 0;
+  long long i = 0;
+  if (vec) {
+    const long long n16 = row_bytes / 16;
+    for (long long k = threadIdx.x; k < n16; k += blockDim.x) {
+      const uint4 x = reinterpret_cast<const uint4*>(ra)[k], y = reinterpret_cast<const uint4*>(rb)[k];
+      same &= (x.x == y.x) & (x.y == y.y) & (x.z == y.z) & (x.w == y.w);
+    }
+    i = n16 * 16;
+  }
+  for (long long k = i + threadIdx.x; k < row_bytes; k += blockDim.x) same &= ra[k] == rb[k];
+  same = __syncthreads_and(same);
+  if (threadIdx.x == 0) flags[blockIdx.x] = same;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_rows_equal(const void* a, const void* b, int rows, long long row_bytes, int* flags, void* stream) {
+  SRGPT_CHECK_ARG(a && b && flags && rows > 0 && row_bytes > 0);
+  rows_equal_kernel<<<rows, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const uint8_t*>(a), reinterpret_cast<const uint8_t*>(b),
+                                                                              row_bytes, flags);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}

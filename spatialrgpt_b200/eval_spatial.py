@@ -218,8 +218,10 @@ def get_depth_predictor(spec: Optional[str] = None) -> Optional[Callable[[np.nda
 
 def answer_questions(line: Dict[str, Any], model, tokenizer, image_processor, image, depth, masks: Optional[torch.Tensor], conv_mode: str,
                      model_name: str, image_file: str, max_new_tokens: int = 128, temperature: float = 0.0, top_p=None,
-                     num_beams: int = 1) -> List[Dict[str, Any]]:
-    """All question turns of one annotation (the conversation accumulates, as in the reference) -> JSONL records."""
+                     num_beams: int = 1, prefix_cache: bool = False) -> List[Dict[str, Any]]:
+    """All question turns of one annotation (the conversation accumulates, as in the reference) -> JSONL records.
+    ``prefix_cache``: each turn reuses the previous turn's encoder outputs and prompt K/V and prefills only the new question
+    (generate(prefix_cache=True)); answers match a full re-prefill up to bf16 rounding."""
     dev = model.device
     images_tensor = process_images([image], image_processor, model.config).to(dev, dtype=model.dtype)
     depths_tensor = None if depth is None else process_images([depth], image_processor, model.config).to(dev, dtype=model.dtype)
@@ -237,7 +239,7 @@ def answer_questions(line: Dict[str, Any], model, tokenizer, image_processor, im
         output_ids = model.generate(input_ids, images=images_tensor, depths=depths_tensor,
                                     masks=None if masks is None else [masks.to(dev, dtype=model.dtype)],
                                     do_sample=temperature > 0, temperature=temperature, top_p=top_p, num_beams=num_beams,
-                                    max_new_tokens=max_new_tokens, use_cache=True)
+                                    max_new_tokens=max_new_tokens, use_cache=True, **({"prefix_cache": True} if prefix_cache else {}))
         pred = clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop)
         records.append({"question_id": line["id"], "image": image_file, "question": line["text_q"], "pred": pred,
                         "gt": conversations[i * 2 + 1]["value"], "model_id": model_name, "qa_info": line["qa_info"]})
@@ -280,7 +282,8 @@ def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tens
             image = Image.open(os.path.join(args.image_folder, image_file)).convert("RGB")
             depth = depth_image(np.array(image), depth_predictor) if depth_predictor is not None else None
             for rec in answer_questions(line, model, tokenizer, image_processor, image, depth, masks, args.conv_mode, model_name, image_file,
-                                        temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams):
+                                        temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams,
+                                        prefix_cache=getattr(args, "prefix_cache", False)):
                 out.write(json.dumps(rec) + "\n")
                 n += 1
     return n
@@ -302,6 +305,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--use-mask", type=lambda s: str(s).lower() not in ("0", "false", "no"), default=True)
     p.add_argument("--depth-predictor", type=str, default=None,
                    help="module:factory of the external depth network (default: DepthAnything from $DEPTH_ANYTHING_PATH, like the reference)")
+    p.add_argument("--prefix-cache", action="store_true",
+                   help="prefill only the new question of each follow-up turn, reusing the earlier turns' encoder outputs and K/V")
     p.add_argument("--allow-no-depth", action="store_true", help="run an enable_depth checkpoint without a depth network (degraded answers)")
     return p
 

@@ -122,6 +122,18 @@ class LlamaDecoder:
         self.sample_logits: Optional[torch.Tensor] = None
         self.sample_seed = 0
         self.sample_seed_dev = torch.zeros(1, dtype=torch.int64, device=dev)  # device copy: the captured graph reads the seed at run time
+        # Reusable prompt prefix of sequence 0: its first `prefix_rows` positions hold K/V that a batch-1 PREFILL wrote and nothing has
+        # overwritten since (generate_from_embeds(reuse_rows=n) continues from them).  Positions written by decode steps are never
+        # counted: the reference prefills them again, and the GEMV decode path rounds differently from the prefill GEMMs.
+        # `prefix_epoch` changes whenever the record does, so a caller can tell that someone else's request came in between.
+        self.prefix_rows = 0
+        self.prefix_epoch = 0
+
+    supports_prefix_reuse = True
+
+    def _record_prefix(self, rows: int) -> None:
+        self.prefix_rows = rows
+        self.prefix_epoch += 1
 
     # ---------------------------------------------------------------------------------------------
     @ops.in_own_dtype
@@ -140,6 +152,7 @@ class LlamaDecoder:
             raise RuntimeError(f"KV cache for {n_seqs} x {tokens_per_seq} tokens needs {need_pages * per_page >> 20} MiB, not available")
         self._graph = None
         self._graph_sample = None
+        self._record_prefix(0)
         n_pages_old, n_seqs_old = c.n_pages, len(c.owned)
         self.cache = None
         del c
@@ -158,18 +171,22 @@ class LlamaDecoder:
 
     @ops.in_own_dtype
     def prefill_hidden(self, inputs_embeds: torch.Tensor, seq: int = 0, start_pos: int = 0) -> torch.Tensor:
-        """Run all layers over one sequence's prompt rows [S, H]; fills the KV cache; returns the
-        final-layer residual stream [S, H] (before the final norm)."""
+        """Run all layers over one sequence's prompt rows [S, H] at positions start_pos .. start_pos + S - 1; fills the KV cache;
+        returns the final-layer residual stream [S, H] (before the final norm).  With start_pos > 0 the rows are a chunk that
+        continues the sequence: positions [0, start_pos) must already be in its pages, and attention reads them from there."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
-        if start_pos + S > self.max_seq_len:
+        if start_pos < 0 or start_pos + S > self.max_seq_len:
             raise RuntimeError(f"prompt of {S} tokens at {start_pos} exceeds max_seq_len {self.max_seq_len}")
+        self._record_prefix(0)
         self.cache.reserve(seq, start_pos + S)
         sp = torch.tensor([start_pos], dtype=torch.int32, device=self.device)
-        pt = self.cache.page_tables[seq]
         x = inputs_embeds.to(self.dtype).contiguous().clone()
         if start_pos != 0:
-            raise NotImplementedError("chunked prefill (prompt attention over cached pages) is a next-round item")
+            cu = torch.tensor([0, S], dtype=torch.int32, device=self.device)
+            return ops.llama_prefill_chunk_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp,
+                                                  self.cache.page_tables[seq:seq + 1], PAGE_SIZE, self.cache.n_pages, cu, S)
+        pt = self.cache.page_tables[seq]
         return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pt, PAGE_SIZE)
 
     @ops.in_own_dtype
@@ -183,6 +200,7 @@ class LlamaDecoder:
             raise RuntimeError("prefill_packed: rows do not match seq_lens")
         if max(seq_lens) > self.max_seq_len:
             raise RuntimeError(f"prompt of {max(seq_lens)} tokens exceeds max_seq_len {self.max_seq_len}")
+        self._record_prefix(0)
         cu = torch.tensor([0] + list(torch.tensor(seq_lens).cumsum(0).tolist()), dtype=torch.int32).to(self.device)
         sp = torch.zeros(B, dtype=torch.int32, device=self.device)
         x = packed_embeds.to(self.dtype).contiguous().clone()
@@ -271,12 +289,19 @@ class LlamaDecoder:
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_from_embeds(self, inputs_embeds: torch.Tensor, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
-                             use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None):
+                             use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0):
         """Greedy (or, with ``sampling=dict(temperature, top_p, seed)``, nucleus-sampled) decoding started from prompt
         embeddings [S, H].  Returns LongTensor [n_new] (and fp32 logits [n_new, V] when return_logits).
-        ``stopping_fn(ids_so_far: LongTensor) -> bool``."""
+        ``stopping_fn(ids_so_far: LongTensor) -> bool``.
+        ``reuse_rows=n`` keeps the K/V of the first n prompt rows of sequence 0 from the previous batch-1 prefill and prefills only
+        rows n..S-1 (chunked prefill at start_pos n); the caller vouches that those rows are the same as before.  n must not exceed
+        ``prefix_rows`` nor S - 1 (the last prompt row is always computed: the first new token needs its hidden state)."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
+        n_reuse = int(reuse_rows)
+        if n_reuse != 0 and (seq != 0 or n_reuse < 0 or n_reuse > self.prefix_rows or n_reuse > S - 1):
+            raise ValueError(f"reuse_rows={n_reuse} is not a reusable prefix here: sequence {seq}, {self.prefix_rows} recorded prefill rows, "
+                             f"{S} prompt rows (at most S - 1 may be reused)")
         if max_new_tokens < 1:
             return torch.empty(0, dtype=torch.int64, device=self.device)
         if max_new_tokens > self.out_ids.numel():
@@ -287,16 +312,19 @@ class LlamaDecoder:
         if eos_token_ids is not None:
             eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
         for b in range(len(self.cache.owned)):  # a previous batched generate leaves pages owned by sequences 1..B-1
-            self.cache.release(b)
+            if not (n_reuse and b == seq):
+                self.cache.release(b)
         self.cache.reserve(seq, S + max_new_tokens)
-        hidden = self.prefill_hidden(inputs_embeds, seq, 0)
+        hidden = self.prefill_hidden(inputs_embeds[n_reuse:], seq, n_reuse)
+        if seq == 0 and self.supports_prefix_reuse:
+            self._record_prefix(S)
         logits = torch.empty((max_new_tokens, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits else None
         # first token: final norm + lm_head + argmax on the last prompt row; afterwards pos == S
         self.pos.fill_(S - 1)
         self.step.zero_()
         sample = self._set_sampling(sampling)
         first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample else None)
-        ops.lm_head_argmax(hidden[S - 1], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
+        ops.lm_head_argmax(hidden[S - 1 - n_reuse], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
                            embed_table=w.embed, next_x=self.h, logits_out=first_logits)
         if sample:
             ops.sample_top_p(first_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)

@@ -18,7 +18,7 @@ from .llama_decoder import LlamaDecoder
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
-from .splice_plan import build_splice_plan
+from .splice_plan import SRC_TOKENS, build_splice_plan, reusable_prefix
 from .weights import ModelWeights
 
 
@@ -71,6 +71,9 @@ class LlavaLlamaModel:
                                       group=tensor_parallel[2] if len(tensor_parallel) > 2 else None, max_seq_len=max_seq_len)
         else:
             self.llm = LlamaDecoder(config.llama, weights.llama, max_seq_len=max_seq_len)
+        # generate(prefix_cache=True): what the previous such request left for the next one to reuse (see _encode_prefix_cached)
+        self._prefix_state = None
+        self.last_prefix_reuse = None
 
     # ---- accessors (llava_arch.py:252-278) -----------------------------------------------------------
     def get_llm(self):
@@ -159,18 +162,20 @@ class LlavaLlamaModel:
         side = ADA_POOL if (self.config.enable_region and self.region_extractor is not None) else self.config.vision.grid
         return self.mm_projector.tokens_out(side)
 
-    def _encode_multimodal(self, images, masks, depths):
-        """llava_arch.py:387-411.  Returns (image_features [N,196,H], mask_embeds, depth_embeds)."""
-        cfg = self.config
+    @staticmethod
+    def _stack_images(images):
+        """A list of [3, R, R] / [n, 3, R, R] tensors, or [B, n, 3, R, R], or [N, 3, R, R] -> [N, 3, R, R]."""
         if isinstance(images, (list, tuple)):
-            images = torch.cat([im if im.dim() == 4 else im[None] for im in images], dim=0)
-        elif images.dim() == 5:
-            images = images.flatten(0, 1)
+            return torch.cat([im if im.dim() == 4 else im[None] for im in images], dim=0)
+        return images.flatten(0, 1) if images.dim() == 5 else images
+
+    def _encode_multimodal(self, images, masks, depths, keep: Optional[dict] = None):
+        """llava_arch.py:387-411.  Returns (image_features [N,196,H], mask_embeds, depth_embeds).  ``keep`` (a dict) receives the
+        encoder outputs a later request may reuse: image_features, hres (nested order) and depth_features."""
+        cfg = self.config
+        images = self._stack_images(images)
         if depths is not None:
-            if isinstance(depths, (list, tuple)):
-                depths = torch.cat([d if d.dim() == 4 else d[None] for d in depths], dim=0)
-            elif depths.dim() == 5:
-                depths = depths.flatten(0, 1)
+            depths = self._stack_images(depths)
         N = images.shape[0]
         mask_embeds = depth_embeds = None
         use_depth = cfg.enable_region and cfg.enable_depth and depths is not None
@@ -191,14 +196,68 @@ class LlavaLlamaModel:
             mask_embeds, depth_embeds = self.region_extractor(hres, None if depth_features is None else depth_features.contiguous(),
                                                               masks, hres_order=ops.ORDER_NESTED)
         else:
-            lres = tower_features
+            hres, lres = None, tower_features
         image_features = self.mm_projector(lres)
+        if keep is not None:
+            keep.update(image_features=image_features, hres=hres, depth_features=depth_features)
         return image_features, mask_embeds, depth_embeds
+
+    def _encode_prefix_cached(self, images, masks, depths, state: dict):
+        """The encoders of a generate(prefix_cache=True) request.  Compares the request's images, depth images and masks bitwise
+        with the copies kept from the previous such request: ONE small device compare (srgpt_rows_equal) and ONE host sync at the
+        start of the request, to learn the outcome.  When every image (and, with the depth branch, every depth image) is
+        unchanged, both tower passes, the refinement and the projector are skipped and only the mask pooling and the region
+        projectors run again (masks may have changed or grown, as in a multi-turn region chat).  Fills ``state`` with the
+        per-image / per-region equality the prompt-prefix rule needs (splice_plan.reusable_prefix) and with what the next
+        request may reuse."""
+        cfg, dev = self.config, self.device
+        images = self._stack_images(images).to(dev)
+        N = images.shape[0]
+        region_on = cfg.enable_region and self.region_extractor is not None
+        use_depth = region_on and cfg.enable_depth and depths is not None
+        depths = self._stack_images(depths).to(dev) if use_depth else None
+        mask_list = (list(masks) if masks is not None else []) + [None] * N
+        mask_list = [None if m is None else m.to(dev) for m in mask_list[:N]]
+        prev = self._prefix_state if (self._prefix_state is not None and self._prefix_state.get("images") is not None) else None
+
+        counts = [0 if m is None else int(m.shape[0]) for m in mask_list]
+        offs = [sum(counts[:i]) for i in range(N + 1)]
+        flags = torch.zeros(2 * N + offs[N], dtype=torch.int32, device=dev)
+
+        def compare(a, b, lo):  # rows of a vs b -> flags[lo:lo + a.shape[0]] when shapes / dtypes allow a bitwise comparison
+            if a is None or b is None or a.dtype != b.dtype or a.shape[1:] != b.shape[1:] or a.shape[0] == 0:
+                return
+            n = min(a.shape[0], b.shape[0])
+            ops.rows_equal(a[:n].contiguous(), b[:n].contiguous(), flags[lo:lo + n])
+
+        if prev is not None and prev["images"].shape[0] == N and (prev["depths"] is None) == (depths is None):
+            compare(images, prev["images"], 0)
+            if depths is not None:
+                compare(depths, prev["depths"], N)
+            prev_offs = prev["mask_offs"]
+            for i in range(N):
+                if i < len(prev["masks"]) and prev_offs[i] == offs[i]:
+                    compare(mask_list[i], prev["masks"][i], 2 * N + offs[i])
+        eq = flags.cpu().bool().tolist()  # the one host sync of a prefix-cached request
+        image_equal = [eq[i] and (depths is None or eq[N + i]) for i in range(N)]
+        mask_equal = [eq[2 * N + offs[i] + k] and image_equal[i] for i in range(N) for k in range(counts[i])]
+        skip = prev is not None and N > 0 and all(image_equal)
+        state.update(images=prev["images"] if skip else images.clone(), depths=prev["depths"] if skip else (None if depths is None else depths.clone()),
+                     masks=[None if m is None else m.contiguous().clone() for m in mask_list], mask_offs=offs, image_equal=image_equal,
+                     mask_equal=mask_equal, encoders_skipped=skip)
+        if not skip:
+            return self._encode_multimodal(images, masks, depths, keep=state)
+        # the encoder outputs of the previous request are this request's
+        state.update(image_features=prev["image_features"], hres=prev["hres"], depth_features=prev["depth_features"])
+        mask_embeds = depth_embeds = None
+        if region_on and masks is not None:
+            mask_embeds, depth_embeds = self.region_extractor(state["hres"], state["depth_features"], mask_list, hres_order=ops.ORDER_NESTED)
+        return state["image_features"], mask_embeds, depth_embeds
 
     # ---- embedding splice (llava_arch.py:333-650) -----------------------------------------------------
     @ops.in_own_dtype
     def prepare_inputs_labels_for_multimodal(self, input_ids, position_ids, attention_mask, past_key_values, labels, images,
-                                             masks=None, depths=None, _packed_only: bool = False):
+                                             masks=None, depths=None, _packed_only: bool = False, _prefix: Optional[dict] = None):
         if images is None or (input_ids is not None and input_ids.shape[1] == 1):
             return input_ids, position_ids, attention_mask, past_key_values, None, labels  # llava_arch.py:355-385
         cfg = self.config
@@ -208,7 +267,7 @@ class LlavaLlamaModel:
         # builds the plan while the GPU runs the tower, (4) plan upload + one gather kernel.  The host never waits on the tower
         # and the GPU never waits on the Python loop below (it cost ~15 % of a 32-request batch when it came in between).
         host_copies, copy_done = self._start_host_copies([input_ids, attention_mask, labels])
-        encoded = self._encode_multimodal(images, masks, depths)
+        encoded = self._encode_multimodal(images, masks, depths) if _prefix is None else self._encode_prefix_cached(images, masks, depths, _prefix)
         if copy_done is not None:
             copy_done.synchronize()
         ids_cpu = host_copies[0].to(torch.int64)
@@ -230,6 +289,8 @@ class LlavaLlamaModel:
         for w in plan.warnings:
             print(w)
         lens, new_labels = plan.lens, plan.labels
+        if _prefix is not None:
+            _prefix.update(src_id=plan.src_id, src_row=plan.src_row, n_tok=n_tok)
         sid_dev, srow_dev = plan.src_id.to(dev, non_blocking=True), plan.src_row.to(dev, non_blocking=True)
 
         # ---- ONE gather kernel builds the embeddings of the whole batch from the encoder outputs
@@ -334,6 +395,11 @@ class LlavaLlamaModel:
         eos_token_id = generation_kwargs.pop("eos_token_id", self.config.llama.eos_token_id)
         return_logits = bool(generation_kwargs.pop("output_logits", False))
         use_graph = bool(generation_kwargs.pop("use_cuda_graph", True))
+        # prefix_cache=True (batch 1, opt-in): keep the previous such request's encoder outputs and the K/V of its prompt rows, and
+        # prefill only the rows after the longest unchanged prefix (a follow-up turn of a conversation).  The new rows run through
+        # short-M GEMMs and the paged attention kernel, so they differ from a full re-prefill by rounding; off, generate() is the
+        # plain path.  model.last_prefix_reuse = (rows_reused, rows_prefilled, encoders_skipped) afterwards.
+        prefix_cache = bool(generation_kwargs.pop("prefix_cache", False))
         # do_sample=True -> HF's TemperatureLogitsWarper + TopPLogitsWarper + multinomial, here one kernel per token
         # (eval_spatial.py:231-236 passes do_sample = temperature > 0, so temperature 0 stays greedy)
         sampling = None
@@ -345,16 +411,30 @@ class LlavaLlamaModel:
             raise NotImplementedError("beam search is implemented for do_sample=False without output_logits (the eval scripts' mode)")
         if generation_kwargs:
             raise TypeError(f"unsupported generation kwargs: {sorted(generation_kwargs)}")
+        prefix = None
+        if prefix_cache:
+            if input_ids is None or input_ids.shape[0] != 1:
+                raise NotImplementedError("prefix_cache=True serves batch-1 requests (no prefix sharing across a batch)")
+            if num_beams != 1:
+                raise NotImplementedError("prefix_cache=True with beam search")
+            if not self.llm.supports_prefix_reuse:
+                raise NotImplementedError("prefix_cache=True on the tensor-parallel decoder")
+            prefix = {}
 
         packed = None
         if images is not None:
-            self.prepare_inputs_labels_for_multimodal(input_ids, None, attention_mask, None, None, images, masks, depths, _packed_only=True)
+            self.prepare_inputs_labels_for_multimodal(input_ids, None, attention_mask, None, None, images, masks, depths, _packed_only=True,
+                                                      _prefix=prefix)
             packed, lens = self._last_packed
             B = len(lens)
         else:
             inputs_embeds = self.llm.embed_tokens(input_ids).view(*input_ids.shape, -1)
             lens = [input_ids.shape[1]] * input_ids.shape[0] if attention_mask is None else attention_mask.sum(-1).tolist()
             B = inputs_embeds.shape[0]
+            if prefix is not None:  # text only: a row is its token id
+                ids = input_ids[0].cpu() if attention_mask is None else input_ids[0].cpu()[attention_mask[0].cpu().bool()]
+                prefix.update(src_id=torch.full((ids.numel(),), SRC_TOKENS, dtype=torch.int32), src_row=ids.to(torch.int32), n_tok=1,
+                              image_equal=[], mask_equal=[], encoders_skipped=False)
         if max_new_tokens is None:
             max_new_tokens = 20 if max_length is None else max(int(max_length) - max(lens), 1)  # HF default max_length=20
         pad = pad_token_id if pad_token_id is not None else (self.config.llama.pad_token_id or 0)
@@ -378,8 +458,19 @@ class LlavaLlamaModel:
         elif B == 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
+            reuse = 0
+            if prefix is not None:
+                prev = self._prefix_state
+                self._prefix_state = None
+                if prev is not None and prev["epoch"] == self.llm.prefix_epoch:  # no other request touched the cache since
+                    reuse = reusable_prefix(prev["src_id"], prev["src_row"], prefix["src_id"], prefix["src_row"], prefix["n_tok"],
+                                            prefix["image_equal"], prefix["mask_equal"], min(self.llm.prefix_rows, n - 1))
             r = self.llm.generate_from_embeds(emb, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling)
+                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse)
+            if prefix is not None:
+                prefix["epoch"] = self.llm.prefix_epoch
+                self._prefix_state = prefix
+                self.last_prefix_reuse = (reuse, n - reuse, bool(prefix["encoders_skipped"]))
             if return_logits:
                 r, lg = r
                 all_logits.append(lg)

@@ -350,6 +350,41 @@ def rope_kv_append(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: i
           "srgpt_rope_kv_append_bf16")
 
 
+def attention_prefill_paged(q: torch.Tensor, kv_pages: torch.Tensor, page_tables: torch.Tensor, page_size: int, start_pos: torch.Tensor,
+                            cu_seqlens: torch.Tensor, max_rows: int, n_heads: int, n_kv_heads: int, head_dim: int, scale: float,
+                            out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Chunked prefill attention: q [rows, >= n_heads*hd] (row-strided view, e.g. the q columns of a fused qkv buffer) of n_seqs
+    chunks packed by cu_seqlens [n_seqs+1]; chunk b continues sequence b at start_pos[b] and attends causally over its pages
+    (kv_pages = one layer [n_pages, 2, page_size, nkv, hd], page_tables [>= n_seqs, cap])."""
+    _need(q, ELEM(), "attention_prefill_paged.q"); _need(kv_pages, ELEM(), "attention_prefill_paged.kv_pages")
+    for t, nm in ((page_tables, "page_tables"), (start_pos, "start_pos"), (cu_seqlens, "cu_seqlens")):
+        _need(t, torch.int32, f"attention_prefill_paged.{nm}")
+    n_seqs = cu_seqlens.numel() - 1
+    if page_tables.dim() != 2 or page_tables.shape[0] < n_seqs or page_tables.stride(1) != 1 or start_pos.numel() < n_seqs:
+        raise SrgptError("attention_prefill_paged: page_tables [n_seqs, cap] / start_pos [n_seqs] expected")
+    if not kv_pages.is_contiguous():
+        raise SrgptError("attention_prefill_paged: kv_pages must be contiguous [n_pages, 2, page_size, nkv, hd]")
+    if out is None:
+        out = torch.empty((q.shape[0], n_heads * head_dim), dtype=ELEM(), device=q.device)
+    check(_lib.load().srgpt_attention_prefill_paged_bf16(_p(q), _rowmajor2d(q, "q"), _p(out), _rowmajor2d(out, "out"), _p(kv_pages), kv_pages.shape[0],
+                                                         _p(page_tables), page_tables.stride(0), page_size, _p(start_pos), _p(cu_seqlens), n_seqs,
+                                                         max_rows, q.shape[0], n_heads, n_kv_heads, head_dim, scale, _stream()),
+          "srgpt_attention_prefill_paged_bf16")
+    return out
+
+
+def rows_equal(a: torch.Tensor, b: torch.Tensor, flags: torch.Tensor) -> torch.Tensor:
+    """flags[r] (int32, device) = 1 when a[r] and b[r] are bitwise equal; a, b contiguous CUDA tensors of one shape and dtype."""
+    if not (a.is_cuda and b.is_cuda and a.is_contiguous() and b.is_contiguous()) or a.shape != b.shape or a.dtype != b.dtype or a.dim() < 1:
+        raise SrgptError("rows_equal: expected two contiguous CUDA tensors of the same shape and dtype")
+    _need(flags, torch.int32, "rows_equal.flags")
+    rows = a.shape[0]
+    if flags.numel() < rows or not flags.is_contiguous():
+        raise SrgptError("rows_equal: flags must be a contiguous int32 vector of at least one entry per row")
+    check(_lib.load().srgpt_rows_equal(_p(a), _p(b), rows, a[0].numel() * a.element_size(), _p(flags), _stream()), "srgpt_rows_equal")
+    return flags
+
+
 def attention_decode(q: torch.Tensor, out: torch.Tensor, kv_pages: torch.Tensor, page_table: torch.Tensor, page_size: int,
                      pos: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: int, scale: float) -> torch.Tensor:
     check(_lib.load().srgpt_attention_decode_bf16(_p(q), _p(out), _p(kv_pages), _p(page_table), page_size, _p(pos), n_heads,
@@ -615,6 +650,32 @@ def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos,
                                                       _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
                                                       _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride,
                                                       _stream()), "srgpt_llama_prefill_layers_bf16")
+    _count(8 * n_layers)
+    return x
+
+
+def llama_prefill_chunk_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
+                               cu_seqlens: torch.Tensor, max_rows: int) -> torch.Tensor:
+    """All decoder layers over x [S, H] in place: n_seqs chunks packed by cu_seqlens [n_seqs+1] that continue their sequences at
+    start_pos [n_seqs] (page_tables [n_seqs, cap]); attention reads every earlier position from the paged cache."""
+    _need(x, ELEM(), "llama_prefill_chunk_layers.x")
+    _need(cu_seqlens, torch.int32, "llama_prefill_chunk_layers.cu_seqlens")
+    _ensure_gemm_workspace(x.device)
+    n_seqs = cu_seqlens.numel() - 1
+    if page_tables.dim() != 2 or page_tables.shape[0] < n_seqs or start_pos.numel() < n_seqs or page_tables.stride(1) != 1:
+        raise SrgptError("llama_prefill_chunk_layers: page_tables [n_seqs, cap] and start_pos [n_seqs] expected")
+    S, H = x.shape
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    dev = x.device
+    ws_h = torch.empty((S, H), dtype=ELEM(), device=dev)
+    ws_qkv = torch.empty((S, (nh + 2 * nkv) * hd), dtype=ELEM(), device=dev)
+    ws_attn = torch.empty((S, nh * hd), dtype=ELEM(), device=dev)
+    ws_act = torch.empty((S, I), dtype=ELEM(), device=dev)
+    import ctypes
+    check(_lib.load().srgpt_llama_prefill_chunk_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
+                                                            _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
+                                                            _p(start_pos), _p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs,
+                                                            _p(cu_seqlens), max_rows, _stream()), "srgpt_llama_prefill_chunk_layers_bf16")
     _count(8 * n_layers)
     return x
 

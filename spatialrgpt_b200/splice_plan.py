@@ -90,3 +90,32 @@ def build_splice_plan(input_ids: torch.Tensor, attention_mask: Optional[torch.Te
             sid, srow, lb = sid[:max_len], srow[:max_len], lb[:max_len]
         plan_sid.append(sid); plan_srow.append(srow); out_labels.append(lb)
     return SplicePlan(torch.cat(plan_sid), torch.cat(plan_srow), [int(x.numel()) for x in plan_sid], out_labels, cur, warns)
+
+
+def reusable_prefix(prev_src_id: Optional[torch.Tensor], prev_src_row: Optional[torch.Tensor], src_id: torch.Tensor, src_row: torch.Tensor,
+                    n_tok: int, image_equal: Sequence[bool], mask_equal: Sequence[bool], limit: int) -> int:
+    """Rows at the start of a batch-1 prompt whose embeddings are the same as in the previous prompt, so that the K/V a prefill
+    wrote for them can be kept (generate(prefix_cache=True)).  Both prompts are given by their splice-plan rows (src_id, src_row).
+    Row r matches when both requests take it from the same source row and that source is unchanged:
+      * a text row: the same token id (src_row is the id);
+      * an image row: image_equal[i] for its image i = src_row // n_tok (the caller folds the depth image of the depth branch in);
+      * a <mask> / <depth> row: mask_equal[g] for its region g = src_row (the caller folds in the region's image as well).
+    Returns the length of the longest matching prefix, at most `limit` (the rows the decoder still holds, capped at S - 1)."""
+    if prev_src_id is None or prev_src_row is None:
+        return 0
+    n = min(int(prev_src_id.numel()), int(src_id.numel()), max(int(limit), 0))
+    if n == 0:
+        return 0
+    sid, srow = src_id[:n].to(torch.int64), src_row[:n].to(torch.int64)
+    ok = (prev_src_id[:n].to(torch.int64) == sid) & (prev_src_row[:n].to(torch.int64) == srow)
+
+    def lookup(table: Sequence[bool], idx: torch.Tensor) -> torch.Tensor:
+        t = torch.tensor([bool(v) for v in table] + [False], dtype=torch.bool)  # the extra False answers any index out of range
+        return t[torch.where((idx >= 0) & (idx < len(table)), idx, len(table))]
+
+    img = sid == SRC_IMAGE
+    ok &= ~img | lookup(image_equal, torch.div(srow, max(int(n_tok), 1), rounding_mode="floor"))
+    region = (sid == SRC_MASK) | (sid == SRC_DEPTH)
+    ok &= ~region | lookup(mask_equal, srow)
+    bad = torch.nonzero(~ok)
+    return int(bad[0, 0]) if bad.numel() else n

@@ -61,6 +61,8 @@ class TPShard:
 
 
 class TPLlamaDecoder(LlamaDecoder):
+    supports_prefix_reuse = False  # prompt-prefix reuse is a batch-1, single-GPU feature: nothing is recorded here
+
     def __init__(self, dims: LlamaDims, w: LlamaW, rank: int, world: int, group=None, max_seq_len: int = 4096, comm: Optional[str] = None, **kw):
         super().__init__(dims, w, max_seq_len=max_seq_len, **kw)
         if dims.num_attention_heads % world or dims.num_key_value_heads % world or dims.intermediate_size % world:
