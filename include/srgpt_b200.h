@@ -200,6 +200,35 @@ long long srgpt_lm_head_workspace(int V);
 int srgpt_lm_head_argmax_bf16(const void* x, const void* W, int ldw, int V, int K, const void* norm_weight, float eps,
                               float* logits_out, void* workspace, const void* embed_table, void* next_x,
                               long long* out_ids, int* step, int* pos, void* stream);
+/* ---- 12-bit lossless packing of decode weights (pack12.cu, gemv.cu; DESIGN.md §3) --------------------------------------
+ * A bf16 matrix [N, K] (K a multiple of 1024) as the batch-1 decode GEMV streams it, 12 bits per weight instead of 16:
+ * sm = sign << 7 | mantissa (1 byte per weight), ex = a 4-bit exponent code per weight against the row's base
+ * (code 0 = exponent field 0, code c = base + c - 1), and a CSR list of the exceptions (nonzero exponents below the window,
+ * stored with code 0): exc[row_ptr[r] .. row_ptr[r+1]) = column << 8 | exponent, sorted by column, at most 32 per row.
+ * The byte order inside the planes follows the GEMV's lanes (pack12.cuh).  Defined for bfloat16 only: the IEEE-half build
+ * exports the same functions and they return SRGPT_ERR_UNSUPPORTED (-3). */
+typedef struct {
+  const void* sm;            /* [N, K] bytes */
+  const void* ex;            /* [N, K / 2] bytes */
+  const unsigned char* base; /* [N] */
+  const int* row_ptr;        /* [N + 1] */
+  const int* exc;            /* [row_ptr[N]] (a valid pointer even when empty) */
+} srgpt_packed12;
+/* Load time, step 1: per row base[r] and the number of exceptions n_exc[r]; *n_bad += the rows holding Inf or NaN (such a
+ * matrix must stay plain bf16).  Step 2 (the caller has decided to pack and built row_ptr from n_exc): write the planes. */
+int srgpt_pack12_scan_bf16(const void* W, int ldw, int N, int K, unsigned char* base, int* n_exc, int* n_bad, void* stream);
+int srgpt_pack12_bf16(const void* W, int ldw, int N, int K, const unsigned char* base, const int* row_ptr, void* sm, void* ex, int* exc,
+                      void* stream);
+/* The inverse (W [N, ldw] bf16), through the GEMV's own decoder: the round-trip check of a packed matrix. */
+int srgpt_unpack12_bf16(const srgpt_packed12* packed, int N, int K, void* W, int ldw, void* stream);
+/* srgpt_gemv_bf16 / srgpt_lm_head_argmax_bf16 over a packed matrix (`packed` is a host pointer; the arrays it names are on
+ * the device).  Every lane sees the same fp32 weights in the same order as the plain kernel, so the results are bit-identical. */
+int srgpt_gemv_packed_bf16(const void* x, const srgpt_packed12* packed, void* y, int N, int K, const void* norm_weight, float eps,
+                           const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
+                           const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream);
+int srgpt_lm_head_argmax_packed_bf16(const void* x, const srgpt_packed12* packed, int V, int K, const void* norm_weight, float eps,
+                                     float* logits_out, void* workspace, const void* embed_table, void* next_x, long long* out_ids,
+                                     int* step, int* pos, void* stream);
 /* Plain argmax over fp32 rows (first index on ties), e.g. first token after prefill. */
 int srgpt_argmax_f32(const float* x, int rows, int cols, long long* out, void* stream);
 /* Same over bf16 rows [rows, ldx] (the bf16-rounded logits of a batched lm_head GEMM, modeling_llama.py:1044). */
@@ -318,6 +347,17 @@ int srgpt_llama_decode_step_bf16(void* h, const srgpt_llama_layer_weights* layer
                                  const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
                                  const void* final_norm, const void* lm_head, int V, const void* embed_table, void* lm_workspace,
                                  float* logits_out, long long* out_ids, int* step, void* stream);
+/* The same step streaming the packed matrices: packed[l].<matrix>.sm == NULL (a matrix kept plain) and lm_packed == NULL or
+ * lm_packed->sm == NULL take the bf16 weight of `layers` / lm_head instead.  Bit-identical to srgpt_llama_decode_step_bf16. */
+typedef struct {
+  srgpt_packed12 qkv, o, gateup, down;
+} srgpt_llama_layer_packed;
+int srgpt_llama_decode_step_packed_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers,
+                                        void* q_buf, void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                        float eps, const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
+                                        const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+                                        const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids, int* step,
+                                        void* stream);
 
 #ifdef __cplusplus
 }

@@ -82,6 +82,13 @@ SIGNATURES = {
                                                    vp]),
     "srgpt_llama_decode_step_bf16":(ci, [vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp, vp,
                                           vp, vp]),
+    "srgpt_pack12_scan_bf16": (ci, [vp, ci, ci, ci, vp, vp, vp, vp]),
+    "srgpt_pack12_bf16": (ci, [vp, ci, ci, ci, vp, vp, vp, vp, vp, vp]),
+    "srgpt_unpack12_bf16": (ci, [vp, ci, ci, vp, ci, vp]),
+    "srgpt_gemv_packed_bf16": (ci, [vp, vp, vp, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_lm_head_argmax_packed_bf16": (ci, [vp, vp, ci, ci, vp, cf, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_llama_decode_step_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp,
+                                                 vp, vp, vp, vp]),
 }
 
 
@@ -91,6 +98,15 @@ class SiglipLayerWeights(C.Structure):
 
 class LlamaLayerWeights(C.Structure):
     _fields_ = [(n, vp) for n in ("in_norm", "qkv_w", "o_w", "post_norm", "gateup_w", "down_w", "kv_pages")]
+
+
+class Packed12(C.Structure):
+    """srgpt_packed12: one matrix in the 12-bit decode packing (all NULL = the matrix stays plain bf16)."""
+    _fields_ = [(n, vp) for n in ("sm", "ex", "base", "row_ptr", "exc")]
+
+
+class LlamaLayerPacked(C.Structure):
+    _fields_ = [(n, Packed12) for n in ("qkv", "o", "gateup", "down")]
 
 
 def lib_path(elem: str = "bf16") -> str:

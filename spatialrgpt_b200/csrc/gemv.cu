@@ -15,9 +15,14 @@
 //   * the pair is chosen so the fused epilogue is warp-local: (gate_i, up_i) for SwiGLU, (d, d + hd/2)
 //     of one head for RoPE + KV-cache append, two vocabulary rows for lm_head + argmax.
 // Rounding points follow the reference's bf16 torch ops (modeling_llama.py:429-431,186-191,221,668,682).
+//
+// The packed variant (PACKED = true) streams the 12-bit lossless packing of pack12.cuh: per batch of 4 chunks a lane loads
+// 3 x 16 bytes per row instead of 4, rebuilds the bf16 pairs in registers (decode_chunk), ORs in the row's few exception
+// exponents, and then runs the very same dot8 / warp_sum / epilogue, so its results are bit-identical.
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "pack12.cuh"
 #include "srgpt_b200.h"
 
 namespace srgpt {
@@ -27,6 +32,7 @@ constexpr int THREADS = 256;
 constexpr int WARPS = THREADS / 32;
 constexpr int SPRE_MAX = 2;                       // up to 2 x 4 chunks per row per lane in shared memory
 constexpr int SPRE_WARP_BYTES = 2 * 4 * 32 * 16;  // per batch: 2 rows x 4 chunks x 32 lanes x 16 B = 4 KB
+constexpr int SPRE_WARP_BYTES12 = 2 * 3 * 32 * 16;  // packed: 2 rows x 3 vectors x 32 lanes x 16 B = 3 KB
 enum { MODE_LM = 3 };
 
 struct Params {
@@ -57,6 +63,7 @@ struct Params {
   int kv_heads_total;         // KV-cache row = kv_heads_total * hd elements (0: n_kv_heads); the rank writes heads [kv_head_off, +n_kv_heads)
   int kv_head_off;
   float* y_f32;               // PLAIN mode: un-rounded fp32 partial dot products go here instead of bf16 y (+ residual)
+  srgpt_packed12 pk;          // the packed kernel's weights (W is unused there)
 };
 
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -144,11 +151,78 @@ __device__ __forceinline__ void pair_rows(const Params& p, int pi, int& r0, int&
   }
 }
 
+// ---- packed weights: one batch (4 chunks = 3 x 16 bytes) of one row for one lane.  Batch b of a row starts at uint4 64 b of its
+//      sm plane row (chunks 0,1 then 2,3 of every lane) and at uint4 32 b of its ex plane row (pack12.cuh).
+struct Raw12 {
+  uint4 s01, s23, e;
+};
+
+__device__ __forceinline__ Raw12 ld_raw12(const uint4* sm_lane, const uint4* ex_lane, int b) {
+  Raw12 q;
+  q.s01 = ld_stream16(sm_lane + b * 64);
+  q.s23 = ld_stream16(sm_lane + b * 64 + 32);
+  q.e = ld_stream16(ex_lane + b * 32);
+  return q;
+}
+
+__device__ __forceinline__ void decode_batch(const Raw12& q, uint32_t bp, uint4 (&w)[4]) {
+  w[0] = pack12::decode_chunk(q.s01.x, q.s01.y, q.e.x, bp);
+  w[1] = pack12::decode_chunk(q.s01.z, q.s01.w, q.e.y, bp);
+  w[2] = pack12::decode_chunk(q.s23.x, q.s23.y, q.e.z, bp);
+  w[3] = pack12::decode_chunk(q.s23.z, q.s23.w, q.e.w, bp);
+}
+
+// The exceptions of one row that fall into batch b: their exponent fields are ORed into the decoded chunks (where code 0 left 0).
+// Lane k holds entry k of the row's list (exc), j is the next entry not yet applied; j and n are warp-uniform and the list is
+// sorted by column, so a batch without exceptions costs one shuffle.  Selects, not indexing, keep w in registers.
+__device__ __forceinline__ void patch_batch(uint4 (&w)[4], int exc, int n, int& j, int b, int lane) {
+  while (j < n) {
+    const int v = __shfl_sync(0xffffffffu, exc, j);
+    const int col = v >> 8;
+    if ((col >> 10) != b) break;
+    const int cc = col >> 3, t = col & 7;
+    const uint32_t bits = ((cc & 31) == lane) ? (uint32_t)(v & 0xFF) << (7 + 16 * (t & 1)) : 0u;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t m = (i == ((cc >> 5) & 3)) ? bits : 0u;
+      w[i].x |= (t >> 1) == 0 ? m : 0u;
+      w[i].y |= (t >> 1) == 1 ? m : 0u;
+      w[i].z |= (t >> 1) == 2 ? m : 0u;
+      w[i].w |= (t >> 1) == 3 ? m : 0u;
+    }
+    ++j;
+  }
+}
+
+struct Rows12 {
+  uint32_t bp0, bp1;  // base - 1 of the two rows
+  int exc0, exc1;     // this lane's entry of each row's exception list
+  int n0, n1;         // list lengths
+  int j0, j1;         // next entry to apply
+};
+
+__device__ __forceinline__ void consume12(const Raw12& q0, const Raw12& q1, Rows12& rs, int b, int lane, const uint4* px, float& a0, float& a1) {
+  uint4 w0[4], w1[4];
+  decode_batch(q0, rs.bp0, w0);
+  decode_batch(q1, rs.bp1, w1);
+  patch_batch(w0, rs.exc0, rs.n0, rs.j0, b, lane);
+  patch_batch(w1, rs.exc1, rs.n1, rs.j1, b, lane);
+  const int c = b * 128 + lane;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float xf[8];
+    unpack8(px[c + 32 * i], xf);
+    a0 += dot8(w0[i], xf);
+    a1 += dot8(w1[i], xf);
+  }
+}
+
 // PRE = number of 4-chunk batches (per row) requested BEFORE the dependency wait: 1 -> 8 loads per lane (3 CTAs/SM),
 // 2 -> 16 loads (2 CTAs/SM), 4 -> 32 loads = a whole K=4096 row pair per warp (1 CTA/SM).  The small matrices of a
 // layer (qkv 50 MB, o_proj 33 MB) run behind a kernel that leaves HBM idle (decode attention / the previous tail), so
 // the more of their weights is in flight before the dependency resolves, the less of them is exposed afterwards.
-template <int MODE, int PRE>
+// PACKED: the weights are p.pk (12-bit packing, K % 1024 == 0, PRE == 1); everything but the weight stream is shared.
+template <int MODE, int PRE, bool PACKED>
 __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) decode_gemv_kernel(const Params p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __shared__ float red[32];
@@ -173,7 +247,7 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   constexpr int NPRE = 4 * PRE;
   uint4 u0[NPRE], u1[NPRE];
   int c = lane;
-  const bool first_full = active && (c + 32 * (NPRE - 1) < nchunk);
+  const bool first_full = !PACKED && active && (c + 32 * (NPRE - 1) < nchunk);
   if (first_full) {
 #pragma unroll
     for (int i = 0; i < NPRE; ++i) {
@@ -184,8 +258,40 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   // ---- a second, register-free prefetch level: the next p.spre batches of both rows go to shared memory with
   //      cp.async (every lane later reads back exactly the 16-byte slots it filled, so no barrier is needed).
   //      Occupancy stays at 3 CTAs/SM, unlike the deeper register prefetch (PRE = 2/4) that was measured and rejected.
-  uint8_t* spre_base = smem_raw + (size_t)p.K * 2 + (size_t)warp * ((size_t)p.spre * SPRE_WARP_BYTES);
+  uint8_t* spre_base = smem_raw + (size_t)p.K * 2 + (size_t)warp * ((size_t)p.spre * (PACKED ? SPRE_WARP_BYTES12 : SPRE_WARP_BYTES));
   int n_spre = 0;
+  // ---- packed: the same two levels (batch 0 in registers, the next p.spre batches in shared memory), plus each row's base and
+  //      exception list; all of it is static, so all of it is requested before the dependency wait
+  const int nbatch = p.K >> 10;
+  Raw12 q0 = {}, q1 = {};
+  Rows12 rs = {};
+  const uint4 *sm0 = nullptr, *ex0 = nullptr;  // this lane's vectors of row r0; row r1 is drow rows further (sm: 2 drow uint4 per ex uint4)
+  const int drow_ex = (r1 - r0) * (p.K >> 5);
+  if (PACKED && active) {
+    sm0 = reinterpret_cast<const uint4*>(p.pk.sm) + (size_t)r0 * (p.K >> 4) + lane;
+    ex0 = reinterpret_cast<const uint4*>(p.pk.ex) + (size_t)r0 * (p.K >> 5) + lane;
+    q0 = ld_raw12(sm0, ex0, 0);
+    q1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, 0);
+    for (int b = 0; b < p.spre && 1 + b < nbatch; ++b) {
+      const uint32_t d = (uint32_t)__cvta_generic_to_shared(spre_base + b * 6 * 512 + lane * 16);
+      const uint4 *s = sm0 + (1 + b) * 64, *e = ex0 + (1 + b) * 32;
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(s) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512), "l"(s + 32) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1024), "l"(e) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1536), "l"(s + 2 * drow_ex) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2048), "l"(s + 2 * drow_ex + 32) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2560), "l"(e + drow_ex) : "memory");
+      ++n_spre;
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    const int e0 = p.pk.row_ptr[r0], e1 = p.pk.row_ptr[r1];
+    rs.n0 = min(p.pk.row_ptr[r0 + 1] - e0, pack12::MAX_EXC_PER_ROW);
+    rs.n1 = min(p.pk.row_ptr[r1 + 1] - e1, pack12::MAX_EXC_PER_ROW);
+    if (lane < rs.n0) rs.exc0 = p.pk.exc[e0 + lane];
+    if (lane < rs.n1) rs.exc1 = p.pk.exc[e1 + lane];
+    rs.bp0 = (uint32_t)p.pk.base[r0] - 1u;
+    rs.bp1 = (uint32_t)p.pk.base[r1] - 1u;
+  }
   if (first_full) {
     for (int b = 0; b < p.spre; ++b) {
       const int cb = c + 32 * NPRE + 128 * b;
@@ -207,7 +313,7 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   //      ~1 us dependency release) then keeps HBM streaming through what used to be idle gaps and later reads L2 hits.
   //      It made the step slower on the in-graph timeline of the earlier target: the prefetch and the demand loads of the same
   //      rows race and both reach DRAM.  Off by default; SRGPT_GEMV_L2PF=1 keeps the experiment reproducible.
-  if (p.l2pf && active && lane < 2) {
+  if (!PACKED && p.l2pf && active && lane < 2) {
     const int c_req = first_full ? (32 * NPRE + 128 * n_spre) : 0;  // chunks per row already requested above
     if (c_req < nchunk) {
       const char* rowp = reinterpret_cast<const char*>(lane == 0 ? p0 : p1) + (size_t)c_req * 16;
@@ -237,7 +343,24 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   stage_x(p.x, p.norm_weight, p.eps, p.K, sx, red, nw_pre, nw_pre_valid);
 
   float a0 = 0.f, a1 = 0.f;
-  if (active) {
+  if constexpr (PACKED) {  // batches in chunk order: the lane's fma chain is the plain kernel's
+    if (active) {
+      consume12(q0, q1, rs, 0, lane, px, a0, a1);
+      if (n_spre > 0) {
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        for (int b = 0; b < n_spre; ++b) {
+          const uint8_t* s = spre_base + b * 6 * 512 + lane * 16;
+          const Raw12 t0 = {*reinterpret_cast<const uint4*>(s), *reinterpret_cast<const uint4*>(s + 512), *reinterpret_cast<const uint4*>(s + 1024)};
+          const Raw12 t1 = {*reinterpret_cast<const uint4*>(s + 1536), *reinterpret_cast<const uint4*>(s + 2048), *reinterpret_cast<const uint4*>(s + 2560)};
+          consume12(t0, t1, rs, 1 + b, lane, px, a0, a1);
+        }
+      }
+      for (int b = 1 + n_spre; b < nbatch; ++b) {
+        const Raw12 t0 = ld_raw12(sm0, ex0, b), t1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, b);
+        consume12(t0, t1, rs, b, lane, px, a0, a1);
+      }
+    }
+  } else if (active) {
     if (first_full) {
 #pragma unroll
       for (int i = 0; i < NPRE; ++i) {
@@ -482,12 +605,12 @@ static int spre_default() {
   return v;
 }
 
-template <int MODE, int PRE>
+template <int MODE, int PRE, bool PACKED = false>
 static int launch_pre(const Params& p, int npairs, cudaStream_t st) {
-  const int smem = p.K * 2 + WARPS * spre_default() * SPRE_WARP_BYTES;
+  const int smem = p.K * 2 + WARPS * spre_default() * (PACKED ? SPRE_WARP_BYTES12 : SPRE_WARP_BYTES);
   static int configured_smem = 0;
   if (smem > 48 * 1024 && smem > configured_smem) {
-    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_kernel<MODE, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_kernel<MODE, PRE, PACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured_smem = smem;
   }
   cudaLaunchConfig_t cfg;
@@ -504,7 +627,7 @@ static int launch_pre(const Params& p, int npairs, cudaStream_t st) {
   // attention leaves HBM idle (its 33 MB fit L2 many times over); 3: o_proj and the qkv GEMV
   const bool small_plain = MODE == SRGPT_GEMV_PLAIN && p.residual != nullptr && (long long)p.N * p.K <= (32LL << 20);
   q.l2pf = (l2pf == 1 || (l2pf >= 2 && small_plain) || (l2pf == 3 && MODE == SRGPT_GEMV_QKV_ROPE)) ? 1 : 0;
-  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, decode_gemv_kernel<MODE, PRE>, q));
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, decode_gemv_kernel<MODE, PRE, PACKED>, q));
   return SRGPT_OK;
 }
 
@@ -524,6 +647,13 @@ static int launch(const Params& p, int npairs, cudaStream_t st) {
   return launch_pre<MODE, 1>(p, npairs, st);
 }
 
+// the packed kernel always runs at the default depth (PRE 1)
+template <int MODE, bool PACKED>
+static int launch_mode(const Params& p, int npairs, cudaStream_t st) {
+  if constexpr (PACKED) return launch_pre<MODE, 1, true>(p, npairs, st);
+  else return launch<MODE>(p, npairs, st);
+}
+
 }  // namespace gemv
 }  // namespace srgpt
 
@@ -531,21 +661,24 @@ using namespace srgpt;
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void* x, const void* W, int ldw, void* y, int N, int K, const void* norm_weight, float eps,
-                               const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
-                               const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size,
-                               void* stream) {
-  SRGPT_CHECK_ARG(x && W && y && N > 0 && K > 0);
-  SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0 && (ldw % 8) == 0 && ldw >= K);
+// a packed matrix the kernel can stream: every array present, vector-aligned planes, K a whole number of batches
+static bool packed_ok(const srgpt_packed12* P, int K) {
+  return P != nullptr && P->sm && P->ex && P->base && P->row_ptr && P->exc && aligned16(P->sm) && aligned16(P->ex) && (K % pack12::BATCH) == 0;
+}
+
+// checks and mode dispatch of srgpt_gemv_bf16 and srgpt_gemv_packed_bf16; p.W / p.ldw or p.pk are set by the caller
+template <bool PACKED>
+static int gemv_modes(gemv::Params& p, const void* x, void* y, int N, int K, const void* norm_weight, float eps, const void* residual, int mode,
+                      int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages,
+                      const int* page_table, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(x && y && N > 0 && K > 0);
+  SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0);
   SRGPT_CHECK_ARG(K * 2 <= 200 * 1024);
-  SRGPT_CHECK_ARG(aligned16(x) && aligned16(W) && (reinterpret_cast<uintptr_t>(y) & 3) == 0);
+  SRGPT_CHECK_ARG(aligned16(x) && (reinterpret_cast<uintptr_t>(y) & 3) == 0);
   SRGPT_CHECK_ARG(norm_weight == nullptr || aligned16(norm_weight));
   SRGPT_CHECK_ARG(mode >= SRGPT_GEMV_PLAIN && mode <= SRGPT_GEMV_QKV_ROPE);
   SRGPT_CHECK_ARG(x != y);  // x is read by late CTAs while early ones already write y
-  gemv::Params p = {};
   p.x = reinterpret_cast<const bf16*>(x);
-  p.W = reinterpret_cast<const bf16*>(W);
-  p.ldw = ldw;
   p.y = reinterpret_cast<bf16*>(y);
   p.N = N; p.K = K;
   p.norm_weight = reinterpret_cast<const bf16*>(norm_weight);
@@ -562,18 +695,47 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void
   switch (mode) {
     case SRGPT_GEMV_PLAIN:
       p.hd = 2;
-      return gemv::launch<SRGPT_GEMV_PLAIN>(p, N / 2, st);
+      return gemv::launch_mode<SRGPT_GEMV_PLAIN, PACKED>(p, N / 2, st);
     case SRGPT_GEMV_SWIGLU:
       SRGPT_CHECK_ARG(residual == nullptr);
       p.hd = 2;
-      return gemv::launch<SRGPT_GEMV_SWIGLU>(p, N / 2, st);
+      return gemv::launch_mode<SRGPT_GEMV_SWIGLU, PACKED>(p, N / 2, st);
     case SRGPT_GEMV_QKV_ROPE:
       SRGPT_CHECK_ARG(residual == nullptr && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && (head_dim % 2) == 0);
       SRGPT_CHECK_ARG(N == (n_heads + 2 * n_kv_heads) * head_dim);
       SRGPT_CHECK_ARG(cos_tab && sin_tab && pos && kv_pages && page_table && page_size > 0);
-      return gemv::launch<SRGPT_GEMV_QKV_ROPE>(p, N / 2, st);
+      return gemv::launch_mode<SRGPT_GEMV_QKV_ROPE, PACKED>(p, N / 2, st);
   }
   return SRGPT_ERR_INVALID;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void* x, const void* W, int ldw, void* y, int N, int K, const void* norm_weight, float eps,
+                               const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
+                               const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size,
+                               void* stream) {
+  SRGPT_CHECK_ARG(W && aligned16(W) && (ldw % 8) == 0 && ldw >= K);
+  gemv::Params p = {};
+  p.W = reinterpret_cast<const bf16*>(W);
+  p.ldw = ldw;
+  return gemv_modes<false>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
+                           page_table, page_size, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_packed_bf16(const void* x, const srgpt_packed12* packed, void* y, int N, int K,
+                                                                               const void* norm_weight, float eps, const void* residual, int mode, int n_heads,
+                                                                               int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+                                                                               const int* pos, void* kv_pages, const int* page_table, int page_size,
+                                                                               void* stream) {
+  SRGPT_CHECK_ARG(packed_ok(packed, K));
+#ifdef SRGPT_ELEM_F16
+  set_last_error("srgpt_gemv_packed_bf16: the 12-bit packing is defined for bfloat16 weights only");
+  return SRGPT_ERR_UNSUPPORTED;
+#else
+  gemv::Params p = {};
+  p.pk = *packed;
+  return gemv_modes<true>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
+                          page_table, page_size, stream);
+#endif
 }
 
 // Tensor-parallel variants of the decode GEMV (SURVEY.md §8e "optional TP", BASELINE config c5): a rank owns n_heads q heads and
@@ -671,20 +833,19 @@ extern "C" __attribute__((visibility("default"))) long long srgpt_lm_head_worksp
   return (long long)g * (long long)(sizeof(float) + sizeof(int));
 }
 
-extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_bf16(const void* x, const void* W, int ldw, int V, int K, const void* norm_weight, float eps,
-                                         float* logits_out, void* workspace, const void* embed_table, void* next_x,
-                                         long long* out_ids, int* step, int* pos, void* stream) {
-  SRGPT_CHECK_ARG(x && W && workspace && out_ids && step && pos && V > 0 && K > 0);
-  SRGPT_CHECK_ARG((K % 8) == 0 && (ldw % 8) == 0 && ldw >= K && K * 2 <= 200 * 1024);
-  SRGPT_CHECK_ARG(aligned16(x) && aligned16(W) && (norm_weight == nullptr || aligned16(norm_weight)));
+// srgpt_lm_head_argmax_bf16 and its packed form; p.W / p.ldw or p.pk are set by the caller
+template <bool PACKED>
+static int lm_head_argmax(gemv::Params& p, const void* x, int V, int K, const void* norm_weight, float eps, float* logits_out, void* workspace,
+                          const void* embed_table, void* next_x, long long* out_ids, int* step, int* pos, void* stream) {
+  SRGPT_CHECK_ARG(x && workspace && out_ids && step && pos && V > 0 && K > 0);
+  SRGPT_CHECK_ARG((K % 8) == 0 && K * 2 <= 200 * 1024);
+  SRGPT_CHECK_ARG(aligned16(x) && (norm_weight == nullptr || aligned16(norm_weight)));
   SRGPT_CHECK_ARG((embed_table == nullptr) == (next_x == nullptr));
   SRGPT_CHECK_ARG(embed_table == nullptr || (aligned16(embed_table) && aligned16(next_x)));
   const int npairs = (V + 1) / 2;
   const int g = gemv::grid_for(npairs);
-  gemv::Params p = {};
   p.x = reinterpret_cast<const bf16*>(x);
-  p.W = reinterpret_cast<const bf16*>(W);
-  p.ldw = ldw; p.N = V; p.K = K;
+  p.N = V; p.K = K;
   p.norm_weight = reinterpret_cast<const bf16*>(norm_weight);
   p.eps = eps;
   p.hd = 2;
@@ -692,7 +853,7 @@ extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_bf16(
   p.part_val = reinterpret_cast<float*>(workspace);
   p.part_idx = reinterpret_cast<int*>(p.part_val + g);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = gemv::launch<gemv::MODE_LM>(p, npairs, st);
+  int rc = gemv::launch_mode<gemv::MODE_LM, PACKED>(p, npairs, st);
   if (rc != SRGPT_OK) return rc;
   // finalize: also a programmatic dependent (its launch latency hides behind the lm_head kernel)
   cudaLaunchConfig_t cfg;
@@ -701,4 +862,29 @@ extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_bf16(
   SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemv::lm_head_finalize_kernel, (const float*)p.part_val, (const int*)p.part_idx, g,
                                       reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(next_x), K, out_ids, step, pos));
   return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_bf16(const void* x, const void* W, int ldw, int V, int K, const void* norm_weight, float eps,
+                                         float* logits_out, void* workspace, const void* embed_table, void* next_x,
+                                         long long* out_ids, int* step, int* pos, void* stream) {
+  SRGPT_CHECK_ARG(W && aligned16(W) && (ldw % 8) == 0 && ldw >= K);
+  gemv::Params p = {};
+  p.W = reinterpret_cast<const bf16*>(W);
+  p.ldw = ldw;
+  return lm_head_argmax<false>(p, x, V, K, norm_weight, eps, logits_out, workspace, embed_table, next_x, out_ids, step, pos, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_packed_bf16(const void* x, const srgpt_packed12* packed, int V, int K,
+                                                                                         const void* norm_weight, float eps, float* logits_out, void* workspace,
+                                                                                         const void* embed_table, void* next_x, long long* out_ids, int* step,
+                                                                                         int* pos, void* stream) {
+  SRGPT_CHECK_ARG(packed_ok(packed, K));
+#ifdef SRGPT_ELEM_F16
+  set_last_error("srgpt_lm_head_argmax_packed_bf16: the 12-bit packing is defined for bfloat16 weights only");
+  return SRGPT_ERR_UNSUPPORTED;
+#else
+  gemv::Params p = {};
+  p.pk = *packed;
+  return lm_head_argmax<true>(p, x, V, K, norm_weight, eps, logits_out, workspace, embed_table, next_x, out_ids, step, pos, stream);
+#endif
 }

@@ -11,6 +11,7 @@ with the position / step counters living in device memory.
 """
 from __future__ import annotations
 
+import os
 from typing import List, Optional
 
 import torch
@@ -128,8 +129,31 @@ class LlamaDecoder:
         # `prefix_epoch` changes whenever the record does, so a caller can tell that someone else's request came in between.
         self.prefix_rows = 0
         self.prefix_epoch = 0
+        # The batch-1 decode step streams its matrices in the lossless 12-bit packing (DESIGN.md §3): 3/4 of the bytes, bit-identical
+        # results.  The bf16 weights stay resident for prefill and batched decode.  decode_pack: matrix -> "packed" or why it is plain.
+        self.decode_pack = {}
+        if self.packs_decode_weights and self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
+            self._pack_decode_weights()
 
     supports_prefix_reuse = True
+    packs_decode_weights = True
+    _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
+    _lm_packed = None
+
+    @ops.in_own_dtype
+    def _pack_decode_weights(self) -> None:
+        packed_layers = []
+        for l, lw in enumerate(self.w.layers):
+            pl = {}
+            for name in ("qkv", "o", "gateup", "down"):
+                pl[name], why = ops.pack12(getattr(lw, name + "_w"))
+                self.decode_pack[f"layers.{l}.{name}"] = why or "packed"
+            packed_layers.append(pl)
+        self._lm_packed, why = ops.pack12(self.w.lm_head)
+        self.decode_pack["lm_head"] = why or "packed"
+        if any(v == "packed" for v in self.decode_pack.values()):
+            self._packed_layers = packed_layers  # keeps the tensors behind the descriptors alive
+            self._packed_array = ops.make_llama_packed_array(packed_layers)
 
     def _record_prefix(self, rows: int) -> None:
         self.prefix_rows = rows
@@ -235,9 +259,14 @@ class LlamaDecoder:
         d, w = self.dims, self.w
         if sample and logits_out is None:
             logits_out = self._sample_buffer()
-        ops.llama_decode_step(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos,
-                              self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, w.embed, self.lm_ws,
-                              self.out_ids, self.step, logits_out)
+        if self._packed_array is not None:
+            ops.llama_decode_step_packed(self.h, self._layer_array, self._packed_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
+                                         d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
+                                         self.lm_ws, self.out_ids, self.step, logits_out)
+        else:
+            ops.llama_decode_step(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos,
+                                  self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, w.embed, self.lm_ws,
+                                  self.out_ids, self.step, logits_out)
         if sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
             ops.sample_top_p(logits_out, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
 

@@ -5,6 +5,7 @@ sm_90a kernel in ``csrc/``.  All wrappers raise ``SrgptError`` on any failure (n
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -13,7 +14,8 @@ from . import _lib
 from ._lib import SrgptError
 from ._lib import check as _check_rc
 
-_KERNELS_PER_CALL = {"srgpt_lm_head_local_best_bf16": 2, "srgpt_mask_pool_bf16": 2, "srgpt_mask_weights": 2, "srgpt_lm_head_argmax_bf16": 2, "srgpt_depth_to_u8x3": 3}
+_KERNELS_PER_CALL = {"srgpt_lm_head_local_best_bf16": 2, "srgpt_mask_pool_bf16": 2, "srgpt_mask_weights": 2, "srgpt_lm_head_argmax_bf16": 2, "srgpt_depth_to_u8x3": 3,
+                     "srgpt_lm_head_argmax_packed_bf16": 2}
 
 
 def check(rc: int, what: str) -> None:
@@ -402,6 +404,78 @@ def gemv(x: torch.Tensor, w: torch.Tensor, y: torch.Tensor, norm_weight: Optiona
     return y
 
 
+# ---- 12-bit lossless packing of decode weights (pack12.cu; DESIGN.md §3) -------------------------------------------
+PACK12_BATCH = 1024          # K must be a multiple: one 4-chunk step of a warp's 32 lanes
+PACK12_MAX_EXC_RATE = 0.01   # a matrix with more exceptions than this stays plain bf16
+PACK12_MAX_EXC_PER_ROW = 32  # the GEMV holds a row's exception list in one register per lane
+
+
+def _packed_desc(p) -> "_lib.Packed12":
+    d = _lib.Packed12()
+    if p is not None:
+        d.sm, d.ex, d.base, d.row_ptr, d.exc = (t.data_ptr() for t in (p.sm, p.ex, p.base, p.row_ptr, p.exc))
+    return d
+
+
+def pack12(w: torch.Tensor, verify: bool = True):
+    """Pack a bf16 matrix [N, K] for the decode GEMV.  Returns (Packed12W, None), or (None, reason) when the matrix must stay
+    plain: K not a multiple of 1024, Inf / NaN, more than 1 % exceptions or more than 32 in one row.  With ``verify`` the packed
+    matrix is unpacked on the device and compared bit for bit with ``w``; a difference raises SrgptError."""
+    from .weights import Packed12W
+    _need(w, torch.bfloat16, "pack12.w")
+    ldw = _rowmajor2d(w, "pack12.w")
+    N, K = w.shape
+    if K % PACK12_BATCH:
+        return None, f"K = {K} is not a multiple of {PACK12_BATCH}"
+    dev, lib = w.device, _lib.load()
+    base = torch.empty(N, dtype=torch.uint8, device=dev)
+    n_exc = torch.empty(N, dtype=torch.int32, device=dev)
+    n_bad = torch.zeros(1, dtype=torch.int32, device=dev)
+    check(lib.srgpt_pack12_scan_bf16(_p(w), ldw, N, K, _p(base), _p(n_exc), _p(n_bad), _stream()), "srgpt_pack12_scan_bf16")
+    total, worst, bad = (int(v) for v in torch.stack([n_exc.sum(), n_exc.max(), n_bad[0]]).cpu())
+    if bad:
+        return None, f"{bad} rows hold Inf or NaN"
+    if total > PACK12_MAX_EXC_RATE * N * K:
+        return None, f"{total / (N * K):.2%} of the weights are exceptions"
+    if worst > PACK12_MAX_EXC_PER_ROW:
+        return None, f"a row has {worst} exceptions"
+    row_ptr = torch.zeros(N + 1, dtype=torch.int32, device=dev)
+    row_ptr[1:] = torch.cumsum(n_exc, 0, dtype=torch.int32)
+    p = Packed12W(sm=torch.empty((N, K), dtype=torch.uint8, device=dev), ex=torch.empty((N, K // 2), dtype=torch.uint8, device=dev), base=base,
+                  row_ptr=row_ptr, exc=torch.empty(max(total, 1), dtype=torch.int32, device=dev))
+    check(lib.srgpt_pack12_bf16(_p(w), ldw, N, K, _p(base), _p(row_ptr), _p(p.sm), _p(p.ex), _p(p.exc), _stream()), "srgpt_pack12_bf16")
+    if verify:
+        verify12(p, w)
+    return p, None
+
+
+def verify12(p, w: torch.Tensor) -> None:
+    """Raises SrgptError unless the Packed12W ``p`` unpacks to exactly the bits of ``w``."""
+    if not torch.equal(unpack12(p).view(torch.int16), w.view(torch.int16)):
+        raise SrgptError(f"pack12: the packed {list(w.shape)} matrix does not unpack to the original bits")
+
+
+def unpack12(p) -> torch.Tensor:
+    """The bf16 matrix [N, K] a Packed12W holds (through the GEMV's own decoder)."""
+    N, K = p.sm.shape
+    out = torch.empty((N, K), dtype=torch.bfloat16, device=p.sm.device)
+    d = _packed_desc(p)
+    check(_lib.load().srgpt_unpack12_bf16(C.byref(d), N, K, _p(out), K, _stream()), "srgpt_unpack12_bf16")
+    return out
+
+
+def gemv_packed(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0,
+                residual: Optional[torch.Tensor] = None, mode: int = GEMV_PLAIN, n_heads: int = 0, n_kv_heads: int = 0,
+                head_dim: int = 0, cos_tab=None, sin_tab=None, pos=None, kv_pages=None, page_table=None, page_size: int = 0) -> torch.Tensor:
+    """gemv() over a Packed12W: bit-identical results, 12 instead of 16 bits of weight stream per element."""
+    N, K = p.sm.shape
+    d = _packed_desc(p)
+    check(_lib.load().srgpt_gemv_packed_bf16(_p(x), C.byref(d), _p(y), N, K, _p(norm_weight), eps, _p(residual), mode, n_heads, n_kv_heads,
+                                             head_dim, _p(cos_tab), _p(sin_tab), _p(pos), _p(kv_pages), _p(page_table), page_size, _stream()),
+          "srgpt_gemv_packed_bf16")
+    return y
+
+
 # ---- host preprocessing on the GPU (preprocess.py) ---------------------------------------------------------------
 def resample_u8(img: torch.Tensor, axis: int, out_size: int, kk: torch.Tensor, bounds: torch.Tensor, ksize: int) -> torch.Tensor:
     _need(img, torch.uint8, "resample_u8.img"); _need(kk, torch.int32, "resample_u8.kk"); _need(bounds, torch.int32, "resample_u8.bounds")
@@ -524,6 +598,17 @@ def lm_head_argmax(x: torch.Tensor, w: torch.Tensor, norm_weight: Optional[torch
                                                 _stream()), "srgpt_lm_head_argmax_bf16")
 
 
+def lm_head_argmax_packed(x: torch.Tensor, p, norm_weight: Optional[torch.Tensor], eps: float, workspace: torch.Tensor,
+                          out_ids: torch.Tensor, step: torch.Tensor, pos: torch.Tensor, embed_table: Optional[torch.Tensor] = None,
+                          next_x: Optional[torch.Tensor] = None, logits_out: Optional[torch.Tensor] = None) -> None:
+    """lm_head_argmax() over a Packed12W lm_head (bit-identical)."""
+    V, K = p.sm.shape
+    d = _packed_desc(p)
+    check(_lib.load().srgpt_lm_head_argmax_packed_bf16(_p(x), C.byref(d), V, K, _p(norm_weight), eps, _p(logits_out), _p(workspace),
+                                                       _p(embed_table), _p(next_x), _p(out_ids), _p(step), _p(pos), _stream()),
+          "srgpt_lm_head_argmax_packed_bf16")
+
+
 def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.Tensor, step_offset: int, out_ids: torch.Tensor,
                  embed_table: Optional[torch.Tensor] = None, next_x: Optional[torch.Tensor] = None) -> None:
     """One token from softmax(logits / T) restricted to its top-p nucleus -> out_ids[step + step_offset] (and next_x = embed row).
@@ -591,6 +676,15 @@ def make_llama_layer_array(layers, kv_pages_per_layer):
         for name in ("in_norm", "qkv_w", "o_w", "post_norm", "gateup_w", "down_w"):
             setattr(arr[i], name, getattr(lw, name).data_ptr())
         arr[i].kv_pages = kv_pages_per_layer[i].data_ptr()
+    return arr
+
+
+def make_llama_packed_array(packed_layers):
+    """ctypes array of srgpt_llama_layer_packed over per-layer dicts {"qkv", "o", "gateup", "down"} -> Packed12W or None (plain)."""
+    arr = (_lib.LlamaLayerPacked * len(packed_layers))()
+    for i, pl in enumerate(packed_layers):
+        for name in ("qkv", "o", "gateup", "down"):
+            setattr(arr[i], name, _packed_desc(pl[name]))
     return arr
 
 
@@ -689,4 +783,17 @@ def llama_decode_step(h, layer_array, n_layers: int, q_buf, attn_buf, act_buf, d
                                                    _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head), dims.vocab_size,
                                                    _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), _stream()),
           "srgpt_llama_decode_step_bf16")
+
+
+def llama_decode_step_packed(h, layer_array, packed_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table,
+                             page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
+    """llama_decode_step() streaming the packed matrices of ``packed_array`` (make_llama_packed_array) and ``lm_packed``
+    (a Packed12W or None); bit-identical."""
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    lm_d = _packed_desc(lm_packed)
+    check(_lib.load().srgpt_llama_decode_step_packed_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(packed_array, C.c_void_p), n_layers,
+                                                          _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
+                                                          _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
+                                                          C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
+                                                          _stream()), "srgpt_llama_decode_step_packed_bf16")
     _count(5 * n_layers + 2)

@@ -108,6 +108,25 @@ class LlamaW:
 
 
 @dataclass
+class Packed12W:
+    """A bf16 weight [N, K] in the lossless 12-bit packing the batch-1 decode GEMV streams (DESIGN.md §3, include/srgpt_b200.h
+    srgpt_packed12): sm [N, K] u8 sign/mantissa, ex [N, K/2] u8 exponent codes, base [N] u8, and the exceptions
+    exc[row_ptr[r]:row_ptr[r+1]] = column << 8 | exponent (int32).  Built by ops.pack12."""
+    sm: torch.Tensor
+    ex: torch.Tensor
+    base: torch.Tensor
+    row_ptr: torch.Tensor
+    exc: torch.Tensor
+
+    @property
+    def shape(self):
+        return self.sm.shape
+
+    def nbytes(self) -> int:
+        return sum(t.numel() * t.element_size() for t in (self.sm, self.ex, self.base, self.row_ptr, self.exc))
+
+
+@dataclass
 class ModelWeights:
     vision: VisionW
     region: Optional[RegionW]

@@ -73,6 +73,21 @@ if "gemv" in which:
                 st.zero_(); ops.lm_head_argmax(x, w, nw, 1e-5, ws, ids, st, ps)
         ms, best = timeit(fn)
         emit(name, ms, best, bytes_=N * K * 2, N=N, K=K)
+    # the same GEMVs over the 12-bit packing (DESIGN.md §3): GBps counts the bytes actually streamed (planes + row metadata)
+    for name, N, K, mode in [("gemv_gateup_swiglu_packed12", 28672, 4096, "swiglu"), ("gemv_down_packed12", 4096, 14336, "plain")]:
+        w, x = rnd(N, K), rnd(K)
+        p, why = ops.pack12(w)
+        if p is None:
+            raise SystemExit(f"{name}: the matrix stays plain ({why})")
+        nw = torch.ones(K, dtype=BF, device=dev)
+        if mode == "plain":
+            y = torch.empty(N, dtype=BF, device=dev); r = rnd(N)
+            fn = lambda: ops.gemv_packed(x, p, y, residual=r)
+        else:
+            y = torch.empty(N // 2, dtype=BF, device=dev)
+            fn = lambda: ops.gemv_packed(x, p, y, norm_weight=nw, eps=1e-5, mode=ops.GEMV_SWIGLU)
+        ms, best = timeit(fn)
+        emit(name, ms, best, bytes_=p.nbytes(), N=N, K=K, bf16_equiv_GBps=round(N * K * 2 / ms / 1e6, 1))
 
 if "maskpool" in which:
     for (n, side, C, M) in [(1, 128, 1152, 8), (1, 128, 1152, 16), (4, 128, 1152, 4), (32, 128, 1152, 4), (1, 32, 1152, 8), (32, 32, 1152, 4)]:
