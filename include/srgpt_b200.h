@@ -359,6 +359,57 @@ int srgpt_llama_decode_step_packed_bf16(void* h, const srgpt_llama_layer_weights
                                         const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids, int* step,
                                         void* stream);
 
+/* ---- prompt-lookup speculative decoding, batch 1, greedy (HF GenerationMixin._assisted_decoding with
+ * PromptLookupCandidateGenerator, i.e. generate(prompt_lookup_num_tokens=k); call site llava_llama.py:212).
+ * A verify pass runs T = k + 1 tokens at positions pos .. pos+T-1: row 0 is the last emitted token, rows 1..T-1 the drafts.
+ * For every token t the kernels below do the fp32 operations of the one-token kernels at position pos+t in the same order, so
+ * the accepted tokens and their logits are bit-identical to plain greedy decoding.  T is 1 .. SRGPT_SPEC_T_MAX. */
+#define SRGPT_SPEC_T_MAX 8
+/* srgpt_gemv_bf16 over T activation rows x [T, ldx] -> y [T, ldy] (residual, when given, has y's layout), each weight streamed
+ * once for all rows.  QKV_ROPE: row t is rotated at and appends K/V at position *pos + t.  T = 1 is srgpt_gemv_bf16. */
+int srgpt_gemv_multi_bf16(const void* x, int ldx, const void* W, int ldw, void* y, int ldy, int T, int N, int K, const void* norm_weight,
+                          float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
+                          const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream);
+int srgpt_gemv_multi_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, void* y, int ldy, int T, int N, int K,
+                                 const void* norm_weight, float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim,
+                                 const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size,
+                                 void* stream);
+/* final norm + lm_head over T rows: fp32 logits [T, V] (optional) and per-(token, CTA) arg max partials in `workspace`
+ * (T * srgpt_lm_head_workspace(V) bytes, token t's block at t * srgpt_lm_head_workspace(V)); srgpt_spec_accept reduces them. */
+int srgpt_lm_head_multi_bf16(const void* x, int ldx, const void* W, int ldw, int T, int V, int K, const void* norm_weight, float eps,
+                             float* logits_out, void* workspace, void* stream);
+int srgpt_lm_head_multi_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, int T, int V, int K, const void* norm_weight, float eps,
+                                    float* logits_out, void* workspace, void* stream);
+/* Decode attention of T consecutive tokens of one sequence: token t (q row t, out row t) attends over kv rows 0 .. pos_rows[t]
+ * (device int32 [T]).  The arithmetic of srgpt_attention_decode_bf16 per token. */
+int srgpt_attention_decode_multi_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages, const int* page_table, int page_size,
+                                      const int* pos_rows, int T, int n_heads, int n_kv_heads, int head_dim, float scale, void* stream);
+/* Start of a verify pass (one CTA): the drafts by n-gram lookup (PromptLookupCandidateGenerator.get_candidates: n-gram sizes from
+ * ngram down to 1, the earliest match with a non-empty continuation, at most T-1 tokens) over the history prompt_ids[0..*prompt_len)
+ * (a negative id is a sentinel that never matches) followed by out_ids[0..*step).  Writes draft_ids [T] (row 0 = the last emitted
+ * token, missing drafts = -1), the embedding rows x [T, H], pos_rows[t] = *pos + t and state[3] = number of drafts. */
+int srgpt_spec_draft(const int* prompt_ids, const int* prompt_len, const long long* out_ids, const int* step, const int* pos, int* pos_rows, int T, int ngram,
+                     const void* embed_table, void* x, int H, int* draft_ids, int* state, void* stream);
+/* End of a verify pass (one CTA): the T arg maxes (lowest index on ties), a = the number of leading drafts equal to the model's
+ * choices, out_ids[*step .. *step + a] = the a + 1 new tokens, *step and *pos advance by a + 1.  state (int32 [8]): [0] passes,
+ * [1] drafted, [2] accepted, [4] step before the pass, [5] tokens emitted, [6] step after.  logits_all != NULL: the accepted
+ * rows of logits_rows [T, V] are copied to logits_all rows *step ...  Writes past out_cap are dropped. */
+int srgpt_spec_accept(const void* workspace, int V, int T, const int* draft_ids, long long* out_ids, int out_cap, int* step, int* pos, int* state,
+                      const float* logits_rows, float* logits_all, void* stream);
+/* One whole verify pass: draft, 5 kernels per layer, lm_head, accept.  Buffers: h [T, H], q_buf / attn_buf [T, nh*hd], act_buf
+ * [T, I], lm_workspace T * srgpt_lm_head_workspace(V) bytes, logits_rows [T, V] (needed when logits_all != NULL). */
+int srgpt_llama_verify_step_bf16(void* h, const srgpt_llama_layer_weights* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int T,
+                                 int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos,
+                                 int* pos_rows, const int* page_table, int page_size, const void* final_norm, const void* lm_head, int V,
+                                 const void* embed_table, void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids,
+                                 const int* prompt_len, int ngram, int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream);
+int srgpt_llama_verify_step_packed_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers,
+                                        void* q_buf, void* attn_buf, void* act_buf, int T, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                        float eps, const void* cos_tab, const void* sin_tab, int* pos, int* pos_rows, const int* page_table,
+                                        int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+                                        const void* embed_table, void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids,
+                                        const int* prompt_len, int ngram, int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

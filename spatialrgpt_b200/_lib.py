@@ -89,7 +89,20 @@ SIGNATURES = {
     "srgpt_lm_head_argmax_packed_bf16": (ci, [vp, vp, ci, ci, vp, cf, vp, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_llama_decode_step_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp,
                                                  vp, vp, vp, vp]),
+    "srgpt_gemv_multi_bf16": (ci, [vp, ci, vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_gemv_multi_packed_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_lm_head_multi_bf16": (ci, [vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, vp, vp]),
+    "srgpt_lm_head_multi_packed_bf16": (ci, [vp, ci, vp, ci, ci, ci, vp, cf, vp, vp, vp]),
+    "srgpt_attention_decode_multi_bf16": (ci, [vp, ci, vp, ci, vp, vp, ci, vp, ci, ci, ci, ci, cf, vp]),
+    "srgpt_spec_draft": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, ci, vp, vp, vp]),
+    "srgpt_spec_accept": (ci, [vp, ci, ci, vp, vp, ci, vp, vp, vp, vp, vp, vp]),
+    "srgpt_llama_verify_step_bf16": (ci, [vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp, vp,
+                                          vp, vp, ci, vp, vp, ci, vp, vp, vp]),
+    "srgpt_llama_verify_step_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp,
+                                                 vp, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp]),
 }
+
+SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)
 
 
 class SiglipLayerWeights(C.Structure):

@@ -516,6 +516,361 @@ lm_head_finalize_kernel(const float* __restrict__ part_val, const int* __restric
   }
 }
 
+// ---- multi-token decode GEMV (verify pass of prompt-lookup speculative decoding) ------------------------------------------------
+// The warp / row-pair layout, chunk ownership (c = lane + 32 i), dot8 chains, warp_sum, stage_x (at 256 threads, so the RMSNorm
+// reduction tree is the same) and epilogues of decode_gemv_kernel, run for MT tokens against one stream of the weights: for every
+// token the fp32 operations and their order are those of the one-token kernel, so each output is bit-identical to it.
+// x is staged in shared memory for all tokens.  With RMSNorm (K = hidden size) the whole row is staged; without (o_proj, down_proj:
+// K up to 14336 = 28 KB per token) x is staged in tiles of MT_TILE_CH chunks, so 8 tokens take 64 KB and 2 CTAs (16 warps) stay
+// resident per SM.  The next 4-chunk batch of weights is loaded into registers while the current one is consumed.
+constexpr int MT_MAX = SRGPT_SPEC_T_MAX;
+constexpr int MT_TILE_CH = 512;  // x chunks (of 8 elements) per staged tile without RMSNorm; a multiple of the 128-chunk batch
+
+struct MParams {
+  Params p;
+  int T;        // tokens (rows of x / y)
+  int ldx, ldy;  // row strides of x and y (residual) in elements
+  int tile_ch;  // chunks of x per staged tile
+};
+
+template <int MODE, bool PACKED>
+__global__ void __launch_bounds__(THREADS, 2) decode_gemv_multi_kernel(const MParams mp) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ float red[32];
+  __shared__ float sv[MT_MAX][WARPS];
+  __shared__ int si[MT_MAX][WARPS];
+  const Params& p = mp.p;
+  const int nt = mp.T, tile_ch = mp.tile_ch;
+  bf16* sx = reinterpret_cast<bf16*>(smem_raw);
+  const uint4* px = reinterpret_cast<const uint4*>(sx);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int npairs = (MODE == MODE_LM) ? ((p.N + 1) >> 1) : (p.N >> 1);
+  const int pi = blockIdx.x * WARPS + warp;
+  const bool active = pi < npairs;
+  int r0 = 0, r1 = 0;
+  if (active) pair_rows<MODE>(p, pi, r0, r1);
+  const int nchunk = p.K >> 3;
+  const int nbatch = (nchunk + 127) >> 7;
+
+  // ---- weights: batch 0 is requested before the dependency wait
+  const uint4* p0 = reinterpret_cast<const uint4*>(p.W + (size_t)r0 * p.ldw);
+  const uint4* p1 = reinterpret_cast<const uint4*>(p.W + (size_t)r1 * p.ldw);
+  uint4 u0[4], u1[4];
+  Raw12 q0 = {}, q1 = {};
+  Rows12 rs = {};
+  const uint4 *sm0 = nullptr, *ex0 = nullptr;
+  const int drow_ex = (r1 - r0) * (p.K >> 5);
+  auto load_plain = [&](int b, uint4 (&w0)[4], uint4 (&w1)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = b * 128 + lane + 32 * i;
+      w0[i] = make_uint4(0, 0, 0, 0);
+      w1[i] = make_uint4(0, 0, 0, 0);
+      if (c < nchunk) {
+        w0[i] = ld_stream16(p0 + c);
+        w1[i] = ld_stream16(p1 + c);
+      }
+    }
+  };
+  if (active) {
+    if constexpr (PACKED) {
+      sm0 = reinterpret_cast<const uint4*>(p.pk.sm) + (size_t)r0 * (p.K >> 4) + lane;
+      ex0 = reinterpret_cast<const uint4*>(p.pk.ex) + (size_t)r0 * (p.K >> 5) + lane;
+      q0 = ld_raw12(sm0, ex0, 0);
+      q1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, 0);
+      const int e0 = p.pk.row_ptr[r0], e1 = p.pk.row_ptr[r1];
+      rs.n0 = min(p.pk.row_ptr[r0 + 1] - e0, pack12::MAX_EXC_PER_ROW);
+      rs.n1 = min(p.pk.row_ptr[r1 + 1] - e1, pack12::MAX_EXC_PER_ROW);
+      if (lane < rs.n0) rs.exc0 = p.pk.exc[e0 + lane];
+      if (lane < rs.n1) rs.exc1 = p.pk.exc[e1 + lane];
+      rs.bp0 = (uint32_t)p.pk.base[r0] - 1u;
+      rs.bp1 = (uint32_t)p.pk.base[r1] - 1u;
+    } else {
+      load_plain(0, u0, u1);
+    }
+  }
+  uint4 nw_pre[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
+  const bool nw_pre_valid = (p.norm_weight != nullptr) && (nchunk <= 2 * THREADS);
+  if (nw_pre_valid) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int cc = threadIdx.x + k * THREADS;
+      if (cc < nchunk) nw_pre[k] = reinterpret_cast<const uint4*>(p.norm_weight)[cc];
+    }
+  }
+  pdl_launch_dependents();
+  pdl_wait();
+
+  float a0[MT_MAX], a1[MT_MAX];
+#pragma unroll
+  for (int t = 0; t < MT_MAX; ++t) a0[t] = a1[t] = 0.f;
+  int b = 0;
+  for (int c0 = 0; c0 < nchunk; c0 += tile_ch) {
+    const int tlen = min(tile_ch, nchunk - c0);
+    if (p.norm_weight != nullptr) {  // one tile holds the whole row (tile_ch == nchunk)
+      for (int t = 0; t < nt; ++t)
+        stage_x(p.x + (size_t)t * mp.ldx, p.norm_weight, p.eps, p.K, sx + (size_t)t * tile_ch * 8, red, nw_pre, nw_pre_valid);
+    } else {
+      __syncthreads();  // the previous tile is consumed
+      for (int t = 0; t < nt; ++t) {
+        const uint4* src = reinterpret_cast<const uint4*>(p.x + (size_t)t * mp.ldx) + c0;
+        uint4* dst = reinterpret_cast<uint4*>(sx) + (size_t)t * tile_ch;
+        for (int cc = threadIdx.x; cc < tlen; cc += THREADS) dst[cc] = src[cc];
+      }
+      __syncthreads();
+    }
+    if (!active) continue;
+    for (; b < nbatch && b * 128 < c0 + tlen; ++b) {
+      // batch 0 was requested before the wait; every later batch is requested here (a double-buffered variant needed more than
+      // the 128 registers of 2 CTAs per SM and spilled)
+      uint4 w0[4], w1[4];
+      if constexpr (PACKED) {
+        if (b > 0) {
+          q0 = ld_raw12(sm0, ex0, b);
+          q1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, b);
+        }
+        decode_batch(q0, rs.bp0, w0);
+        decode_batch(q1, rs.bp1, w1);
+        patch_batch(w0, rs.exc0, rs.n0, rs.j0, b, lane);
+        patch_batch(w1, rs.exc1, rs.n1, rs.j1, b, lane);
+      } else {
+        if (b > 0) load_plain(b, u0, u1);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          w0[i] = u0[i];
+          w1[i] = u1[i];
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int c = b * 128 + lane + 32 * i;
+        if (c < nchunk) {
+#pragma unroll
+          for (int t = 0; t < MT_MAX; ++t) {
+            if (t < nt) {
+              float xf[8];
+              unpack8(px[(size_t)t * tile_ch + (c - c0)], xf);
+              a0[t] += dot8(w0[i], xf);
+              a1[t] += dot8(w1[i], xf);
+            }
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int t = 0; t < MT_MAX; ++t) {
+    if (t < nt) {
+      a0[t] = warp_sum(a0[t]);
+      a1[t] = warp_sum(a1[t]);
+    }
+  }
+  // lane t runs token t's epilogue (every lane holds every token's sums after warp_sum)
+  float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+  for (int t = 0; t < MT_MAX; ++t) {
+    if (t == lane) {
+      s0 = a0[t];
+      s1 = a1[t];
+    }
+  }
+  if (active && lane < nt) {
+    {
+      const int t = lane;
+      bf16* y = p.y + (size_t)t * mp.ldy;
+      if (MODE == SRGPT_GEMV_PLAIN) {
+        float y0 = bf16_round(s0), y1 = bf16_round(s1);
+        if (p.residual != nullptr) {
+          const bf16* res = p.residual + (size_t)t * mp.ldy;
+          y0 += e2f(res[r0]);
+          y1 += e2f(res[r1]);
+        }
+        *reinterpret_cast<uint32_t*>(y + r0) = pack_bf16x2(y0, y1);
+      } else if (MODE == SRGPT_GEMV_SWIGLU) {
+        const float g = bf16_round(s0), u = bf16_round(s1);
+        y[pi] = f2e(bf16_round(silu(g)) * u);
+      } else if (MODE == SRGPT_GEMV_QKV_ROPE) {
+        const int half = p.hd >> 1;
+        const int head = pi / half, j = pi - head * half;
+        float v0 = bf16_round(s0), v1 = bf16_round(s1);
+        const int pos = *p.pos + t;
+        if (head < p.n_heads + p.n_kv_heads) {
+          const float cs = e2f(p.cos_tab[(size_t)pos * half + j]);
+          const float sn = e2f(p.sin_tab[(size_t)pos * half + j]);
+          const float o0 = bf16_round(bf16_round(v0 * cs) + bf16_round(-v1 * sn));
+          const float o1 = bf16_round(bf16_round(v1 * cs) + bf16_round(v0 * sn));
+          v0 = o0;
+          v1 = o1;
+        }
+        if (head < p.n_heads) {
+          y[r0] = f2e(v0);
+          y[r1] = f2e(v1);
+        } else {
+          const int page = p.page_table[pos / p.page_size], slot = pos % p.page_size;
+          const bool is_v = head >= p.n_heads + p.n_kv_heads;
+          const int kh = head - p.n_heads - (is_v ? p.n_kv_heads : 0);
+          bf16* dst = p.kv_pages + (((size_t)page * 2 + (is_v ? 1 : 0)) * p.page_size + slot) * ((size_t)p.n_kv_heads * p.hd) + kh * p.hd;
+          dst[j] = f2e(v0);
+          dst[j + half] = f2e(v1);
+        }
+      } else {  // MODE_LM
+        const float l0 = bf16_round(s0), l1 = bf16_round(s1);
+        if (p.logits_out != nullptr) {
+          float* lo = p.logits_out + (size_t)t * p.N;
+          lo[r0] = l0;
+          if (r1 != r0) lo[r1] = l1;
+        }
+        float best = l0;
+        int besti = r0;
+        if (r1 != r0 && better(l1, r1, best, besti)) { best = l1; besti = r1; }
+        sv[t][warp] = best;
+        si[t][warp] = besti;
+      }
+    }
+  }
+  if (MODE == MODE_LM) {
+    if (!active && lane < nt) {
+      sv[lane][warp] = -INFINITY;
+      si[lane][warp] = 0x7fffffff;
+    }
+    __syncthreads();
+    if (threadIdx.x < nt) {  // the CTA reduction of decode_gemv_kernel, one thread per token
+      const int t = threadIdx.x;
+      float best = sv[t][0];
+      int besti = si[t][0];
+      for (int w = 1; w < WARPS; ++w)
+        if (better(sv[t][w], si[t][w], best, besti)) { best = sv[t][w]; besti = si[t][w]; }
+      float* pv = p.part_val + (size_t)t * 2 * gridDim.x;
+      pv[blockIdx.x] = best;
+      reinterpret_cast<int*>(pv + gridDim.x)[blockIdx.x] = besti;
+    }
+  }
+}
+
+// ---- the two ends of a verify pass -------------------------------------------------------------------------------------------
+// History of the n-gram lookup: the prompt's ids (negative = a row that is not text: never matches), then the generated ids.
+struct SpecHist {
+  const int* prompt;
+  int P;
+  const long long* out;
+  __device__ __forceinline__ int operator()(int i) const { return i < P ? prompt[i] : (int)out[i - P]; }
+};
+
+__global__ void __launch_bounds__(256)
+spec_draft_kernel(const int* __restrict__ prompt_ids, const int* __restrict__ prompt_len, const long long* __restrict__ out_ids, const int* __restrict__ step,
+                  const int* __restrict__ pos, int* __restrict__ pos_rows, int T, int ngram, const bf16* __restrict__ embed_table,
+                  bf16* __restrict__ x, int H, int* __restrict__ draft_ids, int* __restrict__ state) {
+  __shared__ int s_min[8];
+  __shared__ int s_draft[MT_MAX];
+  const int P = prompt_len != nullptr ? *prompt_len : 0;
+  const SpecHist hist{prompt_ids, P, out_ids};
+  const int s = *step, L = P + s;
+  int start = -1;
+  for (int n = min(ngram, L - 1); n >= 1 && start < 0; --n) {
+    // the earliest window i < L - n equal to the last n ids (a window at i < L - n has a non-empty continuation)
+    int best = 0x7fffffff;
+    for (int i = threadIdx.x; i < L - n; i += blockDim.x) {
+      bool eq = true;
+      for (int j = 0; j < n && eq; ++j) {
+        const int v = hist(i + j);
+        eq = v >= 0 && v == hist(L - n + j);
+      }
+      if (eq) { best = i; break; }  // i grows along the loop: the thread's first hit is its earliest
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+    if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = best;
+    __syncthreads();
+    int m = 0x7fffffff;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m = min(m, s_min[w]);
+    __syncthreads();
+    if (m != 0x7fffffff) start = m + n;
+  }
+  if (threadIdx.x == 0) {
+    int nd = 0;
+    s_draft[0] = hist(L - 1);
+    for (int t = 1; t < T; ++t) {
+      int v = -1;
+      if (start >= 0 && nd == t - 1 && start + t - 1 < L) {
+        v = hist(start + t - 1);
+        if (v >= 0) ++nd; else v = -1;  // a draft ends at the first non-text row
+      }
+      s_draft[t] = v;
+    }
+    state[3] = nd;
+  }
+  __syncthreads();
+  if (threadIdx.x < T) {
+    draft_ids[threadIdx.x] = s_draft[threadIdx.x];
+    pos_rows[threadIdx.x] = *pos + (int)threadIdx.x;
+  }
+  for (int t = 0; t < T; ++t) {  // embedding rows of the pass (a missing draft takes row 0: it is never accepted)
+    const uint4* src = reinterpret_cast<const uint4*>(embed_table + (size_t)max(s_draft[t], 0) * H);
+    uint4* dst = reinterpret_cast<uint4*>(x + (size_t)t * H);
+    for (int c = threadIdx.x; c < (H >> 3); c += blockDim.x) dst[c] = src[c];
+  }
+}
+
+// The arg max of every token reduces its partials exactly as lm_head_finalize_kernel does; then the acceptance rule.
+__global__ void __launch_bounds__(256)
+spec_accept_kernel(const float* __restrict__ ws, int nparts, int T, const int* __restrict__ draft_ids, long long* __restrict__ out_ids, int out_cap,
+                   int* step, int* pos, int* state) {
+  __shared__ float sv[8];
+  __shared__ int si[8];
+  __shared__ int s_tok[MT_MAX];
+  pdl_launch_dependents();
+  pdl_wait();
+  for (int t = 0; t < T; ++t) {
+    const float* part_val = ws + (size_t)t * 2 * nparts;
+    const int* part_idx = reinterpret_cast<const int*>(part_val + nparts);
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = threadIdx.x; i < nparts; i += blockDim.x)
+      if (better(part_val[i], part_idx[i], best, bi)) { best = part_val[i]; bi = part_idx[i]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (better(ov, oi, best, bi)) { best = ov; bi = oi; }
+    }
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < 8; ++w)
+        if (better(sv[w], si[w], best, bi)) { best = sv[w]; bi = si[w]; }
+      if (bi == 0x7fffffff) bi = 0;
+      s_tok[t] = bi;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    int a = 0;
+    while (a < T - 1 && draft_ids[a + 1] == s_tok[a]) ++a;
+    const int s0 = *step;
+    for (int t = 0; t <= a; ++t)
+      if (s0 + t < out_cap) out_ids[s0 + t] = (long long)s_tok[t];
+    state[0] += 1;
+    state[1] += state[3];
+    state[2] += a;
+    state[4] = s0;
+    state[5] = a + 1;
+    state[6] = s0 + a + 1;
+    *step = s0 + a + 1;
+    *pos += a + 1;
+  }
+}
+
+// output_logits: the accepted rows of the pass's logits [T, V] go to rows state[4] .. state[4] + state[5] - 1
+__global__ void __launch_bounds__(256) spec_copy_logits_kernel(const float* __restrict__ rows, float* __restrict__ all, int V, const int* __restrict__ state,
+                                                               int out_cap) {
+  const int t = blockIdx.y;
+  if (t >= state[5] || state[4] + t >= out_cap) return;
+  const float* src = rows + (size_t)t * V;
+  float* dst = all + (size_t)(state[4] + t) * V;
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < V; j += gridDim.x * blockDim.x) dst[j] = src[j];
+}
+
 // ---- tensor-parallel helpers ------------------------------------------------------------------------
 // vocabulary-parallel lm_head: this rank's best (bf16-rounded logit, GLOBAL row index) -> best[0] = value bits, best[1] = index
 __global__ void __launch_bounds__(256)
@@ -887,4 +1242,177 @@ extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_argmax_packe
   p.pk = *packed;
   return lm_head_argmax<true>(p, x, V, K, norm_weight, eps, logits_out, workspace, embed_table, next_x, out_ids, step, pos, stream);
 #endif
+}
+
+// ---- prompt-lookup speculative decoding: multi-token GEMV, lm_head, draft and accept ------------------------------------------
+namespace srgpt {
+namespace gemv {
+
+template <int MODE, bool PACKED>
+static int launch_multi(MParams& mp, int npairs, cudaStream_t st) {
+  const int smem = mp.T * mp.tile_ch * 16;
+  static int configured_smem = 0;
+  if (smem > configured_smem) {  // the opt-in counts static shared memory too, so it is set for every size, not only above 48 KB
+    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_multi_kernel<MODE, PACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured_smem = smem;
+  }
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  pdl_config(cfg, attr, grid_for(npairs), THREADS, smem, st);
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, decode_gemv_multi_kernel<MODE, PACKED>, mp));
+  return SRGPT_OK;
+}
+
+// x staged per token: the whole row with RMSNorm, tiles of MT_TILE_CH chunks without
+static int multi_tile(int K, bool norm) { return norm ? (K >> 3) : ((K >> 3) < MT_TILE_CH ? (K >> 3) : MT_TILE_CH); }
+
+}  // namespace gemv
+}  // namespace srgpt
+
+template <bool PACKED>
+static int gemv_multi_modes(gemv::MParams& mp, const void* x, int ldx, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
+                            const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+                            const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(x && y && N > 0 && K > 0 && T >= 1 && T <= gemv::MT_MAX);
+  SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0 && (ldx % 8) == 0 && ldx >= K && (ldy % 2) == 0);
+  SRGPT_CHECK_ARG(aligned16(x) && (reinterpret_cast<uintptr_t>(y) & 3) == 0);
+  SRGPT_CHECK_ARG(norm_weight == nullptr || aligned16(norm_weight));
+  SRGPT_CHECK_ARG(mode >= SRGPT_GEMV_PLAIN && mode <= SRGPT_GEMV_QKV_ROPE);
+  SRGPT_CHECK_ARG(x != y);
+  const int tile = gemv::multi_tile(K, norm_weight != nullptr);
+  SRGPT_CHECK_ARG(T * tile * 16 <= 200 * 1024);
+  gemv::Params& p = mp.p;
+  p.x = reinterpret_cast<const bf16*>(x);
+  p.y = reinterpret_cast<bf16*>(y);
+  p.N = N; p.K = K;
+  p.norm_weight = reinterpret_cast<const bf16*>(norm_weight);
+  p.eps = eps;
+  p.residual = reinterpret_cast<const bf16*>(residual);
+  p.n_heads = n_heads; p.n_kv_heads = n_kv_heads; p.hd = head_dim;
+  p.cos_tab = reinterpret_cast<const bf16*>(cos_tab);
+  p.sin_tab = reinterpret_cast<const bf16*>(sin_tab);
+  p.pos = pos;
+  p.kv_pages = reinterpret_cast<bf16*>(kv_pages);
+  p.page_table = page_table;
+  p.page_size = page_size;
+  mp.T = T; mp.ldx = ldx; mp.ldy = ldy; mp.tile_ch = tile;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (mode) {
+    case SRGPT_GEMV_PLAIN:
+      SRGPT_CHECK_ARG(ldy >= N);
+      p.hd = 2;
+      return gemv::launch_multi<SRGPT_GEMV_PLAIN, PACKED>(mp, N / 2, st);
+    case SRGPT_GEMV_SWIGLU:
+      SRGPT_CHECK_ARG(residual == nullptr && ldy >= N / 2);
+      p.hd = 2;
+      return gemv::launch_multi<SRGPT_GEMV_SWIGLU, PACKED>(mp, N / 2, st);
+    case SRGPT_GEMV_QKV_ROPE:
+      SRGPT_CHECK_ARG(residual == nullptr && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && (head_dim % 2) == 0);
+      SRGPT_CHECK_ARG(N == (n_heads + 2 * n_kv_heads) * head_dim && ldy >= n_heads * head_dim);
+      SRGPT_CHECK_ARG(cos_tab && sin_tab && pos && kv_pages && page_table && page_size > 0);
+      return gemv::launch_multi<SRGPT_GEMV_QKV_ROPE, PACKED>(mp, N / 2, st);
+  }
+  return SRGPT_ERR_INVALID;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_multi_bf16(const void* x, int ldx, const void* W, int ldw, void* y, int ldy, int T, int N, int K,
+                                                                            const void* norm_weight, float eps, const void* residual, int mode, int n_heads,
+                                                                            int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos,
+                                                                            void* kv_pages, const int* page_table, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(W && aligned16(W) && (ldw % 8) == 0 && ldw >= K);
+  gemv::MParams mp = {};
+  mp.p.W = reinterpret_cast<const bf16*>(W);
+  mp.p.ldw = ldw;
+  return gemv_multi_modes<false>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                                 kv_pages, page_table, page_size, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_multi_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, void* y, int ldy, int T,
+                                                                                   int N, int K, const void* norm_weight, float eps, const void* residual,
+                                                                                   int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
+                                                                                   const void* sin_tab, const int* pos, void* kv_pages, const int* page_table,
+                                                                                   int page_size, void* stream) {
+  SRGPT_CHECK_ARG(packed_ok(packed, K));
+#ifdef SRGPT_ELEM_F16
+  set_last_error("srgpt_gemv_multi_packed_bf16: the 12-bit packing is defined for bfloat16 weights only");
+  return SRGPT_ERR_UNSUPPORTED;
+#else
+  gemv::MParams mp = {};
+  mp.p.pk = *packed;
+  return gemv_multi_modes<true>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                                kv_pages, page_table, page_size, stream);
+#endif
+}
+
+template <bool PACKED>
+static int lm_head_multi(gemv::MParams& mp, const void* x, int ldx, int T, int V, int K, const void* norm_weight, float eps, float* logits_out,
+                         void* workspace, void* stream) {
+  SRGPT_CHECK_ARG(x && workspace && V > 0 && K > 0 && T >= 1 && T <= gemv::MT_MAX);
+  SRGPT_CHECK_ARG((K % 8) == 0 && (ldx % 8) == 0 && ldx >= K && aligned16(x) && (norm_weight == nullptr || aligned16(norm_weight)));
+  const int tile = gemv::multi_tile(K, norm_weight != nullptr);
+  SRGPT_CHECK_ARG(T * tile * 16 <= 200 * 1024);
+  gemv::Params& p = mp.p;
+  p.x = reinterpret_cast<const bf16*>(x);
+  p.N = V; p.K = K;
+  p.norm_weight = reinterpret_cast<const bf16*>(norm_weight);
+  p.eps = eps;
+  p.hd = 2;
+  p.logits_out = logits_out;
+  p.part_val = reinterpret_cast<float*>(workspace);
+  mp.T = T; mp.ldx = ldx; mp.ldy = 0; mp.tile_ch = tile;
+  return gemv::launch_multi<gemv::MODE_LM, PACKED>(mp, (V + 1) / 2, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_multi_bf16(const void* x, int ldx, const void* W, int ldw, int T, int V, int K,
+                                                                               const void* norm_weight, float eps, float* logits_out, void* workspace,
+                                                                               void* stream) {
+  SRGPT_CHECK_ARG(W && aligned16(W) && (ldw % 8) == 0 && ldw >= K);
+  gemv::MParams mp = {};
+  mp.p.W = reinterpret_cast<const bf16*>(W);
+  mp.p.ldw = ldw;
+  return lm_head_multi<false>(mp, x, ldx, T, V, K, norm_weight, eps, logits_out, workspace, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_lm_head_multi_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, int T, int V, int K,
+                                                                                      const void* norm_weight, float eps, float* logits_out, void* workspace,
+                                                                                      void* stream) {
+  SRGPT_CHECK_ARG(packed_ok(packed, K));
+#ifdef SRGPT_ELEM_F16
+  set_last_error("srgpt_lm_head_multi_packed_bf16: the 12-bit packing is defined for bfloat16 weights only");
+  return SRGPT_ERR_UNSUPPORTED;
+#else
+  gemv::MParams mp = {};
+  mp.p.pk = *packed;
+  return lm_head_multi<true>(mp, x, ldx, T, V, K, norm_weight, eps, logits_out, workspace, stream);
+#endif
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_spec_draft(const int* prompt_ids, const int* prompt_len, const long long* out_ids, const int* step, const int* pos,
+                                                                       int* pos_rows, int T, int ngram, const void* embed_table, void* x, int H, int* draft_ids,
+                                                                       int* state, void* stream) {
+  SRGPT_CHECK_ARG(out_ids && step && pos && pos_rows && embed_table && x && draft_ids && state && ((prompt_ids == nullptr) == (prompt_len == nullptr)));
+  SRGPT_CHECK_ARG(T >= 1 && T <= gemv::MT_MAX && ngram >= 1 && H > 0 && (H % 8) == 0 && aligned16(embed_table) && aligned16(x));
+  gemv::spec_draft_kernel<<<1, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(prompt_ids, prompt_len, out_ids, step, pos, pos_rows, T, ngram,
+                                                                                 reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(x), H,
+                                                                                 draft_ids, state);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_spec_accept(const void* workspace, int V, int T, const int* draft_ids, long long* out_ids, int out_cap,
+                                                                        int* step, int* pos, int* state, const float* logits_rows, float* logits_all,
+                                                                        void* stream) {
+  SRGPT_CHECK_ARG(workspace && draft_ids && out_ids && step && pos && state && V > 0 && T >= 1 && T <= gemv::MT_MAX && out_cap > 0);
+  SRGPT_CHECK_ARG(logits_all == nullptr || logits_rows != nullptr);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  gemv::pdl_config(cfg, attr, 1, 256, 0, st);
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemv::spec_accept_kernel, reinterpret_cast<const float*>(workspace), gemv::grid_for((V + 1) / 2), T, draft_ids,
+                                      out_ids, out_cap, step, pos, state));
+  if (logits_all != nullptr) {
+    gemv::spec_copy_logits_kernel<<<dim3(ceil_div(V, 256 * 8), T), 256, 0, st>>>(logits_rows, logits_all, V, state, out_cap);
+    SRGPT_CHECK_LAUNCH();
+  }
+  return SRGPT_OK;
 }

@@ -156,3 +156,70 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_pa
   return decode_step(h, layers, packed, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos, page_table,
                      page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
 }
+
+// ---- verify pass of prompt-lookup speculative decoding: T tokens through the layer stack, every weight streamed once -----------
+static int gemv_multi_either(const void* x, int ldx, const void* W, const srgpt_packed12* pk, void* y, int ldy, int T, int N, int K,
+                             const void* norm_weight, float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim,
+                             const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size,
+                             void* stream) {
+  if (pk != nullptr && pk->sm != nullptr)
+    return srgpt_gemv_multi_packed_bf16(x, ldx, pk, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab,
+                                        pos, kv_pages, page_table, page_size, stream);
+  return srgpt_gemv_multi_bf16(x, ldx, W, K, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                               kv_pages, page_table, page_size, stream);
+}
+
+static int verify_step(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers, void* q_buf,
+                       void* attn_buf, void* act_buf, int T, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab,
+                       const void* sin_tab, int* pos, int* pos_rows, const int* page_table, int page_size, const void* final_norm,
+                       const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
+                       float* logits_rows, float* logits_all, const int* prompt_ids, const int* prompt_len, int ngram, int* draft_ids, long long* out_ids,
+                       int out_cap, int* step, int* state, void* stream) {
+  SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos && pos_rows && page_table && final_norm && lm_head && lm_workspace && out_ids &&
+                  step && state && draft_ids);
+  SRGPT_CHECK_ARG(logits_all == nullptr || logits_rows != nullptr);
+  const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
+  const float scale = 1.0f / sqrtf((float)head_dim);
+  SRGPT_TRY(srgpt_spec_draft(prompt_ids, prompt_len, out_ids, step, pos, pos_rows, T, ngram, embed_table, h, H, draft_ids, state, stream));
+  for (int l = 0; l < n_layers; ++l) {
+    const srgpt_llama_layer_weights& w = layers[l];
+    const srgpt_llama_layer_packed* pk = packed != nullptr ? &packed[l] : nullptr;
+    SRGPT_TRY(gemv_multi_either(h, H, w.qkv_w, pk ? &pk->qkv : nullptr, q_buf, qd, T, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads,
+                                n_kv_heads, head_dim, cos_tab, sin_tab, pos, w.kv_pages, page_table, page_size, stream));
+    SRGPT_TRY(srgpt_attention_decode_multi_bf16(q_buf, qd, attn_buf, qd, w.kv_pages, page_table, page_size, pos_rows, T, n_heads, n_kv_heads, head_dim,
+                                                scale, stream));
+    SRGPT_TRY(gemv_multi_either(attn_buf, qd, w.o_w, pk ? &pk->o : nullptr, h, H, T, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr,
+                                nullptr, nullptr, nullptr, 0, stream));
+    SRGPT_TRY(gemv_multi_either(h, H, w.gateup_w, pk ? &pk->gateup : nullptr, act_buf, I, T, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, 0, 0,
+                                0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, stream));
+    SRGPT_TRY(gemv_multi_either(act_buf, I, w.down_w, pk ? &pk->down : nullptr, h, H, T, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr,
+                                nullptr, nullptr, nullptr, nullptr, 0, stream));
+  }
+  if (lm_packed != nullptr && lm_packed->sm != nullptr)
+    SRGPT_TRY(srgpt_lm_head_multi_packed_bf16(h, H, lm_packed, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream));
+  else
+    SRGPT_TRY(srgpt_lm_head_multi_bf16(h, H, lm_head, H, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream));
+  return srgpt_spec_accept(lm_workspace, V, T, draft_ids, out_ids, out_cap, step, pos, state, logits_rows, logits_all, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_verify_step_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int T, int H, int n_heads,
+    int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos, int* pos_rows, const int* page_table,
+    int page_size, const void* final_norm, const void* lm_head, int V, const void* embed_table, void* lm_workspace, float* logits_rows,
+    float* logits_all, const int* prompt_ids, const int* prompt_len, int ngram, int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream) {
+  return verify_step(h, layers, nullptr, n_layers, q_buf, attn_buf, act_buf, T, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos, pos_rows,
+                     page_table, page_size, final_norm, lm_head, nullptr, V, embed_table, lm_workspace, logits_rows, logits_all, prompt_ids, prompt_len, ngram,
+                     draft_ids, out_ids, out_cap, step, state, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_verify_step_packed_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers, void* q_buf, void* attn_buf, void* act_buf,
+    int T, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos, int* pos_rows,
+    const int* page_table, int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
+    void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids, const int* prompt_len, int ngram, int* draft_ids, long long* out_ids, int out_cap,
+    int* step, int* state, void* stream) {
+  SRGPT_CHECK_ARG(packed != nullptr);
+  return verify_step(h, layers, packed, n_layers, q_buf, attn_buf, act_buf, T, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos, pos_rows,
+                     page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows, logits_all, prompt_ids, prompt_len, ngram,
+                     draft_ids, out_ids, out_cap, step, state, stream);
+}

@@ -218,10 +218,12 @@ def get_depth_predictor(spec: Optional[str] = None) -> Optional[Callable[[np.nda
 
 def answer_questions(line: Dict[str, Any], model, tokenizer, image_processor, image, depth, masks: Optional[torch.Tensor], conv_mode: str,
                      model_name: str, image_file: str, max_new_tokens: int = 128, temperature: float = 0.0, top_p=None,
-                     num_beams: int = 1, prefix_cache: bool = False) -> List[Dict[str, Any]]:
+                     num_beams: int = 1, prefix_cache: bool = False, prompt_lookup_num_tokens: int = 0) -> List[Dict[str, Any]]:
     """All question turns of one annotation (the conversation accumulates, as in the reference) -> JSONL records.
     ``prefix_cache``: each turn reuses the previous turn's encoder outputs and prompt K/V and prefills only the new question
-    (generate(prefix_cache=True)); answers match a full re-prefill up to bf16 rounding."""
+    (generate(prefix_cache=True)); answers match a full re-prefill up to bf16 rounding.
+    ``prompt_lookup_num_tokens=k > 0``: greedy answers are decoded by prompt lookup with up to k drafts per verify pass
+    (generate(prompt_lookup_num_tokens=k)); the answers are the same, bit for bit."""
     dev = model.device
     images_tensor = process_images([image], image_processor, model.config).to(dev, dtype=model.dtype)
     depths_tensor = None if depth is None else process_images([depth], image_processor, model.config).to(dev, dtype=model.dtype)
@@ -239,7 +241,8 @@ def answer_questions(line: Dict[str, Any], model, tokenizer, image_processor, im
         output_ids = model.generate(input_ids, images=images_tensor, depths=depths_tensor,
                                     masks=None if masks is None else [masks.to(dev, dtype=model.dtype)],
                                     do_sample=temperature > 0, temperature=temperature, top_p=top_p, num_beams=num_beams,
-                                    max_new_tokens=max_new_tokens, use_cache=True, **({"prefix_cache": True} if prefix_cache else {}))
+                                    max_new_tokens=max_new_tokens, use_cache=True, **({"prefix_cache": True} if prefix_cache else {}),
+                                    **({"prompt_lookup_num_tokens": prompt_lookup_num_tokens} if prompt_lookup_num_tokens else {}))
         pred = clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop)
         records.append({"question_id": line["id"], "image": image_file, "question": line["text_q"], "pred": pred,
                         "gt": conversations[i * 2 + 1]["value"], "model_id": model_name, "qa_info": line["qa_info"]})
@@ -283,7 +286,8 @@ def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tens
             depth = depth_image(np.array(image), depth_predictor) if depth_predictor is not None else None
             for rec in answer_questions(line, model, tokenizer, image_processor, image, depth, masks, args.conv_mode, model_name, image_file,
                                         temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams,
-                                        prefix_cache=getattr(args, "prefix_cache", False)):
+                                        prefix_cache=getattr(args, "prefix_cache", False),
+                                        prompt_lookup_num_tokens=getattr(args, "prompt_lookup_num_tokens", 0)):
                 out.write(json.dumps(rec) + "\n")
                 n += 1
     return n
@@ -307,6 +311,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
                    help="module:factory of the external depth network (default: DepthAnything from $DEPTH_ANYTHING_PATH, like the reference)")
     p.add_argument("--prefix-cache", action="store_true",
                    help="prefill only the new question of each follow-up turn, reusing the earlier turns' encoder outputs and K/V")
+    p.add_argument("--prompt-lookup-num-tokens", type=int, default=0,
+                   help="greedy decoding by prompt lookup: draft up to this many tokens per verify pass (0 = off; same answers)")
     p.add_argument("--allow-no-depth", action="store_true", help="run an enable_depth checkpoint without a depth network (degraded answers)")
     return p
 

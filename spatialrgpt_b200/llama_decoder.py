@@ -136,7 +136,10 @@ class LlamaDecoder:
             self._pack_decode_weights()
 
     supports_prefix_reuse = True
+    supports_prompt_lookup = True
     packs_decode_weights = True
+    _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
+    last_speculation = (0, 0, 0)
     _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
     _lm_packed = None
 
@@ -318,13 +321,20 @@ class LlamaDecoder:
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_from_embeds(self, inputs_embeds: torch.Tensor, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
-                             use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0):
+                             use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0,
+                             lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2):
         """Greedy (or, with ``sampling=dict(temperature, top_p, seed)``, nucleus-sampled) decoding started from prompt
         embeddings [S, H].  Returns LongTensor [n_new] (and fp32 logits [n_new, V] when return_logits).
         ``stopping_fn(ids_so_far: LongTensor) -> bool``.
         ``reuse_rows=n`` keeps the K/V of the first n prompt rows of sequence 0 from the previous batch-1 prefill and prefills only
         rows n..S-1 (chunked prefill at start_pos n); the caller vouches that those rows are the same as before.  n must not exceed
-        ``prefix_rows`` nor S - 1 (the last prompt row is always computed: the first new token needs its hidden state)."""
+        ``prefix_rows`` nor S - 1 (the last prompt row is always computed: the first new token needs its hidden state).
+        ``lookup_k=k > 0`` (greedy, sequence 0): prompt-lookup speculative decoding after the first token (_verify_loop).  Each verify
+        pass drafts up to k tokens (clamped to ops.SPEC_T_MAX - 1) by n-gram lookup (sizes lookup_ngram .. 1) in ``lookup_ids`` (int,
+        negative = a row that never matches) followed by the generated tokens, and keeps the drafts that equal the model's own greedy
+        choices plus one token of its own.  The ids and logits are bit-identical to plain greedy decoding whatever the drafts are.
+        ``last_speculation`` = (verify passes, tokens drafted, tokens accepted) of the passes up to the last returned token; a
+        request whose verify slack does not fit max_seq_len or the decoder's token cap runs the one-token loop and reports (0, 0, 0)."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
         n_reuse = int(reuse_rows)
@@ -340,14 +350,23 @@ class LlamaDecoder:
         eos = set()
         if eos_token_ids is not None:
             eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
+        k = min(int(lookup_k), ops.SPEC_T_MAX - 1) if lookup_k else 0
+        self.last_speculation = (0, 0, 0)
+        if k > 0 and (seq != 0 or sampling or int(lookup_ngram) < 1):
+            raise ValueError("prompt-lookup decoding serves greedy decoding of sequence 0 with lookup_ngram >= 1")
+        # a verify pass writes up to T positions past the last emitted token, and one pass is in flight after the stop is seen
+        slack = 2 * ops.SPEC_T_MAX
+        if k > 0 and (S + max_new_tokens + slack > self.max_seq_len or max_new_tokens + slack > self.out_ids.numel()):
+            k = 0
         for b in range(len(self.cache.owned)):  # a previous batched generate leaves pages owned by sequences 1..B-1
             if not (n_reuse and b == seq):
                 self.cache.release(b)
-        self.cache.reserve(seq, S + max_new_tokens)
+        self.cache.reserve(seq, S + max_new_tokens + (slack if k > 0 else 0))
         hidden = self.prefill_hidden(inputs_embeds[n_reuse:], seq, n_reuse)
         if seq == 0 and self.supports_prefix_reuse:
             self._record_prefix(S)
-        logits = torch.empty((max_new_tokens, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits else None
+        n_rows = max_new_tokens + (slack if k > 0 else 0)  # verify passes write accepted logit rows past the budget too
+        logits = torch.empty((n_rows, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits else None
         # first token: final norm + lm_head + argmax on the last prompt row; afterwards pos == S
         self.pos.fill_(S - 1)
         self.step.zero_()
@@ -357,7 +376,117 @@ class LlamaDecoder:
                            embed_table=w.embed, next_x=self.h, logits_out=first_logits)
         if sample:
             ops.sample_top_p(first_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+        if k > 0 and max_new_tokens > 1:
+            return self._verify_loop(k + 1, int(lookup_ngram), lookup_ids, max_new_tokens, eos, stopping_fn, use_graph, logits)
         return self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample)
+
+    # ---- prompt-lookup speculative decoding: verify passes of T = k + 1 tokens, every weight streamed once per pass ---------------
+    def _verify_buffers(self):
+        st = self._vstate
+        if st is not None:
+            return st
+        d, dev, Tm = self.dims, self.device, ops.SPEC_T_MAX
+        H, qd, I = d.hidden_size, d.num_attention_heads * d.head_dim, d.intermediate_size
+        z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
+        st = dict(h=z(Tm, H), q=z(Tm, qd), attn=z(Tm, qd), act=z(Tm, I), ws=z(Tm * self.lm_ws.numel(), dtype=torch.uint8), logits=None,
+                  pos_rows=z(Tm, dtype=torch.int32), draft=z(Tm, dtype=torch.int32), state=z(8, dtype=torch.int32),
+                  prompt=z(self.max_seq_len, dtype=torch.int32), prompt_len=z(1, dtype=torch.int32),
+                  host_state=torch.zeros((self.out_ids.numel() + 2, 8), dtype=torch.int32, pin_memory=True), graphs={}, cache=self.cache)
+        self._vstate = st
+        return st
+
+    def _verify_launch(self, T: int, ngram: int, logits_all: Optional[torch.Tensor] = None) -> None:
+        d, w, st = self.dims, self.w, self._vstate
+        if logits_all is not None and st["logits"] is None:
+            st["logits"] = torch.empty((ops.SPEC_T_MAX, d.vocab_size), dtype=torch.float32, device=self.device)
+        ops.llama_verify_step(st["h"], self._layer_array, self._packed_array, d.num_hidden_layers, st["q"], st["attn"], st["act"], T, d,
+                              self.cos, self.sin, self.pos, st["pos_rows"], self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed,
+                              w.embed, st["ws"], st["logits"] if logits_all is not None else None, logits_all, st["prompt"], st["prompt_len"],
+                              ngram, st["draft"], self.out_ids, self.step, st["state"])
+
+    def _verify_graph(self, T: int, ngram: int):
+        """One captured verify pass per (T, n-gram size); dropped when the cache is reallocated (its page addresses change)."""
+        st = self._vstate
+        if st["cache"] is not self.cache:
+            st["graphs"], st["cache"] = {}, self.cache
+        g = st["graphs"].get((T, ngram))
+        if g is not None:
+            return g
+        saved = (self.pos.clone(), self.step.clone(), self.out_ids.clone(), st["state"].clone())
+        s = torch.cuda.Stream(device=self.device)
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            self._verify_launch(T, ngram)  # warm-up outside capture (lazy kernel attribute setup); writes only this sequence's slack
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        self.pos.copy_(saved[0]); self.step.copy_(saved[1]); self.out_ids.copy_(saved[2]); st["state"].copy_(saved[3])
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self._verify_launch(T, ngram)
+        st["graphs"][(T, ngram)] = g
+        return g
+
+    def _verify_loop(self, T: int, ngram: int, lookup_ids, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits):
+        """Tokens 1.. of sequence 0 by verify passes; pos / step / out_ids[:1] are set by the first token.  After each pass its state
+        (passes, drafted, accepted, step) and a window of out_ids go to pinned memory on a side stream, and the host inspects pass r-1
+        while pass r runs (the pattern of _decode_loop).  The tokens are cut at the first EOS / stopping criterion / max_new_tokens
+        exactly where the one-token loop cuts them; the pass in flight at the stop writes only this sequence's reserved slack."""
+        st = self._verify_buffers()
+        self.active_pt.copy_(self.cache.page_tables[0])
+        ids = torch.zeros(0, dtype=torch.int64) if lookup_ids is None else torch.as_tensor(lookup_ids).reshape(-1).to("cpu", torch.int64)
+        ids = ids[-st["prompt"].numel():]
+        ids = torch.where(ids < 0, torch.full_like(ids, -1), ids).to(torch.int32)
+        if ids.numel():
+            st["prompt"][: ids.numel()].copy_(ids)
+        st["prompt_len"].fill_(ids.numel())
+        st["state"].zero_()
+        graph = self._verify_graph(T, ngram) if use_graph and logits is None else None
+        if getattr(self, "_host_ids", None) is None:
+            self._host_ids = torch.empty(self.out_ids.numel(), dtype=torch.int64, pin_memory=True)
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        host, side, host_state = self._host_ids, self._copy_stream, st["host_state"]
+        window = 2 * T
+        done = {}
+
+        def fetch(r: int, lo: int) -> None:  # state after pass r and out_ids[lo, lo + 2T) -> host, after the work enqueued so far
+            e = torch.cuda.Event()
+            e.record()
+            side.wait_event(e)
+            with torch.cuda.stream(side):
+                host_state[r].copy_(st["state"], non_blocking=True)
+                host[lo:lo + window].copy_(self.out_ids[lo:lo + window], non_blocking=True)
+                dn = torch.cuda.Event()
+                dn.record(side)
+            done[r] = dn
+
+        def inspect(lo: int, hi: int):  # tokens [lo, hi): the length to return if the request ends among them, else None
+            for kk in range(lo, min(hi, max_new_tokens)):
+                if int(host[kk]) in eos or (stopping_fn is not None and stopping_fn(host[:kk + 1])):
+                    return kk + 1
+            return max_new_tokens if hi >= max_new_tokens else None
+
+        host[0] = int(self.out_ids[0])  # the first token (one sync, as the one-token loop's first inspection)
+        n = inspect(0, 1)
+        stats, known, r = (0, 0, 0), 1, 0
+        while n is None:
+            if graph is not None:
+                graph.replay()
+                ops.LAUNCHES += 5 * self.dims.num_hidden_layers + 3
+            else:
+                self._verify_launch(T, ngram, logits)
+            fetch(r, known)  # pass r's tokens lie in [step after r-1, + T), inside [step after r-2, + 2T)
+            if r > 0:
+                done.pop(r - 1).synchronize()
+                cur = int(host_state[r - 1, 6])
+                stats = tuple(int(v) for v in host_state[r - 1, :3])
+                n = inspect(known, cur)
+                known = cur
+            r += 1
+        self.last_speculation = stats
+        out = self.out_ids[:n].clone()
+        if logits is not None:
+            return out, logits[:n]
+        return out
 
     def _decode_loop(self, seq: int, n: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False):
         """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled); pos / step / h / out_ids[:n] are already set."""

@@ -74,6 +74,8 @@ class LlavaLlamaModel:
         # generate(prefix_cache=True): what the previous such request left for the next one to reuse (see _encode_prefix_cached)
         self._prefix_state = None
         self.last_prefix_reuse = None
+        self.last_speculation = None  # generate(prompt_lookup_num_tokens=k): (verify passes, tokens drafted, tokens accepted)
+        self._last_plan_rows = None
 
     # ---- accessors (llava_arch.py:252-278) -----------------------------------------------------------
     def get_llm(self):
@@ -289,6 +291,7 @@ class LlavaLlamaModel:
         for w in plan.warnings:
             print(w)
         lens, new_labels = plan.lens, plan.labels
+        self._last_plan_rows = (plan.src_id, plan.src_row)
         if _prefix is not None:
             _prefix.update(src_id=plan.src_id, src_row=plan.src_row, n_tok=n_tok)
         sid_dev, srow_dev = plan.src_id.to(dev, non_blocking=True), plan.src_row.to(dev, non_blocking=True)
@@ -375,6 +378,17 @@ class LlavaLlamaModel:
 
     __call__ = forward
 
+    def _lookup_history(self, input_ids, attention_mask, multimodal: bool) -> torch.Tensor:
+        """The prompt rows of a batch-1 request as prompt-lookup history: the token id of a text row, -1 (never matches) for a row
+        taken from image features or region / depth embeddings (the splice plan's rows whose source is not the token table)."""
+        if multimodal:
+            sid, srow = self._last_plan_rows
+            return torch.where(sid == SRC_TOKENS, srow, torch.full_like(srow, -1))
+        ids = input_ids[0].cpu()
+        if attention_mask is not None:
+            ids = ids[attention_mask[0].cpu().bool()]
+        return ids.to(torch.int32)
+
     # ---- generate (llava_llama.py:194-213) --------------------------------------------------------------
     @torch.no_grad()
     @ops.in_own_dtype
@@ -400,6 +414,14 @@ class LlavaLlamaModel:
         # short-M GEMMs and the paged attention kernel, so they differ from a full re-prefill by rounding; off, generate() is the
         # plain path.  model.last_prefix_reuse = (rows_reused, rows_prefilled, encoders_skipped) afterwards.
         prefix_cache = bool(generation_kwargs.pop("prefix_cache", False))
+        # prompt_lookup_num_tokens=k (batch 1, greedy, opt-in; HF's prompt lookup decoding): draft up to k tokens by n-gram lookup
+        # (sizes max_matching_ngram_size .. 1) and verify them in one pass over the weights.  The history searched is the prompt's text
+        # ids (its image / mask / depth rows never match) plus the generated tokens; HF, given only inputs_embeds, searches the
+        # generated tokens alone.  Either way the output does not depend on the drafts: ids and logits are bit-identical to
+        # generate() without the option.  k above ops.SPEC_T_MAX - 1 is clamped to it (only the speed can tell).
+        # model.last_speculation = (verify passes, tokens drafted, tokens accepted) afterwards.
+        lookup_k = int(generation_kwargs.pop("prompt_lookup_num_tokens", 0) or 0)
+        lookup_ngram = int(generation_kwargs.pop("max_matching_ngram_size", 2) or 2)
         # do_sample=True -> HF's TemperatureLogitsWarper + TopPLogitsWarper + multinomial, here one kernel per token
         # (eval_spatial.py:231-236 passes do_sample = temperature > 0, so temperature 0 stays greedy)
         sampling = None
@@ -411,6 +433,15 @@ class LlavaLlamaModel:
             raise NotImplementedError("beam search is implemented for do_sample=False without output_logits (the eval scripts' mode)")
         if generation_kwargs:
             raise TypeError(f"unsupported generation kwargs: {sorted(generation_kwargs)}")
+        if lookup_k:
+            if lookup_k < 0 or lookup_ngram < 1:
+                raise ValueError("prompt_lookup_num_tokens and max_matching_ngram_size must be positive")
+            if sampling is not None:
+                raise NotImplementedError("prompt_lookup_num_tokens with do_sample=True (speculative sampling would change the random stream)")
+            if num_beams != 1:
+                raise NotImplementedError("prompt_lookup_num_tokens with beam search")
+            if not getattr(self.llm, "supports_prompt_lookup", False):
+                raise NotImplementedError("prompt_lookup_num_tokens on the tensor-parallel decoder")
         prefix = None
         if prefix_cache:
             if input_ids is None or input_ids.shape[0] != 1:
@@ -431,6 +462,7 @@ class LlavaLlamaModel:
             inputs_embeds = self.llm.embed_tokens(input_ids).view(*input_ids.shape, -1)
             lens = [input_ids.shape[1]] * input_ids.shape[0] if attention_mask is None else attention_mask.sum(-1).tolist()
             B = inputs_embeds.shape[0]
+            self._last_plan_rows = None
             if prefix is not None:  # text only: a row is its token id
                 ids = input_ids[0].cpu() if attention_mask is None else input_ids[0].cpu()[attention_mask[0].cpu().bool()]
                 prefix.update(src_id=torch.full((ids.numel(),), SRC_TOKENS, dtype=torch.int32), src_row=ids.to(torch.int32), n_tok=1,
@@ -445,6 +477,8 @@ class LlavaLlamaModel:
             def stop_fn(ids, _sc=stopping_criteria):
                 return any(bool(c(ids[None], None)) for c in _sc)
         lens = [int(n) for n in lens]
+        if lookup_k and B != 1:
+            raise NotImplementedError("prompt_lookup_num_tokens serves batch-1 requests")
         left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
         if num_beams != 1 and B != 1:
             raise NotImplementedError("beam search over a batch of prompts (the reference's eval scripts run batch 1)")
@@ -465,8 +499,14 @@ class LlavaLlamaModel:
                 if prev is not None and prev["epoch"] == self.llm.prefix_epoch:  # no other request touched the cache since
                     reuse = reusable_prefix(prev["src_id"], prev["src_row"], prefix["src_id"], prefix["src_row"], prefix["n_tok"],
                                             prefix["image_equal"], prefix["mask_equal"], min(self.llm.prefix_rows, n - 1))
+            spec = {}
+            if lookup_k:
+                spec = dict(lookup_ids=self._lookup_history(input_ids, attention_mask, packed is not None), lookup_k=lookup_k,
+                            lookup_ngram=lookup_ngram)
             r = self.llm.generate_from_embeds(emb, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse)
+                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse, **spec)
+            if lookup_k:
+                self.last_speculation = tuple(self.llm.last_speculation)
             if prefix is not None:
                 prefix["epoch"] = self.llm.prefix_epoch
                 self._prefix_state = prefix

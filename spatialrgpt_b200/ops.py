@@ -797,3 +797,88 @@ def llama_decode_step_packed(h, layer_array, packed_array, n_layers: int, q_buf,
                                                           C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
                                                           _stream()), "srgpt_llama_decode_step_packed_bf16")
     _count(5 * n_layers + 2)
+
+
+# ------------------------------------------------------------------------------------------------ prompt-lookup speculative decoding
+SPEC_T_MAX = _lib.SPEC_T_MAX
+
+
+def gemv_multi(x: torch.Tensor, w: torch.Tensor, y: torch.Tensor, norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0,
+               residual: Optional[torch.Tensor] = None, mode: int = GEMV_PLAIN, n_heads: int = 0, n_kv_heads: int = 0, head_dim: int = 0,
+               cos=None, sin=None, pos=None, kv_pages=None, page_table=None, page_size: int = 0, packed=None) -> torch.Tensor:
+    """gemv() over the T rows of x [T, K] -> y [T, ldy] with every weight streamed once; each row is bit-identical to a one-token gemv()
+    call (QKV_ROPE: row t at position pos + t).  ``packed`` = a Packed12W of ``w`` streams the 12-bit packing instead."""
+    _need(x, ELEM(), "gemv_multi.x")
+    T, K = x.shape
+    N = w.shape[0] if packed is None else packed.sm.shape[0]
+    ldx, ldy = _rowmajor2d(x, "gemv_multi.x"), _rowmajor2d(y, "gemv_multi.y")
+    tail = (_p(norm_weight), eps, _p(residual), mode, n_heads, n_kv_heads, head_dim, _p(cos), _p(sin), _p(pos), _p(kv_pages), _p(page_table),
+            page_size, _stream())
+    if packed is None:
+        check(_lib.load().srgpt_gemv_multi_bf16(_p(x), ldx, _p(w), w.stride(0), _p(y), ldy, T, N, K, *tail), "srgpt_gemv_multi_bf16")
+    else:
+        d = _packed_desc(packed)
+        check(_lib.load().srgpt_gemv_multi_packed_bf16(_p(x), ldx, C.byref(d), _p(y), ldy, T, N, K, *tail), "srgpt_gemv_multi_packed_bf16")
+    return y
+
+
+def lm_head_multi(x: torch.Tensor, w: torch.Tensor, norm_weight: Optional[torch.Tensor], eps: float, workspace: torch.Tensor,
+                  logits_out: Optional[torch.Tensor] = None, packed=None) -> None:
+    """Final norm + lm_head over the T rows of x [T, H]: fp32 logits [T, V] (optional) and the per-token arg max partials in
+    ``workspace`` (T * lm_head_workspace bytes), which spec_accept() reduces."""
+    T, K = x.shape
+    ldx = _rowmajor2d(x, "lm_head_multi.x")
+    if packed is None:
+        V = w.shape[0]
+        check(_lib.load().srgpt_lm_head_multi_bf16(_p(x), ldx, _p(w), w.stride(0), T, V, K, _p(norm_weight), eps, _p(logits_out), _p(workspace),
+                                                   _stream()), "srgpt_lm_head_multi_bf16")
+    else:
+        V = packed.sm.shape[0]
+        d = _packed_desc(packed)
+        check(_lib.load().srgpt_lm_head_multi_packed_bf16(_p(x), ldx, C.byref(d), T, V, K, _p(norm_weight), eps, _p(logits_out), _p(workspace),
+                                                          _stream()), "srgpt_lm_head_multi_packed_bf16")
+
+
+def attention_decode_multi(q: torch.Tensor, out: torch.Tensor, kv_pages: torch.Tensor, page_table: torch.Tensor, page_size: int,
+                           pos_rows: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: int, scale: float) -> torch.Tensor:
+    """Decode attention of T consecutive tokens: row t of q [T, >= nh*hd] attends over kv rows 0 .. pos_rows[t] -> out row t."""
+    _need(pos_rows, torch.int32, "attention_decode_multi.pos_rows")
+    T = q.shape[0]
+    check(_lib.load().srgpt_attention_decode_multi_bf16(_p(q), _rowmajor2d(q, "attention_decode_multi.q"), _p(out),
+                                                        _rowmajor2d(out, "attention_decode_multi.out"), _p(kv_pages), _p(page_table), page_size,
+                                                        _p(pos_rows), T, n_heads, n_kv_heads, head_dim, scale, _stream()),
+          "srgpt_attention_decode_multi_bf16")
+    return out
+
+
+def spec_draft(prompt_ids: Optional[torch.Tensor], prompt_len: Optional[torch.Tensor], out_ids: torch.Tensor, step: torch.Tensor, pos: torch.Tensor, pos_rows: torch.Tensor, T: int,
+               ngram: int, embed_table: torch.Tensor, x: torch.Tensor, draft_ids: torch.Tensor, state: torch.Tensor) -> None:
+    """prompt_ids: device int32 history buffer, prompt_len: device int32 [1] = its length (read at run time)."""
+    check(_lib.load().srgpt_spec_draft(_p(prompt_ids), _p(prompt_len), _p(out_ids), _p(step), _p(pos), _p(pos_rows), T, ngram, _p(embed_table), _p(x),
+                                       embed_table.shape[1], _p(draft_ids), _p(state), _stream()), "srgpt_spec_draft")
+
+
+def spec_accept(workspace: torch.Tensor, V: int, T: int, draft_ids: torch.Tensor, out_ids: torch.Tensor, step: torch.Tensor, pos: torch.Tensor,
+                state: torch.Tensor, logits_rows: Optional[torch.Tensor] = None, logits_all: Optional[torch.Tensor] = None) -> None:
+    check(_lib.load().srgpt_spec_accept(_p(workspace), V, T, _p(draft_ids), _p(out_ids), out_ids.numel(), _p(step), _p(pos), _p(state),
+                                        _p(logits_rows), _p(logits_all), _stream()), "srgpt_spec_accept")
+
+
+def llama_verify_step(h, layer_array, packed_array, n_layers: int, q_buf, attn_buf, act_buf, T: int, dims, cos, sin, pos, pos_rows, page_table,
+                      page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, logits_rows, logits_all, prompt_ids, prompt_len, ngram: int, draft_ids,
+                      out_ids, step, state) -> None:
+    """One verify pass of T tokens (draft, layers, lm_head, accept); packed_array None = the bf16 weights."""
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    common_a = (T, dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(pos_rows), _p(page_table), page_size,
+                _p(final_norm), _p(lm_head))
+    common_b = (dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(logits_all), _p(prompt_ids), _p(prompt_len), ngram, _p(draft_ids), _p(out_ids),
+                out_ids.numel(), _p(step), _p(state), _stream())
+    if packed_array is None:
+        check(_lib.load().srgpt_llama_verify_step_bf16(_p(h), C.cast(layer_array, C.c_void_p), n_layers, _p(q_buf), _p(attn_buf), _p(act_buf),
+                                                       *common_a, *common_b), "srgpt_llama_verify_step_bf16")
+    else:
+        lm_d = _packed_desc(lm_packed)
+        check(_lib.load().srgpt_llama_verify_step_packed_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(packed_array, C.c_void_p), n_layers,
+                                                              _p(q_buf), _p(attn_buf), _p(act_buf), *common_a, C.byref(lm_d), *common_b),
+              "srgpt_llama_verify_step_packed_bf16")
+    _count(5 * n_layers + 3 + (1 if logits_all is not None else 0))
