@@ -18,7 +18,8 @@
 //
 // The packed variant (PACKED = true) streams the 12-bit lossless packing of pack12.cuh: per batch of 4 chunks a lane loads
 // 3 x 16 bytes per row instead of 4, rebuilds the bf16 pairs in registers (decode_chunk), ORs in the row's few exception
-// exponents, and then runs the very same dot8 / warp_sum / epilogue, so its results are bit-identical.
+// exponents, and then runs the very same dot8 / warp_sum / epilogue, so its results are bit-identical.  Its weight stream runs through a
+// per-warp ring of cp.async slots in shared memory (ring_depth), so a warp keeps several batches in flight without spending registers.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -52,6 +53,8 @@ struct Params {
   bf16* kv_pages;
   const int* page_table;
   int page_size;
+  int ring;                   // packed: 1 = the spre slots are a ring that every later batch streams through, 0 = later batches load into
+                              // registers.  It sits in the padding before the next pointer, so no other member (nor MParams) moves.
   // LM
   float* logits_out;
   float* part_val;
@@ -194,6 +197,36 @@ __device__ __forceinline__ void patch_batch(uint4 (&w)[4], int exc, int n, int& 
   }
 }
 
+// Batch b of both rows into one 3 KB slot of the warp's shared memory by cp.async (row r0: sm 01, sm 23, ex at +0 / 512 / 1024, row r1 at
+// +1536 ...).  slot_lane = the slot + 16 * lane: every lane later reads back exactly the 16-byte vectors it requested, so no barrier is needed.
+__device__ __forceinline__ void cp_async_batch12(const uint8_t* slot_lane, const uint4* sm0, const uint4* ex0, int drow_ex, int b) {
+  const uint32_t d = (uint32_t)__cvta_generic_to_shared(slot_lane);
+  const uint4 *s = sm0 + b * 64, *e = ex0 + b * 32;
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(s) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512), "l"(s + 32) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1024), "l"(e) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1536), "l"(s + 2 * drow_ex) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2048), "l"(s + 2 * drow_ex + 32) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2560), "l"(e + drow_ex) : "memory");
+}
+
+__device__ __forceinline__ void ld_slot12(const uint8_t* slot_lane, Raw12& t0, Raw12& t1) {
+  const uint4* s = reinterpret_cast<const uint4*>(slot_lane);
+  t0 = {s[0], s[32], s[64]};
+  t1 = {s[96], s[128], s[160]};
+}
+
+// cp.async.wait_group takes an immediate: wait until at most n (0..RING_MAX - 1) of this thread's newest commit groups are pending
+constexpr int RING_MAX = 4;
+__device__ __forceinline__ void cp_async_wait_pending(int n) {
+  switch (n) {
+    case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
+    case 1: asm volatile("cp.async.wait_group 1;" ::: "memory"); break;
+    case 2: asm volatile("cp.async.wait_group 2;" ::: "memory"); break;
+    default: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
+  }
+}
+
 struct Rows12 {
   uint32_t bp0, bp1;  // base - 1 of the two rows
   int exc0, exc1;     // this lane's entry of each row's exception list
@@ -260,8 +293,8 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   //      Occupancy stays at 3 CTAs/SM, unlike the deeper register prefetch (PRE = 2/4) that was measured and rejected.
   uint8_t* spre_base = smem_raw + (size_t)p.K * 2 + (size_t)warp * ((size_t)p.spre * (PACKED ? SPRE_WARP_BYTES12 : SPRE_WARP_BYTES));
   int n_spre = 0;
-  // ---- packed: the same two levels (batch 0 in registers, the next p.spre batches in shared memory), plus each row's base and
-  //      exception list; all of it is static, so all of it is requested before the dependency wait
+  // ---- packed: the same two levels (batch 0 in registers, the next p.spre batches in shared memory, one commit group each), plus each
+  //      row's base and exception list; all of it is static, so all of it is requested before the dependency wait
   const int nbatch = p.K >> 10;
   Raw12 q0 = {}, q1 = {};
   Rows12 rs = {};
@@ -273,17 +306,10 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
     q0 = ld_raw12(sm0, ex0, 0);
     q1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, 0);
     for (int b = 0; b < p.spre && 1 + b < nbatch; ++b) {
-      const uint32_t d = (uint32_t)__cvta_generic_to_shared(spre_base + b * 6 * 512 + lane * 16);
-      const uint4 *s = sm0 + (1 + b) * 64, *e = ex0 + (1 + b) * 32;
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(s) : "memory");
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512), "l"(s + 32) : "memory");
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1024), "l"(e) : "memory");
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 1536), "l"(s + 2 * drow_ex) : "memory");
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2048), "l"(s + 2 * drow_ex + 32) : "memory");
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 2560), "l"(e + drow_ex) : "memory");
+      cp_async_batch12(spre_base + b * SPRE_WARP_BYTES12 + lane * 16, sm0, ex0, drow_ex, 1 + b);
+      asm volatile("cp.async.commit_group;" ::: "memory");
       ++n_spre;
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
     const int e0 = p.pk.row_ptr[r0], e1 = p.pk.row_ptr[r1];
     rs.n0 = min(p.pk.row_ptr[r0 + 1] - e0, pack12::MAX_EXC_PER_ROW);
     rs.n1 = min(p.pk.row_ptr[r1 + 1] - e1, pack12::MAX_EXC_PER_ROW);
@@ -346,18 +372,36 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
   if constexpr (PACKED) {  // batches in chunk order: the lane's fma chain is the plain kernel's
     if (active) {
       consume12(q0, q1, rs, 0, lane, px, a0, a1);
-      if (n_spre > 0) {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        for (int b = 0; b < n_spre; ++b) {
-          const uint8_t* s = spre_base + b * 6 * 512 + lane * 16;
-          const Raw12 t0 = {*reinterpret_cast<const uint4*>(s), *reinterpret_cast<const uint4*>(s + 512), *reinterpret_cast<const uint4*>(s + 1024)};
-          const Raw12 t1 = {*reinterpret_cast<const uint4*>(s + 1536), *reinterpret_cast<const uint4*>(s + 2048), *reinterpret_cast<const uint4*>(s + 2560)};
-          consume12(t0, t1, rs, 1 + b, lane, px, a0, a1);
+      if (p.ring) {
+        // Ring of n_spre slots: batch b sits in slot (b - 1) % n_spre.  As soon as the lane has read its vectors of batch b back into
+        // registers it requests batch b + n_spre into the same slot (the reads precede the cp.async in the thread's program order), so
+        // n_spre batches stay in flight while batch b is decoded and consumed.  Batches are consumed in chunk order, as above.
+        int slot = 0;
+        for (int b = 1; b < nbatch; ++b) {
+          cp_async_wait_pending(min(n_spre - 1, nbatch - 1 - b));  // groups committed after batch b's own may still be pending
+          const uint8_t* s = spre_base + slot * SPRE_WARP_BYTES12 + lane * 16;
+          Raw12 t0, t1;
+          ld_slot12(s, t0, t1);
+          if (b + n_spre < nbatch) {
+            cp_async_batch12(s, sm0, ex0, drow_ex, b + n_spre);
+            asm volatile("cp.async.commit_group;" ::: "memory");
+          }
+          consume12(t0, t1, rs, b, lane, px, a0, a1);
+          if (++slot == n_spre) slot = 0;
         }
-      }
-      for (int b = 1 + n_spre; b < nbatch; ++b) {
-        const Raw12 t0 = ld_raw12(sm0, ex0, b), t1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, b);
-        consume12(t0, t1, rs, b, lane, px, a0, a1);
+      } else {
+        if (n_spre > 0) {
+          asm volatile("cp.async.wait_group 0;" ::: "memory");
+          for (int b = 0; b < n_spre; ++b) {
+            Raw12 t0, t1;
+            ld_slot12(spre_base + b * SPRE_WARP_BYTES12 + lane * 16, t0, t1);
+            consume12(t0, t1, rs, 1 + b, lane, px, a0, a1);
+          }
+        }
+        for (int b = 1 + n_spre; b < nbatch; ++b) {
+          const Raw12 t0 = ld_raw12(sm0, ex0, b), t1 = ld_raw12(sm0 + 2 * drow_ex, ex0 + drow_ex, b);
+          consume12(t0, t1, rs, b, lane, px, a0, a1);
+        }
       }
     }
   } else if (active) {
@@ -960,9 +1004,26 @@ static int spre_default() {
   return v;
 }
 
+// Depth of the packed kernel's per-warp ring (slots of 3 KB per warp).  SRGPT_GEMV_RING = 0 keeps the two fixed levels (batch 0 in
+// registers, spre_default() batches in shared memory, the rest loaded into registers one batch at a time); n > 0 sets the depth (default
+// 2).  Read at every launch, so a captured graph keeps the depth it was captured with.  At K = 4096 a depth of 2 is 56 KB per CTA, so
+// the 3 CTAs per SM the registers allow still fit and 3 of a row's 4 batches are requested before the dependency wait.  Deeper rings
+// (2 CTAs per SM) made o_proj and down_proj stream faster but delayed the kernel after them by more (DESIGN.md §5).  Returns -1 for the
+// fixed levels, else the depth clamped to the batches after batch 0.
+static int ring_depth(int K) {
+  const char* e = getenv("SRGPT_GEMV_RING");
+  int d = (e != nullptr && e[0] != 0) ? atoi(e) : 2;
+  if (d <= 0) return -1;
+  d = d > RING_MAX ? RING_MAX : d;
+  const int later = (K >> 10) - 1;
+  return d < later ? d : later;
+}
+
 template <int MODE, int PRE, bool PACKED = false>
 static int launch_pre(const Params& p, int npairs, cudaStream_t st) {
-  const int smem = p.K * 2 + WARPS * spre_default() * (PACKED ? SPRE_WARP_BYTES12 : SPRE_WARP_BYTES);
+  const int ring = PACKED ? ring_depth(p.K) : -1;
+  const int spre = ring >= 0 ? ring : spre_default();
+  const int smem = p.K * 2 + WARPS * spre * (PACKED ? SPRE_WARP_BYTES12 : SPRE_WARP_BYTES);
   static int configured_smem = 0;
   if (smem > 48 * 1024 && smem > configured_smem) {
     SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_kernel<MODE, PRE, PACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -973,7 +1034,8 @@ static int launch_pre(const Params& p, int npairs, cudaStream_t st) {
   pdl_config(cfg, attr, grid_for(npairs), THREADS, smem, st);
   Params q = p;
   q.trace = trace_next_slot();
-  q.spre = spre_default();
+  q.spre = spre;
+  q.ring = ring >= 0 ? 1 : 0;
   static const int l2pf = [] {
     const char* v = getenv("SRGPT_GEMV_L2PF");
     return (v != nullptr && v[0] != 0) ? atoi(v) : 0;

@@ -1,6 +1,6 @@
 """Kernel micro-benchmarks (CUDA events on the launching stream, warm-up, L2 flush between timed
 launches).  Prints one JSON object per kernel."""
-import json, os, sys
+import json, os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from spatialrgpt_b200 import ops
@@ -47,6 +47,15 @@ def rnd(*s):
 
 which = sys.argv[1:] or ["gemv", "maskpool", "gemm", "attn", "rowops"]
 
+# the card and its clocks belong beside every number below (nvidia-smi reads them, it changes nothing)
+try:
+    q = "name,power.limit,clocks.max.sm,clocks.sm"
+    smi = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
+                         capture_output=True, text=True, timeout=30).stdout.strip()
+    print(json.dumps({"gpu": dict(zip(q.split(","), (v.strip() for v in smi.split(","))))}), flush=True)
+except (OSError, subprocess.SubprocessError):
+    print(json.dumps({"gpu": torch.cuda.get_device_name()}), flush=True)
+
 if "gemv" in which:
     for name, N, K, mode in [("gemv_qkv_rope", 6144, 4096, "qkv"), ("gemv_o", 4096, 4096, "plain"), ("gemv_gateup_swiglu", 28672, 4096, "swiglu"),
                              ("gemv_down", 4096, 14336, "plain"), ("lm_head_argmax", 128259, 4096, "lm")]:
@@ -74,18 +83,34 @@ if "gemv" in which:
         ms, best = timeit(fn)
         emit(name, ms, best, bytes_=N * K * 2, N=N, K=K)
     # the same GEMVs over the 12-bit packing (DESIGN.md §3): GBps counts the bytes actually streamed (planes + row metadata)
-    for name, N, K, mode in [("gemv_gateup_swiglu_packed12", 28672, 4096, "swiglu"), ("gemv_down_packed12", 4096, 14336, "plain")]:
+    for name, N, K, mode in [("gemv_qkv_rope_packed12", 6144, 4096, "qkv"), ("gemv_o_packed12", 4096, 4096, "plain"),
+                             ("gemv_gateup_swiglu_packed12", 28672, 4096, "swiglu"), ("gemv_down_packed12", 4096, 14336, "plain"),
+                             ("lm_head_argmax_packed12", 128256, 4096, "lm")]:
         w, x = rnd(N, K), rnd(K)
         p, why = ops.pack12(w)
         if p is None:
             raise SystemExit(f"{name}: the matrix stays plain ({why})")
+        del w
         nw = torch.ones(K, dtype=BF, device=dev)
         if mode == "plain":
             y = torch.empty(N, dtype=BF, device=dev); r = rnd(N)
             fn = lambda: ops.gemv_packed(x, p, y, residual=r)
-        else:
+        elif mode == "swiglu":
             y = torch.empty(N // 2, dtype=BF, device=dev)
             fn = lambda: ops.gemv_packed(x, p, y, norm_weight=nw, eps=1e-5, mode=ops.GEMV_SWIGLU)
+        elif mode == "qkv":
+            from spatialrgpt_b200.config import LlamaDims
+            from spatialrgpt_b200.llama_decoder import build_rope_tables
+            cos, sin = build_rope_tables(LlamaDims(), 1024, dev)
+            pages = torch.zeros(64, 2, 16, 8, 128, dtype=BF, device=dev); pt = torch.arange(64, dtype=torch.int32, device=dev)
+            pos = torch.tensor([300], dtype=torch.int32, device=dev); y = torch.empty(4096, dtype=BF, device=dev)
+            fn = lambda: ops.gemv_packed(x, p, y, norm_weight=nw, eps=1e-5, mode=ops.GEMV_QKV_ROPE, n_heads=32, n_kv_heads=8, head_dim=128,
+                                         cos_tab=cos, sin_tab=sin, pos=pos, kv_pages=pages, page_table=pt, page_size=16)
+        else:
+            ws = ops.lm_head_workspace(N, dev); ids = torch.zeros(8, dtype=torch.int64, device=dev)
+            st = torch.zeros(1, dtype=torch.int32, device=dev); ps = torch.zeros(1, dtype=torch.int32, device=dev)
+            def fn():
+                st.zero_(); ops.lm_head_argmax_packed(x, p, nw, 1e-5, ws, ids, st, ps)
         ms, best = timeit(fn)
         emit(name, ms, best, bytes_=p.nbytes(), N=N, K=K, bf16_equiv_GBps=round(N * K * 2 / ms / 1e6, 1))
 
