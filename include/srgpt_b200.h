@@ -248,6 +248,23 @@ int srgpt_beam_candidates_bf16(const void* logits, int ldx, int n_beams, int V, 
  * srgpt_lm_head_argmax_bf16 / srgpt_llama_decode_step_bf16 (which advanced *step) with step_offset = -1. */
 int srgpt_sample_top_p_f32(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step, int step_offset,
                            long long* out_ids, const void* embed_table, void* next_x, int K, void* stream);
+/* HF's logits processors on the device (logits_process.cu): replaces RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
+ * NoBadWordsLogitsProcessor, MinLengthLogitsProcessor and MinNewTokensLengthLogitsProcessor (transformers generation/logits_process.py),
+ * which HF runs on the host behind generate(repetition_penalty=, no_repeat_ngram_size=, bad_words_ids=, min_length=, min_new_tokens=)
+ * (llava/model/language_model/llava_llama.py:212 forwards them; llava/eval/model_vqa.py:76), plus the greedy arg max after them.
+ * logits: rows [rows, ld], fp32 (logits_f32 = 1) or the element type.  Row r's history is hist[r * hist_row_stride + t * hist_tok_stride]
+ * for t < min(*step + step_offset, hist_cap) (step NULL: step_offset alone).  fparams = device float[2] {penalty, 1 / penalty};
+ * spec = device int[spec_cap] {flags (1 penalty, 2 n-gram, 4 bad words, 8 minimum length), n-gram size, minimum new tokens, n_eos,
+ * n_bad, eos ids[n_eos], bad-word offsets[n_bad + 1], bad-word tokens[]} - both read at run time, so a captured graph serves every
+ * setting.  Writes the processed fp32 rows to out [rows, ldo] (may be NULL) and, when ids is given, the arg max of each processed
+ * row to ids[rows] (lowest index on ties, NaN never wins). */
+int srgpt_logits_process(const void* logits, int logits_f32, int ld, int rows, int V, const long long* hist, int hist_row_stride,
+                         int hist_tok_stride, int hist_cap, const int* step, int step_offset, const float* fparams, const int* spec,
+                         int spec_cap, float* out, int ldo, long long* ids, void* stream);
+/* out_ids[*step + step_offset] = ids[0] and, when given, next_x[K] = embed_table[ids[0]]: the processed greedy choice replaces the one
+ * srgpt_lm_head_argmax_bf16 / srgpt_llama_decode_step_bf16 wrote (call with step_offset = -1, as srgpt_sample_top_p_f32). */
+int srgpt_logits_pick_token(const long long* ids, const int* step, int step_offset, long long* out_ids, const void* embed_table,
+                            void* next_x, int K, void* stream);
 
 /* ---- host preprocessing on the GPU (preprocess.cu; llava/mm_utils.py:421-542: process_images / process_regions) ----------
  * The pinned image processor (transformers 4.37.2 SiglipImageProcessor) = Pillow BICUBIC resize of the uint8 image + rescale +

@@ -61,6 +61,8 @@ SIGNATURES = {
     "srgpt_argmax_bf16": (ci, [vp, ci, ci, ci, vp, vp]),
     "srgpt_beam_candidates_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp, vp]),
     "srgpt_sample_top_p_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp]),
+    "srgpt_logits_process": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, ci, vp, ci, vp, vp, ci, vp, ci, vp, vp]),
+    "srgpt_logits_pick_token": (ci, [vp, vp, ci, vp, vp, vp, ci, vp]),
     "srgpt_resample_u8": (ci, [vp, vp, ci, ci, ci, ci, ci, vp, vp, ci, vp]),
     "srgpt_u8_to_normalized_chw": (ci, [vp, vp, ci, ci, ci, C.c_double, vp, vp, ci, vp]),
     "srgpt_resize_nearest_u8": (ci, [vp, vp, ci, ci, ci, ci, vp, vp, vp]),

@@ -26,11 +26,14 @@ from .mm_utils import KeywordsStoppingCriteria, process_images, process_regions,
 
 class RegionChat:
     def __init__(self, model, tokenizer, image_processor, conv_mode: str = "llama_3", temperature: float = 0.0, max_new_tokens: int = 512,
-                 prefix_cache: bool = False, prompt_lookup_num_tokens: int = 0):
+                 prefix_cache: bool = False, prompt_lookup_num_tokens: int = 0, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0):
         """``prefix_cache``: a follow-up reuses the earlier turns' encoder outputs and prompt K/V and prefills only the new rows
         (generate(prefix_cache=True)); answers match a full re-prefill up to bf16 rounding.
         ``prompt_lookup_num_tokens=k > 0``: greedy answers are decoded by prompt lookup (generate(prompt_lookup_num_tokens=k)),
-        the same answers bit for bit."""
+        the same answers bit for bit.
+        ``repetition_penalty`` / ``no_repeat_ngram_size``: HF's processors of the same name (generate()), against the loops greedy answers
+        fall into; forwarded only when not neutral (1.0 / 0)."""
+        self.repetition_penalty, self.no_repeat_ngram_size = repetition_penalty, no_repeat_ngram_size
         self.prompt_lookup_num_tokens = prompt_lookup_num_tokens
         self.model, self.tokenizer, self.image_processor = model, tokenizer, image_processor
         self.prefix_cache = prefix_cache
@@ -68,7 +71,9 @@ class RegionChat:
                              do_sample=self.temperature > 0, temperature=self.temperature, max_new_tokens=self.max_new_tokens, use_cache=True,
                              stopping_criteria=[KeywordsStoppingCriteria([stop], self.tokenizer, input_ids)],
                              **({"prefix_cache": True} if self.prefix_cache else {}),
-                             **({"prompt_lookup_num_tokens": self.prompt_lookup_num_tokens} if self.prompt_lookup_num_tokens else {}))
+                             **({"prompt_lookup_num_tokens": self.prompt_lookup_num_tokens} if self.prompt_lookup_num_tokens else {}),
+                             **({"repetition_penalty": self.repetition_penalty} if self.repetition_penalty != 1.0 else {}),
+                             **({"no_repeat_ngram_size": self.no_repeat_ngram_size} if self.no_repeat_ngram_size else {}))
         answer = clean_output(self.tokenizer.batch_decode(out, skip_special_tokens=True)[0], stop)
         turn_regions = re.findall(r"<region(\d+)>", text)
         mapping = {str(k): r for k, r in enumerate(turn_regions)}

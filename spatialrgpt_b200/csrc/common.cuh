@@ -148,6 +148,16 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return t;
 }
 
+// Arg max over wide rows (rowops.cu argmax_wide_kernel, logits_process.cu): one CTA per ARGMAX_SEG columns, the segments of a row
+// meet in a 64-bit atomicMax on (float_order_bits(value) << 32 | ~index) - max value first, lowest index on ties.
+constexpr int ARGMAX_SEG = 4096;
+__device__ __forceinline__ unsigned int float_order_bits(float f) {
+  const unsigned int u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+// host: keys [rows] (u64, as above) -> the arg max index of each row, in place (rowops.cu)
+void argmax_unpack(long long* keys, int rows, cudaStream_t stream);
+
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float gelu_tanh(float x) {
   // tanh on the SFU (MUFU.TANH, rel. error ~2^-11): the result is rounded to bf16 (2^-8) right after, and the

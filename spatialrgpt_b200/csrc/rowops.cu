@@ -268,11 +268,7 @@ __global__ void __launch_bounds__(256) argmax_kernel(const T* __restrict__ x, in
 // Wide rows (a vocabulary of 128 K per sequence of a batched decode step): one CTA per 4096-column segment, the segments of a row
 // meet in a 64-bit atomicMax on (order-preserving value bits << 32 | ~index) - max value first, lowest index on ties, and
 // associative, so the result does not depend on the arrival order.  out[] holds the packed key until argmax_unpack_kernel.
-constexpr int ARGMAX_SEG = 4096;
-__device__ __forceinline__ unsigned int float_order_bits(float f) {
-  const unsigned int u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
+// (ARGMAX_SEG and float_order_bits live in common.cuh: logits_process.cu builds the same key)
 template <typename T>
 __global__ void __launch_bounds__(256) argmax_wide_kernel(const T* __restrict__ x, int ldx, int cols, unsigned long long* __restrict__ keys) {
   __shared__ unsigned long long sk[8];
@@ -304,6 +300,10 @@ __global__ void argmax_unpack_kernel(long long* __restrict__ out, int rows) {
     const unsigned long long k = reinterpret_cast<unsigned long long*>(out)[r];
     out[r] = k == 0ull ? 0ll : (long long)(0xFFFFFFFFu - (unsigned int)(k & 0xFFFFFFFFull));
   }
+}
+
+void argmax_unpack(long long* keys, int rows, cudaStream_t stream) {
+  argmax_unpack_kernel<<<ceil_div(rows, 256), 256, 0, stream>>>(keys, rows);
 }
 
 // ---------------------------------------------------------------------------------------------

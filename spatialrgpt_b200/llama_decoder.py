@@ -16,7 +16,7 @@ from typing import List, Optional
 
 import torch
 
-from . import ops
+from . import logits_processors, ops
 from .config import LlamaDims
 from .weights import LlamaW
 
@@ -123,6 +123,14 @@ class LlamaDecoder:
         self.sample_logits: Optional[torch.Tensor] = None
         self.sample_seed = 0
         self.sample_seed_dev = torch.zeros(1, dtype=torch.int64, device=dev)  # device copy: the captured graph reads the seed at run time
+        # logits processors (repetition penalty, no-repeat n-grams, bad words, minimum length; logits_processors.py): the parameters live
+        # in device memory so one captured graph per mode serves every setting.  The spec buffer is sized at first use and grown when a
+        # request needs more, which drops the graphs that read it.
+        self.proc_fparams = torch.ones(2, dtype=torch.float32, device=dev)
+        self.proc_spec: Optional[torch.Tensor] = None
+        self.proc_logits: Optional[torch.Tensor] = None  # the processed fp32 row of the one-token step (sampling reads it)
+        self.proc_ids = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._proc_graphs = {}  # sample flag -> decode-step graph with processing on
         # Reusable prompt prefix of sequence 0: its first `prefix_rows` positions hold K/V that a batch-1 PREFILL wrote and nothing has
         # overwritten since (generate_from_embeds(reuse_rows=n) continues from them).  Positions written by decode steps are never
         # counted: the reference prefills them again, and the GEMV decode path rounds differently from the prefill GEMMs.
@@ -137,6 +145,7 @@ class LlamaDecoder:
 
     supports_prefix_reuse = True
     supports_prompt_lookup = True
+    supports_logits_processors = True
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     last_speculation = (0, 0, 0)
@@ -179,6 +188,7 @@ class LlamaDecoder:
             raise RuntimeError(f"KV cache for {n_seqs} x {tokens_per_seq} tokens needs {need_pages * per_page >> 20} MiB, not available")
         self._graph = None
         self._graph_sample = None
+        self._proc_graphs = {}
         self._record_prefix(0)
         n_pages_old, n_seqs_old = c.n_pages, len(c.owned)
         self.cache = None
@@ -258,9 +268,9 @@ class LlamaDecoder:
         return lg.float()
 
     # ---------------------------------------------------------------------------------------------
-    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False) -> None:
+    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False) -> None:
         d, w = self.dims, self.w
-        if sample and logits_out is None:
+        if (sample or proc) and logits_out is None:
             logits_out = self._sample_buffer()
         if self._packed_array is not None:
             ops.llama_decode_step_packed(self.h, self._layer_array, self._packed_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
@@ -270,30 +280,72 @@ class LlamaDecoder:
             ops.llama_decode_step(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos,
                                   self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, w.embed, self.lm_ws,
                                   self.out_ids, self.step, logits_out)
-        if sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
+        if proc:
+            self._process_row(logits_out, sample)
+        elif sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
             ops.sample_top_p(logits_out, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+
+    def _process_row(self, raw: torch.Tensor, sample: bool) -> None:
+        """After an lm_head that advanced the step: the processors over the raw fp32 row (history = out_ids[:step - 1]), then the
+        processed greedy choice, or a draw from the processed row, replaces out_ids[step - 1] and the next embedding row."""
+        w = self.w
+        if sample:
+            if self.proc_logits is None:
+                self.proc_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
+            ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, out=self.proc_logits)
+            ops.sample_top_p(self.proc_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+        else:
+            ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, ids=self.proc_ids)
+            ops.logits_pick_token(self.proc_ids, self.step, -1, self.out_ids, w.embed, self.h)
+
+    def _proc_kernels(self, sample: bool) -> int:
+        """Kernels the processing adds to a graph-replayed one-token step (ops.LAUNCHES accounting)."""
+        return 1 if sample else 3  # processing (+ key unpack and pick when greedy); sampling's own kernel is counted by the caller
+
+    def _set_processors(self, processors) -> bool:
+        """processors = None or a spec of logits_processors.parse / resolve_min_length.  Writes its device encoding; True when on."""
+        if not processors:
+            return False
+        V = self.dims.vocab_size
+        if any(t < 0 or t >= V for s in processors.get("bad_words_ids") or [] for t in s):
+            raise ValueError(f"bad_words_ids holds a token outside the vocabulary [0, {V})")
+        fparams, ints = logits_processors.encode(processors)
+        if self.proc_spec is None or self.proc_spec.numel() < ints.size:
+            cap = 256
+            while cap < ints.size:
+                cap *= 2
+            self.proc_spec = torch.zeros(cap, dtype=torch.int32, device=self.device)
+            self._proc_graphs = {}  # they read the old buffer
+            if getattr(self, "_bstate", None) is not None:
+                self._bstate["graph_proc"] = None
+        self.proc_spec[: ints.size].copy_(torch.from_numpy(ints))
+        self.proc_fparams.copy_(torch.from_numpy(fparams))
+        return True
 
     def _sample_buffer(self) -> torch.Tensor:
         if self.sample_logits is None:
             self.sample_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
         return self.sample_logits
 
-    def _ensure_graph(self, seq: int, sample: bool = False) -> None:
-        if (self._graph_sample if sample else self._graph) is not None:
+    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False) -> None:
+        if (self._proc_graphs.get(sample) if proc else (self._graph_sample if sample else self._graph)) is not None:
             return
         # warm up once outside capture (lazy cudaFuncSetAttribute calls etc.), on a side stream
         saved = (self.pos.clone(), self.step.clone(), self.h.clone(), self.out_ids.clone())
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())  # after the clones are enqueued
+        kw = {"proc": True} if proc else {}  # the plain call keeps the signature subclasses override
         with torch.cuda.stream(s):
-            self._decode_step_launch(seq, sample=sample)
+            self._decode_step_launch(seq, sample=sample, **kw)
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.pos.copy_(saved[0]); self.step.copy_(saved[1]); self.h.copy_(saved[2]); self.out_ids.copy_(saved[3])
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            self._decode_step_launch(seq, sample=sample)
-        if sample:
+            self._decode_step_launch(seq, sample=sample, **kw)
+        if proc:
+            self._proc_graphs[sample] = g
+        elif sample:
             self._graph_sample = g
         else:
             self._graph = g
@@ -322,7 +374,7 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def generate_from_embeds(self, inputs_embeds: torch.Tensor, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
                              use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0,
-                             lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2):
+                             lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2, processors=None):
         """Greedy (or, with ``sampling=dict(temperature, top_p, seed)``, nucleus-sampled) decoding started from prompt
         embeddings [S, H].  Returns LongTensor [n_new] (and fp32 logits [n_new, V] when return_logits).
         ``stopping_fn(ids_so_far: LongTensor) -> bool``.
@@ -334,7 +386,10 @@ class LlamaDecoder:
         negative = a row that never matches) followed by the generated tokens, and keeps the drafts that equal the model's own greedy
         choices plus one token of its own.  The ids and logits are bit-identical to plain greedy decoding whatever the drafts are.
         ``last_speculation`` = (verify passes, tokens drafted, tokens accepted) of the passes up to the last returned token; a
-        request whose verify slack does not fit max_seq_len or the decoder's token cap runs the one-token loop and reports (0, 0, 0)."""
+        request whose verify slack does not fit max_seq_len or the decoder's token cap runs the one-token loop and reports (0, 0, 0).
+        ``processors`` (a spec of logits_processors.resolve_min_length, or None): HF's repetition penalty / no-repeat n-gram / bad words /
+        minimum length over every token's logits, the first one included, before the greedy choice or the sampling warpers; the history
+        is the generated tokens.  Returned logits stay raw, as HF's output_logits."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
         n_reuse = int(reuse_rows)
@@ -352,8 +407,9 @@ class LlamaDecoder:
             eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
         k = min(int(lookup_k), ops.SPEC_T_MAX - 1) if lookup_k else 0
         self.last_speculation = (0, 0, 0)
-        if k > 0 and (seq != 0 or sampling or int(lookup_ngram) < 1):
-            raise ValueError("prompt-lookup decoding serves greedy decoding of sequence 0 with lookup_ngram >= 1")
+        if k > 0 and (seq != 0 or sampling or int(lookup_ngram) < 1 or processors):
+            raise ValueError("prompt-lookup decoding serves greedy decoding of sequence 0 with lookup_ngram >= 1, without logits processors")
+        proc = self._set_processors(processors)
         # a verify pass writes up to T positions past the last emitted token, and one pass is in flight after the stop is seen
         slack = 2 * ops.SPEC_T_MAX
         if k > 0 and (S + max_new_tokens + slack > self.max_seq_len or max_new_tokens + slack > self.out_ids.numel()):
@@ -371,14 +427,16 @@ class LlamaDecoder:
         self.pos.fill_(S - 1)
         self.step.zero_()
         sample = self._set_sampling(sampling)
-        first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample else None)
+        first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample or proc else None)
         ops.lm_head_argmax(hidden[S - 1 - n_reuse], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
                            embed_table=w.embed, next_x=self.h, logits_out=first_logits)
-        if sample:
+        if proc:
+            self._process_row(first_logits, sample)
+        elif sample:
             ops.sample_top_p(first_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
         if k > 0 and max_new_tokens > 1:
             return self._verify_loop(k + 1, int(lookup_ngram), lookup_ids, max_new_tokens, eos, stopping_fn, use_graph, logits)
-        return self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample)
+        return self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc)
 
     # ---- prompt-lookup speculative decoding: verify passes of T = k + 1 tokens, every weight streamed once per pass ---------------
     def _verify_buffers(self):
@@ -488,22 +546,25 @@ class LlamaDecoder:
             return out, logits[:n]
         return out
 
-    def _decode_loop(self, seq: int, n: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False):
-        """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled); pos / step / h / out_ids[:n] are already set."""
+    def _decode_loop(self, seq: int, n: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False,
+                     proc: bool = False):
+        """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
+        out_ids[:n] are already set."""
         self.active_pt.copy_(self.cache.page_tables[seq])
         need_host_check = bool(eos) or stopping_fn is not None
         return_logits = logits is not None
         graph = None
         if use_graph and not return_logits:
-            self._ensure_graph(seq, sample)
-            graph = self._graph_sample if sample else self._graph
+            self._ensure_graph(seq, sample, proc=True) if proc else self._ensure_graph(seq, sample)
+            graph = self._proc_graphs[sample] if proc else (self._graph_sample if sample else self._graph)
+        per_replay = self.kernels_per_decode_step + (1 if sample else 0) + (self._proc_kernels(sample) if proc else 0)
 
         def launch_step(k: int) -> None:
             if graph is not None:
                 graph.replay()
-                ops.LAUNCHES += self.kernels_per_decode_step + (1 if sample else 0)
+                ops.LAUNCHES += per_replay
             else:
-                self._decode_step_launch(seq, None if logits is None else logits[k], sample)
+                self._decode_step_launch(seq, None if logits is None else logits[k], sample, **({"proc": True} if proc else {}))
 
         if not need_host_check:
             while n < max_new_tokens:
@@ -565,14 +626,14 @@ class LlamaDecoder:
         d, dev = self.dims, self.device
         H, nh, nkv, hd, I, V = d.hidden_size, d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.intermediate_size, d.vocab_size
         z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
-        st = dict(B=B, cache=self.cache, graph=None, h=z(B, H), xn=z(B, H), qkv=z(B, (nh + 2 * nkv) * hd), attn=z(B, nh * hd), act=z(B, I),
+        st = dict(B=B, cache=self.cache, graph=None, graph_proc=None, h=z(B, H), xn=z(B, H), qkv=z(B, (nh + 2 * nkv) * hd), attn=z(B, nh * hd), act=z(B, I),
                   logits=z(B, (V + 7) // 8 * 8), pos=z(B, dtype=torch.int32), step=z(1, dtype=torch.int32), ids=z(B, dtype=torch.int64),
                   out=z(self.out_ids.numel() * B, dtype=torch.int64), ticket=z(1, dtype=torch.int32),
                   cu=torch.arange(B + 1, dtype=torch.int32, device=dev))
         self._bstate = st
         return st
 
-    def _batch_step_launch(self, st, logits_only: bool = False) -> None:
+    def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False) -> None:
         """One decode step of all B sequences (llava_arch.py:549-611 + modeling_llama.py:540-562 semantics without padding): the
         projections are wgmma GEMMs over the B rows (tall stream-K configuration), RoPE / KV append and attention per sequence."""
         d, w, B = self.dims, self.w, st["B"]
@@ -595,10 +656,14 @@ class LlamaDecoder:
         ops.gemm(xn, w.lm_head, out=lg)  # bf16 logits (modeling_llama.py:1044), arg max with the lowest index on ties
         if logits_only:  # beam search: the host picks the next tokens from the candidates of these logits
             return
-        ops.argmax_bf16(lg, out=st["ids"])
+        if proc:  # the processors over each sequence's bf16 row and its history st["out"][t * B + b], t < step; then the arg max
+            ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, ids=st["ids"])
+        else:
+            ops.argmax_bf16(lg, out=st["ids"])
         ops.decode_batch_advance(st["ids"], w.embed, h, st["out"], st["step"], st["pos"], st["ticket"])
 
-    def _decode_batched(self, first: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos, stopping_fn, use_graph: bool):
+    def _decode_batched(self, first: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos, stopping_fn, use_graph: bool,
+                        proc: bool = False):
         """Greedy decode of B prefilled sequences together.  Returns a list of LongTensor [n_b] (each cut at its own stop)."""
         B = len(seq_lens)
         st = self._batch_state(B)
@@ -607,21 +672,22 @@ class LlamaDecoder:
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        if use_graph and st["graph"] is None:
+        gkey = "graph_proc" if proc else "graph"
+        if use_graph and st[gkey] is None:
             saved = {k: st[k].clone() for k in ("h", "pos", "step", "out")}
             s = torch.cuda.Stream(device=self.device)
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._batch_step_launch(st)  # warm-up outside capture (lazy kernel attribute setup)
+                self._batch_step_launch(st, proc=proc)  # warm-up outside capture (lazy kernel attribute setup)
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
             for k, v in saved.items():
                 st[k].copy_(v)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._batch_step_launch(st)
-            st["graph"] = g
-        kernels = 8 * self.dims.num_hidden_layers + 4
+                self._batch_step_launch(st, proc=proc)
+            st[gkey] = g
+        kernels = 8 * self.dims.num_hidden_layers + (5 if proc else 4)  # the processing kernel + key unpack replace the arg max
         need_check = bool(eos) or stopping_fn is not None
         host = torch.empty((max_new_tokens, B), dtype=torch.int64, pin_memory=True) if need_check else None
         side = getattr(self, "_copy_stream", None) or torch.cuda.Stream(device=self.device)
@@ -646,10 +712,10 @@ class LlamaDecoder:
         checked = 0
         while n < max_new_tokens:
             if use_graph:
-                st["graph"].replay()
+                st[gkey].replay()
                 ops.LAUNCHES += kernels
             else:
-                self._batch_step_launch(st)
+                self._batch_step_launch(st, proc=proc)
             if need_check:  # same pipelining as the single-sequence loop: inspect row n-1 while row n is being computed
                 fetch(n)
                 for k in range(checked, n):
@@ -787,11 +853,12 @@ class LlamaDecoder:
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos_token_ids=None,
-                       stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None):
+                       stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None, processors=None):
         """Decoding of B prompts: ONE packed prefill pass (tensor-core bound, all prompts share every GEMM), one lm_head GEMM for the
         B first tokens, then BATCHED decode: every step advances all B sequences, each weight streamed once per step for the
         whole batch (_decode_batched).  With ``return_logits`` or sampling the sequences are decoded one after the other with the
-        single-sequence weight-streaming step.  Returns a list of LongTensor [n_b] (and a list of fp32 logits)."""
+        single-sequence weight-streaming step.  Returns a list of LongTensor [n_b] (and a list of fp32 logits).
+        ``processors``: the logits processors of generate_from_embeds, on every path (the first tokens included)."""
         d, w = self.dims, self.w
         B = len(seq_lens)
         if max_new_tokens < 1:
@@ -803,6 +870,7 @@ class LlamaDecoder:
         eos = set()
         if eos_token_ids is not None:
             eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
+        proc = self._set_processors(processors)
         for b in range(len(self.cache.owned)):
             self.cache.release(b)
         self.ensure_capacity(B, max(seq_lens) + max_new_tokens)
@@ -811,10 +879,14 @@ class LlamaDecoder:
         first, lg = self.first_tokens(hidden, seq_lens, return_logits=True)
         outs, all_logits = [], []
         sample = self._set_sampling(sampling)
+        first_rows = None  # the processed first-token rows a sampled sequence draws from
+        if proc:  # the first tokens with an empty history: only the minimum length and single-token bad words act
+            first_rows = torch.empty((B, d.vocab_size), dtype=torch.float32, device=self.device) if sample else None
+            ops.logits_process(lg, None, 0, 1, None, 0, self.proc_fparams, self.proc_spec, out=first_rows, ids=first)
         if max_new_tokens == 1 and not return_logits and not sample:
             return [first[b:b + 1] for b in range(B)]
         if not return_logits and not sample and B > 1:
-            return self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph)
+            return self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc)
         zero = torch.zeros(1, dtype=torch.int32, device=self.device)
         for b in range(B):
             logits = None
@@ -828,8 +900,9 @@ class LlamaDecoder:
             self.step.fill_(1)
             if sample:  # re-draw the first token of this sequence from its logits row (a different draw per sequence: the seed moves)
                 self._set_seed(self.sample_seed + 0x9E3779B97F4A7C15 * (b + 1))
-                ops.sample_top_p(lg[b].float().contiguous(), self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
-            r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample)
+                row = first_rows[b] if proc else lg[b].float().contiguous()
+                ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+            r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc)
             if return_logits:
                 outs.append(r[0]); all_logits.append(r[1])
             else:

@@ -11,7 +11,7 @@ from typing import Any, List, Optional, Sequence, Tuple, Union
 
 import torch
 
-from . import ops
+from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
 from .llama_decoder import LlamaDecoder
@@ -429,10 +429,23 @@ class LlavaLlamaModel:
             sampling = dict(temperature=1.0 if temperature is None else float(temperature), top_p=top_p, top_k=top_k, seed=seed)
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
+        # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
+        # device inside the decode step before the greedy choice or the sampling warpers (logits_processors.py, csrc/logits_process.cu).
+        # The history is the generated tokens, as HF's given only inputs_embeds.  Neutral values leave generate() unchanged.
+        proc_kw = {k: generation_kwargs.pop(k, None) for k in ("repetition_penalty", "no_repeat_ngram_size", "bad_words_ids", "min_new_tokens",
+                                                              "min_length")}
         if num_beams != 1 and (sampling is not None or return_logits):
             raise NotImplementedError("beam search is implemented for do_sample=False without output_logits (the eval scripts' mode)")
         if generation_kwargs:
             raise TypeError(f"unsupported generation kwargs: {sorted(generation_kwargs)}")
+        processors = logits_processors.parse(**proc_kw, eos_token_id=eos_token_id, vocab_size=getattr(self.config.llama, "vocab_size", None))
+        if processors is not None:
+            if num_beams != 1:
+                raise NotImplementedError("logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length) with beam search")
+            if lookup_k:
+                raise NotImplementedError("logits processors with prompt_lookup_num_tokens (the verify pass would process every draft position)")
+            if not getattr(self.llm, "supports_logits_processors", False):
+                raise NotImplementedError("logits processors on the tensor-parallel decoder (its logits are vocabulary-parallel)")
         if lookup_k:
             if lookup_k < 0 or lookup_ngram < 1:
                 raise ValueError("prompt_lookup_num_tokens and max_matching_ngram_size must be positive")
@@ -477,6 +490,8 @@ class LlavaLlamaModel:
             def stop_fn(ids, _sc=stopping_criteria):
                 return any(bool(c(ids[None], None)) for c in _sc)
         lens = [int(n) for n in lens]
+        processors = logits_processors.resolve_min_length(processors, max(lens))  # HF subtracts the (padded) inputs_embeds length
+        proc = {} if processors is None else {"processors": processors}
         if lookup_k and B != 1:
             raise NotImplementedError("prompt_lookup_num_tokens serves batch-1 requests")
         left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
@@ -504,7 +519,8 @@ class LlavaLlamaModel:
                 spec = dict(lookup_ids=self._lookup_history(input_ids, attention_mask, packed is not None), lookup_k=lookup_k,
                             lookup_ngram=lookup_ngram)
             r = self.llm.generate_from_embeds(emb, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse, **spec)
+                                              use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse, **spec,
+                                              **proc)
             if lookup_k:
                 self.last_speculation = tuple(self.llm.last_speculation)
             if prefix is not None:
@@ -522,7 +538,7 @@ class LlavaLlamaModel:
                 T = inputs_embeds.shape[1]
                 packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
             r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                        use_graph=use_graph, return_logits=return_logits, sampling=sampling)
+                                        use_graph=use_graph, return_logits=return_logits, sampling=sampling, **proc)
             if return_logits:
                 outs, all_logits = r
             else:

@@ -626,6 +626,55 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
                                              _p(out_ids), _p(embed_table), _p(next_x), K, _stream()), "srgpt_sample_top_p_f32")
 
 
+def logits_process(logits: torch.Tensor, hist: Optional[torch.Tensor], hist_row_stride: int, hist_tok_stride: int, step: Optional[torch.Tensor],
+                   step_offset: int, fparams: torch.Tensor, spec: torch.Tensor, out: Optional[torch.Tensor] = None,
+                   ids: Optional[torch.Tensor] = None) -> None:
+    """HF's repetition penalty / no-repeat n-gram / bad words / minimum length processors over the rows of ``logits`` ([rows, V] fp32 or
+    the element type, unit inner stride; a 1-D fp32 row counts as one row), then the greedy choice.  Row r's history is
+    ``hist.view(-1)[r * hist_row_stride + t * hist_tok_stride]`` for t < step + step_offset (``step`` = device int32 [1], or None:
+    step_offset tokens).  ``fparams`` = device float32 [penalty, 1 / penalty], ``spec`` = device int32 (layout: include/srgpt_b200.h).
+    Writes the processed fp32 rows to ``out`` [rows, V] and / or the arg max of each processed row to ``ids`` int64 [rows]."""
+    x = logits if logits.dim() == 2 else logits.view(1, -1)
+    rows, V = x.shape
+    f32 = x.dtype == torch.float32
+    _need(x, torch.float32 if f32 else ELEM(), "logits_process.logits")
+    _need(fparams, torch.float32, "logits_process.fparams"); _need(spec, torch.int32, "logits_process.spec")
+    if out is not None:
+        out = out if out.dim() == 2 else out.view(1, -1)
+        _need(out, torch.float32, "logits_process.out")
+        if out.shape != x.shape:
+            raise SrgptError(f"logits_process: out {tuple(out.shape)} does not match logits {tuple(x.shape)}")
+    if ids is not None:
+        _need(ids, torch.int64, "logits_process.ids")
+        if ids.numel() < rows or not ids.is_contiguous():
+            raise SrgptError("logits_process: ids must be a contiguous int64 vector of at least `rows` entries")
+    cap = 0
+    if hist is not None:
+        _need(hist, torch.int64, "logits_process.hist")
+        if not hist.is_contiguous():
+            raise SrgptError("logits_process: hist must be contiguous")
+        last = (rows - 1) * hist_row_stride  # the history of every row must lie inside hist
+        cap = max(0, (hist.numel() - 1 - last) // max(hist_tok_stride, 1) + 1) if hist.numel() > last else 0
+    if step is not None:
+        _need(step, torch.int32, "logits_process.step")
+    check(_lib.load().srgpt_logits_process(_p(x), int(f32), _rowmajor2d(x, "logits_process.logits"), rows, V, _p(hist), hist_row_stride,
+                                           hist_tok_stride, cap, _p(step), step_offset, _p(fparams), _p(spec), spec.numel(), _p(out),
+                                           0 if out is None else _rowmajor2d(out, "logits_process.out"), _p(ids), _stream()),
+          "srgpt_logits_process")
+    if ids is not None:
+        _count(2)  # the processing kernel and the key unpack
+
+
+def logits_pick_token(ids: torch.Tensor, step: torch.Tensor, step_offset: int, out_ids: torch.Tensor, embed_table: Optional[torch.Tensor] = None,
+                      next_x: Optional[torch.Tensor] = None) -> None:
+    """out_ids[step + step_offset] = ids[0] (and next_x = embed_table[ids[0]]): the processed greedy choice of a one-token step."""
+    _need(ids, torch.int64, "logits_pick_token.ids"); _need(step, torch.int32, "logits_pick_token.step")
+    _need(out_ids, torch.int64, "logits_pick_token.out_ids")
+    K = 0 if embed_table is None else embed_table.shape[1]
+    check(_lib.load().srgpt_logits_pick_token(_p(ids), _p(step), step_offset, _p(out_ids), _p(embed_table), _p(next_x), K, _stream()),
+          "srgpt_logits_pick_token")
+
+
 def beam_candidates(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores: torch.Tensor, cand_tokens: torch.Tensor) -> None:
     """Per beam row: the n_cand best (log_softmax(logits)[token] + beam_scores[row], token) -> cand_scores / cand_tokens [k, n_cand]."""
     _need(logits, ELEM(), "beam_candidates.logits"); _need(beam_scores, torch.float32, "beam_candidates.beam_scores")

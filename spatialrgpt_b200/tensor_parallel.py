@@ -64,6 +64,7 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_prefix_reuse = False  # prompt-prefix reuse is a batch-1, single-GPU feature: nothing is recorded here
     packs_decode_weights = False   # the ranks stream their bf16 shards
     supports_prompt_lookup = False  # the verify pass is a single-GPU kernel sequence
+    supports_logits_processors = False  # the logits are vocabulary-parallel: no rank holds a whole row
 
     def __init__(self, dims: LlamaDims, w: LlamaW, rank: int, world: int, group=None, max_seq_len: int = 4096, comm: Optional[str] = None, **kw):
         super().__init__(dims, w, max_seq_len=max_seq_len, **kw)
