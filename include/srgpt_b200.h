@@ -229,6 +229,35 @@ int srgpt_gemv_packed_bf16(const void* x, const srgpt_packed12* packed, void* y,
 int srgpt_lm_head_argmax_packed_bf16(const void* x, const srgpt_packed12* packed, int V, int K, const void* norm_weight, float eps,
                                      float* logits_out, void* workspace, const void* embed_table, void* next_x, long long* out_ids,
                                      int* step, int* pos, void* stream);
+/* ---- NF4 weight-only quantization of the decoder-layer matrices (nf4.cu, gemv.cu; DESIGN.md §3) ------------------------
+ * Stands for the reference's load_pretrained_model(load_4bit=True) (llava/model/builder.py:51-60): bitsandbytes NF4 codes,
+ * blocksize 64, double-quantized absmax, applied to the LLM only (llava/model/llava_arch.py:99-101).  A weight's value is
+ * round_to_elem(fl32(code[q] * scale)), dequantized to the element type before the multiply as bitsandbytes' Linear4bit does.
+ * Computed in the build's element type: bfloat16 in libsrgpt_b200.so, IEEE half in libsrgpt_b200_f16.so (the loader's default).
+ * The decode GEMV's planes (nf4.cuh): q [N, K / 2] codes in the GEMV's lane order (K a multiple of 1024), scale [N, K / 64]
+ * fp32 resolved scales in natural order. */
+typedef struct {
+  const unsigned char* q; /* [N, K / 2] */
+  const float* scale;     /* [N, K / 64] */
+} srgpt_nf4;
+/* Load time, step 1 (one original [N, K] matrix, K a multiple of 64): codes [N, K / 2] in natural order (weight 2j in the high
+ * nibble of byte j) chosen against the exact fp32 absmax [N, K / 64] of each block of 64; *n_bad += the blocks holding Inf or NaN. */
+int srgpt_nf4_quantize_bf16(const void* W, int ldw, int N, int K, unsigned char* codes, float* absmax, int* n_bad, void* stream);
+/* Step 2, double quantization of the n absmax values of one matrix: *offset = their mean (fp64 sum in index order, rounded to
+ * fp32), blocks of 256 of (absmax - offset) to the nearest entry of the 256-value signed dynamic map dyn_map, and
+ * scale[i] = fl32(map[c] * absmax2) + offset, the scale the weights are dequantized with. */
+int srgpt_nf4_double_quant(const float* absmax, long long n, const float* dyn_map, float* offset, float* scale, void* stream);
+/* Natural-order codes + scales -> the element-type matrix W [N, ldw] (the resident dequantized copy). */
+int srgpt_nf4_dequantize_bf16(const unsigned char* codes, const float* scale, int N, int K, void* W, int ldw, void* stream);
+/* Natural-order codes [N, K / 2] -> the GEMV's lane order (K a multiple of 1024); run on a fused matrix. */
+int srgpt_nf4_lane_order(const unsigned char* codes, int N, int K, unsigned char* q, void* stream);
+/* The lane-ordered planes -> W [N, ldw], through the GEMV's own dequantization: the round-trip check of the planes. */
+int srgpt_nf4_unpack_bf16(const srgpt_nf4* nf4, int N, int K, void* W, int ldw, void* stream);
+/* srgpt_gemv_bf16 (PLAIN + residual, SWIGLU + RMSNorm, QKV_ROPE + KV append) streaming the NF4 planes: bit-identical to
+ * srgpt_gemv_bf16 over the dequantized matrix.  `nf4` is a host pointer; K a multiple of 1024. */
+int srgpt_gemv_nf4_bf16(const void* x, const srgpt_nf4* nf4, void* y, int N, int K, const void* norm_weight, float eps, const void* residual,
+                        int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos,
+                        void* kv_pages, const int* page_table, int page_size, void* stream);
 /* Plain argmax over fp32 rows (first index on ties), e.g. first token after prefill. */
 int srgpt_argmax_f32(const float* x, int rows, int cols, long long* out, void* stream);
 /* Same over bf16 rows [rows, ldx] (the bf16-rounded logits of a batched lm_head GEMM, modeling_llama.py:1044). */
@@ -375,6 +404,18 @@ int srgpt_llama_decode_step_packed_bf16(void* h, const srgpt_llama_layer_weights
                                         const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
                                         const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids, int* step,
                                         void* stream);
+/* The same step streaming NF4 layer matrices (the reference's load_4bit decode, llava/model/builder.py:51-60): nf4[l].<matrix>.q
+ * == NULL (K not a multiple of 1024) takes the dequantized weight of `layers`; lm_head stays unquantized, streamed from lm_packed
+ * when lm_packed->sm != NULL (bfloat16 build) and from lm_head otherwise.  Bit-identical to srgpt_llama_decode_step_bf16 over the
+ * dequantized weights. */
+typedef struct {
+  srgpt_nf4 qkv, o, gateup, down;
+} srgpt_llama_layer_nf4;
+int srgpt_llama_decode_step_nf4_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf,
+                                     void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                                     const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
+                                     const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
+                                     void* lm_workspace, float* logits_out, long long* out_ids, int* step, void* stream);
 
 /* ---- prompt-lookup speculative decoding, batch 1, greedy (HF GenerationMixin._assisted_decoding with
  * PromptLookupCandidateGenerator, i.e. generate(prompt_lookup_num_tokens=k); call site llava_llama.py:212).

@@ -91,6 +91,14 @@ SIGNATURES = {
     "srgpt_lm_head_argmax_packed_bf16": (ci, [vp, vp, ci, ci, vp, cf, vp, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_llama_decode_step_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp,
                                                  vp, vp, vp, vp]),
+    "srgpt_nf4_quantize_bf16": (ci, [vp, ci, ci, ci, vp, vp, vp, vp]),
+    "srgpt_nf4_double_quant": (ci, [vp, cll, vp, vp, vp, vp]),
+    "srgpt_nf4_dequantize_bf16": (ci, [vp, vp, ci, ci, vp, ci, vp]),
+    "srgpt_nf4_lane_order": (ci, [vp, ci, ci, vp, vp]),
+    "srgpt_nf4_unpack_bf16": (ci, [vp, ci, ci, vp, ci, vp]),
+    "srgpt_gemv_nf4_bf16": (ci, [vp, vp, vp, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_llama_decode_step_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp,
+                                              vp, vp, vp, vp]),
     "srgpt_gemv_multi_bf16": (ci, [vp, ci, vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
     "srgpt_gemv_multi_packed_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
     "srgpt_lm_head_multi_bf16": (ci, [vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, vp, vp]),
@@ -122,6 +130,15 @@ class Packed12(C.Structure):
 
 class LlamaLayerPacked(C.Structure):
     _fields_ = [(n, Packed12) for n in ("qkv", "o", "gateup", "down")]
+
+
+class Nf4(C.Structure):
+    """srgpt_nf4: one matrix's NF4 planes for the decode GEMV (q NULL = the step reads the dequantized matrix)."""
+    _fields_ = [("q", vp), ("scale", vp)]
+
+
+class LlamaLayerNf4(C.Structure):
+    _fields_ = [(n, Nf4) for n in ("qkv", "o", "gateup", "down")]
 
 
 def lib_path(elem: str = "bf16") -> str:

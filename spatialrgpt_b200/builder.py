@@ -216,7 +216,9 @@ def load_pretrained_model(model_path: str, model_name: str, model_base: Optional
 
     The model comes back in fp16 like the reference's (builder.py:62 sets torch_dtype = float16 unconditionally); callers that want
     bf16 cast afterwards exactly as the reference's do (``model.to(dtype=torch.bfloat16)``, eval_spatial.py:221).  ``torch_dtype=``
-    (torch.float16 / torch.bfloat16) is an extension that loads straight into that dtype."""
+    (torch.float16 / torch.bfloat16) is an extension that loads straight into that dtype.  ``quantization="nf4"`` is an extension too:
+    the decoder-layer linears are NF4-quantized at load (weights.from_state_dicts) and dequantized into that dtype; the batch-1 decode
+    step streams the 4-bit planes.  ``load_4bit`` / ``load_8bit`` (bitsandbytes) still raise."""
     if load_8bit or load_4bit:
         raise NotImplementedError("bitsandbytes quantised loading is outside the hot path (builder.py:51-60)")
     if model_base is not None:
@@ -232,8 +234,9 @@ def load_pretrained_model(model_path: str, model_name: str, model_base: Optional
     dtype = kwargs.pop("torch_dtype", None) or torch.float16
     if dtype not in (torch.float16, torch.bfloat16):
         raise NotImplementedError(f"torch_dtype {dtype}: the sm_90a kernels compute in torch.float16 or torch.bfloat16")
-    model = LlavaLlamaModel(cfg, from_state_dicts(cfg, sd, dev, dtype=dtype), tokenizer=tokenizer, image_processor=image_processor,
-                            max_seq_len=max_seq)
+    quantization = kwargs.pop("quantization", None)
+    model = LlavaLlamaModel(cfg, from_state_dicts(cfg, sd, dev, dtype=dtype, quantization=quantization), tokenizer=tokenizer,
+                            image_processor=image_processor, max_seq_len=max_seq)
     context_len = getattr(cfg.llama, "max_sequence_length", 2048) if hasattr(cfg.llama, "max_sequence_length") else 2048
     return tokenizer, model, image_processor, context_len
 

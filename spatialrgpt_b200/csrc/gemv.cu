@@ -23,6 +23,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "nf4.cuh"
 #include "pack12.cuh"
 #include "srgpt_b200.h"
 
@@ -255,6 +256,10 @@ __device__ __forceinline__ void consume12(const Raw12& q0, const Raw12& q1, Rows
 // layer (qkv 50 MB, o_proj 33 MB) run behind a kernel that leaves HBM idle (decode attention / the previous tail), so
 // the more of their weights is in flight before the dependency resolves, the less of them is exposed afterwards.
 // PACKED: the weights are p.pk (12-bit packing, K % 1024 == 0, PRE == 1); everything but the weight stream is shared.
+template <int MODE>
+__device__ __forceinline__ void epilogue(const Params& p, bool active, int pi, int r0, int r1, int warp, int lane, float a0, float a1, float* sv,
+                                         int* si);
+
 template <int MODE, int PRE, bool PACKED>
 __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) decode_gemv_kernel(const Params p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -451,6 +456,15 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
       a1 += dot8(ld_stream16(p1 + c), xf);
     }
   }
+  epilogue<MODE>(p, active, pi, r0, r1, warp, lane, a0, a1, sv, si);
+  trace_mark(p.trace, 2);
+}
+
+// The end of every one-token decode GEMV: the warp sums of the lane partials a0 / a1 of rows r0 / r1, then the mode's epilogue
+// (rounding points of the reference's torch ops, see the top of the file) and, for lm_head, the CTA's arg max partial.
+template <int MODE>
+__device__ __forceinline__ void epilogue(const Params& p, bool active, int pi, int r0, int r1, int warp, int lane, float a0, float a1, float* sv,
+                                         int* si) {
   a0 = warp_sum(a0);
   a1 = warp_sum(a1);
   float best = -INFINITY;
@@ -516,6 +530,144 @@ __global__ void __launch_bounds__(THREADS, PRE == 1 ? 3 : (PRE == 2 ? 2 : 1)) de
       p.part_idx[blockIdx.x] = besti;
     }
   }
+}
+
+// ---- NF4 weights (nf4.cuh): per batch a lane streams one 16-byte vector of codes per row (its 4 chunks) and lanes 0-15 / 16-31 one
+//      scale each of row r0 / r1 (the row's 16 blocks of the batch, 64 bytes per row).  Lane l's chunk i lies in block 4 i + l / 8 of
+//      the batch, so its two scales come from lanes 4 i + l / 8 and 16 + 4 i + l / 8 by shuffle.
+struct NParams {
+  Params p;
+  srgpt_nf4 nf;
+};
+constexpr int SLOT_NF4 = 2 * 32 * 16 + 32 * 4;  // one ring slot per warp: both rows' code vectors (2 x 512 B) and the 32 scales (128 B)
+
+struct Raw4 {
+  uint4 q0, q1;
+  float s;
+};
+
+__device__ __forceinline__ Raw4 ld_raw4(const uint4* q0, const uint4* q1, const float* s_lane, int b) {
+  Raw4 t;
+  t.q0 = ld_stream16(q0 + b * 32);
+  t.q1 = ld_stream16(q1 + b * 32);
+  t.s = __ldg(s_lane + b * 16);
+  return t;
+}
+
+// batch b of both rows and the scales into one slot of the warp's ring (codes of r0 / r1 at +0 / +512, scales at +1024); every lane
+// later reads back exactly what it requested, so no barrier is needed
+__device__ __forceinline__ void cp_async_batch4(uint8_t* slot, int lane, const uint4* q0, const uint4* q1, const float* s_lane, int b) {
+  const uint32_t d = (uint32_t)__cvta_generic_to_shared(slot + lane * 16);
+  const uint32_t ds = (uint32_t)__cvta_generic_to_shared(slot + 1024 + lane * 4);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(q0 + b * 32) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512), "l"(q1 + b * 32) : "memory");
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(ds), "l"(s_lane + b * 16) : "memory");
+}
+
+__device__ __forceinline__ Raw4 ld_slot4(const uint8_t* slot, int lane) {
+  Raw4 t;
+  t.q0 = *reinterpret_cast<const uint4*>(slot + lane * 16);
+  t.q1 = *reinterpret_cast<const uint4*>(slot + 512 + lane * 16);
+  t.s = *reinterpret_cast<const float*>(slot + 1024 + lane * 4);
+  return t;
+}
+
+__device__ __forceinline__ uint32_t word_of(const uint4& v, int i) { return i == 0 ? v.x : (i == 1 ? v.y : (i == 2 ? v.z : v.w)); }
+
+// batch b in chunk order through the plain kernel's dot8 chain: the lane's fp32 sums are those of the element-type kernel over the
+// dequantized matrix
+__device__ __forceinline__ void consume_nf4(const Raw4& t, const float* tab, int b, int lane, const uint4* px, float& a0, float& a1) {
+  const int c = b * 128 + lane;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float s0 = __shfl_sync(0xffffffffu, t.s, 4 * i + (lane >> 3));
+    const float s1 = __shfl_sync(0xffffffffu, t.s, 16 + 4 * i + (lane >> 3));
+    const uint4 w0 = nf4::dequant8(word_of(t.q0, i), s0, tab);
+    const uint4 w1 = nf4::dequant8(word_of(t.q1, i), s1, tab);
+    float xf[8];
+    unpack8(px[c + 32 * i], xf);
+    a0 += dot8(w0, xf);
+    a1 += dot8(w1, xf);
+  }
+}
+
+// The one-token decode GEMV over NF4 planes (PLAIN, SWIGLU, QKV_ROPE; K % 1024 == 0).  The structure of the packed kernel: batch 0 in
+// registers and the next p.spre batches in the warp's shared-memory slots, all requested before the dependency wait; with p.ring the
+// slots are a ring every later batch streams through, else later batches load into registers.  Same x staging, row pairs and epilogue.
+template <int MODE>
+__global__ void __launch_bounds__(THREADS, 3) decode_gemv_nf4_kernel(const NParams np) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ float red[32];
+  __shared__ float sv[WARPS];
+  __shared__ int si[WARPS];
+  __shared__ float tab[16];
+  const Params& p = np.p;
+  bf16* sx = reinterpret_cast<bf16*>(smem_raw);
+  const uint4* px = reinterpret_cast<const uint4*>(sx);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  trace_mark(p.trace, 0);
+  const int pi = blockIdx.x * WARPS + warp;
+  const bool active = pi < (p.N >> 1);
+  int r0 = 0, r1 = 0;
+  if (active) pair_rows<MODE>(p, pi, r0, r1);
+  if (threadIdx.x < 16) tab[threadIdx.x] = nf4::code_value(threadIdx.x);  // published by stage_x's barrier
+
+  const int nbatch = p.K >> 10;
+  uint8_t* ring = smem_raw + (size_t)p.K * 2 + (size_t)warp * p.spre * SLOT_NF4;
+  const uint4 *q0 = nullptr, *q1 = nullptr;
+  const float* s_lane = nullptr;
+  Raw4 t0 = {};
+  int n_spre = 0;
+  if (active) {
+    q0 = reinterpret_cast<const uint4*>(np.nf.q + (size_t)r0 * (p.K >> 1)) + lane;
+    q1 = reinterpret_cast<const uint4*>(np.nf.q + (size_t)r1 * (p.K >> 1)) + lane;
+    s_lane = np.nf.scale + (size_t)(lane < 16 ? r0 : r1) * (p.K >> 6) + (lane & 15);
+    t0 = ld_raw4(q0, q1, s_lane, 0);
+    for (int b = 0; b < p.spre && 1 + b < nbatch; ++b) {
+      cp_async_batch4(ring + b * SLOT_NF4, lane, q0, q1, s_lane, 1 + b);
+      asm volatile("cp.async.commit_group;" ::: "memory");
+      ++n_spre;
+    }
+  }
+  uint4 nw_pre[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
+  const bool nw_pre_valid = (p.norm_weight != nullptr) && ((p.K >> 3) <= 2 * THREADS);
+  if (nw_pre_valid) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int cc = threadIdx.x + k * THREADS;
+      if (cc < (p.K >> 3)) nw_pre[k] = reinterpret_cast<const uint4*>(p.norm_weight)[cc];
+    }
+  }
+  pdl_launch_dependents();
+  pdl_wait();
+  trace_mark(p.trace, 1);
+
+  stage_x(p.x, p.norm_weight, p.eps, p.K, sx, red, nw_pre, nw_pre_valid);
+
+  float a0 = 0.f, a1 = 0.f;
+  if (active) {
+    consume_nf4(t0, tab, 0, lane, px, a0, a1);
+    int slot = 0;
+    for (int b = 1; b < nbatch; ++b) {
+      Raw4 t;
+      if (p.ring || b <= n_spre) {
+        // batch b sits in slot `slot`; the groups committed after its own may still be pending
+        cp_async_wait_pending(p.ring ? min(n_spre - 1, nbatch - 1 - b) : n_spre - b);
+        uint8_t* s = ring + slot * SLOT_NF4;
+        t = ld_slot4(s, lane);
+        if (p.ring && b + n_spre < nbatch) {
+          cp_async_batch4(s, lane, q0, q1, s_lane, b + n_spre);
+          asm volatile("cp.async.commit_group;" ::: "memory");
+        }
+        if (++slot == n_spre) slot = 0;
+      } else {
+        t = ld_raw4(q0, q1, s_lane, b);
+      }
+      consume_nf4(t, tab, b, lane, px, a0, a1);
+    }
+  }
+  epilogue<MODE>(p, active, pi, r0, r1, warp, lane, a0, a1, sv, si);
   trace_mark(p.trace, 2);
 }
 
@@ -1071,6 +1223,37 @@ static int launch_mode(const Params& p, int npairs, cudaStream_t st) {
   else return launch<MODE>(p, npairs, st);
 }
 
+// The NF4 kernel's ring: the packed kernel's depth (ring_depth, SRGPT_GEMV_RING) in slots of SLOT_NF4 bytes per warp; depth 0 keeps the
+// fixed levels (spre_default() batches in shared memory, the rest loaded into registers).
+template <int MODE>
+static int launch_nf4(const Params& p, const srgpt_nf4& nf, int npairs, cudaStream_t st) {
+  const int ring = ring_depth(p.K);
+  const int spre = ring >= 0 ? ring : spre_default();
+  const int smem = p.K * 2 + WARPS * spre * SLOT_NF4;
+  static int configured_smem = 0;
+  if (smem > 48 * 1024 && smem > configured_smem) {
+    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_nf4_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured_smem = smem;
+  }
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  pdl_config(cfg, attr, grid_for(npairs), THREADS, smem, st);
+  NParams q = {p, nf};
+  q.p.trace = trace_next_slot();
+  q.p.spre = spre;
+  q.p.ring = ring >= 0 ? 1 : 0;
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, decode_gemv_nf4_kernel<MODE>, q));
+  return SRGPT_OK;
+}
+
+enum { W_PLAIN = 0, W_PACKED12 = 1, W_NF4 = 2 };  // the weight stream of a one-token decode GEMV
+
+template <int MODE, int KIND>
+static int launch_kind(const Params& p, const srgpt_nf4* nf, int npairs, cudaStream_t st) {
+  if constexpr (KIND == W_NF4) return launch_nf4<MODE>(p, *nf, npairs, st);
+  else return launch_mode<MODE, KIND == W_PACKED12>(p, npairs, st);
+}
+
 }  // namespace gemv
 }  // namespace srgpt
 
@@ -1083,11 +1266,12 @@ static bool packed_ok(const srgpt_packed12* P, int K) {
   return P != nullptr && P->sm && P->ex && P->base && P->row_ptr && P->exc && aligned16(P->sm) && aligned16(P->ex) && (K % pack12::BATCH) == 0;
 }
 
-// checks and mode dispatch of srgpt_gemv_bf16 and srgpt_gemv_packed_bf16; p.W / p.ldw or p.pk are set by the caller
-template <bool PACKED>
-static int gemv_modes(gemv::Params& p, const void* x, void* y, int N, int K, const void* norm_weight, float eps, const void* residual, int mode,
-                      int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages,
-                      const int* page_table, int page_size, void* stream) {
+// checks and mode dispatch of srgpt_gemv_bf16, srgpt_gemv_packed_bf16 and srgpt_gemv_nf4_bf16 (KIND = gemv::W_*); p.W / p.ldw, p.pk or nf
+// are set by the caller
+template <int KIND>
+static int gemv_modes(gemv::Params& p, const srgpt_nf4* nf, const void* x, void* y, int N, int K, const void* norm_weight, float eps,
+                      const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+                      const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream) {
   SRGPT_CHECK_ARG(x && y && N > 0 && K > 0);
   SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0);
   SRGPT_CHECK_ARG(K * 2 <= 200 * 1024);
@@ -1112,18 +1296,31 @@ static int gemv_modes(gemv::Params& p, const void* x, void* y, int N, int K, con
   switch (mode) {
     case SRGPT_GEMV_PLAIN:
       p.hd = 2;
-      return gemv::launch_mode<SRGPT_GEMV_PLAIN, PACKED>(p, N / 2, st);
+      return gemv::launch_kind<SRGPT_GEMV_PLAIN, KIND>(p, nf, N / 2, st);
     case SRGPT_GEMV_SWIGLU:
       SRGPT_CHECK_ARG(residual == nullptr);
       p.hd = 2;
-      return gemv::launch_mode<SRGPT_GEMV_SWIGLU, PACKED>(p, N / 2, st);
+      return gemv::launch_kind<SRGPT_GEMV_SWIGLU, KIND>(p, nf, N / 2, st);
     case SRGPT_GEMV_QKV_ROPE:
       SRGPT_CHECK_ARG(residual == nullptr && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && (head_dim % 2) == 0);
       SRGPT_CHECK_ARG(N == (n_heads + 2 * n_kv_heads) * head_dim);
       SRGPT_CHECK_ARG(cos_tab && sin_tab && pos && kv_pages && page_table && page_size > 0);
-      return gemv::launch_mode<SRGPT_GEMV_QKV_ROPE, PACKED>(p, N / 2, st);
+      return gemv::launch_kind<SRGPT_GEMV_QKV_ROPE, KIND>(p, nf, N / 2, st);
   }
   return SRGPT_ERR_INVALID;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_nf4_bf16(const void* x, const srgpt_nf4* nf4, void* y, int N, int K, const void* norm_weight,
+                                                                          float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim,
+                                                                          const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages,
+                                                                          const int* page_table, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(nf4 && nf4->q && nf4->scale && aligned16(nf4->q) && (reinterpret_cast<uintptr_t>(nf4->scale) & 3) == 0);
+  SRGPT_CHECK_ARG(K > 0 && (K % nf4::BLOCK) == 0);
+  SRGPT_CHECK_ARG((K % nf4::BATCH) == 0);
+  SRGPT_CHECK_ARG(K * 2 + gemv::WARPS * gemv::RING_MAX * gemv::SLOT_NF4 <= 227 * 1024);
+  gemv::Params p = {};
+  return gemv_modes<gemv::W_NF4>(p, nf4, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
+                                 page_table, page_size, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void* x, const void* W, int ldw, void* y, int N, int K, const void* norm_weight, float eps,
@@ -1134,8 +1331,8 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void
   gemv::Params p = {};
   p.W = reinterpret_cast<const bf16*>(W);
   p.ldw = ldw;
-  return gemv_modes<false>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
-                           page_table, page_size, stream);
+  return gemv_modes<gemv::W_PLAIN>(p, nullptr, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                                   kv_pages, page_table, page_size, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_gemv_packed_bf16(const void* x, const srgpt_packed12* packed, void* y, int N, int K,
@@ -1150,8 +1347,8 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_packed_bf16(con
 #else
   gemv::Params p = {};
   p.pk = *packed;
-  return gemv_modes<true>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
-                          page_table, page_size, stream);
+  return gemv_modes<gemv::W_PACKED12>(p, nullptr, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                                      kv_pages, page_table, page_size, stream);
 #endif
 }
 

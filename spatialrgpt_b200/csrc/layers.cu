@@ -100,10 +100,14 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_chunk_
   return SRGPT_OK;
 }
 
-// one decode GEMV over the packed matrix when there is one (pk->sm != NULL), else over the plain bf16 weight W [N, K]
-static int gemv_either(const void* x, const void* W, const srgpt_packed12* pk, void* y, int N, int K, const void* norm_weight, float eps,
-                       const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+// one decode GEMV over the NF4 planes when there are some (nf->q != NULL), else over the packed matrix when there is one (pk->sm != NULL),
+// else over the plain weight W [N, K]
+static int gemv_either(const void* x, const void* W, const srgpt_packed12* pk, const srgpt_nf4* nf, void* y, int N, int K, const void* norm_weight,
+                       float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
                        const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream) {
+  if (nf != nullptr && nf->q != nullptr)
+    return srgpt_gemv_nf4_bf16(x, nf, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
+                               page_table, page_size, stream);
   if (pk != nullptr && pk->sm != nullptr)
     return srgpt_gemv_packed_bf16(x, pk, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
                                   page_table, page_size, stream);
@@ -111,26 +115,27 @@ static int gemv_either(const void* x, const void* W, const srgpt_packed12* pk, v
                          page_size, stream);
 }
 
-static int decode_step(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers, void* q_buf,
-                       void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab,
-                       const void* sin_tab, int* pos, const int* page_table, int page_size, const void* final_norm, const void* lm_head,
-                       const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids,
-                       int* step, void* stream) {
+static int decode_step(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4,
+                       int n_layers, void* q_buf, void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                       const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size, const void* final_norm,
+                       const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out,
+                       long long* out_ids, int* step, void* stream) {
   SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos && page_table && final_norm && lm_head && lm_workspace && out_ids && step);
   const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
   const float scale = 1.0f / sqrtf((float)head_dim);
   for (int l = 0; l < n_layers; ++l) {
     const srgpt_llama_layer_weights& w = layers[l];
     const srgpt_llama_layer_packed* pk = packed != nullptr ? &packed[l] : nullptr;
-    SRGPT_TRY(gemv_either(h, w.qkv_w, pk ? &pk->qkv : nullptr, q_buf, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim,
-                          cos_tab, sin_tab, pos, w.kv_pages, page_table, page_size, stream));
+    const srgpt_llama_layer_nf4* nf = nf4 != nullptr ? &nf4[l] : nullptr;
+    SRGPT_TRY(gemv_either(h, w.qkv_w, pk ? &pk->qkv : nullptr, nf ? &nf->qkv : nullptr, q_buf, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE,
+                          n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, w.kv_pages, page_table, page_size, stream));
     SRGPT_TRY(srgpt_attention_decode_bf16(q_buf, attn_buf, w.kv_pages, page_table, page_size, pos, n_heads, n_kv_heads, head_dim, scale, stream));
-    SRGPT_TRY(gemv_either(attn_buf, w.o_w, pk ? &pk->o : nullptr, h, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr,
-                          nullptr, 0, stream));
-    SRGPT_TRY(gemv_either(h, w.gateup_w, pk ? &pk->gateup : nullptr, act_buf, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, 0, 0, 0, nullptr,
+    SRGPT_TRY(gemv_either(attn_buf, w.o_w, pk ? &pk->o : nullptr, nf ? &nf->o : nullptr, h, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr,
                           nullptr, nullptr, nullptr, nullptr, 0, stream));
-    SRGPT_TRY(gemv_either(act_buf, w.down_w, pk ? &pk->down : nullptr, h, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr,
-                          nullptr, nullptr, 0, stream));
+    SRGPT_TRY(gemv_either(h, w.gateup_w, pk ? &pk->gateup : nullptr, nf ? &nf->gateup : nullptr, act_buf, 2 * I, H, w.post_norm, eps, nullptr,
+                          SRGPT_GEMV_SWIGLU, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, stream));
+    SRGPT_TRY(gemv_either(act_buf, w.down_w, pk ? &pk->down : nullptr, nf ? &nf->down : nullptr, h, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0,
+                          nullptr, nullptr, nullptr, nullptr, nullptr, 0, stream));
   }
   if (lm_packed != nullptr && lm_packed->sm != nullptr)
     return srgpt_lm_head_argmax_packed_bf16(h, lm_packed, V, H, final_norm, eps, logits_out, lm_workspace, embed_table, h, out_ids, step, pos, stream);
@@ -143,8 +148,8 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_bf
                                                                                      int page_size, const void* final_norm, const void* lm_head, int V,
                                                                                      const void* embed_table, void* lm_workspace, float* logits_out,
                                                                                      long long* out_ids, int* step, void* stream) {
-  return decode_step(h, layers, nullptr, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos, page_table,
-                     page_size, final_norm, lm_head, nullptr, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
+  return decode_step(h, layers, nullptr, nullptr, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
+                     page_table, page_size, final_norm, lm_head, nullptr, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_packed_bf16(
@@ -153,8 +158,18 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_pa
     int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
     float* logits_out, long long* out_ids, int* step, void* stream) {
   SRGPT_CHECK_ARG(packed != nullptr);
-  return decode_step(h, layers, packed, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos, page_table,
-                     page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
+  return decode_step(h, layers, packed, nullptr, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
+                     page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_nf4_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int H,
+    int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
+    const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out,
+    long long* out_ids, int* step, void* stream) {
+  SRGPT_CHECK_ARG(nf4 != nullptr);
+  return decode_step(h, layers, nullptr, nf4, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
+                     page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
 }
 
 // ---- verify pass of prompt-lookup speculative decoding: T tokens through the layer stack, every weight streamed once -----------

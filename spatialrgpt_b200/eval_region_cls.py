@@ -149,7 +149,8 @@ def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
         from .builder import load_pretrained_model as loader
     model_path = os.path.expanduser(args.model_path)
     model_name = get_model_name_from_path(model_path)
-    tokenizer, model, image_processor, _ = loader(model_path, model_name, getattr(args, "model_base", None))
+    quant = {"quantization": args.quantization} if getattr(args, "quantization", None) else {}
+    tokenizer, model, image_processor, _ = loader(model_path, model_name, getattr(args, "model_base", None), **quant)
     data = get_chunk(generate_data_list(args.annotation_file), args.num_chunks, args.chunk_idx)
     answers_file = os.path.expanduser(args.answers_file)
     os.makedirs(os.path.dirname(answers_file) or ".", exist_ok=True)
@@ -190,6 +191,7 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--dataset", type=str, default="lvis")
     p.add_argument("--prompt_type", type=str, default="seg")
     p.add_argument("--seed", type=int, default=None, help="seed of the prompt choice (the reference draws unseeded)")
+    p.add_argument("--quantization", choices=["nf4"], default=None, help="NF4 weight-only quantization of the LLM's layer matrices")
     return p
 
 

@@ -140,7 +140,13 @@ class LlamaDecoder:
         # The batch-1 decode step streams its matrices in the lossless 12-bit packing (DESIGN.md §3): 3/4 of the bytes, bit-identical
         # results.  The bf16 weights stay resident for prefill and batched decode.  decode_pack: matrix -> "packed" or why it is plain.
         self.decode_pack = {}
-        if self.packs_decode_weights and self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
+        # NF4 layer matrices (weights.from_state_dicts(quantization="nf4")): the layer matrices hold the dequantized values for every path,
+        # and the batch-1 decode step streams the NF4 planes instead (bit-identical).  decode_quant: matrix -> "nf4" or why the step reads
+        # its dequantized copy.  SRGPT_DECODE_NF4=0 runs the usual step over the dequantized copies.
+        self.decode_quant = {}
+        if getattr(w, "quantization", None) == "nf4" and os.environ.get("SRGPT_DECODE_NF4", "1") != "0":
+            self._nf4_decode_weights()
+        elif self.packs_decode_weights and self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
             self._pack_decode_weights()
 
     supports_prefix_reuse = True
@@ -151,6 +157,20 @@ class LlamaDecoder:
     last_speculation = (0, 0, 0)
     _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
     _lm_packed = None
+    _nf4_array = None  # srgpt_llama_layer_nf4[] of the decode step
+
+    @ops.in_own_dtype
+    def _nf4_decode_weights(self) -> None:
+        """The NF4 step's layer array; lm_head stays unquantized and is packed in the bf16 build (SRGPT_DECODE_PACK=0: plain)."""
+        for l, lw in enumerate(self.w.layers):
+            for name in ("qkv", "o", "gateup", "down"):
+                K = getattr(lw, name + "_w").shape[1]
+                self.decode_quant[f"layers.{l}.{name}"] = "nf4" if lw.nf4[name] is not None else f"K = {K} is not a multiple of {ops.NF4_BATCH}"
+        if self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
+            self._lm_packed, why = ops.pack12(self.w.lm_head)
+            self.decode_pack["lm_head"] = why or "packed"
+        if any(v == "nf4" for v in self.decode_quant.values()):
+            self._nf4_array = ops.make_llama_nf4_array([lw.nf4 for lw in self.w.layers])
 
     @ops.in_own_dtype
     def _pack_decode_weights(self) -> None:
@@ -272,7 +292,11 @@ class LlamaDecoder:
         d, w = self.dims, self.w
         if (sample or proc) and logits_out is None:
             logits_out = self._sample_buffer()
-        if self._packed_array is not None:
+        if self._nf4_array is not None:
+            ops.llama_decode_step_nf4(self.h, self._layer_array, self._nf4_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
+                                      d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
+                                      self.lm_ws, self.out_ids, self.step, logits_out)
+        elif self._packed_array is not None:
             ops.llama_decode_step_packed(self.h, self._layer_array, self._packed_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
                                          d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
                                          self.lm_ws, self.out_ids, self.step, logits_out)

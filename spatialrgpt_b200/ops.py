@@ -15,7 +15,7 @@ from ._lib import SrgptError
 from ._lib import check as _check_rc
 
 _KERNELS_PER_CALL = {"srgpt_lm_head_local_best_bf16": 2, "srgpt_mask_pool_bf16": 2, "srgpt_mask_weights": 2, "srgpt_lm_head_argmax_bf16": 2, "srgpt_depth_to_u8x3": 3,
-                     "srgpt_lm_head_argmax_packed_bf16": 2}
+                     "srgpt_lm_head_argmax_packed_bf16": 2, "srgpt_nf4_double_quant": 2}
 
 
 def check(rc: int, what: str) -> None:
@@ -476,6 +476,104 @@ def gemv_packed(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch
     return y
 
 
+# ---- NF4 weight-only quantization of the decoder-layer matrices (nf4.cu; DESIGN.md §3) ------------------------------
+NF4_BLOCK = 64     # weights per scale; a matrix's in_features must be a multiple
+NF4_BATCH = 1024   # K must be a multiple for the decode GEMV's lane-ordered planes
+_NF4_MAPS = {}
+
+
+def nf4_dynamic_map(device) -> torch.Tensor:
+    """The 256 fp32 values of bitsandbytes' create_dynamic_map(signed=True), the second-level code of double quantization: for
+    i = 0..6, +-10^(i-6) times the midpoints of linspace(0.1, 1, 2^i + 1), plus 0 and 1, sorted.  The linspace points are
+    fl32(0.1 + 0.9 j / (n - 1)) computed in fp64, the midpoints and products in fp32."""
+    key = str(device)
+    if key not in _NF4_MAPS:
+        import numpy as np
+        vals = []
+        for i in range(7):
+            n = 2 ** i + 1
+            b = np.array([0.1 + 0.9 * j / (n - 1) for j in range(n)], dtype=np.float32)
+            means = (b[:-1] + b[1:]) * np.float32(0.5)
+            s = np.float32(10.0 ** (i - 6))
+            vals += list(s * means) + list(-(s * means))
+        vals += [np.float32(0.0), np.float32(1.0)]
+        _NF4_MAPS[key] = torch.from_numpy(np.sort(np.array(vals, dtype=np.float32))).to(device)
+    return _NF4_MAPS[key]
+
+
+def nf4_quantize(w: torch.Tensor):
+    """NF4 codes of an element-type matrix [N, K] (K a multiple of 64): (codes [N, K/2] uint8 in natural order, scale [N, K/64]
+    fp32 resolved scales).  Raises NotImplementedError for K % 64 != 0 and SrgptError when w holds Inf or NaN."""
+    _need(w, ELEM(), "nf4_quantize.w")
+    ldw = _rowmajor2d(w, "nf4_quantize.w")
+    N, K = w.shape
+    if K % NF4_BLOCK:
+        raise NotImplementedError(f"NF4 quantization needs in_features to be a multiple of {NF4_BLOCK}, got {K}")
+    dev, lib = w.device, _lib.load()
+    codes = torch.empty((N, K // 2), dtype=torch.uint8, device=dev)
+    absmax = torch.empty((N, K // NF4_BLOCK), dtype=torch.float32, device=dev)
+    n_bad = torch.zeros(1, dtype=torch.int32, device=dev)
+    check(lib.srgpt_nf4_quantize_bf16(_p(w), ldw, N, K, _p(codes), _p(absmax), _p(n_bad), _stream()), "srgpt_nf4_quantize_bf16")
+    if int(n_bad[0]):
+        raise SrgptError(f"nf4_quantize: the {list(w.shape)} matrix holds Inf or NaN in {int(n_bad[0])} blocks of {NF4_BLOCK}")
+    offset = torch.empty(1, dtype=torch.float32, device=dev)
+    scale = torch.empty_like(absmax)
+    check(lib.srgpt_nf4_double_quant(_p(absmax), absmax.numel(), _p(nf4_dynamic_map(dev)), _p(offset), _p(scale), _stream()),
+          "srgpt_nf4_double_quant")
+    return codes, scale
+
+
+def nf4_dequantize(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+    """The element-type matrix [N, K] of natural-order codes and scales: round_to_elem(fl32(code_value * scale))."""
+    N, K = codes.shape[0], codes.shape[1] * 2
+    out = torch.empty((N, K), dtype=ELEM(), device=codes.device)
+    check(_lib.load().srgpt_nf4_dequantize_bf16(_p(codes), _p(scale), N, K, _p(out), K, _stream()), "srgpt_nf4_dequantize_bf16")
+    return out
+
+
+def _nf4_desc(p) -> "_lib.Nf4":
+    d = _lib.Nf4()
+    if p is not None:
+        d.q, d.scale = p.q.data_ptr(), p.scale.data_ptr()
+    return d
+
+
+def nf4_planes(codes: torch.Tensor, scale: torch.Tensor, deq: torch.Tensor):
+    """The decode GEMV's planes of a (fused) matrix: (Nf4W, None), or (None, reason) when K is not a multiple of 1024 and the decode
+    step reads the dequantized matrix instead.  The lane-ordered planes must dequantize to exactly ``deq``; SrgptError otherwise."""
+    from .weights import Nf4W
+    N, K = codes.shape[0], codes.shape[1] * 2
+    if K % NF4_BATCH:
+        return None, f"K = {K} is not a multiple of {NF4_BATCH}"
+    q = torch.empty_like(codes)
+    check(_lib.load().srgpt_nf4_lane_order(_p(codes), N, K, _p(q), _stream()), "srgpt_nf4_lane_order")
+    p = Nf4W(q=q, scale=scale.contiguous())
+    if not torch.equal(nf4_unpack(p).view(torch.int16), deq.view(torch.int16)):
+        raise SrgptError(f"nf4: the lane-ordered planes of the {list(deq.shape)} matrix do not dequantize to its resident copy")
+    return p, None
+
+
+def nf4_unpack(p) -> torch.Tensor:
+    """The element-type matrix [N, K] an Nf4W's lane-ordered planes hold (through the GEMV's own dequantization)."""
+    N, K = p.q.shape[0], p.q.shape[1] * 2
+    out = torch.empty((N, K), dtype=ELEM(), device=p.q.device)
+    d = _nf4_desc(p)
+    check(_lib.load().srgpt_nf4_unpack_bf16(C.byref(d), N, K, _p(out), K, _stream()), "srgpt_nf4_unpack_bf16")
+    return out
+
+
+def gemv_nf4(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0,
+             residual: Optional[torch.Tensor] = None, mode: int = GEMV_PLAIN, n_heads: int = 0, n_kv_heads: int = 0,
+             head_dim: int = 0, cos_tab=None, sin_tab=None, pos=None, kv_pages=None, page_table=None, page_size: int = 0) -> torch.Tensor:
+    """gemv() over an Nf4W: bit-identical to gemv() over the dequantized matrix, 4.5 bits of weight stream per element."""
+    N, K = p.q.shape[0], p.q.shape[1] * 2
+    d = _nf4_desc(p)
+    check(_lib.load().srgpt_gemv_nf4_bf16(_p(x), C.byref(d), _p(y), N, K, _p(norm_weight), eps, _p(residual), mode, n_heads, n_kv_heads,
+                                          head_dim, _p(cos_tab), _p(sin_tab), _p(pos), _p(kv_pages), _p(page_table), page_size, _stream()),
+          "srgpt_gemv_nf4_bf16")
+    return y
+
+
 # ---- host preprocessing on the GPU (preprocess.py) ---------------------------------------------------------------
 def resample_u8(img: torch.Tensor, axis: int, out_size: int, kk: torch.Tensor, bounds: torch.Tensor, ksize: int) -> torch.Tensor:
     _need(img, torch.uint8, "resample_u8.img"); _need(kk, torch.int32, "resample_u8.kk"); _need(bounds, torch.int32, "resample_u8.bounds")
@@ -737,6 +835,15 @@ def make_llama_packed_array(packed_layers):
     return arr
 
 
+def make_llama_nf4_array(nf4_layers):
+    """ctypes array of srgpt_llama_layer_nf4 over per-layer dicts {"qkv", "o", "gateup", "down"} -> Nf4W or None (dequantized weight)."""
+    arr = (_lib.LlamaLayerNf4 * len(nf4_layers))()
+    for i, pl in enumerate(nf4_layers):
+        for name in ("qkv", "o", "gateup", "down"):
+            setattr(arr[i], name, _nf4_desc(pl[name]))
+    return arr
+
+
 def clip_embed(patch_embeds: torch.Tensor, class_embedding: torch.Tensor, position_embedding: torch.Tensor, n_img: int, T: int) -> torch.Tensor:
     """[n_img*T, D] patch embeddings -> [n_img*(T+1), D]: class token prepended, position embedding added (CLIPVisionEmbeddings)."""
     _need(patch_embeds, ELEM(), "clip_embed.patch_embeds")
@@ -845,6 +952,20 @@ def llama_decode_step_packed(h, layer_array, packed_array, n_layers: int, q_buf,
                                                           _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
                                                           C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
                                                           _stream()), "srgpt_llama_decode_step_packed_bf16")
+    _count(5 * n_layers + 2)
+
+
+def llama_decode_step_nf4(h, layer_array, nf4_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table,
+                          page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
+    """llama_decode_step() streaming the NF4 planes of ``nf4_array`` (make_llama_nf4_array) and lm_head from ``lm_packed`` (a
+    Packed12W or None); bit-identical to the plain step over the dequantized weights."""
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    lm_d = _packed_desc(lm_packed)
+    check(_lib.load().srgpt_llama_decode_step_nf4_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(nf4_array, C.c_void_p), n_layers,
+                                                       _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
+                                                       _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
+                                                       C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
+                                                       _stream()), "srgpt_llama_decode_step_nf4_bf16")
     _count(5 * n_layers + 2)
 
 

@@ -67,6 +67,8 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_logits_processors = False  # the logits are vocabulary-parallel: no rank holds a whole row
 
     def __init__(self, dims: LlamaDims, w: LlamaW, rank: int, world: int, group=None, max_seq_len: int = 4096, comm: Optional[str] = None, **kw):
+        if getattr(w, "quantization", None) is not None:
+            raise NotImplementedError(f"the tensor-parallel decoder streams unquantized shards; quantization={w.quantization!r} is single-GPU only")
         super().__init__(dims, w, max_seq_len=max_seq_len, **kw)
         if dims.num_attention_heads % world or dims.num_key_value_heads % world or dims.intermediate_size % world:
             raise ValueError(f"heads {dims.num_attention_heads}/{dims.num_key_value_heads} and intermediate size {dims.intermediate_size} must divide by TP={world}")

@@ -97,6 +97,9 @@ class LlamaLayerW:
     post_norm: torch.Tensor
     gateup_w: torch.Tensor  # [2 I, H], rows interleaved (gate_i, up_i)
     down_w: torch.Tensor  # [H, I]
+    # quantization="nf4": {"qkv", "o", "gateup", "down"} -> the fused matrix's Nf4W planes, or None where K is not a multiple of 1024
+    # (the *_w tensors above are then the dequantized matrices)
+    nf4: Optional[Dict[str, Optional["Nf4W"]]] = None
 
 
 @dataclass
@@ -105,6 +108,7 @@ class LlamaW:
     norm: torch.Tensor
     lm_head: torch.Tensor  # [V, H]
     layers: List[LlamaLayerW] = field(default_factory=list)
+    quantization: Optional[str] = None  # None or "nf4" (the decoder-layer linears only)
 
 
 @dataclass
@@ -124,6 +128,17 @@ class Packed12W:
 
     def nbytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in (self.sm, self.ex, self.base, self.row_ptr, self.exc))
+
+
+@dataclass
+class Nf4W:
+    """An NF4-quantized weight [N, K] as the batch-1 decode GEMV streams it (DESIGN.md §3, include/srgpt_b200.h srgpt_nf4): q [N, K/2]
+    uint8 codes in the GEMV's lane order, scale [N, K/64] fp32 resolved scales.  Built by ops.nf4_planes."""
+    q: torch.Tensor
+    scale: torch.Tensor
+
+    def nbytes(self) -> int:
+        return self.q.numel() + self.scale.numel() * 4
 
 
 @dataclass
@@ -157,6 +172,10 @@ class ModelWeights:
     def to(self, dtype: torch.dtype) -> "ModelWeights":
         """In-place cast of every floating-point weight (what ``model.to(dtype=...)`` does to the reference's modules,
         llava/eval/eval_spatial.py:221); the kernel layouts (padding, interleaving, fused qkv) are dtype independent."""
+        if self.llama.quantization is not None and dtype != self.dtype:
+            raise NotImplementedError(f"the {self.llama.quantization} layer matrices are dequantized into the element type they were loaded in "
+                                      f"({self.dtype}); load the model with torch_dtype={dtype} instead of casting it")
+
         def walk(o):
             if isinstance(o, torch.Tensor):
                 return o.to(dtype) if o.is_floating_point() else o
@@ -184,9 +203,15 @@ def interleave_rows(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
 
 
 def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], device, n_tower_layers: Optional[int] = None,
-                     dtype: torch.dtype = BF16) -> ModelWeights:
+                     dtype: torch.dtype = BF16, quantization: Optional[str] = None) -> ModelWeights:
     """sd = {"vision_tower": ..., "region_extractor": ..., "mm_projector": ..., "llm": ...} with the
-    reference's key names; tensors may live on the CPU in any float dtype.  ``dtype``: torch.bfloat16 or torch.float16."""
+    reference's key names; tensors may live on the CPU in any float dtype.  ``dtype``: torch.bfloat16 or torch.float16.
+    ``quantization="nf4"``: every decoder-layer linear (q/k/v/o/gate/up/down_proj) is NF4-quantized on the device as its own [out, in]
+    matrix, before qkv is fused and gate/up interleaved (the reference's load_4bit, llava/model/builder.py:51-60); the layer keeps the
+    dequantized matrices for every path and the NF4 planes for the batch-1 decode step.  Embeddings, lm_head, norms, towers, projector
+    and region extractor stay unquantized."""
+    if quantization not in (None, "nf4"):
+        raise ValueError(f"quantization={quantization!r}: supported are None and 'nf4'")
     dev = torch.device(device)
 
     def g(d, k):
@@ -251,9 +276,12 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
 
     l, lc = sd["llm"], cfg.llama
     llama = LlamaW(embed=g(l, "model.embed_tokens.weight").contiguous(), norm=g(l, "model.norm.weight"),
-                   lm_head=g(l, "lm_head.weight" if "lm_head.weight" in l else "model.embed_tokens.weight").contiguous())
+                   lm_head=g(l, "lm_head.weight" if "lm_head.weight" in l else "model.embed_tokens.weight").contiguous(), quantization=quantization)
     for i in range(lc.num_hidden_layers):
         p = f"model.layers.{i}."
+        if quantization == "nf4":
+            llama.layers.append(_nf4_layer(l, p, g, dtype))
+            continue
         llama.layers.append(LlamaLayerW(
             in_norm=g(l, p + "input_layernorm.weight"),
             qkv_w=torch.cat([g(l, p + f"self_attn.{n}.weight") for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous(),
@@ -262,6 +290,28 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
             gateup_w=interleave_rows(g(l, p + "mlp.gate_proj.weight"), g(l, p + "mlp.up_proj.weight")),
             down_w=g(l, p + "mlp.down_proj.weight").contiguous()))
     return ModelWeights(vision, region, projector, llama)
+
+
+def _nf4_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> LlamaLayerW:
+    """One decoder layer with NF4 linears: each original matrix quantized and dequantized on its own, then the codes, scales and
+    dequantized matrices fused exactly as the plain layer's weights (q/k/v rows concatenated, gate/up rows interleaved)."""
+    from . import ops
+    with ops.elem_dtype(dtype):
+        quant = {}
+        for n in ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj"):
+            key = p + ("self_attn." if n.endswith(("q_proj", "k_proj", "v_proj", "o_proj")) else "mlp.") + n + ".weight"
+            codes, scale = ops.nf4_quantize(g(l, key).contiguous())
+            quant[n] = (codes, scale, ops.nf4_dequantize(codes, scale))
+        fused = {
+            "qkv": [torch.cat([quant[n][k] for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous() for k in range(3)],
+            "o": list(quant["o_proj"]),
+            "gateup": [interleave_rows(quant["gate_proj"][k], quant["up_proj"][k]) for k in range(3)],
+            "down": list(quant["down_proj"]),
+        }
+        del quant
+        planes = {name: ops.nf4_planes(*f)[0] for name, f in fused.items()}
+    return LlamaLayerW(in_norm=g(l, p + "input_layernorm.weight"), qkv_w=fused["qkv"][2], o_w=fused["o"][2],
+                       post_norm=g(l, p + "post_attention_layernorm.weight"), gateup_w=fused["gateup"][2], down_w=fused["down"][2], nf4=planes)
 
 
 def random_init(cfg: LlavaConfig, device, seed: int = 0, std: float = 0.02, n_tower_layers: Optional[int] = None,

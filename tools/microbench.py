@@ -113,6 +113,30 @@ if "gemv" in which:
                 st.zero_(); ops.lm_head_argmax_packed(x, p, nw, 1e-5, ws, ids, st, ps)
         ms, best = timeit(fn)
         emit(name, ms, best, bytes_=p.nbytes(), N=N, K=K, bf16_equiv_GBps=round(N * K * 2 / ms / 1e6, 1))
+    # the layer GEMVs over NF4 planes (4.5 bits per weight; DESIGN.md §3): GBps counts the codes and scales streamed
+    for name, N, K, mode in [("gemv_qkv_rope_nf4", 6144, 4096, "qkv"), ("gemv_o_nf4", 4096, 4096, "plain"),
+                             ("gemv_gateup_swiglu_nf4", 28672, 4096, "swiglu"), ("gemv_down_nf4", 4096, 14336, "plain")]:
+        x = rnd(K)
+        codes, scale = ops.nf4_quantize(rnd(N, K))
+        p, _ = ops.nf4_planes(codes, scale, ops.nf4_dequantize(codes, scale))
+        del codes
+        nw = torch.ones(K, dtype=BF, device=dev)
+        if mode == "plain":
+            y = torch.empty(N, dtype=BF, device=dev); r = rnd(N)
+            fn = lambda: ops.gemv_nf4(x, p, y, residual=r)
+        elif mode == "swiglu":
+            y = torch.empty(N // 2, dtype=BF, device=dev)
+            fn = lambda: ops.gemv_nf4(x, p, y, norm_weight=nw, eps=1e-5, mode=ops.GEMV_SWIGLU)
+        else:
+            from spatialrgpt_b200.config import LlamaDims
+            from spatialrgpt_b200.llama_decoder import build_rope_tables
+            cos, sin = build_rope_tables(LlamaDims(), 1024, dev)
+            pages = torch.zeros(64, 2, 16, 8, 128, dtype=BF, device=dev); pt = torch.arange(64, dtype=torch.int32, device=dev)
+            pos = torch.tensor([300], dtype=torch.int32, device=dev); y = torch.empty(4096, dtype=BF, device=dev)
+            fn = lambda: ops.gemv_nf4(x, p, y, norm_weight=nw, eps=1e-5, mode=ops.GEMV_QKV_ROPE, n_heads=32, n_kv_heads=8, head_dim=128,
+                                      cos_tab=cos, sin_tab=sin, pos=pos, kv_pages=pages, page_table=pt, page_size=16)
+        ms, best = timeit(fn)
+        emit(name, ms, best, bytes_=p.nbytes(), N=N, K=K, bf16_equiv_GBps=round(N * K * 2 / ms / 1e6, 1))
 
 if "maskpool" in which:
     for (n, side, C, M) in [(1, 128, 1152, 8), (1, 128, 1152, 16), (4, 128, 1152, 4), (32, 128, 1152, 4), (1, 32, 1152, 8), (32, 32, 1152, 4)]:
