@@ -94,12 +94,9 @@ def _quantized(ops, w, dtype):
     return ops.nf4_planes(codes, scale, deq)[0], deq
 
 
-@pytest.mark.parametrize("ring", [None, "0"])
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("K", [1024, 2048, 4096, 5120, 14336])
-def test_plain_and_swiglu_modes_are_bit_identical(ops, monkeypatch, dtype, K, ring):
-    if ring is not None:
-        monkeypatch.setenv("SRGPT_GEMV_RING", ring)
+def test_plain_and_swiglu_modes_are_bit_identical(ops, dtype, K):
     N = 1024
     with ops.elem_dtype(dtype):
         p, deq = _quantized(ops, matrix(N, K, K + 1, dtype).to(DEV), dtype)
@@ -117,13 +114,10 @@ def test_plain_and_swiglu_modes_are_bit_identical(ops, monkeypatch, dtype, K, ri
         assert _same(a0, a1)
 
 
-@pytest.mark.parametrize("ring", [None, "0"])
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_qkv_rope_mode_and_kv_pages_are_bit_identical(ops, monkeypatch, dtype, ring):
+def test_qkv_rope_mode_and_kv_pages_are_bit_identical(ops, dtype):
     from spatialrgpt_b200.config import LlamaDims
     from spatialrgpt_b200.llama_decoder import build_rope_tables
-    if ring is not None:
-        monkeypatch.setenv("SRGPT_GEMV_RING", ring)
     nh, nkv, hd, K, page = 32, 8, 128, 4096, 16
     N = (nh + 2 * nkv) * hd
     with ops.elem_dtype(dtype):

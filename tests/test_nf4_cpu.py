@@ -187,7 +187,7 @@ def test_c_abi_rejects_bad_arguments_without_a_gpu(lib):
                                                 *([None] * 6)) == -1
 
 
-NF4_KERNELS = r"_ZN5srgpt4gemv22decode_gemv_nf4_kernelILi[0-2]EEEvNS0_7NParamsE"
+NF4_KERNELS = r"_ZN5srgpt4gemv18decode_gemv_kernelILi[0-2]ENS0_3Nf4EEEvNS0_6ParamsE"
 NEW_SYMBOLS = ["srgpt_nf4_quantize_bf16", "srgpt_nf4_double_quant", "srgpt_nf4_dequantize_bf16", "srgpt_nf4_lane_order", "srgpt_nf4_unpack_bf16",
                "srgpt_gemv_nf4_bf16", "srgpt_llama_decode_step_nf4_bf16"]
 
@@ -202,7 +202,7 @@ def test_both_builds_export_the_nf4_entries(elem):
 
 
 @pytest.mark.parametrize("elem", ["bf16", "f16"])
-def test_nf4_gemv_kernels_fit_three_ctas_per_sm_without_local_memory(elem):
+def test_nf4_format_gemv_kernels_fit_three_ctas_per_sm_without_local_memory(elem):
     """The plain decode GEMV runs 3 CTAs of 256 threads per SM (80 registers); the NF4 kernels must allow the same."""
     from spatialrgpt_b200 import _lib
     _lib.load(elem=elem)

@@ -226,14 +226,14 @@ def test_f16_build_refuses_the_packing():
     assert "bfloat16" in lib.srgpt_last_error().decode()
 
 
-def test_packed_gemv_kernels_are_in_the_library_without_spills():
+def test_packed12_gemv_kernels_are_in_the_library_without_spills():
     from spatialrgpt_b200 import _lib
     _lib.load()
     r = subprocess.run(["cuobjdump", "-sass", _lib.lib_path()], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     funcs = re.split(r"\n\s*Function : ", r.stdout)
-    packed = [f for f in funcs if re.match(r"_ZN5srgpt4gemv18decode_gemv_kernelILi[0-3]ELi1ELb1EEE", f)]
+    packed = [f for f in funcs if re.match(r"_ZN5srgpt4gemv18decode_gemv_kernelILi[0-3]ENS0_8Packed12EEE", f)]
     assert len(packed) == 4, "one packed GEMV per mode (plain, SwiGLU, QKV + RoPE, lm_head)"
     for f in packed:
         assert "PRMT" in f and "LDG.E.NA.128" in f
