@@ -35,6 +35,22 @@ def build_rope_tables(dims: LlamaDims, max_pos: int, device, dtype: torch.dtype 
     return freqs.cos().to(dtype).to(device).contiguous(), freqs.sin().to(dtype).to(device).contiguous()
 
 
+def eos_list(eos_token_ids) -> List[int]:
+    """eos_token_ids as generate() takes it (None, one id or several) -> the ids in the given order (beam search appends the first)."""
+    if eos_token_ids is None:
+        return []
+    return [int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids])]
+
+
+def first_stop(host_ids, lo: int, hi: int, eos, stopping_fn, limit: int) -> Optional[int]:
+    """Where a request ends among the generated tokens [lo, hi) already on the host: k + 1 for the first k whose id is in `eos` or for
+    which ``stopping_fn(host_ids[:k + 1])`` fires, else `limit` (the token budget) when the window reaches it, else None."""
+    for k in range(lo, min(hi, limit)):
+        if int(host_ids[k]) in eos or (stopping_fn is not None and stopping_fn(host_ids[:k + 1])):
+            return k + 1
+    return limit if hi >= limit else None
+
+
 class PagedKVCache:
     """KV pages for all layers: [layers, n_pages, 2 (k,v), PAGE_SIZE, n_kv_heads, head_dim] bf16, a free list
     and per-sequence page tables (int32, device) of fixed capacity so decode graphs stay valid."""
@@ -115,8 +131,11 @@ class LlamaDecoder:
         self.lm_ws = ops.lm_head_workspace(dims.vocab_size, dev)
         self.scale = hd ** -0.5
         self._layer_array = ops.make_llama_layer_array(w.layers, [self.cache.layer(l) for l in range(dims.num_hidden_layers)])
-        self._graph: Optional[torch.cuda.CUDAGraph] = None
-        self._graph_sample: Optional[torch.cuda.CUDAGraph] = None
+        # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
+        # ("verify", T, ngram), ("batch", B, proc) and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
+        # dropped whenever one of them is replaced: the KV cache and layer array (ensure_capacity), the processor spec (_set_processors)
+        # and the batched-decode buffers (_batch_state).
+        self._graphs = {}
         self.kernels_per_decode_step = 5 * dims.num_hidden_layers + 2
         # sampling mode (do_sample=True): temperature / top_p live in device memory so one captured graph serves any setting
         self.sample_params = torch.tensor([1.0, 1.0, 0.0], dtype=torch.float32, device=dev)
@@ -130,7 +149,6 @@ class LlamaDecoder:
         self.proc_spec: Optional[torch.Tensor] = None
         self.proc_logits: Optional[torch.Tensor] = None  # the processed fp32 row of the one-token step (sampling reads it)
         self.proc_ids = torch.zeros(1, dtype=torch.int64, device=dev)
-        self._proc_graphs = {}  # sample flag -> decode-step graph with processing on
         # Reusable prompt prefix of sequence 0: its first `prefix_rows` positions hold K/V that a batch-1 PREFILL wrote and nothing has
         # overwritten since (generate_from_embeds(reuse_rows=n) continues from them).  Positions written by decode steps are never
         # counted: the reference prefills them again, and the GEMV decode path rounds differently from the prefill GEMMs.
@@ -154,6 +172,9 @@ class LlamaDecoder:
     supports_logits_processors = True
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
+    _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
+    _host_ids = None  # pinned host copy of generated ids for the stop checks, and the stream that fills it (_pinned_ids)
+    _copy_stream = None
     last_speculation = (0, 0, 0)
     _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
     _lm_packed = None
@@ -195,7 +216,7 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def ensure_capacity(self, n_seqs: int, tokens_per_seq: int) -> None:
         """Grow the paged cache so `n_seqs` sequences of `tokens_per_seq` tokens fit at once (batched prefill).
-        Re-allocation drops all cached sequences and the captured decode graph (page addresses change)."""
+        Re-allocation drops all cached sequences and the captured graphs (page addresses change)."""
         c = self.cache
         need_pages = n_seqs * ((tokens_per_seq + PAGE_SIZE - 1) // PAGE_SIZE)
         if n_seqs <= len(c.owned) and need_pages <= c.n_pages:
@@ -206,9 +227,7 @@ class LlamaDecoder:
         cur_b = c.pages.numel() * 2
         if need_pages * per_page > free_b + cur_b - (2 << 30):
             raise RuntimeError(f"KV cache for {n_seqs} x {tokens_per_seq} tokens needs {need_pages * per_page >> 20} MiB, not available")
-        self._graph = None
-        self._graph_sample = None
-        self._proc_graphs = {}
+        self._drop_graphs()
         self._record_prefix(0)
         n_pages_old, n_seqs_old = c.n_pages, len(c.owned)
         self.cache = None
@@ -322,10 +341,6 @@ class LlamaDecoder:
             ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, ids=self.proc_ids)
             ops.logits_pick_token(self.proc_ids, self.step, -1, self.out_ids, w.embed, self.h)
 
-    def _proc_kernels(self, sample: bool) -> int:
-        """Kernels the processing adds to a graph-replayed one-token step (ops.LAUNCHES accounting)."""
-        return 1 if sample else 3  # processing (+ key unpack and pick when greedy); sampling's own kernel is counted by the caller
-
     def _set_processors(self, processors) -> bool:
         """processors = None or a spec of logits_processors.parse / resolve_min_length.  Writes its device encoding; True when on."""
         if not processors:
@@ -339,9 +354,7 @@ class LlamaDecoder:
             while cap < ints.size:
                 cap *= 2
             self.proc_spec = torch.zeros(cap, dtype=torch.int32, device=self.device)
-            self._proc_graphs = {}  # they read the old buffer
-            if getattr(self, "_bstate", None) is not None:
-                self._bstate["graph_proc"] = None
+            self._drop_graphs(lambda key: key[0] in ("step", "batch") and key[-1])  # the graphs with processing on read the old buffer
         self.proc_spec[: ints.size].copy_(torch.from_numpy(ints))
         self.proc_fparams.copy_(torch.from_numpy(fparams))
         return True
@@ -351,28 +364,73 @@ class LlamaDecoder:
             self.sample_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
         return self.sample_logits
 
-    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False) -> None:
-        if (self._proc_graphs.get(sample) if proc else (self._graph_sample if sample else self._graph)) is not None:
-            return
-        # warm up once outside capture (lazy cudaFuncSetAttribute calls etc.), on a side stream
-        saved = (self.pos.clone(), self.step.clone(), self.h.clone(), self.out_ids.clone())
+    # ---- captured graphs ---------------------------------------------------------------------------------------------------------
+    def _capture(self, key, launch, restore, kernels: int) -> torch.cuda.CUDAGraph:
+        """The graph stored under `key`, captured from `launch()` if there is none: one warm-up run outside capture (lazy kernel
+        attribute setup) on a side stream, the tensors in `restore` put back as they were, then the capture.  `kernels` is what one
+        replay launches (ops.LAUNCHES accounting)."""
+        if key in self._graphs:
+            return self._graphs[key][0]
+        saved = [t.clone() for t in restore]
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())  # after the clones are enqueued
-        kw = {"proc": True} if proc else {}  # the plain call keeps the signature subclasses override
         with torch.cuda.stream(s):
-            self._decode_step_launch(seq, sample=sample, **kw)
+            launch()
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
-        self.pos.copy_(saved[0]); self.step.copy_(saved[1]); self.h.copy_(saved[2]); self.out_ids.copy_(saved[3])
+        for t, v in zip(restore, saved):
+            t.copy_(v)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            self._decode_step_launch(seq, sample=sample, **kw)
-        if proc:
-            self._proc_graphs[sample] = g
-        elif sample:
-            self._graph_sample = g
-        else:
-            self._graph = g
+            launch()
+        self._graphs[key] = (g, kernels)
+        return g
+
+    def _replay(self, key) -> None:
+        g, kernels = self._graphs[key]
+        g.replay()
+        ops.LAUNCHES += kernels
+
+    def _drop_graphs(self, match=lambda key: True) -> None:
+        """Forget the captured graphs whose key matches (all of them by default)."""
+        self._graphs = {k: v for k, v in self._graphs.items() if not match(k)}
+
+    @property
+    def _graph(self) -> Optional[torch.cuda.CUDAGraph]:
+        """The greedy one-token step graph, once _ensure_graph has captured it."""
+        entry = self._graphs.get(("step", False, False))
+        return None if entry is None else entry[0]
+
+    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False) -> torch.cuda.CUDAGraph:
+        """The one-token step graph of this mode.  Sampling adds its kernel; processing adds 1 more when sampling, 3 when greedy
+        (processing, key unpack and pick)."""
+        kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0)
+        return self._capture(("step", sample, proc), lambda: self._decode_step_launch(seq, sample=sample, proc=proc),
+                             (self.pos, self.step, self.h, self.out_ids), kernels)
+
+    # ---- stop checks: generated ids reach the host through pinned memory while the next step runs --------------------------------
+    def _pinned_ids(self, n: int) -> torch.Tensor:
+        """n elements of pinned int64 host memory, and the copy stream _to_host fills it on; created on first use, grown when a batch
+        needs more."""
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        if self._host_ids is None or self._host_ids.numel() < n:
+            self._host_ids = torch.empty(max(n, self.out_ids.numel()), dtype=torch.int64, pin_memory=True)
+        return self._host_ids[:n]
+
+    def _to_host(self, *copies) -> torch.cuda.Event:
+        """Enqueue each (device slice, pinned slice) copy on the copy stream, ordered after the work enqueued so far; returns the event
+        that marks their completion."""
+        side = self._copy_stream
+        e = torch.cuda.Event()
+        e.record()
+        side.wait_event(e)
+        with torch.cuda.stream(side):
+            for src, dst in copies:
+                dst.copy_(src, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(side)
+        return done
 
     def _set_sampling(self, sampling) -> bool:
         """sampling = None (greedy) or dict(temperature=, top_p=, top_k=, seed=).  Returns True when tokens are sampled."""
@@ -426,9 +484,7 @@ class LlamaDecoder:
             raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
         if S + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
-        eos = set()
-        if eos_token_ids is not None:
-            eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
+        eos = eos_list(eos_token_ids)
         k = min(int(lookup_k), ops.SPEC_T_MAX - 1) if lookup_k else 0
         self.last_speculation = (0, 0, 0)
         if k > 0 and (seq != 0 or sampling or int(lookup_ngram) < 1 or processors):
@@ -473,7 +529,7 @@ class LlamaDecoder:
         st = dict(h=z(Tm, H), q=z(Tm, qd), attn=z(Tm, qd), act=z(Tm, I), ws=z(Tm * self.lm_ws.numel(), dtype=torch.uint8), logits=None,
                   pos_rows=z(Tm, dtype=torch.int32), draft=z(Tm, dtype=torch.int32), state=z(8, dtype=torch.int32),
                   prompt=z(self.max_seq_len, dtype=torch.int32), prompt_len=z(1, dtype=torch.int32),
-                  host_state=torch.zeros((self.out_ids.numel() + 2, 8), dtype=torch.int32, pin_memory=True), graphs={}, cache=self.cache)
+                  host_state=torch.zeros((self.out_ids.numel() + 2, 8), dtype=torch.int32, pin_memory=True))
         self._vstate = st
         return st
 
@@ -486,27 +542,10 @@ class LlamaDecoder:
                               w.embed, st["ws"], st["logits"] if logits_all is not None else None, logits_all, st["prompt"], st["prompt_len"],
                               ngram, st["draft"], self.out_ids, self.step, st["state"])
 
-    def _verify_graph(self, T: int, ngram: int):
-        """One captured verify pass per (T, n-gram size); dropped when the cache is reallocated (its page addresses change)."""
-        st = self._vstate
-        if st["cache"] is not self.cache:
-            st["graphs"], st["cache"] = {}, self.cache
-        g = st["graphs"].get((T, ngram))
-        if g is not None:
-            return g
-        saved = (self.pos.clone(), self.step.clone(), self.out_ids.clone(), st["state"].clone())
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._verify_launch(T, ngram)  # warm-up outside capture (lazy kernel attribute setup); writes only this sequence's slack
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        self.pos.copy_(saved[0]); self.step.copy_(saved[1]); self.out_ids.copy_(saved[2]); st["state"].copy_(saved[3])
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._verify_launch(T, ngram)
-        st["graphs"][(T, ngram)] = g
-        return g
+    def _verify_graph(self, T: int, ngram: int) -> torch.cuda.CUDAGraph:
+        """The captured verify pass of this (T, n-gram size); its warm-up writes only this sequence's slack."""
+        return self._capture(("verify", T, ngram), lambda: self._verify_launch(T, ngram),
+                             (self.pos, self.step, self.out_ids, self._vstate["state"]), 5 * self.dims.num_hidden_layers + 3)
 
     def _verify_loop(self, T: int, ngram: int, lookup_ids, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits):
         """Tokens 1.. of sequence 0 by verify passes; pos / step / out_ids[:1] are set by the first token.  After each pass its state
@@ -522,47 +561,27 @@ class LlamaDecoder:
             st["prompt"][: ids.numel()].copy_(ids)
         st["prompt_len"].fill_(ids.numel())
         st["state"].zero_()
-        graph = self._verify_graph(T, ngram) if use_graph and logits is None else None
-        if getattr(self, "_host_ids", None) is None:
-            self._host_ids = torch.empty(self.out_ids.numel(), dtype=torch.int64, pin_memory=True)
-            self._copy_stream = torch.cuda.Stream(device=self.device)
-        host, side, host_state = self._host_ids, self._copy_stream, st["host_state"]
-        window = 2 * T
-        done = {}
-
-        def fetch(r: int, lo: int) -> None:  # state after pass r and out_ids[lo, lo + 2T) -> host, after the work enqueued so far
-            e = torch.cuda.Event()
-            e.record()
-            side.wait_event(e)
-            with torch.cuda.stream(side):
-                host_state[r].copy_(st["state"], non_blocking=True)
-                host[lo:lo + window].copy_(self.out_ids[lo:lo + window], non_blocking=True)
-                dn = torch.cuda.Event()
-                dn.record(side)
-            done[r] = dn
-
-        def inspect(lo: int, hi: int):  # tokens [lo, hi): the length to return if the request ends among them, else None
-            for kk in range(lo, min(hi, max_new_tokens)):
-                if int(host[kk]) in eos or (stopping_fn is not None and stopping_fn(host[:kk + 1])):
-                    return kk + 1
-            return max_new_tokens if hi >= max_new_tokens else None
-
+        graph = use_graph and logits is None
+        if graph:
+            self._verify_graph(T, ngram)
+        host, host_state, window = self._pinned_ids(self.out_ids.numel()), st["host_state"], 2 * T
         host[0] = int(self.out_ids[0])  # the first token (one sync, as the one-token loop's first inspection)
-        n = inspect(0, 1)
-        stats, known, r = (0, 0, 0), 1, 0
+        n = first_stop(host, 0, 1, eos, stopping_fn, max_new_tokens)
+        stats, known, r, prev = (0, 0, 0), 1, 0, None
         while n is None:
-            if graph is not None:
-                graph.replay()
-                ops.LAUNCHES += 5 * self.dims.num_hidden_layers + 3
+            if graph:
+                self._replay(("verify", T, ngram))
             else:
                 self._verify_launch(T, ngram, logits)
-            fetch(r, known)  # pass r's tokens lie in [step after r-1, + T), inside [step after r-2, + 2T)
+            # the state after pass r and out_ids[known, + 2T): pass r's tokens lie in [step after r-1, + T), inside [step after r-2, + 2T)
+            copied = self._to_host((st["state"], host_state[r]), (self.out_ids[known:known + window], host[known:known + window]))
             if r > 0:
-                done.pop(r - 1).synchronize()
+                prev.synchronize()
                 cur = int(host_state[r - 1, 6])
                 stats = tuple(int(v) for v in host_state[r - 1, :3])
-                n = inspect(known, cur)
+                n = first_stop(host, known, cur, eos, stopping_fn, max_new_tokens)
                 known = cur
+            prev = copied
             r += 1
         self.last_speculation = stats
         out = self.out_ids[:n].clone()
@@ -575,22 +594,17 @@ class LlamaDecoder:
         """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
         out_ids[:n] are already set."""
         self.active_pt.copy_(self.cache.page_tables[seq])
-        need_host_check = bool(eos) or stopping_fn is not None
-        return_logits = logits is not None
-        graph = None
-        if use_graph and not return_logits:
-            self._ensure_graph(seq, sample, proc=True) if proc else self._ensure_graph(seq, sample)
-            graph = self._proc_graphs[sample] if proc else (self._graph_sample if sample else self._graph)
-        per_replay = self.kernels_per_decode_step + (1 if sample else 0) + (self._proc_kernels(sample) if proc else 0)
+        key = ("step", sample, proc) if use_graph and logits is None else None
+        if key is not None:
+            self._ensure_graph(seq, sample, proc)
 
         def launch_step(k: int) -> None:
-            if graph is not None:
-                graph.replay()
-                ops.LAUNCHES += per_replay
+            if key is not None:
+                self._replay(key)
             else:
-                self._decode_step_launch(seq, None if logits is None else logits[k], sample, **({"proc": True} if proc else {}))
+                self._decode_step_launch(seq, None if logits is None else logits[k], sample, proc)
 
-        if not need_host_check:
+        if not eos and stopping_fn is None:
             while n < max_new_tokens:
                 launch_step(n)
                 n += 1
@@ -600,57 +614,34 @@ class LlamaDecoder:
             # pinned memory, and the host inspects token n-1 while the GPU computes token n.  On a stop the one speculative
             # step is discarded (it only touched this sequence's own KV slot and the step counters, which the next request
             # resets).  HF inspects after every token too (a blocking .item()); the result is identical.
-            if getattr(self, "_host_ids", None) is None:
-                self._host_ids = torch.empty(self.out_ids.numel(), dtype=torch.int64, pin_memory=True)
-                self._copy_stream = torch.cuda.Stream(device=self.device)
-            host, side = self._host_ids, self._copy_stream
-            done = {}
-
-            def fetch(lo: int, hi: int) -> None:  # tokens [lo, hi) -> host, ordered after the work enqueued so far
-                e = torch.cuda.Event()
-                e.record()
-                side.wait_event(e)
-                with torch.cuda.stream(side):
-                    host[lo:hi].copy_(self.out_ids[lo:hi], non_blocking=True)
-                    d = torch.cuda.Event()
-                    d.record(side)
-                for k in range(lo, hi):
-                    done[k] = d
-
-            fetch(0, n)
+            host = self._pinned_ids(self.out_ids.numel())
+            copied = self._to_host((self.out_ids[:n], host[:n]))
             checked = 0
-            while True:
-                launched = n < max_new_tokens
-                if launched:
-                    launch_step(n)
-                    fetch(n, n + 1)
-                else:
-                    break  # the token budget is spent: the last token is returned whatever it is (HF semantics)
-                stop_len = None
-                for k in range(checked, n):
-                    done.pop(k).synchronize()
-                    if int(host[k]) in eos or (stopping_fn is not None and stopping_fn(host[:k + 1])):
-                        stop_len = k + 1
-                        break
-                checked = n
-                if stop_len is not None:
-                    n = stop_len
+            while n < max_new_tokens:  # once the budget is spent the last token is returned whatever it is (HF semantics)
+                launch_step(n)
+                nxt = self._to_host((self.out_ids[n:n + 1], host[n:n + 1]))
+                copied.synchronize()
+                stop = first_stop(host, checked, n, eos, stopping_fn, max_new_tokens)
+                if stop is not None:
+                    n = stop
                     break
+                checked, copied = n, nxt
                 n += 1
         out = self.out_ids[:n].clone()
-        if return_logits:
+        if logits is not None:
             return out, logits[:n]
         return out
 
     # ---- batched decode: B sequences advance one token per step, every weight streamed ONCE for the whole batch ----------------
     def _batch_state(self, B: int):
-        st = getattr(self, "_bstate", None)
-        if st is not None and st["B"] == B and st["cache"] is self.cache:
+        st = self._bstate
+        if st is not None and st["B"] == B:
             return st
+        self._drop_graphs(lambda key: key[0] in ("batch", "beam"))  # they read the buffers replaced here
         d, dev = self.dims, self.device
         H, nh, nkv, hd, I, V = d.hidden_size, d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.intermediate_size, d.vocab_size
         z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
-        st = dict(B=B, cache=self.cache, graph=None, graph_proc=None, h=z(B, H), xn=z(B, H), qkv=z(B, (nh + 2 * nkv) * hd), attn=z(B, nh * hd), act=z(B, I),
+        st = dict(B=B, h=z(B, H), xn=z(B, H), qkv=z(B, (nh + 2 * nkv) * hd), attn=z(B, nh * hd), act=z(B, I),
                   logits=z(B, (V + 7) // 8 * 8), pos=z(B, dtype=torch.int32), step=z(1, dtype=torch.int32), ids=z(B, dtype=torch.int64),
                   out=z(self.out_ids.numel() * B, dtype=torch.int64), ticket=z(1, dtype=torch.int32),
                   cu=torch.arange(B + 1, dtype=torch.int32, device=dev))
@@ -696,58 +687,30 @@ class LlamaDecoder:
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        gkey = "graph_proc" if proc else "graph"
-        if use_graph and st[gkey] is None:
-            saved = {k: st[k].clone() for k in ("h", "pos", "step", "out")}
-            s = torch.cuda.Stream(device=self.device)
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._batch_step_launch(st, proc=proc)  # warm-up outside capture (lazy kernel attribute setup)
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            for k, v in saved.items():
-                st[k].copy_(v)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._batch_step_launch(st, proc=proc)
-            st[gkey] = g
-        kernels = 8 * self.dims.num_hidden_layers + (5 if proc else 4)  # the processing kernel + key unpack replace the arg max
+        key = ("batch", B, proc)
+        if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max
+            self._capture(key, lambda: self._batch_step_launch(st, proc=proc), (st["h"], st["pos"], st["step"], st["out"]),
+                          8 * self.dims.num_hidden_layers + (5 if proc else 4))
         need_check = bool(eos) or stopping_fn is not None
-        host = torch.empty((max_new_tokens, B), dtype=torch.int64, pin_memory=True) if need_check else None
-        side = getattr(self, "_copy_stream", None) or torch.cuda.Stream(device=self.device)
-        self._copy_stream = side
         out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
-        stopped = [None] * B  # length at which sequence b stopped
-        done = {}
-
-        def fetch(k: int) -> None:
-            e = torch.cuda.Event()
-            e.record()
-            side.wait_event(e)
-            with torch.cuda.stream(side):
-                host[k].copy_(out2d[k], non_blocking=True)
-                dn = torch.cuda.Event()
-                dn.record(side)
-            done[k] = dn
-
-        n = 1
         if need_check:
-            fetch(0)
-        checked = 0
+            host = self._pinned_ids(max_new_tokens * B).view(max_new_tokens, B)
+            cols = [host[:, b] for b in range(B)]
+            copied = self._to_host((out2d[0], host[0]))
+        stopped = [None] * B  # length at which sequence b stopped
+        n = 1
         while n < max_new_tokens:
             if use_graph:
-                st[gkey].replay()
-                ops.LAUNCHES += kernels
+                self._replay(key)
             else:
                 self._batch_step_launch(st, proc=proc)
             if need_check:  # same pipelining as the single-sequence loop: inspect row n-1 while row n is being computed
-                fetch(n)
-                for k in range(checked, n):
-                    done.pop(k).synchronize()
-                    for b in range(B):
-                        if stopped[b] is None and (int(host[k, b]) in eos or (stopping_fn is not None and stopping_fn(host[:k + 1, b]))):
-                            stopped[b] = k + 1
-                checked = n
+                nxt = self._to_host((out2d[n], host[n]))
+                copied.synchronize()
+                for b in range(B):
+                    if stopped[b] is None:
+                        stopped[b] = first_stop(cols[b], n - 1, n, eos, stopping_fn, max_new_tokens)
+                copied = nxt
                 if all(s is not None for s in stopped):
                     break
             n += 1
@@ -773,9 +736,7 @@ class LlamaDecoder:
             return torch.empty(0, dtype=torch.int64, device=self.device)
         if S + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
-        eos = []
-        if eos_token_ids is not None:
-            eos = [int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids])]
+        eos = eos_list(eos_token_ids)
         n_cand = max(2, 1 + len(eos)) * k
         for b in range(len(self.cache.owned)):
             self.cache.release(b)
@@ -799,7 +760,6 @@ class LlamaDecoder:
         zero = torch.zeros(k, dtype=torch.int32, device=dev)
         tables = [list(self.cache.owned[b]) for b in range(k)]  # page ids by position // PAGE_SIZE
         pages_all = self.cache.pages
-        graph = st.get("beam_graph") if use_graph else None
 
         def keep(score: float, toks: List[int]) -> None:
             nonlocal worst
@@ -852,18 +812,9 @@ class LlamaDecoder:
             st["h"].copy_(ops.splice_rows(w.embed, None, None, None, zero, ids))
             st["pos"].fill_(S + step)
             d_scores.copy_(beam_scores, non_blocking=True)
-            if use_graph and graph is None:
-                saved = st["h"].clone()
-                self._batch_step_launch(st, logits_only=True)  # warm-up outside capture; rewrites only this step's own KV rows
-                torch.cuda.synchronize()
-                st["h"].copy_(saved)
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    self._batch_step_launch(st, logits_only=True)
-                st["beam_graph"] = graph
-            if graph is not None:
-                graph.replay()
-                ops.LAUNCHES += 8 * d.num_hidden_layers + 2
+            if use_graph:  # the warm-up before the capture rewrites only this step's own KV rows
+                self._capture(("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), 8 * d.num_hidden_layers + 2)
+                self._replay(("beam", k))
             else:
                 self._batch_step_launch(st, logits_only=True)
         if not done:  # finalize (beam_search.py): the running beams become hypotheses over their generated length
@@ -891,9 +842,7 @@ class LlamaDecoder:
             raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
         if max(seq_lens) + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{max(seq_lens)} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
-        eos = set()
-        if eos_token_ids is not None:
-            eos = set(int(e) for e in (eos_token_ids if isinstance(eos_token_ids, (list, tuple, set)) else [eos_token_ids]))
+        eos = eos_list(eos_token_ids)
         proc = self._set_processors(processors)
         for b in range(len(self.cache.owned)):
             self.cache.release(b)

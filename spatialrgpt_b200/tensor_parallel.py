@@ -126,11 +126,13 @@ class TPLlamaDecoder(LlamaDecoder):
         self.best_slot = self.slots[-1].view(torch.int32)[:2]
         self.kernels_per_decode_step = 6 * d.num_hidden_layers + 2
 
-    def _ensure_graph(self, seq: int, sample: bool = False) -> None:
-        had = (self._graph_sample if sample else self._graph) is not None
-        super()._ensure_graph(seq, sample)
-        if not had:  # the warm-up step before the capture ran real collectives with the current (epoch, step): retire those flag values
+    def _capture(self, key, launch, restore, kernels: int) -> torch.cuda.CUDAGraph:
+        had = key in self._graphs
+        g = super()._capture(key, launch, restore, kernels)
+        if not had and key[0] == "step":
+            # the warm-up step before the capture ran real collectives with the current (epoch, step): retire those flag values
             self.tp_epoch.add_(1)
+        return g
 
     def _decode_loop(self, *args, **kwargs):
         self.tp_epoch.add_(1)  # a new request: flag values of the previous one can never match (tp_comm.cu seq_value)
@@ -150,9 +152,9 @@ class TPLlamaDecoder(LlamaDecoder):
             out.copy_(t)
 
     # ---- one decode step of this rank ------------------------------------------------------------------------------------
-    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False) -> None:
-        if sample or logits_out is not None:
-            raise NotImplementedError("the tensor-parallel decoder implements greedy decoding (the mode config c5 names)")
+    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False) -> None:
+        if sample or proc or logits_out is not None:
+            raise NotImplementedError("the tensor-parallel decoder implements greedy decoding without logits processors (the mode config c5 names)")
         d, w = self.dims, self.w
         hd = d.head_dim
         group = d.num_attention_heads // d.num_key_value_heads

@@ -17,7 +17,7 @@ llm = model.llm
 n = 5 * cfg.llama.num_hidden_layers + 1   # traced launches per step (the 1-CTA finalize kernel is not traced)
 buf = torch.zeros(2 * n + 8, 4, dtype=torch.int64, device=dev)
 lib = _lib.load()
-llm._graph = None
+llm._drop_graphs()
 lib.srgpt_trace_begin(buf.data_ptr(), 2 * n + 8)
 llm._ensure_graph(0)           # capture with trace records baked into the kernel parameters
 used = lib.srgpt_trace_end()

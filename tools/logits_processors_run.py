@@ -79,9 +79,8 @@ def main():
            "processors": PROCESSORS, "decode_tokens_per_s": {m: round((N - 1) / (t / 1e3), 1) for m, t in med.items()},
            "ids_differ": bool(not torch.equal(ids["off"], ids["on"]))}
     dec.generate_from_embeds(x, N, processors=spec)
-    dec._ensure_graph(0)
-    dec._ensure_graph(0, proc=True)
-    off_ms, on_ms = replay_ms(dec, dec._graph, PROMPT_ROWS, 60), replay_ms(dec, dec._proc_graphs[False], PROMPT_ROWS, 60)
+    g_off, g_on = dec._ensure_graph(0), dec._ensure_graph(0, proc=True)
+    off_ms, on_ms = replay_ms(dec, g_off, PROMPT_ROWS, 60), replay_ms(dec, g_on, PROMPT_ROWS, 60)
     out["graph_replay_ms"] = {"off": round(off_ms, 4), "on": round(on_ms, 4), "delta_pct": round(100 * (on_ms - off_ms) / off_ms, 2)}
     out["processing_kernels_us"] = {f"history_{n}": round(kernel_us(dec, n), 2) for n in (0, 128, 4096)}
     print(json.dumps(out))
