@@ -417,6 +417,60 @@ int srgpt_llama_decode_step_nf4_bf16(void* h, const srgpt_llama_layer_weights* l
                                      const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
                                      void* lm_workspace, float* logits_out, long long* out_ids, int* step, void* stream);
 
+/* ---- FP8 (E4M3) W8A8 quantization of the decoder-layer linears (fp8.cu, gemm_wgmma.cu; DESIGN.md §3, §7) ---------------------------
+ * Every row r of a weight W [N, K] (once, at load) and of an activation x [M, K] (before every linear) is quantized alike:
+ * a = max_k |x[r, k]| (fp32), inv = 448 / a, scale[r] = a / 448 (both 1 when a == 0), q[r, k] = e4m3(fl32(x[r, k] * inv)), rounded to
+ * nearest even and saturated to +-448 (cvt.rn.satfinite).  A linear is y[m, n] = acc[m, n] * (scale_x[m] * scale_w[n]) in fp32, acc the fp32
+ * sum of the exact E4M3 products; the epilogue's rounding points follow.  K must be a multiple of 16. */
+typedef struct {
+  const void* q;       /* [N, K] E4M3 codes, row-major, K bytes per row */
+  const float* scale;  /* [N] */
+} srgpt_fp8;
+/* *n_bad += 1 for every row holding Inf or NaN (such a matrix must not be used). */
+int srgpt_fp8_quantize_weight_bf16(const void* W, int ldw, int N, int K, void* q, float* scale, int* n_bad, void* stream);
+/* q [M, ldq] bytes (ldq a multiple of 16), scale [M] */
+int srgpt_fp8_quantize_act_bf16(const void* x, int ldx, int M, int K, void* q, int ldq, float* scale, void* stream);
+/* srgpt_gemm_bf16 over E4M3 operands: A [M, lda] and W [N, ldw] bytes with their row scales sx [M] and sw [N]; epilogue SRGPT_EPI_NONE,
+ * SRGPT_EPI_BIAS_RESIDUAL (no bias) or SRGPT_EPI_SWIGLU; C in the element type.  Tiles, ring, tile order and stream-K as the 16-bit
+ * kernel, with K blocks of 128 elements (wgmma m64n128k32 e4m3). */
+int srgpt_gemm_fp8_bf16(const void* A, int lda, const float* sx, const void* W, int ldw, const float* sw, void* C, int ldc, int M, int N, int K,
+                        const void* residual, int ldr, int epilogue, void* stream);
+/* A decoder layer with FP8 linears (no element-type copy of its matrices). */
+typedef struct {
+  const void* in_norm;
+  srgpt_fp8 qkv;     /* [(nh + 2 nkv) hd, H] */
+  srgpt_fp8 o;       /* [H, nh hd] */
+  const void* post_norm;
+  srgpt_fp8 gateup;  /* [2 I, H], rows interleaved (gate_i, up_i) */
+  srgpt_fp8 down;    /* [H, I] */
+  void* kv_pages;
+} srgpt_llama_layer_fp8;
+/* srgpt_llama_prefill_layers_bf16 / srgpt_llama_prefill_chunk_layers_bf16 with every linear as activation quantizer + FP8 GEMM.
+ * Extra workspaces: ws_q8 [S, max(H, nh hd, I)] bytes and ws_scale [S] fp32. */
+int srgpt_llama_prefill_layers_fp8_bf16(void* x, const srgpt_llama_layer_fp8* layers, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn,
+                                        void* ws_act, void* ws_q8, float* ws_scale, int S, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                        float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables,
+                                        int page_size, int n_seqs, const int* cu_seqlens, int max_seqlen, int page_table_stride, void* stream);
+int srgpt_llama_prefill_chunk_layers_fp8_bf16(void* x, const srgpt_llama_layer_fp8* layers, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn,
+                                              void* ws_act, void* ws_q8, float* ws_scale, int S, int H, int n_heads, int n_kv_heads, int head_dim,
+                                              int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
+                                              const int* page_tables, int page_table_stride, int page_size, int n_pages, int n_seqs,
+                                              const int* cu_seqlens, int max_rows, void* stream);
+/* srgpt_gemv_bf16 over FP8 planes (fp8_gemv_kernel, gemv.cu), every mode: x (RMS-normalised first when norm_weight is given) is quantized
+ * in the kernel by the activation definition above, the weight codes are turned into their element-type values exactly, and a row's sum
+ * acc of exact products (fp32) becomes acc * fl32(s_x * scale[row]) before the mode's stores and rounding points.  `w` is a host pointer;
+ * K a multiple of 16. */
+int srgpt_gemv_fp8_bf16(const void* x, const srgpt_fp8* w, void* y, int N, int K, const void* norm_weight, float eps, const void* residual,
+                        int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos,
+                        void* kv_pages, const int* page_table, int page_size, void* stream);
+/* One decode step over FP8 layers: srgpt_llama_decode_step_nf4_bf16's 5 kernels per layer with every layer matrix streamed by
+ * srgpt_gemv_fp8_bf16, then lm_head + argmax (lm_packed may be NULL).  Buffers as srgpt_llama_decode_step_bf16's. */
+int srgpt_llama_decode_step_fp8_bf16(void* h, const srgpt_llama_layer_fp8* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf,
+                                     int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab,
+                                     int* pos, const int* page_table, int page_size, const void* final_norm, const void* lm_head,
+                                     const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out,
+                                     long long* out_ids, int* step, void* stream);
+
 /* ---- prompt-lookup speculative decoding, batch 1, greedy (HF GenerationMixin._assisted_decoding with
  * PromptLookupCandidateGenerator, i.e. generate(prompt_lookup_num_tokens=k); call site llava_llama.py:212).
  * A verify pass runs T = k + 1 tokens at positions pos .. pos+T-1: row 0 is the last emitted token, rows 1..T-1 the drafts.

@@ -99,6 +99,16 @@ SIGNATURES = {
     "srgpt_gemv_nf4_bf16": (ci, [vp, vp, vp, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
     "srgpt_llama_decode_step_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp,
                                               vp, vp, vp, vp]),
+    "srgpt_fp8_quantize_weight_bf16": (ci, [vp, ci, ci, ci, vp, vp, vp, vp]),
+    "srgpt_fp8_quantize_act_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp]),
+    "srgpt_gemm_fp8_bf16": (ci, [vp, ci, vp, vp, ci, vp, vp, ci, ci, ci, ci, vp, ci, ci, vp]),
+    "srgpt_llama_prefill_layers_fp8_bf16": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, ci, ci,
+                                                 vp]),
+    "srgpt_llama_prefill_chunk_layers_fp8_bf16": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, ci,
+                                                       ci, vp, ci, vp]),
+    "srgpt_gemv_fp8_bf16": (ci, [vp, vp, vp, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_llama_decode_step_fp8_bf16": (ci, [vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp, vp, vp, vp,
+                                              vp, vp]),
     "srgpt_gemv_multi_bf16": (ci, [vp, ci, vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
     "srgpt_gemv_multi_packed_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
     "srgpt_lm_head_multi_bf16": (ci, [vp, ci, vp, ci, ci, ci, ci, vp, cf, vp, vp, vp]),
@@ -139,6 +149,15 @@ class Nf4(C.Structure):
 
 class LlamaLayerNf4(C.Structure):
     _fields_ = [(n, Nf4) for n in ("qkv", "o", "gateup", "down")]
+
+
+class Fp8(C.Structure):
+    """srgpt_fp8: one matrix's E4M3 codes [N, K] and row scales [N]."""
+    _fields_ = [("q", vp), ("scale", vp)]
+
+
+class LlamaLayerFp8(C.Structure):
+    _fields_ = [("in_norm", vp), ("qkv", Fp8), ("o", Fp8), ("post_norm", vp), ("gateup", Fp8), ("down", Fp8), ("kv_pages", vp)]
 
 
 def lib_path(elem: str = "bf16") -> str:

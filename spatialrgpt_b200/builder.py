@@ -218,7 +218,10 @@ def load_pretrained_model(model_path: str, model_name: str, model_base: Optional
     bf16 cast afterwards exactly as the reference's do (``model.to(dtype=torch.bfloat16)``, eval_spatial.py:221).  ``torch_dtype=``
     (torch.float16 / torch.bfloat16) is an extension that loads straight into that dtype.  ``quantization="nf4"`` is an extension too:
     the decoder-layer linears are NF4-quantized at load (weights.from_state_dicts) and dequantized into that dtype; the batch-1 decode
-    step streams the 4-bit planes.  ``load_4bit`` / ``load_8bit`` (bitsandbytes) still raise."""
+    step streams the 4-bit planes.  ``quantization="fp8"`` quantizes the same linears to per-row E4M3 weights (W8A8: every activation row
+    is quantized alike before each linear), keeps no element-type copy of them, and runs them on the FP8 tensor cores (prefill, batched
+    decode, beams) and through the FP8 decode GEMV (the one-token step); ``prompt_lookup_num_tokens`` then raises.  ``load_4bit`` /
+    ``load_8bit`` (bitsandbytes) still raise."""
     if load_8bit or load_4bit:
         raise NotImplementedError("bitsandbytes quantised loading is outside the hot path (builder.py:51-60)")
     if model_base is not None:

@@ -14,6 +14,9 @@
 // Out-of-bounds rows/cols/K are zero-filled by TMA, so M, N need no padding and K only has to
 // be a multiple of 8 elements (16-byte global strides).
 //
+// FP8: gemm_fp8_kernel runs the same body over E4M3 operands (K blocks of 128 one-byte elements, the same 128-byte rows, wgmma
+// m64n128k32.e4m3) and scales the accumulators by the row scales of both operands before the epilogue (W8A8 decoder linears, fp8.cu).
+//
 // Short problems (M <= 128 rows: the projections and the lm_head of a batched decode step) have N / 128 tiles, too few to
 // fill 132 SMs.  With a registered workspace they run "stream-K": the (n-tile, k-block) units are cut into gridDim.x equal
 // contiguous ranges, one per SM.  A tile whose k-range is split is owned by the CTA holding its first k-block; the other CTAs
@@ -76,6 +79,35 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a
       : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
+
+// The E4M3 form (FP8 operands, gemm_fp8_kernel): one wgmma consumes 32 one-byte elements = the same 32 bytes of K, so the descriptor
+// step and the accumulator layout are those of wgmma_m64n128k16.
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b)
+      : "memory");
+}
+
+// per-row / per-column fp32 scales of the FP8 operands: y[m, n] = acc[m, n] * (sx[m] * sw[n])
+struct Fp8Scales {
+  const float* sx;  // [M]
+  const float* sw;  // [N]
+};
 
 struct Params {
   int M, N, K;
@@ -176,11 +208,30 @@ __device__ __forceinline__ void store_acc(const float (&d)[64], const Params& p,
   }
 }
 
+// FP8: the fp32 accumulators of one consumer thread times sx[row] * sw[col], before the epilogue rounds them (rows / columns past M / N
+// are never stored and keep their value)
+__device__ __forceinline__ void scale_acc(float (&d)[64], const Fp8Scales& sc, const Params& p, int row0, int col0) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = row0 + 8 * i;
+    if (row >= p.M) continue;
+    const float sx = sc.sx[row];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = col0 + 8 * j;
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+        if (col + c < p.N) d[4 * j + 2 * i + c] *= sx * sc.sw[col + c];
+    }
+  }
+}
+
 // SK = false: persistent over whole 128 x 128 tiles.  SK = true: stream-K over the (n-tile, k-block) units of an M <= 128
-// problem (see the file comment).
-template <int EPI, bool SK>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p, const TskWs ws) {
+// problem (see the file comment).  FP8 = true: E4M3 operands, a K block of 128 one-byte elements (the same 128-byte rows, so the
+// stage size, swizzle, ring and tile order are those of the 16-bit kernel), and the accumulators scaled by `sc` before the epilogue.
+template <int EPI, bool SK, bool FP8>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const Params& p, const TskWs& ws, const Fp8Scales& sc) {
+  constexpr int KB = FP8 ? 128 : BK;  // elements per k-block
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned stage buffers
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -189,7 +240,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 
   const int tiles_m = (p.M + BM - 1) / BM;
   const int tiles_n = (p.N + BN - 1) / BN;
-  const int num_kb = (p.K + BK - 1) / BK;
+  const int num_kb = (p.K + KB - 1) / KB;
   const int num_units = tiles_m * tiles_n;
   const int G = (int)gridDim.x, cta = (int)blockIdx.x;
   const long long total = (long long)tiles_n * num_kb;  // stream-K units (M <= 128: one m-tile)
@@ -197,8 +248,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int u_begin = SK ? range_begin(cta) : 0, u_end = SK ? range_begin(cta + 1) : 0;
 
   if (threadIdx.x == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
+    prefetch_tmap(tmap_a);
+    prefetch_tmap(tmap_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
       mbar_init(smem_u32(&empty_bar[s]), 2);  // one arrive per consumer warpgroup
@@ -217,8 +268,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         const uint32_t fb = smem_u32(&full_bar[stage]);
         mbar_expect_tx(fb, STAGE_BYTES);  // out-of-bounds rows / columns are zero-filled and still counted
         uint8_t* sa = smem + stage * STAGE_BYTES;
-        tma_load_2d(smem_u32(sa), &tmap_a, fb, kb * BK, m0);
-        tma_load_2d(smem_u32(sa + A_BYTES), &tmap_b, fb, kb * BK, n0);
+        tma_load_2d(smem_u32(sa), tmap_a, fb, kb * KB, m0);
+        tma_load_2d(smem_u32(sa + A_BYTES), tmap_b, fb, kb * KB, n0);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       };
       if (SK) {
@@ -255,7 +306,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       const uint64_t a_desc = make_desc_sw128(a_addr), b_desc = make_desc_sw128(b_addr);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BK / WG_K; ++k) wgmma_m64n128k16(d, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k));
+      for (int k = 0; k < BK / WG_K; ++k) {
+        if constexpr (FP8)
+          wgmma_m64n128k32_e4m3(d, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k));
+        else
+          wgmma_m64n128k16(d, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k));
+      }
       wgmma_commit();
       if (kb > 0) {
         wgmma_wait<1>();  // the previous k-block's wgmma has read its stage
@@ -273,6 +329,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       int mt, nt;
       unit_to_tile(unit, tiles_m, tiles_n, p.gm, mt, nt);
       mainloop(num_kb);
+      if constexpr (FP8) scale_acc(d, sc, p, mt * BM + r_in_tile, nt * BN + c_in_tile);
       store_acc<EPI>(d, p, mt * BM + r_in_tile, nt * BN + c_in_tile);
     }
     return;
@@ -312,6 +369,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int i = 0; i < 64; ++i) d[i] += __ldcg(src + i * 256 + ct);
       }
+      if constexpr (FP8) scale_acc(d, sc, p, r_in_tile, tile * BN + c_in_tile);
       store_acc<EPI>(d, p, r_in_tile, tile * BN + c_in_tile);
       if (c_last > cta) {
         // every consumer has read the contributors' partials: clear their flags, so that a CUDA-graph REPLAY of this launch
@@ -325,15 +383,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
 }
 
+template <int EPI, bool SK>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p, const TskWs ws) {
+  gemm_body<EPI, SK, false>(&tmap_a, &tmap_b, p, ws, Fp8Scales{nullptr, nullptr});
+}
+
+template <int EPI, bool SK>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p, const TskWs ws,
+                const Fp8Scales sc) {
+  gemm_body<EPI, SK, true>(&tmap_a, &tmap_b, p, ws, sc);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-// [rows, k] row-major 16-bit matrix with `ld` elements between rows -> box {BK, 128 rows}, 128B swizzle
-static int make_tmap(CUtensorMap* tm, const void* ptr, int rows, int k, int ld) {
+// [rows, k] row-major matrix with `ld` elements between rows -> box {128 bytes, 128 rows}, 128B swizzle; 16-bit elements, or E4M3
+// bytes when fp8
+static int make_tmap(CUtensorMap* tm, const void* ptr, int rows, int k, int ld, bool fp8 = false) {
   const cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)BK, 128u};
-  const int r = encode_tmap_bf16(tm, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * (fp8 ? 1 : 2)};
+  const cuuint32_t box[2] = {fp8 ? 128u : (cuuint32_t)BK, 128u};
+  const int r = fp8 ? encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)
+                    : encode_tmap_bf16(tm, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
   if (r != 0) {
     set_last_error("cuTensorMapEncodeTiled failed: %d (rows=%d k=%d ld=%d ptr=%p)", r, rows, k, ld, ptr);
     return SRGPT_ERR_CUDA;
@@ -355,32 +428,42 @@ static TskState g_tsk;
 
 static long long tsk_workspace_bytes(int ctas) { return TSK_FLAG_BYTES + (long long)ctas * TSK_SLOT_FLOATS * 4; }
 
-template <int EPI, bool SK>
-static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, const TskWs& ws, int grid, cudaStream_t stream) {
+template <int EPI, bool SK, bool FP8>
+static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, const TskWs& ws, const Fp8Scales& sc, int grid,
+                         cudaStream_t stream) {
   static bool configured = false;
   if (!configured) {
-    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    if constexpr (FP8)
+      SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    else
+      SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  gemm_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p, ws);
+  if constexpr (FP8)
+    gemm_fp8_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p, ws, sc);
+  else
+    gemm_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p, ws);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }
 
-template <int EPI>
-static int launch(const void* A, int lda, const void* W, int ldw, const Params& p, cudaStream_t stream) {
+// FP8: A and W hold E4M3 bytes (lda / ldw in bytes) and `sc` their scales
+template <int EPI, bool FP8 = false>
+static int launch(const void* A, int lda, const void* W, int ldw, const Params& p, cudaStream_t stream, const Fp8Scales& sc = Fp8Scales{nullptr, nullptr}) {
+  constexpr int EB = FP8 ? 1 : 2;           // bytes per element
+  constexpr int KB = FP8 ? 128 : BK;        // elements per k-block
   CUtensorMap ta, tb;
-  int rc = make_tmap(&ta, A, p.M, p.K, lda);
+  int rc = make_tmap(&ta, A, p.M, p.K, lda, FP8);
   if (rc != SRGPT_OK) return rc;
-  rc = make_tmap(&tb, W, p.N, p.K, ldw);
+  rc = make_tmap(&tb, W, p.N, p.K, ldw, FP8);
   if (rc != SRGPT_OK) return rc;
   const int sms = sm_count();
   TskWs ws = {nullptr, nullptr, 0};
   // one-tile-high problems whose weights are worth streaming (>= 4 MB) take the stream-K split when the caller registered a
   // workspace (srgpt_gemm_set_workspace); SRGPT_GEMM_TSK=-1 turns it off
   static const int tsk_env = env_int("SRGPT_GEMM_TSK");
-  const long long sk_units = (long long)ceil_div(p.N, BN) * ceil_div(p.K, BK);
-  if (tsk_env >= 0 && g_tsk.base != nullptr && p.M <= BM && (long long)p.N * p.K * 2 >= (4LL << 20) &&
+  const long long sk_units = (long long)ceil_div(p.N, BN) * ceil_div(p.K, KB);
+  if (tsk_env >= 0 && g_tsk.base != nullptr && p.M <= BM && (long long)p.N * p.K * EB >= (4LL << 20) &&
       g_tsk.bytes >= tsk_workspace_bytes(8)) {
     int grid = sms < TSK_MAX_CTAS ? sms : TSK_MAX_CTAS;
     if ((long long)grid > sk_units) grid = (int)sk_units;
@@ -389,7 +472,7 @@ static int launch(const void* A, int lda, const void* W, int ldw, const Params& 
     ws.partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(g_tsk.base) + TSK_FLAG_BYTES);
     if (++g_tsk.epoch == 0) g_tsk.epoch = 1;  // flags start at 0 (zeroed workspace) and never equal a future epoch
     ws.epoch = g_tsk.epoch;
-    return launch_kernel<EPI, true>(ta, tb, p, ws, grid, stream);
+    return launch_kernel<EPI, true, FP8>(ta, tb, p, ws, sc, grid, stream);
   }
   // rasterisation group: the whole M when the activation fits L2 (50 MB), else as many m-tiles as keep a group's rows <= 20 MB;
   // SRGPT_GEMM_GM forces the group size
@@ -397,14 +480,14 @@ static int launch(const void* A, int lda, const void* W, int ldw, const Params& 
   const int tiles_m = ceil_div(p.M, BM);
   Params pg = p;
   pg.gm = tiles_m;
-  if (2.0 * p.M * p.K > 40e6) {
-    const int g = (int)(20e6 / (2.0 * BM * p.K));
+  if ((double)EB * p.M * p.K > 40e6) {
+    const int g = (int)(20e6 / ((double)EB * BM * p.K));
     pg.gm = g < 1 ? 1 : (g < tiles_m ? g : tiles_m);
   }
   if (gm_env > 0) pg.gm = gm_env < tiles_m ? gm_env : tiles_m;
   const long long units = (long long)tiles_m * ceil_div(p.N, BN);
   const int grid = (int)(units < sms ? units : sms);
-  return launch_kernel<EPI, false>(ta, tb, pg, ws, grid, stream);
+  return launch_kernel<EPI, false, FP8>(ta, tb, pg, ws, sc, grid, stream);
 }
 
 }  // namespace gemm
@@ -469,6 +552,43 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemm_bf16(const void
     case SRGPT_EPI_BIAS_RESIDUAL: return gemm::launch<SRGPT_EPI_BIAS_RESIDUAL>(A, lda, W, ldw, p, st);
     case SRGPT_EPI_SWIGLU: return gemm::launch<SRGPT_EPI_SWIGLU>(A, lda, W, ldw, p, st);
     case SRGPT_EPI_BIAS_QUICK_GELU: return gemm::launch<SRGPT_EPI_BIAS_QUICK_GELU>(A, lda, W, ldw, p, st);
+  }
+  return SRGPT_ERR_INVALID;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemm_fp8_bf16(const void* A, int lda, const float* sx, const void* W, int ldw, const float* sw,
+                                                                            void* C, int ldc, int M, int N, int K, const void* residual, int ldr,
+                                                                            int epilogue, void* stream) {
+  SRGPT_CHECK_ARG(A != nullptr && W != nullptr && C != nullptr && sx != nullptr && sw != nullptr);
+  SRGPT_CHECK_ARG(M > 0 && N > 0 && K > 0 && (K % 16) == 0);
+  SRGPT_CHECK_ARG(lda >= K && ldw >= K && (lda % 16) == 0 && (ldw % 16) == 0);  // 16-byte global strides for TMA
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0);
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(C) & 15) == 0);
+  SRGPT_CHECK_ARG(epilogue == SRGPT_EPI_NONE || epilogue == SRGPT_EPI_BIAS_RESIDUAL || epilogue == SRGPT_EPI_SWIGLU);
+  if (epilogue == SRGPT_EPI_SWIGLU) {
+    SRGPT_CHECK_ARG((N % 2) == 0 && ldc >= N / 2 && (ldc % 8) == 0);
+  } else {
+    SRGPT_CHECK_ARG(ldc >= N && (ldc % 8) == 0);
+  }
+  if (residual != nullptr) {
+    SRGPT_CHECK_ARG(epilogue == SRGPT_EPI_BIAS_RESIDUAL && ldr >= N && (ldr % 8) == 0);
+    SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(residual) & 15) == 0);
+  }
+
+  gemm::Params p;
+  p.gm = 1;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc;
+  p.bias = nullptr;
+  p.residual = reinterpret_cast<const bf16*>(residual);
+  p.ldr = ldr; p.res_row_mod = 0;
+  p.C = C; p.out_fp32 = 0;
+  const gemm::Fp8Scales sc = {sx, sw};
+
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (epilogue) {
+    case SRGPT_EPI_NONE: return gemm::launch<SRGPT_EPI_NONE, true>(A, lda, W, ldw, p, st, sc);
+    case SRGPT_EPI_BIAS_RESIDUAL: return gemm::launch<SRGPT_EPI_BIAS_RESIDUAL, true>(A, lda, W, ldw, p, st, sc);
+    case SRGPT_EPI_SWIGLU: return gemm::launch<SRGPT_EPI_SWIGLU, true>(A, lda, W, ldw, p, st, sc);
   }
   return SRGPT_ERR_INVALID;
 }

@@ -20,7 +20,10 @@
 // A format only says how a batch of 4 chunks per lane and row is loaded and turned into the element-type chunks dot8 reads; the kernel
 // around it (row pairs, x staging, the prefetch before the dependency wait, the chunk order of every lane's fma chain and the epilogue)
 // is one, so the packed and NF4 kernels are bit-identical to the bf16 kernel over the same (dequantized) matrix.
+#include <type_traits>
+
 #include "common.cuh"
+#include "fp8.cuh"
 #include "nf4.cuh"
 #include "pack12.cuh"
 #include "srgpt_b200.h"
@@ -586,6 +589,131 @@ __global__ void __launch_bounds__(THREADS, 3) decode_gemv_kernel(const Params p)
   trace_mark(p.trace, 2);
 }
 
+// ---- FP8 (E4M3) W8A8 one-token GEMV (the decode step of a quantization="fp8" model; definition: include/srgpt_b200.h srgpt_fp8) ----------
+// x (RMS-normalised when norm_weight is given) is staged as by the kernels above, then quantized in place by the activation quantizer's
+// definition: the CTA's max |x|, inv = 448 / a, and every element replaced by its E4M3 value, held exactly as an element-type value.  A
+// warp streams a row pair of codes (one 16-byte vector = 16 weights per lane and load, 4 loads per row and batch, the next batch
+// requested while the current one is consumed), turns each vector into two element-type chunks (exact) and runs dot8 over them: every
+// product is exact and acc is their fp32 sum.  The epilogue multiplies acc by fl32(s_x * s_w[row]) and stores through store_pair, the
+// rounding points of the other formats.  K % 16 == 0.
+__device__ __forceinline__ float stage_quantize_e4m3(bf16* sx, int K, float* red) {
+  const int nchunk = K >> 3;
+  float m = 0.f;
+  for (int c = threadIdx.x; c < nchunk; c += THREADS) {
+    float f[8];
+    unpack8(reinterpret_cast<const uint4*>(sx)[c], f);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) m = fmaxf(m, fabsf(f[t]));
+  }
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int w = 1; w < WARPS; ++w) m = fmaxf(m, red[w]);
+  float inv, scale;
+  fp8::row_scales(m, inv, scale);
+  for (int c = threadIdx.x; c < nchunk; c += THREADS) {  // a thread rewrites only the chunks it read
+    float f[8];
+    unpack8(reinterpret_cast<const uint4*>(sx)[c], f);
+    uint4 v;
+    v.x = fp8::e4m3x2_to_elem2(fp8::e4m3x2(__fmul_rn(f[0], inv), __fmul_rn(f[1], inv)));
+    v.y = fp8::e4m3x2_to_elem2(fp8::e4m3x2(__fmul_rn(f[2], inv), __fmul_rn(f[3], inv)));
+    v.z = fp8::e4m3x2_to_elem2(fp8::e4m3x2(__fmul_rn(f[4], inv), __fmul_rn(f[5], inv)));
+    v.w = fp8::e4m3x2_to_elem2(fp8::e4m3x2(__fmul_rn(f[6], inv), __fmul_rn(f[7], inv)));
+    reinterpret_cast<uint4*>(sx)[c] = v;
+  }
+  __syncthreads();
+  return scale;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(THREADS, 2) fp8_gemv_kernel(const Params p, const srgpt_fp8 w8) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ float red[32];
+  bf16* sx = reinterpret_cast<bf16*>(smem_raw);
+  const uint4* px = reinterpret_cast<const uint4*>(sx);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  trace_mark(p.trace, 0);
+  const int pi = blockIdx.x * WARPS + warp;
+  const bool active = pi < (p.N >> 1);
+  int r0, r1;
+  pair_rows<MODE>(p, pi, r0, r1);
+  const int nvec = p.K >> 4;  // 16-byte code vectors per row
+  const uint4* q0 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(w8.q) + (size_t)r0 * p.K);
+  const uint4* q1 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(w8.q) + (size_t)r1 * p.K);
+  // batch b: vectors v = 128 b + lane + 32 i, i = 0..3, of both rows (zero past the row's end)
+  auto load = [&](int b, uint4 (&u0)[4], uint4 (&u1)[4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int v = b * 128 + lane + 32 * i;
+      u0[i] = make_uint4(0, 0, 0, 0);
+      u1[i] = make_uint4(0, 0, 0, 0);
+      if (active && v < nvec) {
+        u0[i] = ld_stream16(q0 + v);
+        u1[i] = ld_stream16(q1 + v);
+      }
+    }
+  };
+  uint4 c0[4], c1[4];
+  load(0, c0, c1);  // static weights: requested before the dependency wait, like the row scales and the norm weights
+  const float sw0 = active ? __ldg(w8.scale + r0) : 0.f, sw1 = active ? __ldg(w8.scale + r1) : 0.f;
+  uint4 nw_pre[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
+  const bool nw_pre_valid = (p.norm_weight != nullptr) && ((p.K >> 3) <= 2 * THREADS);
+  if (nw_pre_valid) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int cc = threadIdx.x + k * THREADS;
+      if (cc < (p.K >> 3)) nw_pre[k] = reinterpret_cast<const uint4*>(p.norm_weight)[cc];
+    }
+  }
+  pdl_launch_dependents();
+  pdl_wait();
+  trace_mark(p.trace, 1);
+
+  stage_x(p.x, p.norm_weight, p.eps, p.K, sx, red, nw_pre, nw_pre_valid);
+  const float s_x = stage_quantize_e4m3(sx, p.K, red);
+
+  float a0 = 0.f, a1 = 0.f;
+  const int nb = (nvec + 127) >> 7;
+  for (int b = 0; b < nb; ++b) {
+    uint4 n0[4], n1[4];
+    if (b + 1 < nb) load(b + 1, n0, n1);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int v = b * 128 + lane + 32 * i;
+      if (v < nvec) {
+        uint4 w0[2], w1[2];
+        fp8::e4m3x16_to_elem(c0[i], w0[0], w0[1]);
+        fp8::e4m3x16_to_elem(c1[i], w1[0], w1[1]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float xf[8];
+          unpack8(px[2 * v + h], xf);
+          a0 += dot8(w0[h], xf);
+          a1 += dot8(w1[h], xf);
+        }
+      }
+    }
+    if (b + 1 < nb) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        c0[i] = n0[i];
+        c1[i] = n1[i];
+      }
+    }
+  }
+  a0 = warp_sum(a0);
+  a1 = warp_sum(a1);
+  if (active && lane == 0) {
+    float best;
+    int besti;
+    store_pair<MODE>(p, p.y, p.residual, nullptr, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos : 0, pi, r0, r1, a0 * (s_x * sw0), a1 * (s_x * sw1), best,
+                     besti);
+  }
+  trace_mark(p.trace, 2);
+}
+
 // The best (value, index) of part_val / part_idx [0, n) over a CTA of 256 threads: `better` (the larger value, the lower index on ties)
 // per thread, across the warp by shuffles, then across the 8 warps by thread 0, which alone holds the result.  (-INFINITY, 0x7fffffff)
 // when n = 0 or every value is NaN.  A caller that runs it again first synchronises the CTA: it reuses its shared memory.
@@ -972,6 +1100,34 @@ static int launch(const Params& p, int npairs, cudaStream_t st) {
   return SRGPT_OK;
 }
 
+template <int MODE>
+static int launch_fp8(const Params& p, const srgpt_fp8& w8, int npairs, cudaStream_t st) {
+  const int smem = p.K * 2;
+  static int configured_smem = 0;
+  if (smem > 48 * 1024 && smem > configured_smem) {
+    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(fp8_gemv_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured_smem = smem;
+  }
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  pdl_config(cfg, attr, grid_for(npairs), THREADS, smem, st);
+  Params q = p;
+  q.trace = trace_next_slot();
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fp8_gemv_kernel<MODE>, q, w8));
+  return SRGPT_OK;
+}
+
+// the FP8 planes are not a decode_gemv_kernel format: their kernel is fp8_gemv_kernel, which takes them beside Params
+struct Fp8 {};
+
+template <int MODE, class Fmt>
+static int launch_format(const Params& p, const srgpt_fp8* w8, int npairs, cudaStream_t st) {
+  if constexpr (std::is_same<Fmt, Fp8>::value)
+    return launch_fp8<MODE>(p, *w8, npairs, st);
+  else
+    return launch<MODE, Fmt>(p, npairs, st);
+}
+
 }  // namespace gemv
 }  // namespace srgpt
 
@@ -1017,11 +1173,12 @@ static void set_rope(gemv::Params& p, int n_heads, int n_kv_heads, int head_dim,
   p.page_size = page_size;
 }
 
-// checks and mode dispatch of srgpt_gemv_bf16, srgpt_gemv_packed_bf16 and srgpt_gemv_nf4_bf16; p's weights are set by the caller
+// checks and mode dispatch of srgpt_gemv_bf16, srgpt_gemv_packed_bf16, srgpt_gemv_nf4_bf16 and srgpt_gemv_fp8_bf16; p's weights are set by
+// the caller
 template <class Fmt>
 static int gemv_modes(gemv::Params& p, const void* x, void* y, int N, int K, const void* norm_weight, float eps, const void* residual, int mode,
                       int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages,
-                      const int* page_table, int page_size, void* stream) {
+                      const int* page_table, int page_size, void* stream, const srgpt_fp8* w8 = nullptr) {
   SRGPT_CHECK_ARG(x && y && N > 0 && K > 0);
   SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0);
   SRGPT_CHECK_ARG(K * 2 <= 200 * 1024);
@@ -1033,16 +1190,16 @@ static int gemv_modes(gemv::Params& p, const void* x, void* y, int N, int K, con
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   switch (mode) {
     case SRGPT_GEMV_PLAIN:
-      return gemv::launch<SRGPT_GEMV_PLAIN, Fmt>(p, N / 2, st);
+      return gemv::launch_format<SRGPT_GEMV_PLAIN, Fmt>(p, w8, N / 2, st);
     case SRGPT_GEMV_SWIGLU:
       SRGPT_CHECK_ARG(residual == nullptr);
-      return gemv::launch<SRGPT_GEMV_SWIGLU, Fmt>(p, N / 2, st);
+      return gemv::launch_format<SRGPT_GEMV_SWIGLU, Fmt>(p, w8, N / 2, st);
     case SRGPT_GEMV_QKV_ROPE:
       SRGPT_CHECK_ARG(residual == nullptr && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && (head_dim % 2) == 0);
       SRGPT_CHECK_ARG(N == (n_heads + 2 * n_kv_heads) * head_dim);
       SRGPT_CHECK_ARG(cos_tab && sin_tab && pos && kv_pages && page_table && page_size > 0);
       set_rope(p, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages, page_table, page_size);
-      return gemv::launch<SRGPT_GEMV_QKV_ROPE, Fmt>(p, N / 2, st);
+      return gemv::launch_format<SRGPT_GEMV_QKV_ROPE, Fmt>(p, w8, N / 2, st);
   }
   return SRGPT_ERR_INVALID;
 }
@@ -1059,6 +1216,17 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_nf4_bf16(const 
   p.nf = *nf4;
   return gemv_modes<gemv::Nf4>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
                                page_table, page_size, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_fp8_bf16(const void* x, const srgpt_fp8* w, void* y, int N, int K, const void* norm_weight,
+                                                                          float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim,
+                                                                          const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages,
+                                                                          const int* page_table, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(w && w->q && w->scale && aligned16(w->q) && (reinterpret_cast<uintptr_t>(w->scale) & 3) == 0);
+  SRGPT_CHECK_ARG(K > 0 && (K % 16) == 0);
+  gemv::Params p = {};
+  return gemv_modes<gemv::Fp8>(p, x, y, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages,
+                               page_table, page_size, stream, w);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_gemv_bf16(const void* x, const void* W, int ldw, void* y, int N, int K, const void* norm_weight, float eps,

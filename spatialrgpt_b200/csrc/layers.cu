@@ -44,20 +44,47 @@ extern "C" __attribute__((visibility("default"))) int srgpt_siglip_layers_bf16(v
   return srgpt_vit_layers_bf16(x, layers, n_layers, ws_h, ws_qkv, ws_attn, ws_mlp, n_img, T, D, heads, I, eps, SRGPT_EPI_BIAS_GELU_TANH, stream);
 }
 
-extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers_bf16(void* x, const srgpt_llama_layer_weights* layers, int n_layers, void* ws_h, void* ws_qkv,
-                                                                                        void* ws_attn, void* ws_act, int S, int H, int n_heads, int n_kv_heads,
-                                                                                        int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab,
-                                                                                        const int* start_pos, const int* page_table, int page_size, int n_seqs, const int* cu_seqlens,
-                                                                                        int max_seqlen, int page_table_stride, void* stream) {
-  SRGPT_CHECK_ARG(x && layers && ws_h && ws_qkv && ws_attn && ws_act && n_layers >= 0 && S > 0 && H > 0 && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && I > 0);
+// One decoder layer as the prefill stacks see it: the element-type matrices of `srgpt_llama_layer_weights`, or the FP8 planes of
+// `srgpt_llama_layer_fp8` (w8 != NULL).
+struct LayerRef {
+  const void* in_norm;
+  const void* post_norm;
+  void* kv_pages;
+  const void* w[4];        // qkv, o, gateup, down
+  const srgpt_fp8* w8[4];  // the same, FP8; NULL for element-type layers
+};
+
+static LayerRef layer_ref(const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_fp8* layers8, int l) {
+  if (layers8 != nullptr) {
+    const srgpt_llama_layer_fp8& w = layers8[l];
+    return LayerRef{w.in_norm, w.post_norm, w.kv_pages, {nullptr, nullptr, nullptr, nullptr}, {&w.qkv, &w.o, &w.gateup, &w.down}};
+  }
+  const srgpt_llama_layer_weights& w = layers[l];
+  return LayerRef{w.in_norm, w.post_norm, w.kv_pages, {w.qkv_w, w.o_w, w.gateup_w, w.down_w}, {nullptr, nullptr, nullptr, nullptr}};
+}
+
+// y = epilogue(x [M, K] · W [N, K]^T): the element-type GEMM, or with w8 the activation quantizer (into q8 [M, K], s [M]) and the FP8 GEMM
+static int linear(const void* x, int ldx, const void* W, const srgpt_fp8* w8, void* q8, float* s, void* y, int ldy, int M, int N, int K,
+                  const void* residual, int ldr, int epilogue, void* stream) {
+  if (w8 == nullptr) return srgpt_gemm_bf16(x, ldx, W, K, y, ldy, M, N, K, nullptr, residual, ldr, 0, epilogue, 0, stream);
+  SRGPT_TRY(srgpt_fp8_quantize_act_bf16(x, ldx, M, K, q8, K, s, stream));
+  return srgpt_gemm_fp8_bf16(q8, K, s, w8->q, K, w8->scale, y, ldy, M, N, K, residual, ldr, epilogue, stream);
+}
+
+static int prefill_layers(void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_fp8* layers8, int n_layers, void* ws_h,
+                          void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_s, int S, int H, int n_heads, int n_kv_heads,
+                          int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_table,
+                          int page_size, int n_seqs, const int* cu_seqlens, int max_seqlen, int page_table_stride, void* stream) {
+  SRGPT_CHECK_ARG(x && (layers || layers8) && ws_h && ws_qkv && ws_attn && ws_act && n_layers >= 0 && S > 0 && H > 0 && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && I > 0);
+  SRGPT_CHECK_ARG(layers8 == nullptr || (ws_q8 && ws_s));
   const bool packed = cu_seqlens != nullptr;
   SRGPT_CHECK_ARG(packed ? (n_seqs >= 1 && max_seqlen >= 1 && max_seqlen <= S && page_table_stride > 0) : (n_seqs == 1));
   const int qd = n_heads * head_dim, kd = n_kv_heads * head_dim, nqkv = qd + 2 * kd;
   const float scale = 1.0f / sqrtf((float)head_dim);
   for (int l = 0; l < n_layers; ++l) {
-    const srgpt_llama_layer_weights& w = layers[l];
+    const LayerRef w = layer_ref(layers, layers8, l);
     SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.in_norm, ws_h, H, S, H, eps, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_h, H, w.qkv_w, H, ws_qkv, nqkv, S, nqkv, H, nullptr, nullptr, 0, 0, SRGPT_EPI_NONE, 0, stream));
+    SRGPT_TRY(linear(ws_h, H, w.w[0], w.w8[0], ws_q8, ws_s, ws_qkv, nqkv, S, nqkv, H, nullptr, 0, SRGPT_EPI_NONE, stream));
     if (packed) {
       SRGPT_TRY(srgpt_rope_kv_append_varlen_bf16(ws_qkv, S, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, start_pos, w.kv_pages, page_table, page_table_stride,
                                                  page_size, n_seqs, cu_seqlens, stream));
@@ -68,10 +95,54 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers
       SRGPT_TRY(srgpt_attention_prefill_bf16(ws_qkv, cptr(ws_qkv, (size_t)qd * 2), cptr(ws_qkv, (size_t)(qd + kd) * 2), ws_attn, nqkv, nqkv, qd, 1, S, n_heads,
                                              n_kv_heads, head_dim, scale, 1, stream));
     }
-    SRGPT_TRY(srgpt_gemm_bf16(ws_attn, qd, w.o_w, qd, x, H, S, H, qd, nullptr, x, H, 0, SRGPT_EPI_BIAS_RESIDUAL, 0, stream));
+    SRGPT_TRY(linear(ws_attn, qd, w.w[1], w.w8[1], ws_q8, ws_s, x, H, S, H, qd, x, H, SRGPT_EPI_BIAS_RESIDUAL, stream));
     SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.post_norm, ws_h, H, S, H, eps, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_h, H, w.gateup_w, H, ws_act, I, S, 2 * I, H, nullptr, nullptr, 0, 0, SRGPT_EPI_SWIGLU, 0, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_act, I, w.down_w, I, x, H, S, H, I, nullptr, x, H, 0, SRGPT_EPI_BIAS_RESIDUAL, 0, stream));
+    SRGPT_TRY(linear(ws_h, H, w.w[2], w.w8[2], ws_q8, ws_s, ws_act, I, S, 2 * I, H, nullptr, 0, SRGPT_EPI_SWIGLU, stream));
+    SRGPT_TRY(linear(ws_act, I, w.w[3], w.w8[3], ws_q8, ws_s, x, H, S, H, I, x, H, SRGPT_EPI_BIAS_RESIDUAL, stream));
+  }
+  return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers_bf16(void* x, const srgpt_llama_layer_weights* layers, int n_layers, void* ws_h, void* ws_qkv,
+                                                                                        void* ws_attn, void* ws_act, int S, int H, int n_heads, int n_kv_heads,
+                                                                                        int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab,
+                                                                                        const int* start_pos, const int* page_table, int page_size, int n_seqs, const int* cu_seqlens,
+                                                                                        int max_seqlen, int page_table_stride, void* stream) {
+  SRGPT_CHECK_ARG(layers != nullptr);
+  return prefill_layers(x, layers, nullptr, n_layers, ws_h, ws_qkv, ws_attn, ws_act, nullptr, nullptr, S, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab,
+                        sin_tab, start_pos, page_table, page_size, n_seqs, cu_seqlens, max_seqlen, page_table_stride, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers_fp8_bf16(
+    void* x, const srgpt_llama_layer_fp8* layers, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_scale, int S,
+    int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_table,
+    int page_size, int n_seqs, const int* cu_seqlens, int max_seqlen, int page_table_stride, void* stream) {
+  SRGPT_CHECK_ARG(layers != nullptr);
+  return prefill_layers(x, nullptr, layers, n_layers, ws_h, ws_qkv, ws_attn, ws_act, ws_q8, ws_scale, S, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab,
+                        sin_tab, start_pos, page_table, page_size, n_seqs, cu_seqlens, max_seqlen, page_table_stride, stream);
+}
+
+static int prefill_chunk_layers(void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_fp8* layers8, int n_layers, void* ws_h,
+                                void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_s, int S, int H, int n_heads, int n_kv_heads,
+                                int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables,
+                                int page_table_stride, int page_size, int n_pages, int n_seqs, const int* cu_seqlens, int max_rows, void* stream) {
+  SRGPT_CHECK_ARG(x && (layers || layers8) && ws_h && ws_qkv && ws_attn && ws_act && n_layers >= 0 && S > 0 && H > 0 && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && I > 0);
+  SRGPT_CHECK_ARG(layers8 == nullptr || (ws_q8 && ws_s));
+  SRGPT_CHECK_ARG(start_pos && page_tables && cu_seqlens && n_seqs >= 1 && max_rows >= 1 && max_rows <= S && page_table_stride > 0 && n_pages > 0);
+  const int qd = n_heads * head_dim, kd = n_kv_heads * head_dim, nqkv = qd + 2 * kd;
+  const float scale = 1.0f / sqrtf((float)head_dim);
+  for (int l = 0; l < n_layers; ++l) {
+    const LayerRef w = layer_ref(layers, layers8, l);
+    SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.in_norm, ws_h, H, S, H, eps, stream));
+    SRGPT_TRY(linear(ws_h, H, w.w[0], w.w8[0], ws_q8, ws_s, ws_qkv, nqkv, S, nqkv, H, nullptr, 0, SRGPT_EPI_NONE, stream));
+    SRGPT_TRY(srgpt_rope_kv_append_varlen_bf16(ws_qkv, S, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, start_pos, w.kv_pages, page_tables, page_table_stride,
+                                               page_size, n_seqs, cu_seqlens, stream));
+    SRGPT_TRY(srgpt_attention_prefill_paged_bf16(ws_qkv, nqkv, ws_attn, qd, w.kv_pages, n_pages, page_tables, page_table_stride, page_size, start_pos, cu_seqlens,
+                                                 n_seqs, max_rows, S, n_heads, n_kv_heads, head_dim, scale, stream));
+    SRGPT_TRY(linear(ws_attn, qd, w.w[1], w.w8[1], ws_q8, ws_s, x, H, S, H, qd, x, H, SRGPT_EPI_BIAS_RESIDUAL, stream));
+    SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.post_norm, ws_h, H, S, H, eps, stream));
+    SRGPT_TRY(linear(ws_h, H, w.w[2], w.w8[2], ws_q8, ws_s, ws_act, I, S, 2 * I, H, nullptr, 0, SRGPT_EPI_SWIGLU, stream));
+    SRGPT_TRY(linear(ws_act, I, w.w[3], w.w8[3], ws_q8, ws_s, x, H, S, H, I, x, H, SRGPT_EPI_BIAS_RESIDUAL, stream));
   }
   return SRGPT_OK;
 }
@@ -80,24 +151,18 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_chunk_
     void* x, const srgpt_llama_layer_weights* layers, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act, int S, int H, int n_heads,
     int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables,
     int page_table_stride, int page_size, int n_pages, int n_seqs, const int* cu_seqlens, int max_rows, void* stream) {
-  SRGPT_CHECK_ARG(x && layers && ws_h && ws_qkv && ws_attn && ws_act && n_layers >= 0 && S > 0 && H > 0 && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && I > 0);
-  SRGPT_CHECK_ARG(start_pos && page_tables && cu_seqlens && n_seqs >= 1 && max_rows >= 1 && max_rows <= S && page_table_stride > 0 && n_pages > 0);
-  const int qd = n_heads * head_dim, kd = n_kv_heads * head_dim, nqkv = qd + 2 * kd;
-  const float scale = 1.0f / sqrtf((float)head_dim);
-  for (int l = 0; l < n_layers; ++l) {
-    const srgpt_llama_layer_weights& w = layers[l];
-    SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.in_norm, ws_h, H, S, H, eps, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_h, H, w.qkv_w, H, ws_qkv, nqkv, S, nqkv, H, nullptr, nullptr, 0, 0, SRGPT_EPI_NONE, 0, stream));
-    SRGPT_TRY(srgpt_rope_kv_append_varlen_bf16(ws_qkv, S, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, start_pos, w.kv_pages, page_tables, page_table_stride,
-                                               page_size, n_seqs, cu_seqlens, stream));
-    SRGPT_TRY(srgpt_attention_prefill_paged_bf16(ws_qkv, nqkv, ws_attn, qd, w.kv_pages, n_pages, page_tables, page_table_stride, page_size, start_pos, cu_seqlens,
-                                                 n_seqs, max_rows, S, n_heads, n_kv_heads, head_dim, scale, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_attn, qd, w.o_w, qd, x, H, S, H, qd, nullptr, x, H, 0, SRGPT_EPI_BIAS_RESIDUAL, 0, stream));
-    SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.post_norm, ws_h, H, S, H, eps, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_h, H, w.gateup_w, H, ws_act, I, S, 2 * I, H, nullptr, nullptr, 0, 0, SRGPT_EPI_SWIGLU, 0, stream));
-    SRGPT_TRY(srgpt_gemm_bf16(ws_act, I, w.down_w, I, x, H, S, H, I, nullptr, x, H, 0, SRGPT_EPI_BIAS_RESIDUAL, 0, stream));
-  }
-  return SRGPT_OK;
+  SRGPT_CHECK_ARG(layers != nullptr);
+  return prefill_chunk_layers(x, layers, nullptr, n_layers, ws_h, ws_qkv, ws_attn, ws_act, nullptr, nullptr, S, H, n_heads, n_kv_heads, head_dim, I, eps,
+                              cos_tab, sin_tab, start_pos, page_tables, page_table_stride, page_size, n_pages, n_seqs, cu_seqlens, max_rows, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_chunk_layers_fp8_bf16(
+    void* x, const srgpt_llama_layer_fp8* layers, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_scale, int S,
+    int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
+    const int* page_tables, int page_table_stride, int page_size, int n_pages, int n_seqs, const int* cu_seqlens, int max_rows, void* stream) {
+  SRGPT_CHECK_ARG(layers != nullptr);
+  return prefill_chunk_layers(x, nullptr, layers, n_layers, ws_h, ws_qkv, ws_attn, ws_act, ws_q8, ws_scale, S, H, n_heads, n_kv_heads, head_dim, I, eps,
+                              cos_tab, sin_tab, start_pos, page_tables, page_table_stride, page_size, n_pages, n_seqs, cu_seqlens, max_rows, stream);
 }
 
 // one decode GEMV over the NF4 planes when there are some (nf->q != NULL), else over the packed matrix when there is one (pk->sm != NULL),
@@ -170,6 +235,31 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_nf
   SRGPT_CHECK_ARG(nf4 != nullptr);
   return decode_step(h, layers, nullptr, nf4, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
                      page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_fp8_bf16(
+    void* h, const srgpt_llama_layer_fp8* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads,
+    int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size, const void* final_norm,
+    const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids,
+    int* step, void* stream) {
+  SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos && page_table && final_norm && lm_head && lm_workspace && out_ids && step);
+  const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
+  const float scale = 1.0f / sqrtf((float)head_dim);
+  for (int l = 0; l < n_layers; ++l) {
+    const srgpt_llama_layer_fp8& w = layers[l];
+    SRGPT_TRY(srgpt_gemv_fp8_bf16(h, &w.qkv, q_buf, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim, cos_tab,
+                                  sin_tab, pos, w.kv_pages, page_table, page_size, stream));
+    SRGPT_TRY(srgpt_attention_decode_bf16(q_buf, attn_buf, w.kv_pages, page_table, page_size, pos, n_heads, n_kv_heads, head_dim, scale, stream));
+    SRGPT_TRY(srgpt_gemv_fp8_bf16(attn_buf, &w.o, h, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  0, stream));
+    SRGPT_TRY(srgpt_gemv_fp8_bf16(h, &w.gateup, act_buf, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, 0, 0, 0, nullptr, nullptr,
+                                  nullptr, nullptr, nullptr, 0, stream));
+    SRGPT_TRY(srgpt_gemv_fp8_bf16(act_buf, &w.down, h, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  0, stream));
+  }
+  if (lm_packed != nullptr && lm_packed->sm != nullptr)
+    return srgpt_lm_head_argmax_packed_bf16(h, lm_packed, V, H, final_norm, eps, logits_out, lm_workspace, embed_table, h, out_ids, step, pos, stream);
+  return srgpt_lm_head_argmax_bf16(h, lm_head, H, V, H, final_norm, eps, logits_out, lm_workspace, embed_table, h, out_ids, step, pos, stream);
 }
 
 // ---- verify pass of prompt-lookup speculative decoding: T tokens through the layer stack, every weight streamed once -----------

@@ -90,14 +90,18 @@ inline EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 // 0 on success, -1 without the driver entry point, else the CUresult
-inline int encode_tmap_bf16(CUtensorMap* tm, const void* ptr, int ndim, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
-                            CUtensorMapSwizzle swizzle) {
+inline int encode_tmap(CUtensorMap* tm, CUtensorMapDataType dtype, const void* ptr, int ndim, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+                       const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (fn == nullptr) return -1;
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(tm, SRGPT_TMAP_DTYPE, (cuuint32_t)ndim, const_cast<void*>(ptr), dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = fn(tm, dtype, (cuuint32_t)ndim, const_cast<void*>(ptr), dims, strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+inline int encode_tmap_bf16(CUtensorMap* tm, const void* ptr, int ndim, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
+                            CUtensorMapSwizzle swizzle) {
+  return encode_tmap(tm, SRGPT_TMAP_DTYPE, ptr, ndim, dims, strides_bytes, box, swizzle);
 }
 
 }  // namespace tma

@@ -191,7 +191,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--dataset", type=str, default="lvis")
     p.add_argument("--prompt_type", type=str, default="seg")
     p.add_argument("--seed", type=int, default=None, help="seed of the prompt choice (the reference draws unseeded)")
-    p.add_argument("--quantization", choices=["nf4"], default=None, help="NF4 weight-only quantization of the LLM's layer matrices")
+    p.add_argument("--quantization", choices=["nf4", "fp8"], default=None,
+                   help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
     return p
 
 

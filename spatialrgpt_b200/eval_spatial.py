@@ -257,7 +257,7 @@ def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tens
         from .builder import load_pretrained_model as loader
     model_path = os.path.expanduser(args.model_path)
     model_name = get_model_name_from_path(model_path)
-    # --quantization nf4 dequantizes into the compute dtype at load, so the model is loaded in bf16 instead of cast to it
+    # --quantization quantizes from (and computes in) the element type it is loaded in, so the model is loaded in bf16 instead of cast to it
     quant = {"quantization": args.quantization, "torch_dtype": torch.bfloat16} if getattr(args, "quantization", None) else {}
     tokenizer, model, image_processor, _ = loader(model_path, model_name, getattr(args, "model_base", None), **quant)
     model.to(dtype=torch.bfloat16)  # eval_spatial.py:221: the loader returns fp16, this script computes in bf16
@@ -316,7 +316,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--prompt-lookup-num-tokens", type=int, default=0,
                    help="greedy decoding by prompt lookup: draft up to this many tokens per verify pass (0 = off; same answers)")
     p.add_argument("--allow-no-depth", action="store_true", help="run an enable_depth checkpoint without a depth network (degraded answers)")
-    p.add_argument("--quantization", choices=["nf4"], default=None, help="NF4 weight-only quantization of the LLM's layer matrices")
+    p.add_argument("--quantization", choices=["nf4", "fp8"], default=None,
+                   help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
     return p
 
 

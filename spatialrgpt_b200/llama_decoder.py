@@ -130,13 +130,21 @@ class LlamaDecoder:
         self.act_buf = torch.zeros(I, dtype=self.dtype, device=dev)
         self.lm_ws = ops.lm_head_workspace(dims.vocab_size, dev)
         self.scale = hd ** -0.5
-        self._layer_array = ops.make_llama_layer_array(w.layers, [self.cache.layer(l) for l in range(dims.num_hidden_layers)])
+        # quantization="fp8" (weights.from_state_dicts): the layers hold only E4M3 codes and row scales; prefill, batched decode and beams
+        # run their linears as the activation quantizer + an FP8 GEMM, the one-token step streams the codes through the FP8 GEMV (DESIGN.md
+        # §3).  The verify pass of prompt-lookup decoding has no FP8 form.
+        self.fp8 = getattr(w, "quantization", None) == "fp8"
+        if self.fp8:
+            self.supports_prompt_lookup = False
+        self._layer_array = self._make_layer_array()
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
         # ("verify", T, ngram), ("batch", B, proc) and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
         # dropped whenever one of them is replaced: the KV cache and layer array (ensure_capacity), the processor spec (_set_processors)
         # and the batched-decode buffers (_batch_state).
         self._graphs = {}
         self.kernels_per_decode_step = 5 * dims.num_hidden_layers + 2
+        # batched decode step: 8 kernels per layer, 12 with the FP8 activation quantizers
+        self._batch_kernels_per_layer = 12 if self.fp8 else 8
         # sampling mode (do_sample=True): temperature / top_p live in device memory so one captured graph serves any setting
         self.sample_params = torch.tensor([1.0, 1.0, 0.0], dtype=torch.float32, device=dev)
         self.sample_logits: Optional[torch.Tensor] = None
@@ -162,7 +170,9 @@ class LlamaDecoder:
         # and the batch-1 decode step streams the NF4 planes instead (bit-identical).  decode_quant: matrix -> "nf4" or why the step reads
         # its dequantized copy.  SRGPT_DECODE_NF4=0 runs the usual step over the dequantized copies.
         self.decode_quant = {}
-        if getattr(w, "quantization", None) == "nf4" and os.environ.get("SRGPT_DECODE_NF4", "1") != "0":
+        if self.fp8:
+            self._fp8_decode_weights()
+        elif getattr(w, "quantization", None) == "nf4" and os.environ.get("SRGPT_DECODE_NF4", "1") != "0":
             self._nf4_decode_weights()
         elif self.packs_decode_weights and self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
             self._pack_decode_weights()
@@ -179,6 +189,22 @@ class LlamaDecoder:
     _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
     _lm_packed = None
     _nf4_array = None  # srgpt_llama_layer_nf4[] of the decode step
+
+    def _make_layer_array(self):
+        """The layer descriptors of the prefill stacks and the decode step over the current KV cache."""
+        pages = [self.cache.layer(l) for l in range(self.dims.num_hidden_layers)]
+        return ops.make_llama_fp8_array(self.w.layers, pages) if self.fp8 else ops.make_llama_layer_array(self.w.layers, pages)
+
+    @ops.in_own_dtype
+    def _fp8_decode_weights(self) -> None:
+        """The FP8 step streams every layer matrix through the FP8 GEMV; lm_head stays unquantized and is packed in the bf16 build
+        (SRGPT_DECODE_PACK=0: plain)."""
+        for l in range(self.dims.num_hidden_layers):
+            for name in ("qkv", "o", "gateup", "down"):
+                self.decode_quant[f"layers.{l}.{name}"] = "fp8"
+        if self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
+            self._lm_packed, why = ops.pack12(self.w.lm_head)
+            self.decode_pack["lm_head"] = why or "packed"
 
     @ops.in_own_dtype
     def _nf4_decode_weights(self) -> None:
@@ -233,7 +259,7 @@ class LlamaDecoder:
         self.cache = None
         del c
         self.cache = PagedKVCache(d, max(need_pages, n_pages_old), max(n_seqs, n_seqs_old), (self.max_seq_len + PAGE_SIZE - 1) // PAGE_SIZE, self.device, self.dtype)
-        self._layer_array = ops.make_llama_layer_array(self.w.layers, [self.cache.layer(l) for l in range(d.num_hidden_layers)])
+        self._layer_array = self._make_layer_array()
 
     @ops.in_own_dtype
     def embed_tokens(self, ids: torch.Tensor) -> torch.Tensor:
@@ -311,7 +337,11 @@ class LlamaDecoder:
         d, w = self.dims, self.w
         if (sample or proc) and logits_out is None:
             logits_out = self._sample_buffer()
-        if self._nf4_array is not None:
+        if self.fp8:
+            ops.llama_decode_step_fp8(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos, self.sin,
+                                      self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed, self.lm_ws, self.out_ids,
+                                      self.step, logits_out)
+        elif self._nf4_array is not None:
             ops.llama_decode_step_nf4(self.h, self._layer_array, self._nf4_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
                                       d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
                                       self.lm_ws, self.out_ids, self.step, logits_out)
@@ -484,6 +514,8 @@ class LlamaDecoder:
             raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
         if S + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
+        if lookup_k and self.fp8:
+            raise NotImplementedError("prompt-lookup decoding (prompt_lookup_num_tokens) has no FP8 verify pass; decode FP8 weights without it")
         eos = eos_list(eos_token_ids)
         k = min(int(lookup_k), ops.SPEC_T_MAX - 1) if lookup_k else 0
         self.last_speculation = (0, 0, 0)
@@ -645,6 +677,8 @@ class LlamaDecoder:
                   logits=z(B, (V + 7) // 8 * 8), pos=z(B, dtype=torch.int32), step=z(1, dtype=torch.int32), ids=z(B, dtype=torch.int64),
                   out=z(self.out_ids.numel() * B, dtype=torch.int64), ticket=z(1, dtype=torch.int32),
                   cu=torch.arange(B + 1, dtype=torch.int32, device=dev))
+        if self.fp8:  # the activation quantizer's codes and row scales
+            st.update(q8=z(B, max(H, nh * hd, I), dtype=torch.uint8), s8=z(B, dtype=torch.float32))
         self._bstate = st
         return st
 
@@ -656,16 +690,21 @@ class LlamaDecoder:
         qd = nh * hd
         h, xn, qkv, attn, act = st["h"], st["xn"], st["qkv"], st["attn"], st["act"]
         pts = self.cache.page_tables
+        if self.fp8:  # every linear as the activation quantizer + the FP8 GEMM
+            def linear(x, wt, **kw):
+                return ops.linear_fp8(x, wt, q=st["q8"][:, :x.shape[1]], scale=st["s8"], **kw)
+        else:
+            linear = ops.gemm
         for l, lw in enumerate(w.layers):
             pages = self.cache.layer(l)
             ops.rmsnorm(h, lw.in_norm, d.rms_norm_eps, out=xn)
-            ops.gemm(xn, lw.qkv_w, out=qkv)
+            linear(xn, lw.qkv_w, out=qkv)
             ops.rope_kv_append_varlen(qkv, nh, nkv, hd, self.cos, self.sin, st["pos"], pages, pts, PAGE_SIZE, st["cu"])
             ops.attention_decode_batched(qkv[:, :qd], attn, pages, pts, PAGE_SIZE, st["pos"], nh, nkv, hd, self.scale)
-            ops.gemm(attn, lw.o_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
+            linear(attn, lw.o_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
             ops.rmsnorm(h, lw.post_norm, d.rms_norm_eps, out=xn)
-            ops.gemm(xn, lw.gateup_w, epilogue=ops.EPI_SWIGLU, out=act)
-            ops.gemm(act, lw.down_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
+            linear(xn, lw.gateup_w, epilogue=ops.EPI_SWIGLU, out=act)
+            linear(act, lw.down_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
         ops.rmsnorm(h, w.norm, d.rms_norm_eps, out=xn)
         lg = st["logits"][:, :V]
         ops.gemm(xn, w.lm_head, out=lg)  # bf16 logits (modeling_llama.py:1044), arg max with the lowest index on ties
@@ -690,7 +729,7 @@ class LlamaDecoder:
         key = ("batch", B, proc)
         if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max
             self._capture(key, lambda: self._batch_step_launch(st, proc=proc), (st["h"], st["pos"], st["step"], st["out"]),
-                          8 * self.dims.num_hidden_layers + (5 if proc else 4))
+                          self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4))
         need_check = bool(eos) or stopping_fn is not None
         out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
         if need_check:
@@ -813,7 +852,7 @@ class LlamaDecoder:
             st["pos"].fill_(S + step)
             d_scores.copy_(beam_scores, non_blocking=True)
             if use_graph:  # the warm-up before the capture rewrites only this step's own KV rows
-                self._capture(("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), 8 * d.num_hidden_layers + 2)
+                self._capture(("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), self._batch_kernels_per_layer * d.num_hidden_layers + 2)
                 self._replay(("beam", k))
             else:
                 self._batch_step_launch(st, logits_only=True)

@@ -453,6 +453,8 @@ class LlavaLlamaModel:
                 raise NotImplementedError("prompt_lookup_num_tokens with do_sample=True (speculative sampling would change the random stream)")
             if num_beams != 1:
                 raise NotImplementedError("prompt_lookup_num_tokens with beam search")
+            if getattr(self.llm, "fp8", False):
+                raise NotImplementedError("prompt_lookup_num_tokens with quantization='fp8' (the verify pass has no FP8 form)")
             if not getattr(self.llm, "supports_prompt_lookup", False):
                 raise NotImplementedError("prompt_lookup_num_tokens on the tensor-parallel decoder")
         prefix = None

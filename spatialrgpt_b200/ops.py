@@ -574,6 +574,95 @@ def gemv_nf4(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch.Te
     return y
 
 
+# ---- FP8 (E4M3) W8A8 quantization of the decoder-layer linears (fp8.cu, gemm_wgmma.cu; DESIGN.md §3) ------------------------------
+FP8_K_MULTIPLE = 16  # in_features must be a multiple (16-byte rows for TMA)
+
+
+def fp8_quantize_weight(w: torch.Tensor, name: str = "matrix"):
+    """Per-row E4M3 codes of an element-type matrix [N, K]: (q [N, K] uint8, scale [N] fp32), include/srgpt_b200.h's definition.  Raises
+    NotImplementedError for K % 16 != 0 and SrgptError when w holds Inf or NaN; `name` names the matrix in both."""
+    N, K = w.shape
+    if K % FP8_K_MULTIPLE:
+        raise NotImplementedError(f"FP8 quantization needs in_features to be a multiple of {FP8_K_MULTIPLE}; {name} has {K}")
+    _need(w, ELEM(), "fp8_quantize_weight.w")
+    ldw = _rowmajor2d(w, "fp8_quantize_weight.w")
+    q = torch.empty((N, K), dtype=torch.uint8, device=w.device)
+    scale = torch.empty(N, dtype=torch.float32, device=w.device)
+    n_bad = torch.zeros(1, dtype=torch.int32, device=w.device)
+    check(_lib.load().srgpt_fp8_quantize_weight_bf16(_p(w), ldw, N, K, _p(q), _p(scale), _p(n_bad), _stream()), "srgpt_fp8_quantize_weight_bf16")
+    if int(n_bad[0]):
+        raise SrgptError(f"fp8_quantize_weight: {name} {list(w.shape)} holds Inf or NaN in {int(n_bad[0])} rows")
+    return q, scale
+
+
+def fp8_quantize_act(x: torch.Tensor, q: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None):
+    """The activation quantizer: per-row E4M3 codes of x [M, K] -> (q [M, K] uint8, scale [M] fp32), the weights' definition."""
+    _need(x, ELEM(), "fp8_quantize_act.x")
+    ldx = _rowmajor2d(x, "fp8_quantize_act.x")
+    M, K = x.shape
+    q = torch.empty((M, K), dtype=torch.uint8, device=x.device) if q is None else q
+    scale = torch.empty(M, dtype=torch.float32, device=x.device) if scale is None else scale
+    _need(q, torch.uint8, "fp8_quantize_act.q"); _need(scale, torch.float32, "fp8_quantize_act.scale")
+    if q.shape != (M, K) or scale.numel() < M:
+        raise SrgptError(f"fp8_quantize_act: q {tuple(q.shape)} / scale {tuple(scale.shape)} do not fit x {(M, K)}")
+    check(_lib.load().srgpt_fp8_quantize_act_bf16(_p(x), ldx, M, K, _p(q), _rowmajor2d(q, "fp8_quantize_act.q"), _p(scale), _stream()),
+          "srgpt_fp8_quantize_act_bf16")
+    return q, scale
+
+
+def gemm_fp8(q: torch.Tensor, sx: torch.Tensor, w, residual: Optional[torch.Tensor] = None, epilogue: int = EPI_NONE,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[M, N] = epilogue(acc * (sx[m] * w.scale[n])) with acc = q [M, K] · w.q [N, K]^T over E4M3 codes (an Fp8W), on the FP8 tensor
+    cores.  Epilogues: EPI_NONE, EPI_BIAS_RESIDUAL (no bias), EPI_SWIGLU."""
+    _need(q, torch.uint8, "gemm_fp8.q"); _need(sx, torch.float32, "gemm_fp8.sx")
+    _ensure_gemm_workspace(q.device)
+    lda, ldw = _rowmajor2d(q, "gemm_fp8.q"), _rowmajor2d(w.q, "gemm_fp8.w")
+    M, K = q.shape
+    N, K2 = w.q.shape
+    if K != K2:
+        raise SrgptError(f"gemm_fp8: K mismatch {K} vs {K2}")
+    n_out = N // 2 if epilogue == EPI_SWIGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=ELEM(), device=q.device)
+    _need(out, ELEM(), "gemm_fp8.out")
+    if out.shape != (M, n_out):
+        raise SrgptError(f"gemm_fp8.out: expected {(M, n_out)}, got {tuple(out.shape)}")
+    ldr = 0
+    if residual is not None:
+        _need(residual, ELEM(), "gemm_fp8.residual")
+        ldr = _rowmajor2d(residual, "gemm_fp8.residual")
+    check(_lib.load().srgpt_gemm_fp8_bf16(_p(q), lda, _p(sx), _p(w.q), ldw, _p(w.scale), _p(out), _rowmajor2d(out, "gemm_fp8.out"), M, N, K,
+                                          _p(residual), ldr, epilogue, _stream()), "srgpt_gemm_fp8_bf16")
+    return out
+
+
+def linear_fp8(x: torch.Tensor, w, residual: Optional[torch.Tensor] = None, epilogue: int = EPI_NONE, out: Optional[torch.Tensor] = None,
+               q: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """A W8A8 linear over the element-type activation x [M, K]: the activation quantizer (into q / scale when given), then gemm_fp8."""
+    q, scale = fp8_quantize_act(x, q, scale)
+    return gemm_fp8(q, scale, w, residual=residual, epilogue=epilogue, out=out)
+
+
+def gemv_fp8(x: torch.Tensor, w, y: torch.Tensor, norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0,
+             residual: Optional[torch.Tensor] = None, mode: int = GEMV_PLAIN, n_heads: int = 0, n_kv_heads: int = 0,
+             head_dim: int = 0, cos_tab=None, sin_tab=None, pos=None, kv_pages=None, page_table=None, page_size: int = 0) -> torch.Tensor:
+    """gemv() over an Fp8W: x (RMS-normalised first with norm_weight) quantized in the kernel by the activation definition, the W8A8
+    linear of fp8_quantize_act + gemm_fp8 at M = 1 with the one-token GEMV's modes and rounding points; 1 byte of weight stream per element."""
+    _need(x, ELEM(), "gemv_fp8.x"); _need(y, ELEM(), "gemv_fp8.y")
+    N, K = w.q.shape
+    d = _fp8_desc(w)
+    check(_lib.load().srgpt_gemv_fp8_bf16(_p(x), C.byref(d), _p(y), N, K, _p(norm_weight), eps, _p(residual), mode, n_heads, n_kv_heads, head_dim,
+                                          _p(cos_tab), _p(sin_tab), _p(pos), _p(kv_pages), _p(page_table), page_size, _stream()),
+          "srgpt_gemv_fp8_bf16")
+    return y
+
+
+def _fp8_desc(p) -> "_lib.Fp8":
+    d = _lib.Fp8()
+    d.q, d.scale = p.q.data_ptr(), p.scale.data_ptr()
+    return d
+
+
 # ---- host preprocessing on the GPU (preprocess.py) ---------------------------------------------------------------
 def resample_u8(img: torch.Tensor, axis: int, out_size: int, kk: torch.Tensor, bounds: torch.Tensor, ksize: int) -> torch.Tensor:
     _need(img, torch.uint8, "resample_u8.img"); _need(kk, torch.int32, "resample_u8.kk"); _need(bounds, torch.int32, "resample_u8.bounds")
@@ -844,6 +933,17 @@ def make_llama_nf4_array(nf4_layers):
     return arr
 
 
+def make_llama_fp8_array(layers, kv_pages_per_layer):
+    """ctypes array of srgpt_llama_layer_fp8 over FP8 LlamaLayerW (their *_w fields hold Fp8W)."""
+    arr = (_lib.LlamaLayerFp8 * len(layers))()
+    for i, lw in enumerate(layers):
+        arr[i].in_norm, arr[i].post_norm = lw.in_norm.data_ptr(), lw.post_norm.data_ptr()
+        for name in ("qkv", "o", "gateup", "down"):
+            setattr(arr[i], name, _fp8_desc(getattr(lw, name + "_w")))
+        arr[i].kv_pages = kv_pages_per_layer[i].data_ptr()
+    return arr
+
+
 def clip_embed(patch_embeds: torch.Tensor, class_embedding: torch.Tensor, position_embedding: torch.Tensor, n_img: int, T: int) -> torch.Tensor:
     """[n_img*T, D] patch embeddings -> [n_img*(T+1), D]: class token prepended, position embedding added (CLIPVisionEmbeddings)."""
     _need(patch_embeds, ELEM(), "clip_embed.patch_embeds")
@@ -874,6 +974,16 @@ def siglip_layers(x: torch.Tensor, layer_array, n_layers: int, n_img: int, T: in
     return x
 
 
+def _is_fp8_array(layer_array) -> bool:
+    return getattr(layer_array, "_type_", None) is _lib.LlamaLayerFp8
+
+
+def _fp8_workspaces(S: int, dims, dev):
+    """The activation quantizer's codes [S, max(H, nh hd, I)] and scales [S] of the FP8 layer stacks."""
+    K = max(dims.hidden_size, dims.num_attention_heads * dims.head_dim, dims.intermediate_size)
+    return torch.empty(S * K, dtype=torch.uint8, device=dev), torch.empty(S, dtype=torch.float32, device=dev)
+
+
 def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_table, page_size: int,
                          cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0) -> torch.Tensor:
     """All decoder layers over the prompt rows x [S, H] in place (K/V appended to the paged cache).  One prompt
@@ -896,6 +1006,14 @@ def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos,
     ws_attn = torch.empty((S, nh * hd), dtype=ELEM(), device=dev)
     ws_act = torch.empty((S, I), dtype=ELEM(), device=dev)
     import ctypes
+    if _is_fp8_array(layer_array):
+        ws_q8, ws_s = _fp8_workspaces(S, dims, dev)
+        check(_lib.load().srgpt_llama_prefill_layers_fp8_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
+                                                              _p(ws_attn), _p(ws_act), _p(ws_q8), _p(ws_s), S, H, nh, nkv, hd, I, dims.rms_norm_eps,
+                                                              _p(cos), _p(sin), _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens),
+                                                              max_seqlen, pt_stride, _stream()), "srgpt_llama_prefill_layers_fp8_bf16")
+        _count(12 * n_layers)
+        return x
     check(_lib.load().srgpt_llama_prefill_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
                                                       _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
                                                       _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride,
@@ -922,6 +1040,15 @@ def llama_prefill_chunk_layers(x: torch.Tensor, layer_array, n_layers: int, dims
     ws_attn = torch.empty((S, nh * hd), dtype=ELEM(), device=dev)
     ws_act = torch.empty((S, I), dtype=ELEM(), device=dev)
     import ctypes
+    if _is_fp8_array(layer_array):
+        ws_q8, ws_s = _fp8_workspaces(S, dims, dev)
+        check(_lib.load().srgpt_llama_prefill_chunk_layers_fp8_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
+                                                                    _p(ws_attn), _p(ws_act), _p(ws_q8), _p(ws_s), S, H, nh, nkv, hd, I,
+                                                                    dims.rms_norm_eps, _p(cos), _p(sin), _p(start_pos), _p(page_tables),
+                                                                    page_tables.stride(0), page_size, n_pages, n_seqs, _p(cu_seqlens), max_rows,
+                                                                    _stream()), "srgpt_llama_prefill_chunk_layers_fp8_bf16")
+        _count(12 * n_layers)
+        return x
     check(_lib.load().srgpt_llama_prefill_chunk_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
                                                             _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
                                                             _p(start_pos), _p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs,
@@ -966,6 +1093,20 @@ def llama_decode_step_nf4(h, layer_array, nf4_array, n_layers: int, q_buf, attn_
                                                        _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
                                                        C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
                                                        _stream()), "srgpt_llama_decode_step_nf4_bf16")
+    _count(5 * n_layers + 2)
+
+
+def llama_decode_step_fp8(h, fp8_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table, page_size: int,
+                          final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
+    """llama_decode_step() over FP8 layers (make_llama_fp8_array): every layer matrix streamed by the FP8 GEMV (gemv_fp8), lm_head from
+    ``lm_packed`` (a Packed12W or None) or lm_head."""
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    lm_d = _packed_desc(lm_packed)
+    check(_lib.load().srgpt_llama_decode_step_fp8_bf16(_p(h), C.cast(fp8_array, C.c_void_p), n_layers, _p(q_buf), _p(attn_buf), _p(act_buf),
+                                                       dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos),
+                                                       _p(page_table), page_size, _p(final_norm), _p(lm_head), C.byref(lm_d), dims.vocab_size,
+                                                       _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), _stream()),
+          "srgpt_llama_decode_step_fp8_bf16")
     _count(5 * n_layers + 2)
 
 

@@ -98,7 +98,8 @@ class LlamaLayerW:
     gateup_w: torch.Tensor  # [2 I, H], rows interleaved (gate_i, up_i)
     down_w: torch.Tensor  # [H, I]
     # quantization="nf4": {"qkv", "o", "gateup", "down"} -> the fused matrix's Nf4W planes, or None where K is not a multiple of 1024
-    # (the *_w tensors above are then the dequantized matrices)
+    # (the *_w tensors above are then the dequantized matrices).  quantization="fp8": the *_w fields hold Fp8W and there is no
+    # element-type copy of the matrices.
     nf4: Optional[Dict[str, Optional["Nf4W"]]] = None
 
 
@@ -108,7 +109,7 @@ class LlamaW:
     norm: torch.Tensor
     lm_head: torch.Tensor  # [V, H]
     layers: List[LlamaLayerW] = field(default_factory=list)
-    quantization: Optional[str] = None  # None or "nf4" (the decoder-layer linears only)
+    quantization: Optional[str] = None  # None, "nf4" or "fp8" (the decoder-layer linears only)
 
 
 @dataclass
@@ -136,6 +137,21 @@ class Nf4W:
     uint8 codes in the GEMV's lane order, scale [N, K/64] fp32 resolved scales.  Built by ops.nf4_planes."""
     q: torch.Tensor
     scale: torch.Tensor
+
+    def nbytes(self) -> int:
+        return self.q.numel() + self.scale.numel() * 4
+
+
+@dataclass
+class Fp8W:
+    """An FP8 (E4M3) weight [N, K] of the W8A8 decoder-layer linears (DESIGN.md §3, include/srgpt_b200.h srgpt_fp8): q [N, K] uint8 codes,
+    scale [N] fp32 row scales; the weight stands for q * scale.  Built by ops.fp8_quantize_weight."""
+    q: torch.Tensor
+    scale: torch.Tensor
+
+    @property
+    def shape(self):
+        return self.q.shape
 
     def nbytes(self) -> int:
         return self.q.numel() + self.scale.numel() * 4
@@ -209,9 +225,13 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
     ``quantization="nf4"``: every decoder-layer linear (q/k/v/o/gate/up/down_proj) is NF4-quantized on the device as its own [out, in]
     matrix, before qkv is fused and gate/up interleaved (the reference's load_4bit, llava/model/builder.py:51-60); the layer keeps the
     dequantized matrices for every path and the NF4 planes for the batch-1 decode step.  Embeddings, lm_head, norms, towers, projector
-    and region extractor stay unquantized."""
-    if quantization not in (None, "nf4"):
-        raise ValueError(f"quantization={quantization!r}: supported are None and 'nf4'")
+    and region extractor stay unquantized.
+    ``quantization="fp8"``: W8A8 with E4M3 codes (DESIGN.md §3): every decoder-layer linear is quantized on the device per output row, one
+    matrix at a time, and the layer holds only the codes and row scales; every path (prefill, batched decode, beams, the one-token step)
+    quantizes each activation row the same way before the FP8 GEMM.  Embeddings, lm_head, norms, towers, projector and region extractor
+    stay unquantized."""
+    if quantization not in (None, "nf4", "fp8"):
+        raise ValueError(f"quantization={quantization!r}: supported are None, 'nf4' and 'fp8'")
     dev = torch.device(device)
 
     def g(d, k):
@@ -282,6 +302,9 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
         if quantization == "nf4":
             llama.layers.append(_nf4_layer(l, p, g, dtype))
             continue
+        if quantization == "fp8":
+            llama.layers.append(_fp8_layer(l, p, g, dtype))
+            continue
         llama.layers.append(LlamaLayerW(
             in_norm=g(l, p + "input_layernorm.weight"),
             qkv_w=torch.cat([g(l, p + f"self_attn.{n}.weight") for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous(),
@@ -312,6 +335,29 @@ def _nf4_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> Lla
         planes = {name: ops.nf4_planes(*f)[0] for name, f in fused.items()}
     return LlamaLayerW(in_norm=g(l, p + "input_layernorm.weight"), qkv_w=fused["qkv"][2], o_w=fused["o"][2],
                        post_norm=g(l, p + "post_attention_layernorm.weight"), gateup_w=fused["gateup"][2], down_w=fused["down"][2], nf4=planes)
+
+
+def _fp8_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> LlamaLayerW:
+    """One decoder layer with FP8 linears.  The scales are per output row, so each original matrix is quantized on its own (only one
+    element-type matrix is on the device at a time) and the codes and scales are fused as the plain layer's weights are (q/k/v rows
+    concatenated, gate/up rows interleaved)."""
+    from . import ops
+    with ops.elem_dtype(dtype):
+        quant = {}
+        for n in ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj"):
+            key = p + ("self_attn." if n.endswith(("q_proj", "k_proj", "v_proj", "o_proj")) else "mlp.") + n + ".weight"
+            quant[n] = ops.fp8_quantize_weight(g(l, key).contiguous(), name=key)
+        fused = {
+            "qkv": [torch.cat([quant[n][k] for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous() for k in range(2)],
+            "o": list(quant["o_proj"]),
+            "gateup": [interleave_rows(quant["gate_proj"][0], quant["up_proj"][0]),
+                       torch.stack((quant["gate_proj"][1], quant["up_proj"][1]), 1).reshape(-1).contiguous()],
+            "down": list(quant["down_proj"]),
+        }
+        del quant
+    w = {name: Fp8W(q=f[0], scale=f[1]) for name, f in fused.items()}
+    return LlamaLayerW(in_norm=g(l, p + "input_layernorm.weight"), qkv_w=w["qkv"], o_w=w["o"], post_norm=g(l, p + "post_attention_layernorm.weight"),
+                       gateup_w=w["gateup"], down_w=w["down"])
 
 
 def random_init(cfg: LlavaConfig, device, seed: int = 0, std: float = 0.02, n_tower_layers: Optional[int] = None,
