@@ -258,6 +258,12 @@ int srgpt_nf4_unpack_bf16(const srgpt_nf4* nf4, int N, int K, void* W, int ldw, 
 int srgpt_gemv_nf4_bf16(const void* x, const srgpt_nf4* nf4, void* y, int N, int K, const void* norm_weight, float eps, const void* residual,
                         int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos,
                         void* kv_pages, const int* page_table, int page_size, void* stream);
+/* srgpt_gemm_bf16 (epilogue SRGPT_EPI_NONE, SRGPT_EPI_BIAS_RESIDUAL without bias, or SRGPT_EPI_SWIGLU) with the weight W [N, K] read from
+ * the decode GEMV's NF4 planes `w` (a host pointer; K a multiple of 1024): the producer warpgroup dequantizes each B tile into shared
+ * memory.  Tiles, tile order, stream-K and its workspace are chosen as for a 16-bit [N, K] matrix, so the result is bit-identical to
+ * srgpt_gemm_bf16 over the dequantized matrix. */
+int srgpt_gemm_nf4_bf16(const void* A, int lda, const srgpt_nf4* w, void* C, int ldc, int M, int N, int K, const void* residual, int ldr,
+                        int epilogue, void* stream);
 /* Plain argmax over fp32 rows (first index on ties), e.g. first token after prefill. */
 int srgpt_argmax_f32(const float* x, int rows, int cols, long long* out, void* stream);
 /* Same over bf16 rows [rows, ldx] (the bf16-rounded logits of a batched lm_head GEMM, modeling_llama.py:1044). */
@@ -416,6 +422,18 @@ int srgpt_llama_decode_step_nf4_bf16(void* h, const srgpt_llama_layer_weights* l
                                      const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
                                      const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
                                      void* lm_workspace, float* logits_out, long long* out_ids, int* step, void* stream);
+/* srgpt_llama_prefill_layers_bf16 / srgpt_llama_prefill_chunk_layers_bf16 with every matrix whose nf4[l].<matrix>.q != NULL taken by
+ * srgpt_gemm_nf4_bf16 from its planes; the element-type pointer of `layers` is then unused and may be NULL.  Bit-identical to the
+ * element-type stacks over the dequantized weights. */
+int srgpt_llama_prefill_layers_nf4_bf16(void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* ws_h,
+                                        void* ws_qkv, void* ws_attn, void* ws_act, int S, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                        float eps, const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables,
+                                        int page_size, int n_seqs, const int* cu_seqlens, int max_seqlen, int page_table_stride, void* stream);
+int srgpt_llama_prefill_chunk_layers_nf4_bf16(void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers,
+                                              void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act, int S, int H, int n_heads, int n_kv_heads,
+                                              int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
+                                              const int* page_tables, int page_table_stride, int page_size, int n_pages, int n_seqs,
+                                              const int* cu_seqlens, int max_rows, void* stream);
 
 /* ---- FP8 (E4M3) W8A8 quantization of the decoder-layer linears (fp8.cu, gemm_wgmma.cu; DESIGN.md §3, §7) ---------------------------
  * Every row r of a weight W [N, K] (once, at load) and of an activation x [M, K] (before every linear) is quantized alike:
@@ -486,6 +504,10 @@ int srgpt_gemv_multi_packed_bf16(const void* x, int ldx, const srgpt_packed12* p
                                  const void* norm_weight, float eps, const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim,
                                  const void* cos_tab, const void* sin_tab, const int* pos, void* kv_pages, const int* page_table, int page_size,
                                  void* stream);
+/* srgpt_gemv_multi_bf16 streaming NF4 planes (a host pointer; K a multiple of 1024): bit-identical to it over the dequantized matrix. */
+int srgpt_gemv_multi_nf4_bf16(const void* x, int ldx, const srgpt_nf4* nf4, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
+                              const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+                              const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream);
 /* final norm + lm_head over T rows: fp32 logits [T, V] (optional) and per-(token, CTA) arg max partials in `workspace`
  * (T * srgpt_lm_head_workspace(V) bytes, token t's block at t * srgpt_lm_head_workspace(V)); srgpt_spec_accept reduces them. */
 int srgpt_lm_head_multi_bf16(const void* x, int ldx, const void* W, int ldw, int T, int V, int K, const void* norm_weight, float eps,
@@ -521,6 +543,14 @@ int srgpt_llama_verify_step_packed_bf16(void* h, const srgpt_llama_layer_weights
                                         int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
                                         const void* embed_table, void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids,
                                         const int* prompt_len, int ngram, int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream);
+/* The verify pass streaming NF4 layer matrices: nf4[l].<matrix>.q != NULL takes srgpt_gemv_multi_nf4_bf16 (the element-type pointer of
+ * `layers` may then be NULL), q == NULL the element-type matrix; lm_head as in srgpt_llama_decode_step_nf4_bf16. */
+int srgpt_llama_verify_step_nf4_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf,
+                                     void* attn_buf, void* act_buf, int T, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                                     const void* cos_tab, const void* sin_tab, int* pos, int* pos_rows, const int* page_table, int page_size,
+                                     const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
+                                     void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids, const int* prompt_len, int ngram,
+                                     int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream);
 
 #ifdef __cplusplus
 }

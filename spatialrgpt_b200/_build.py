@@ -37,7 +37,7 @@ def _nvcc() -> str:
 
 def _deps():
     files = [os.path.join(CSRC, s) for s in SOURCES]
-    files += [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tma.cuh"), os.path.join(CSRC, "pack12.cuh"), os.path.join(CSRC, "nf4.cuh"), os.path.join(CSRC, "fp8.cuh"),
+    files += [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "tma.cuh"), os.path.join(CSRC, "pack12.cuh"), os.path.join(CSRC, "nf4.cuh"), os.path.join(CSRC, "gemv_multi_kernel.inc"), os.path.join(CSRC, "fp8.cuh"),
               os.path.join(INCLUDE, "srgpt_b200.h")]
     return files
 

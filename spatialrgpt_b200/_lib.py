@@ -120,6 +120,13 @@ SIGNATURES = {
                                           vp, vp, ci, vp, vp, ci, vp, vp, vp]),
     "srgpt_llama_verify_step_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp,
                                                  vp, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp]),
+    "srgpt_gemm_nf4_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, ci, ci, vp]),
+    "srgpt_gemv_multi_nf4_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, vp, ci, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp]),
+    "srgpt_llama_prefill_layers_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp]),
+    "srgpt_llama_prefill_chunk_layers_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, ci, ci,
+                                                       vp, ci, vp]),
+    "srgpt_llama_verify_step_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp,
+                                              vp, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)

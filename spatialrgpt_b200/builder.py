@@ -220,12 +220,16 @@ def load_pretrained_model(model_path: str, model_name: str, model_base: Optional
     the decoder-layer linears are NF4-quantized at load (weights.from_state_dicts) and dequantized into that dtype; the batch-1 decode
     step streams the 4-bit planes.  ``quantization="fp8"`` quantizes the same linears to per-row E4M3 weights (W8A8: every activation row
     is quantized alike before each linear), keeps no element-type copy of them, and runs them on the FP8 tensor cores (prefill, batched
-    decode, beams) and through the FP8 decode GEMV (the one-token step); ``prompt_lookup_num_tokens`` then raises.  ``load_4bit`` /
-    ``load_8bit`` (bitsandbytes) still raise."""
+    decode, beams) and through the FP8 decode GEMV (the one-token step); ``prompt_lookup_num_tokens`` then raises.
+    ``nf4_dequantized_copy=False`` (with ``quantization="nf4"`` only) keeps no dequantized copy of the layer matrices that have NF4 planes:
+    prefill, batched decode, beams and the verify pass read the planes too (bit-identical).  ``load_4bit`` / ``load_8bit`` (bitsandbytes)
+    still raise."""
     if load_8bit or load_4bit:
         raise NotImplementedError("bitsandbytes quantised loading is outside the hot path (builder.py:51-60)")
     if model_base is not None:
         raise NotImplementedError("LoRA / delta checkpoints (builder.py:66-140) are outside the hot path")
+    if not kwargs.get("nf4_dequantized_copy", True) and kwargs.get("quantization") != "nf4":
+        raise ValueError(f"nf4_dequantized_copy=False needs quantization='nf4', not {kwargs.get('quantization')!r}")
     if not is_mm_model(model_path):
         raise ValueError(f"{model_path} is not a llava-style VLM checkpoint (config.json 'architectures')")
     from .llava_llama import LlavaLlamaModel
@@ -238,7 +242,9 @@ def load_pretrained_model(model_path: str, model_name: str, model_base: Optional
     if dtype not in (torch.float16, torch.bfloat16):
         raise NotImplementedError(f"torch_dtype {dtype}: the sm_90a kernels compute in torch.float16 or torch.bfloat16")
     quantization = kwargs.pop("quantization", None)
-    model = LlavaLlamaModel(cfg, from_state_dicts(cfg, sd, dev, dtype=dtype, quantization=quantization), tokenizer=tokenizer,
+    nf4_dequantized_copy = kwargs.pop("nf4_dequantized_copy", True)
+    model = LlavaLlamaModel(cfg, from_state_dicts(cfg, sd, dev, dtype=dtype, quantization=quantization, nf4_dequantized_copy=nf4_dequantized_copy),
+                            tokenizer=tokenizer,
                             image_processor=image_processor, max_seq_len=max_seq)
     context_len = getattr(cfg.llama, "max_sequence_length", 2048) if hasattr(cfg.llama, "max_sequence_length") else 2048
     return tokenizer, model, image_processor, context_len

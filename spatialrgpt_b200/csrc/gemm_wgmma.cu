@@ -17,6 +17,12 @@
 // FP8: gemm_fp8_kernel runs the same body over E4M3 operands (K blocks of 128 one-byte elements, the same 128-byte rows, wgmma
 // m64n128k32.e4m3) and scales the accumulators by the row scales of both operands before the epilogue (W8A8 decoder linears, fp8.cu).
 //
+// NF4: gemm_nf4_kernel runs the same body over the decode GEMV's NF4 planes (nf4.cuh) instead of a 16-bit weight matrix.  The A operand
+// still comes by TMA; the producer warpgroup builds each B stage itself: every thread loads its code words and block scales two stages
+// ahead, dequantizes them with nf4::dequant8 into the 16-byte chunks TMA would have written (128B swizzle), then fences the generic-proxy
+// stores against the wgmma reads (fence.proxy.async) and arrives on the stage's full barrier.  The consumers, the tile order and stream-K
+// are those of the 16-bit kernel over the dequantized matrix, so the results are bit-identical to it.
+//
 // Short problems (M <= 128 rows: the projections and the lm_head of a batched decode step) have N / 128 tiles, too few to
 // fill 132 SMs.  With a registered workspace they run "stream-K": the (n-tile, k-block) units are cut into gridDim.x equal
 // contiguous ranges, one per SM.  A tile whose k-range is split is owned by the CTA holding its first k-block; the other CTAs
@@ -27,6 +33,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "nf4.cuh"
 #include "srgpt_b200.h"
 #include "tma.cuh"
 
@@ -226,11 +233,59 @@ __device__ __forceinline__ void scale_acc(float (&d)[64], const Fp8Scales& sc, c
   }
 }
 
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// NF4 B operand: the code words and block scales of one k-block for one producer thread.  Thread pt fills 16-byte slot j = pt % 8 (the
+// chunk of weights 8 j .. 8 j + 7 of the k-block) of tile rows pt / 8 + 16 i, i = 0..7: a warp's load covers 4 rows x 8 chunks.  A k-block
+// is one scale block (BK == nf4::BLOCK), so a row's 8 chunks share one scale.
+struct Nf4Raw {
+  uint32_t w[8];
+  float s[8];
+};
+
+// Load i of the producer's sequence: the same (m-tile, n-tile, k-block) order as the TMA producer of gemm_body
+__device__ __forceinline__ void nf4_coords(bool sk, int i, int u_begin, int num_kb, int cta, int G, int tiles_m, int tiles_n, int gm, int& m0,
+                                           int& n0, int& kb) {
+  if (sk) {
+    const int u = u_begin + i, tile = u / num_kb;
+    m0 = 0;
+    n0 = tile * BN;
+    kb = u - tile * num_kb;
+  } else {
+    const int ui = i / num_kb;
+    int mt, nt;
+    unit_to_tile(cta + ui * G, tiles_m, tiles_n, gm, mt, nt);
+    m0 = mt * BM;
+    n0 = nt * BN;
+    kb = i - ui * num_kb;
+  }
+}
+
+// code word of chunk 8 kb + j of a row at nf4::lane_offset(8 kb + j); rows at or beyond N are not read and hold code 7 (the value +0)
+__device__ __forceinline__ void nf4_fetch(const srgpt_nf4& w4, const Params& p, int n0, int kb, int r0, int j, Nf4Raw& c) {
+  const size_t row_bytes = (size_t)(p.K >> 1);
+  const int row_scales = p.K / nf4::BLOCK;
+  const uint8_t* q = w4.q + (size_t)(n0 + r0) * row_bytes + nf4::lane_offset(8 * kb + j);
+  const float* s = w4.scale + (size_t)(n0 + r0) * row_scales + kb;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    c.w[i] = 0x77777777u;
+    c.s[i] = 0.f;
+    if (n0 + r0 + 16 * i < p.N) {
+      c.w[i] = __ldg(reinterpret_cast<const uint32_t*>(q + (size_t)(16 * i) * row_bytes));
+      c.s[i] = __ldg(s + (size_t)(16 * i) * row_scales);
+    }
+  }
+}
+
 // SK = false: persistent over whole 128 x 128 tiles.  SK = true: stream-K over the (n-tile, k-block) units of an M <= 128
 // problem (see the file comment).  FP8 = true: E4M3 operands, a K block of 128 one-byte elements (the same 128-byte rows, so the
 // stage size, swizzle, ring and tile order are those of the 16-bit kernel), and the accumulators scaled by `sc` before the epilogue.
-template <int EPI, bool SK, bool FP8>
-__device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const Params& p, const TskWs& ws, const Fp8Scales& sc) {
+// NF4 = true: the B stages are dequantized from the planes `w4` by the producer warpgroup (tmap_b unused); everything else is the
+// 16-bit kernel.
+template <int EPI, bool SK, bool FP8, bool NF4 = false>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const Params& p, const TskWs& ws, const Fp8Scales& sc,
+                                          const srgpt_nf4& w4 = srgpt_nf4{nullptr, nullptr}) {
   constexpr int KB = FP8 ? 128 : BK;  // elements per k-block
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned stage buffers
@@ -247,11 +302,16 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a, const CUten
   auto range_begin = [&](int c) { return (int)(total * c / G); };
   const int u_begin = SK ? range_begin(cta) : 0, u_end = SK ? range_begin(cta + 1) : 0;
 
+  // NF4: the 16 code values, behind the barriers (the 256 bytes reserved for them hold both)
+  float* nf4_tab = reinterpret_cast<float*>(empty_bar + STAGES);
+  if constexpr (NF4) {
+    if (threadIdx.x < 16) nf4_tab[threadIdx.x] = nf4::code_value(threadIdx.x);
+  }
   if (threadIdx.x == 0) {
     prefetch_tmap(tmap_a);
-    prefetch_tmap(tmap_b);
+    if constexpr (!NF4) prefetch_tmap(tmap_b);
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&full_bar[s]), 1);
+      mbar_init(smem_u32(&full_bar[s]), NF4 ? 1 + 128 : 1);  // NF4: the A transaction plus one arrive per producer thread
       mbar_init(smem_u32(&empty_bar[s]), 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
@@ -259,6 +319,55 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmap_a, const CUten
   __syncthreads();
 
   const int wg = threadIdx.x >> 7;
+  if constexpr (NF4) {
+    if (wg == 0) {
+      // ===================== NF4 producer: A by TMA, B dequantized by the whole warpgroup =====================
+      const int pt = threadIdx.x, j = pt & 7, r0 = pt >> 3;
+      const int n_loads = SK ? u_end - u_begin : (cta < num_units ? (num_units - 1 - cta) / G + 1 : 0) * num_kb;
+      uint32_t stage = 0, phase = 0;
+      auto fetch = [&](int i, Nf4Raw& c) {
+        int m0, n0, kb;
+        nf4_coords(SK, i, u_begin, num_kb, cta, G, tiles_m, tiles_n, p.gm, m0, n0, kb);
+        nf4_fetch(w4, p, n0, kb, r0, j, c);
+      };
+      auto put = [&](int i, const Nf4Raw& c) {
+        int m0, n0, kb;
+        nf4_coords(SK, i, u_begin, num_kb, cta, G, tiles_m, tiles_n, p.gm, m0, n0, kb);
+        mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
+        const uint32_t fb = smem_u32(&full_bar[stage]);
+        uint8_t* sa = smem + stage * STAGE_BYTES;
+        if (pt == 0) {
+          mbar_expect_tx(fb, A_BYTES);
+          tma_load_2d(smem_u32(sa), tmap_a, fb, kb * BK, m0);
+        }
+        // row r, 16-byte chunk c of a 128B-swizzled K-major tile sits at r * 128 + ((c ^ (r & 7)) << 4); r & 7 == r0 & 7 for all 8 rows
+        uint8_t* sb = sa + A_BYTES + r0 * 128 + ((j ^ (r0 & 7)) << 4);
+#pragma unroll
+        for (int i2 = 0; i2 < 8; ++i2) *reinterpret_cast<uint4*>(sb + i2 * 16 * 128) = nf4::dequant8(c.w[i2], c.s[i2], nf4_tab);
+        fence_proxy_async_shared();  // the generic-proxy stores before the wgmma (async proxy) reads them
+        mbar_arrive(fb);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      };
+      // three register buffers: the loads of a stage are issued two stages before it is dequantized
+      Nf4Raw b0, b1, b2;
+      if (n_loads > 0) fetch(0, b0);
+      if (n_loads > 1) fetch(1, b1);
+      if (n_loads > 2) fetch(2, b2);
+      for (int i = 0; i < n_loads; i += 3) {
+        put(i, b0);
+        if (i + 3 < n_loads) fetch(i + 3, b0);
+        if (i + 1 < n_loads) {
+          put(i + 1, b1);
+          if (i + 4 < n_loads) fetch(i + 4, b1);
+        }
+        if (i + 2 < n_loads) {
+          put(i + 2, b2);
+          if (i + 5 < n_loads) fetch(i + 5, b2);
+        }
+      }
+      return;
+    }
+  }
   if (wg == 0) {
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
@@ -396,6 +505,12 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   gemm_body<EPI, SK, true>(&tmap_a, &tmap_b, p, ws, sc);
 }
 
+template <int EPI, bool SK>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_nf4_kernel(const __grid_constant__ CUtensorMap tmap_a, const Params p, const TskWs ws, const srgpt_nf4 w4) {
+  gemm_body<EPI, SK, false, true>(&tmap_a, nullptr, p, ws, Fp8Scales{nullptr, nullptr}, w4);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -428,18 +543,22 @@ static TskState g_tsk;
 
 static long long tsk_workspace_bytes(int ctas) { return TSK_FLAG_BYTES + (long long)ctas * TSK_SLOT_FLOATS * 4; }
 
-template <int EPI, bool SK, bool FP8>
-static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, const TskWs& ws, const Fp8Scales& sc, int grid,
-                         cudaStream_t stream) {
+template <int EPI, bool SK, bool FP8, bool NF4>
+static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, const TskWs& ws, const Fp8Scales& sc, const srgpt_nf4& w4,
+                         int grid, cudaStream_t stream) {
   static bool configured = false;
   if (!configured) {
-    if constexpr (FP8)
+    if constexpr (NF4)
+      SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_nf4_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    else if constexpr (FP8)
       SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     else
       SRGPT_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  if constexpr (FP8)
+  if constexpr (NF4)
+    gemm_nf4_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, p, ws, w4);
+  else if constexpr (FP8)
     gemm_fp8_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p, ws, sc);
   else
     gemm_kernel<EPI, SK><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p, ws);
@@ -447,16 +566,20 @@ static int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const Par
   return SRGPT_OK;
 }
 
-// FP8: A and W hold E4M3 bytes (lda / ldw in bytes) and `sc` their scales
-template <int EPI, bool FP8 = false>
-static int launch(const void* A, int lda, const void* W, int ldw, const Params& p, cudaStream_t stream, const Fp8Scales& sc = Fp8Scales{nullptr, nullptr}) {
+// FP8: A and W hold E4M3 bytes (lda / ldw in bytes) and `sc` their scales.  NF4: W is unused and the weights are the planes `w4`, a 16-bit
+// [N, K] matrix for every choice made here (stream-K or not, grid, rasterisation), so the partition is the 16-bit kernel's.
+template <int EPI, bool FP8 = false, bool NF4 = false>
+static int launch(const void* A, int lda, const void* W, int ldw, const Params& p, cudaStream_t stream, const Fp8Scales& sc = Fp8Scales{nullptr, nullptr},
+                  const srgpt_nf4& w4 = srgpt_nf4{nullptr, nullptr}) {
   constexpr int EB = FP8 ? 1 : 2;           // bytes per element
   constexpr int KB = FP8 ? 128 : BK;        // elements per k-block
   CUtensorMap ta, tb;
   int rc = make_tmap(&ta, A, p.M, p.K, lda, FP8);
   if (rc != SRGPT_OK) return rc;
-  rc = make_tmap(&tb, W, p.N, p.K, ldw, FP8);
-  if (rc != SRGPT_OK) return rc;
+  if (!NF4) {
+    rc = make_tmap(&tb, W, p.N, p.K, ldw, FP8);
+    if (rc != SRGPT_OK) return rc;
+  }
   const int sms = sm_count();
   TskWs ws = {nullptr, nullptr, 0};
   // one-tile-high problems whose weights are worth streaming (>= 4 MB) take the stream-K split when the caller registered a
@@ -472,7 +595,7 @@ static int launch(const void* A, int lda, const void* W, int ldw, const Params& 
     ws.partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(g_tsk.base) + TSK_FLAG_BYTES);
     if (++g_tsk.epoch == 0) g_tsk.epoch = 1;  // flags start at 0 (zeroed workspace) and never equal a future epoch
     ws.epoch = g_tsk.epoch;
-    return launch_kernel<EPI, true, FP8>(ta, tb, p, ws, sc, grid, stream);
+    return launch_kernel<EPI, true, FP8, NF4>(ta, tb, p, ws, sc, w4, grid, stream);
   }
   // rasterisation group: the whole M when the activation fits L2 (50 MB), else as many m-tiles as keep a group's rows <= 20 MB;
   // SRGPT_GEMM_GM forces the group size
@@ -487,7 +610,7 @@ static int launch(const void* A, int lda, const void* W, int ldw, const Params& 
   if (gm_env > 0) pg.gm = gm_env < tiles_m ? gm_env : tiles_m;
   const long long units = (long long)tiles_m * ceil_div(p.N, BN);
   const int grid = (int)(units < sms ? units : sms);
-  return launch_kernel<EPI, false, FP8>(ta, tb, pg, ws, sc, grid, stream);
+  return launch_kernel<EPI, false, FP8, NF4>(ta, tb, pg, ws, sc, w4, grid, stream);
 }
 
 }  // namespace gemm
@@ -589,6 +712,42 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemm_fp8_bf16(const 
     case SRGPT_EPI_NONE: return gemm::launch<SRGPT_EPI_NONE, true>(A, lda, W, ldw, p, st, sc);
     case SRGPT_EPI_BIAS_RESIDUAL: return gemm::launch<SRGPT_EPI_BIAS_RESIDUAL, true>(A, lda, W, ldw, p, st, sc);
     case SRGPT_EPI_SWIGLU: return gemm::launch<SRGPT_EPI_SWIGLU, true>(A, lda, W, ldw, p, st, sc);
+  }
+  return SRGPT_ERR_INVALID;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemm_nf4_bf16(const void* A, int lda, const srgpt_nf4* w, void* C, int ldc, int M, int N, int K,
+                                                                            const void* residual, int ldr, int epilogue, void* stream) {
+  SRGPT_CHECK_ARG(A != nullptr && w != nullptr && w->q != nullptr && w->scale != nullptr && C != nullptr);
+  SRGPT_CHECK_ARG(M > 0 && N > 0 && K > 0 && (K % nf4::BATCH) == 0);
+  SRGPT_CHECK_ARG(lda >= K && (lda % 8) == 0);  // 16-byte global strides for TMA
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0);
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(w->q) & 15) == 0 && (reinterpret_cast<uintptr_t>(w->scale) & 3) == 0);
+  SRGPT_CHECK_ARG(epilogue == SRGPT_EPI_NONE || epilogue == SRGPT_EPI_BIAS_RESIDUAL || epilogue == SRGPT_EPI_SWIGLU);
+  if (epilogue == SRGPT_EPI_SWIGLU) {
+    SRGPT_CHECK_ARG((N % 2) == 0 && ldc >= N / 2 && (ldc % 8) == 0);
+  } else {
+    SRGPT_CHECK_ARG(ldc >= N && (ldc % 8) == 0);
+  }
+  if (residual != nullptr) {
+    SRGPT_CHECK_ARG(epilogue == SRGPT_EPI_BIAS_RESIDUAL && ldr >= N && (ldr % 8) == 0);
+    SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(residual) & 15) == 0);
+  }
+
+  gemm::Params p;
+  p.gm = 1;
+  p.M = M; p.N = N; p.K = K; p.ldc = ldc;
+  p.bias = nullptr;
+  p.residual = reinterpret_cast<const bf16*>(residual);
+  p.ldr = ldr; p.res_row_mod = 0;
+  p.C = C; p.out_fp32 = 0;
+  const gemm::Fp8Scales none = {nullptr, nullptr};
+
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (epilogue) {
+    case SRGPT_EPI_NONE: return gemm::launch<SRGPT_EPI_NONE, false, true>(A, lda, nullptr, K, p, st, none, *w);
+    case SRGPT_EPI_BIAS_RESIDUAL: return gemm::launch<SRGPT_EPI_BIAS_RESIDUAL, false, true>(A, lda, nullptr, K, p, st, none, *w);
+    case SRGPT_EPI_SWIGLU: return gemm::launch<SRGPT_EPI_SWIGLU, false, true>(A, lda, nullptr, K, p, st, none, *w);
   }
   return SRGPT_ERR_INVALID;
 }

@@ -382,6 +382,8 @@ struct Nf4 {
   __device__ __forceinline__ void load_side(const Params&, int, int, int) {}
   __device__ __forceinline__ int nbatch(const Params& p, int) const { return p.K >> 10; }
   __device__ __forceinline__ Raw load(int b) const { return {ld_stream16(q0 + b * 32), ld_stream16(q1 + b * 32), __ldg(s_lane + b * 16)}; }
+  // the verify kernel's batches: rows are whole batches (K % 1024 == 0)
+  __device__ __forceinline__ Raw load_bounded(int b, int, int) const { return load(b); }
   // codes of r0 / r1 at +0 / +512, scales at +1024
   __device__ __forceinline__ void cp_async(uint8_t* slot, int lane, int b) const {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(slot + lane * 16);
@@ -782,134 +784,14 @@ struct MParams {
   int tile_ch;  // chunks of x per staged tile
 };
 
-template <int MODE, class Fmt>
-__global__ void __launch_bounds__(THREADS, 2) decode_gemv_multi_kernel(const MParams mp) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __shared__ float red[32];
-  __shared__ float sv[MT_MAX][WARPS];
-  __shared__ int si[MT_MAX][WARPS];
-  const Params& p = mp.p;
-  const int nt = mp.T, tile_ch = mp.tile_ch;
-  bf16* sx = reinterpret_cast<bf16*>(smem_raw);
-  const uint4* px = reinterpret_cast<const uint4*>(sx);
+#define SRGPT_GEMV_MULTI_KERNEL decode_gemv_multi_kernel
+#include "gemv_multi_kernel.inc"
+#undef SRGPT_GEMV_MULTI_KERNEL
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int npairs = (MODE == MODE_LM) ? ((p.N + 1) >> 1) : (p.N >> 1);
-  const int pi = blockIdx.x * WARPS + warp;
-  const bool active = pi < npairs;
-  int r0, r1;
-  pair_rows<MODE>(p, pi, r0, r1);  // every warp, as in decode_gemv_kernel
-  const int nchunk = p.K >> 3;
-  const int nbatch = (nchunk + 127) >> 7;
-
-  // ---- weights: batch 0 is requested before the dependency wait
-  Fmt f{};
-  f.setup(p, r0, r1, lane);
-  typename Fmt::Raw raw{};
-  if (active) {
-    raw = f.load_bounded(0, nchunk, lane);
-    f.load_side(p, r0, r1, lane);
-  }
-  uint4 nw_pre[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-  const bool nw_pre_valid = (p.norm_weight != nullptr) && (nchunk <= 2 * THREADS);
-  if (nw_pre_valid) {
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const int cc = threadIdx.x + k * THREADS;
-      if (cc < nchunk) nw_pre[k] = reinterpret_cast<const uint4*>(p.norm_weight)[cc];
-    }
-  }
-  pdl_launch_dependents();
-  pdl_wait();
-
-  float a0[MT_MAX], a1[MT_MAX];
-#pragma unroll
-  for (int t = 0; t < MT_MAX; ++t) a0[t] = a1[t] = 0.f;
-  int b = 0;
-  for (int c0 = 0; c0 < nchunk; c0 += tile_ch) {
-    const int tlen = min(tile_ch, nchunk - c0);
-    if (p.norm_weight != nullptr) {  // one tile holds the whole row (tile_ch == nchunk)
-      for (int t = 0; t < nt; ++t)
-        stage_x(p.x + (size_t)t * mp.ldx, p.norm_weight, p.eps, p.K, sx + (size_t)t * tile_ch * 8, red, nw_pre, nw_pre_valid);
-    } else {
-      __syncthreads();  // the previous tile is consumed
-      for (int t = 0; t < nt; ++t) {
-        const uint4* src = reinterpret_cast<const uint4*>(p.x + (size_t)t * mp.ldx) + c0;
-        uint4* dst = reinterpret_cast<uint4*>(sx) + (size_t)t * tile_ch;
-        for (int cc = threadIdx.x; cc < tlen; cc += THREADS) dst[cc] = src[cc];
-      }
-      __syncthreads();
-    }
-    if (!active) continue;
-    for (; b < nbatch && b * 128 < c0 + tlen; ++b) {
-      // batch 0 was requested before the wait; every later batch is requested here (a double-buffered variant needed more than
-      // the 128 registers of 2 CTAs per SM and spilled)
-      if (b > 0) raw = f.load_bounded(b, nchunk, lane);
-      uint4 w0[4], w1[4];
-      f.decode(raw, b, lane, w0, w1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int c = b * 128 + lane + 32 * i;
-        if (c < nchunk) {
-#pragma unroll
-          for (int t = 0; t < MT_MAX; ++t) {
-            if (t < nt) {
-              float xf[8];
-              unpack8(px[(size_t)t * tile_ch + (c - c0)], xf);
-              a0[t] += dot8(w0[i], xf);
-              a1[t] += dot8(w1[i], xf);
-            }
-          }
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int t = 0; t < MT_MAX; ++t) {
-    if (t < nt) {
-      a0[t] = warp_sum(a0[t]);
-      a1[t] = warp_sum(a1[t]);
-    }
-  }
-  // lane t runs token t's stores (every lane holds every token's sums after warp_sum)
-  float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-  for (int t = 0; t < MT_MAX; ++t) {
-    if (t == lane) {
-      s0 = a0[t];
-      s1 = a1[t];
-    }
-  }
-  if (active && lane < nt) {
-    const int t = lane;
-    float best;
-    int besti;
-    store_pair<MODE>(p, p.y + (size_t)t * mp.ldy, p.residual != nullptr ? p.residual + (size_t)t * mp.ldy : nullptr,
-                     p.logits_out != nullptr ? p.logits_out + (size_t)t * p.N : nullptr, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos + t : 0, pi, r0,
-                     r1, s0, s1, best, besti);
-    if (MODE == MODE_LM) {
-      sv[t][warp] = best;
-      si[t][warp] = besti;
-    }
-  }
-  if (MODE == MODE_LM) {
-    if (!active && lane < nt) {
-      sv[lane][warp] = -INFINITY;
-      si[lane][warp] = 0x7fffffff;
-    }
-    __syncthreads();
-    if (threadIdx.x < nt) {  // the CTA reduction of decode_gemv_kernel, one thread per token
-      const int t = threadIdx.x;
-      float best = sv[t][0];
-      int besti = si[t][0];
-      for (int w = 1; w < WARPS; ++w)
-        if (better(sv[t][w], si[t][w], best, besti)) { best = sv[t][w]; besti = si[t][w]; }
-      float* pv = p.part_val + (size_t)t * 2 * gridDim.x;
-      pv[blockIdx.x] = best;
-      reinterpret_cast<int*>(pv + gridDim.x)[blockIdx.x] = besti;
-    }
-  }
-}
+// the NF4 planes (srgpt_gemv_multi_nf4_bf16, the verify pass of a planes-only NF4 model): the same kernel under its own name
+#define SRGPT_GEMV_MULTI_KERNEL nf4_gemv_multi_kernel
+#include "gemv_multi_kernel.inc"
+#undef SRGPT_GEMV_MULTI_KERNEL
 
 // ---- the two ends of a verify pass -------------------------------------------------------------------------------------------
 // History of the n-gram lookup: the prompt's ids (negative = a row that is not text: never matches), then the generated ids.
@@ -1394,17 +1276,25 @@ namespace srgpt {
 namespace gemv {
 
 template <int MODE, class Fmt>
+static auto multi_kernel() {
+  if constexpr (std::is_same<Fmt, Nf4>::value)
+    return &nf4_gemv_multi_kernel<MODE, Nf4>;
+  else
+    return &decode_gemv_multi_kernel<MODE, Fmt>;
+}
+
+template <int MODE, class Fmt>
 static int launch_multi(MParams& mp, int npairs, cudaStream_t st) {
   const int smem = mp.T * mp.tile_ch * 16;
   static int configured_smem = 0;
   if (smem > configured_smem) {  // the opt-in counts static shared memory too, so it is set for every size, not only above 48 KB
-    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(decode_gemv_multi_kernel<MODE, Fmt>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    SRGPT_CHECK_CUDA(cudaFuncSetAttribute(multi_kernel<MODE, Fmt>(), cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured_smem = smem;
   }
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
   pdl_config(cfg, attr, grid_for(npairs), THREADS, smem, st);
-  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, decode_gemv_multi_kernel<MODE, Fmt>, mp));
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, multi_kernel<MODE, Fmt>(), mp));
   return SRGPT_OK;
 }
 
@@ -1472,6 +1362,19 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_multi_packed_bf
   return gemv_multi_modes<gemv::Packed12>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab,
                                           pos, kv_pages, page_table, page_size, stream);
 #endif
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_multi_nf4_bf16(const void* x, int ldx, const srgpt_nf4* nf4, void* y, int ldy, int T, int N,
+                                                                                int K, const void* norm_weight, float eps, const void* residual, int mode,
+                                                                                int n_heads, int n_kv_heads, int head_dim, const void* cos_tab,
+                                                                                const void* sin_tab, const int* pos, void* kv_pages, const int* page_table,
+                                                                                int page_size, void* stream) {
+  SRGPT_CHECK_ARG(nf4 && nf4->q && nf4->scale && aligned16(nf4->q) && (reinterpret_cast<uintptr_t>(nf4->scale) & 3) == 0);
+  SRGPT_CHECK_ARG(K > 0 && (K % nf4::BATCH) == 0);
+  gemv::MParams mp = {};
+  mp.p.nf = *nf4;
+  return gemv_multi_modes<gemv::Nf4>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
+                                     kv_pages, page_table, page_size, stream);
 }
 
 template <class Fmt>

@@ -150,6 +150,10 @@ def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
     model_path = os.path.expanduser(args.model_path)
     model_name = get_model_name_from_path(model_path)
     quant = {"quantization": args.quantization} if getattr(args, "quantization", None) else {}
+    if getattr(args, "nf4_planes_only", False):
+        if getattr(args, "quantization", None) != "nf4":
+            raise ValueError("--nf4-planes-only needs --quantization nf4")
+        quant["nf4_dequantized_copy"] = False
     tokenizer, model, image_processor, _ = loader(model_path, model_name, getattr(args, "model_base", None), **quant)
     data = get_chunk(generate_data_list(args.annotation_file), args.num_chunks, args.chunk_idx)
     answers_file = os.path.expanduser(args.answers_file)
@@ -193,6 +197,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--seed", type=int, default=None, help="seed of the prompt choice (the reference draws unseeded)")
     p.add_argument("--quantization", choices=["nf4", "fp8"], default=None,
                    help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
+    p.add_argument("--nf4-planes-only", action="store_true",
+                   help="with --quantization nf4: keep only the 4-bit planes of the layer matrices, no dequantized copy (same answers)")
     return p
 
 

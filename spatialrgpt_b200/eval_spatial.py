@@ -259,6 +259,10 @@ def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tens
     model_name = get_model_name_from_path(model_path)
     # --quantization quantizes from (and computes in) the element type it is loaded in, so the model is loaded in bf16 instead of cast to it
     quant = {"quantization": args.quantization, "torch_dtype": torch.bfloat16} if getattr(args, "quantization", None) else {}
+    if getattr(args, "nf4_planes_only", False):
+        if getattr(args, "quantization", None) != "nf4":
+            raise ValueError("--nf4-planes-only needs --quantization nf4")
+        quant["nf4_dequantized_copy"] = False
     tokenizer, model, image_processor, _ = loader(model_path, model_name, getattr(args, "model_base", None), **quant)
     model.to(dtype=torch.bfloat16)  # eval_spatial.py:221: the loader returns fp16, this script computes in bf16
     if depth_predictor is None:
@@ -318,6 +322,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--allow-no-depth", action="store_true", help="run an enable_depth checkpoint without a depth network (degraded answers)")
     p.add_argument("--quantization", choices=["nf4", "fp8"], default=None,
                    help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
+    p.add_argument("--nf4-planes-only", action="store_true",
+                   help="with --quantization nf4: keep only the 4-bit planes of the layer matrices, no dequantized copy (same answers)")
     return p
 
 

@@ -18,7 +18,7 @@ import torch
 
 from . import logits_processors, ops
 from .config import LlamaDims
-from .weights import LlamaW
+from .weights import LlamaW, Nf4W
 
 PAGE_SIZE = 16
 
@@ -136,6 +136,12 @@ class LlamaDecoder:
         self.fp8 = getattr(w, "quantization", None) == "fp8"
         if self.fp8:
             self.supports_prompt_lookup = False
+        # quantization="nf4" with nf4_dequantized_copy=False: the matrices with planes have no dequantized copy, so prefill, batched decode,
+        # beams and the verify pass read the planes as well (srgpt_gemm_nf4_bf16, srgpt_gemv_multi_nf4_bf16; bit-identical to the copy)
+        self.nf4_planes_only = getattr(w, "quantization", None) == "nf4" and not getattr(w, "nf4_dequantized_copy", True)
+        if self.nf4_planes_only and os.environ.get("SRGPT_DECODE_NF4", "1") == "0":
+            raise ValueError("SRGPT_DECODE_NF4=0 runs the decode step over the dequantized copies, which a model loaded with "
+                             "nf4_dequantized_copy=False does not keep")
         self._layer_array = self._make_layer_array()
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
         # ("verify", T, ngram), ("batch", B, proc) and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
@@ -189,6 +195,12 @@ class LlamaDecoder:
     _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
     _lm_packed = None
     _nf4_array = None  # srgpt_llama_layer_nf4[] of the decode step
+    nf4_planes_only = False
+
+    @property
+    def _planes_array(self):
+        """The srgpt_llama_layer_nf4[] the prefill stacks and the verify pass take (planes-only NF4 models), else None."""
+        return self._nf4_array if self.nf4_planes_only else None
 
     def _make_layer_array(self):
         """The layer descriptors of the prefill stacks and the decode step over the current KV cache."""
@@ -287,9 +299,11 @@ class LlamaDecoder:
         if start_pos != 0:
             cu = torch.tensor([0, S], dtype=torch.int32, device=self.device)
             return ops.llama_prefill_chunk_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp,
-                                                  self.cache.page_tables[seq:seq + 1], PAGE_SIZE, self.cache.n_pages, cu, S)
+                                                  self.cache.page_tables[seq:seq + 1], PAGE_SIZE, self.cache.n_pages, cu, S,
+                                                  nf4_array=self._planes_array)
         pt = self.cache.page_tables[seq]
-        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pt, PAGE_SIZE)
+        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pt, PAGE_SIZE,
+                                        nf4_array=self._planes_array)
 
     @ops.in_own_dtype
     def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int]) -> torch.Tensor:
@@ -307,7 +321,7 @@ class LlamaDecoder:
         sp = torch.zeros(B, dtype=torch.int32, device=self.device)
         x = packed_embeds.to(self.dtype).contiguous().clone()
         return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, self.cache.page_tables[:B],
-                                        PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens))
+                                        PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens), nf4_array=self._planes_array)
 
     @ops.in_own_dtype
     def first_tokens(self, hidden_packed: torch.Tensor, seq_lens: List[int], return_logits: bool = False):
@@ -572,7 +586,7 @@ class LlamaDecoder:
         ops.llama_verify_step(st["h"], self._layer_array, self._packed_array, d.num_hidden_layers, st["q"], st["attn"], st["act"], T, d,
                               self.cos, self.sin, self.pos, st["pos_rows"], self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed,
                               w.embed, st["ws"], st["logits"] if logits_all is not None else None, logits_all, st["prompt"], st["prompt_len"],
-                              ngram, st["draft"], self.out_ids, self.step, st["state"])
+                              ngram, st["draft"], self.out_ids, self.step, st["state"], nf4_array=self._planes_array)
 
     def _verify_graph(self, T: int, ngram: int) -> torch.cuda.CUDAGraph:
         """The captured verify pass of this (T, n-gram size); its warm-up writes only this sequence's slack."""
@@ -693,6 +707,9 @@ class LlamaDecoder:
         if self.fp8:  # every linear as the activation quantizer + the FP8 GEMM
             def linear(x, wt, **kw):
                 return ops.linear_fp8(x, wt, q=st["q8"][:, :x.shape[1]], scale=st["s8"], **kw)
+        elif self.nf4_planes_only:  # the NF4 GEMM where a matrix is held as planes
+            def linear(x, wt, **kw):
+                return ops.gemm_nf4(x, wt, **kw) if isinstance(wt, Nf4W) else ops.gemm(x, wt, **kw)
         else:
             linear = ops.gemm
         for l, lw in enumerate(w.layers):

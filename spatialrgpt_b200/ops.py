@@ -574,6 +574,34 @@ def gemv_nf4(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch.Te
     return y
 
 
+def gemm_nf4(a: torch.Tensor, w, residual: Optional[torch.Tensor] = None, epilogue: int = EPI_NONE,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemm() with the weight [N, K] read from an Nf4W's planes (K a multiple of 1024; epilogue EPI_NONE, EPI_BIAS_RESIDUAL without bias
+    or EPI_SWIGLU): the producer warpgroup dequantizes each weight tile in shared memory, so no element-type copy of the matrix is read
+    or kept.  Bit-identical to gemm() over the dequantized matrix."""
+    _need(a, ELEM(), "gemm_nf4.a")
+    _ensure_gemm_workspace(a.device)
+    lda = _rowmajor2d(a, "gemm_nf4.a")
+    M, K = a.shape
+    N, K2 = w.q.shape[0], w.q.shape[1] * 2
+    if K != K2:
+        raise SrgptError(f"gemm_nf4: K mismatch {K} vs {K2}")
+    n_out = N // 2 if epilogue == EPI_SWIGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=ELEM(), device=a.device)
+    _need(out, ELEM(), "gemm_nf4.out")
+    if out.shape != (M, n_out):
+        raise SrgptError(f"gemm_nf4.out: expected {(M, n_out)}, got {tuple(out.shape)}")
+    ldr = 0
+    if residual is not None:
+        _need(residual, ELEM(), "gemm_nf4.residual")
+        ldr = _rowmajor2d(residual, "gemm_nf4.residual")
+    d = _nf4_desc(w)
+    check(_lib.load().srgpt_gemm_nf4_bf16(_p(a), lda, C.byref(d), _p(out), _rowmajor2d(out, "gemm_nf4.out"), M, N, K, _p(residual), ldr, epilogue,
+                                          _stream()), "srgpt_gemm_nf4_bf16")
+    return out
+
+
 # ---- FP8 (E4M3) W8A8 quantization of the decoder-layer linears (fp8.cu, gemm_wgmma.cu; DESIGN.md §3) ------------------------------
 FP8_K_MULTIPLE = 16  # in_features must be a multiple (16-byte rows for TMA)
 
@@ -907,10 +935,13 @@ def make_siglip_layer_array(layers):
 
 
 def make_llama_layer_array(layers, kv_pages_per_layer):
+    """ctypes array of srgpt_llama_layer_weights; a matrix held only as NF4 planes (an Nf4W in its *_w field) gets NULL, and the NF4
+    entry points take it from the srgpt_llama_layer_nf4 array instead."""
     arr = (_lib.LlamaLayerWeights * len(layers))()
     for i, lw in enumerate(layers):
         for name in ("in_norm", "qkv_w", "o_w", "post_norm", "gateup_w", "down_w"):
-            setattr(arr[i], name, getattr(lw, name).data_ptr())
+            t = getattr(lw, name)
+            setattr(arr[i], name, t.data_ptr() if isinstance(t, torch.Tensor) else None)
         arr[i].kv_pages = kv_pages_per_layer[i].data_ptr()
     return arr
 
@@ -985,10 +1016,10 @@ def _fp8_workspaces(S: int, dims, dev):
 
 
 def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_table, page_size: int,
-                         cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0) -> torch.Tensor:
+                         cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0, nf4_array=None) -> torch.Tensor:
     """All decoder layers over the prompt rows x [S, H] in place (K/V appended to the paged cache).  One prompt
     (page_table [cap], start_pos [1]) or, with cu_seqlens [n_seqs+1], n_seqs prompts packed back to back
-    (page_table [n_seqs, cap], start_pos [n_seqs])."""
+    (page_table [n_seqs, cap], start_pos [n_seqs]).  ``nf4_array`` (make_llama_nf4_array): every matrix with planes through gemm_nf4."""
     _need(x, ELEM(), "llama_prefill_layers.x")
     _ensure_gemm_workspace(x.device)
     n_seqs, pt_stride = 1, 0
@@ -1014,6 +1045,13 @@ def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos,
                                                               max_seqlen, pt_stride, _stream()), "srgpt_llama_prefill_layers_fp8_bf16")
         _count(12 * n_layers)
         return x
+    if nf4_array is not None:
+        check(_lib.load().srgpt_llama_prefill_layers_nf4_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), ctypes.cast(nf4_array, ctypes.c_void_p),
+                                                              n_layers, _p(ws_h), _p(ws_qkv), _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I,
+                                                              dims.rms_norm_eps, _p(cos), _p(sin), _p(start_pos), _p(page_table), page_size, n_seqs,
+                                                              _p(cu_seqlens), max_seqlen, pt_stride, _stream()), "srgpt_llama_prefill_layers_nf4_bf16")
+        _count(8 * n_layers)
+        return x
     check(_lib.load().srgpt_llama_prefill_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
                                                       _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
                                                       _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride,
@@ -1023,9 +1061,10 @@ def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos,
 
 
 def llama_prefill_chunk_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
-                               cu_seqlens: torch.Tensor, max_rows: int) -> torch.Tensor:
+                               cu_seqlens: torch.Tensor, max_rows: int, nf4_array=None) -> torch.Tensor:
     """All decoder layers over x [S, H] in place: n_seqs chunks packed by cu_seqlens [n_seqs+1] that continue their sequences at
-    start_pos [n_seqs] (page_tables [n_seqs, cap]); attention reads every earlier position from the paged cache."""
+    start_pos [n_seqs] (page_tables [n_seqs, cap]); attention reads every earlier position from the paged cache.  ``nf4_array``: as
+    llama_prefill_layers()."""
     _need(x, ELEM(), "llama_prefill_chunk_layers.x")
     _need(cu_seqlens, torch.int32, "llama_prefill_chunk_layers.cu_seqlens")
     _ensure_gemm_workspace(x.device)
@@ -1048,6 +1087,14 @@ def llama_prefill_chunk_layers(x: torch.Tensor, layer_array, n_layers: int, dims
                                                                     page_tables.stride(0), page_size, n_pages, n_seqs, _p(cu_seqlens), max_rows,
                                                                     _stream()), "srgpt_llama_prefill_chunk_layers_fp8_bf16")
         _count(12 * n_layers)
+        return x
+    if nf4_array is not None:
+        check(_lib.load().srgpt_llama_prefill_chunk_layers_nf4_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p),
+                                                                    ctypes.cast(nf4_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
+                                                                    _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
+                                                                    _p(start_pos), _p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs,
+                                                                    _p(cu_seqlens), max_rows, _stream()), "srgpt_llama_prefill_chunk_layers_nf4_bf16")
+        _count(8 * n_layers)
         return x
     check(_lib.load().srgpt_llama_prefill_chunk_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
                                                             _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
@@ -1133,6 +1180,20 @@ def gemv_multi(x: torch.Tensor, w: torch.Tensor, y: torch.Tensor, norm_weight: O
     return y
 
 
+def gemv_multi_nf4(x: torch.Tensor, p, y: torch.Tensor, norm_weight: Optional[torch.Tensor] = None, eps: float = 0.0,
+                   residual: Optional[torch.Tensor] = None, mode: int = GEMV_PLAIN, n_heads: int = 0, n_kv_heads: int = 0, head_dim: int = 0,
+                   cos=None, sin=None, pos=None, kv_pages=None, page_table=None, page_size: int = 0) -> torch.Tensor:
+    """gemv_multi() streaming an Nf4W's planes: bit-identical to gemv_multi() over the dequantized matrix."""
+    _need(x, ELEM(), "gemv_multi_nf4.x")
+    T, K = x.shape
+    N = p.q.shape[0]
+    d = _nf4_desc(p)
+    check(_lib.load().srgpt_gemv_multi_nf4_bf16(_p(x), _rowmajor2d(x, "gemv_multi_nf4.x"), C.byref(d), _p(y), _rowmajor2d(y, "gemv_multi_nf4.y"), T, N, K,
+                                                _p(norm_weight), eps, _p(residual), mode, n_heads, n_kv_heads, head_dim, _p(cos), _p(sin), _p(pos),
+                                                _p(kv_pages), _p(page_table), page_size, _stream()), "srgpt_gemv_multi_nf4_bf16")
+    return y
+
+
 def lm_head_multi(x: torch.Tensor, w: torch.Tensor, norm_weight: Optional[torch.Tensor], eps: float, workspace: torch.Tensor,
                   logits_out: Optional[torch.Tensor] = None, packed=None) -> None:
     """Final norm + lm_head over the T rows of x [T, H]: fp32 logits [T, V] (optional) and the per-token arg max partials in
@@ -1177,14 +1238,20 @@ def spec_accept(workspace: torch.Tensor, V: int, T: int, draft_ids: torch.Tensor
 
 def llama_verify_step(h, layer_array, packed_array, n_layers: int, q_buf, attn_buf, act_buf, T: int, dims, cos, sin, pos, pos_rows, page_table,
                       page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, logits_rows, logits_all, prompt_ids, prompt_len, ngram: int, draft_ids,
-                      out_ids, step, state) -> None:
-    """One verify pass of T tokens (draft, layers, lm_head, accept); packed_array None = the bf16 weights."""
+                      out_ids, step, state, nf4_array=None) -> None:
+    """One verify pass of T tokens (draft, layers, lm_head, accept); packed_array None = the bf16 weights.  ``nf4_array``
+    (make_llama_nf4_array): every matrix with planes streamed by gemv_multi_nf4, lm_head from ``lm_packed`` or lm_head."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
     common_a = (T, dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(pos_rows), _p(page_table), page_size,
                 _p(final_norm), _p(lm_head))
     common_b = (dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(logits_all), _p(prompt_ids), _p(prompt_len), ngram, _p(draft_ids), _p(out_ids),
                 out_ids.numel(), _p(step), _p(state), _stream())
-    if packed_array is None:
+    if nf4_array is not None:
+        lm_d = _packed_desc(lm_packed)
+        check(_lib.load().srgpt_llama_verify_step_nf4_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(nf4_array, C.c_void_p), n_layers,
+                                                           _p(q_buf), _p(attn_buf), _p(act_buf), *common_a, C.byref(lm_d), *common_b),
+              "srgpt_llama_verify_step_nf4_bf16")
+    elif packed_array is None:
         check(_lib.load().srgpt_llama_verify_step_bf16(_p(h), C.cast(layer_array, C.c_void_p), n_layers, _p(q_buf), _p(attn_buf), _p(act_buf),
                                                        *common_a, *common_b), "srgpt_llama_verify_step_bf16")
     else:

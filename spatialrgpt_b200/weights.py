@@ -98,8 +98,9 @@ class LlamaLayerW:
     gateup_w: torch.Tensor  # [2 I, H], rows interleaved (gate_i, up_i)
     down_w: torch.Tensor  # [H, I]
     # quantization="nf4": {"qkv", "o", "gateup", "down"} -> the fused matrix's Nf4W planes, or None where K is not a multiple of 1024
-    # (the *_w tensors above are then the dequantized matrices).  quantization="fp8": the *_w fields hold Fp8W and there is no
-    # element-type copy of the matrices.
+    # (the *_w tensors above are then the dequantized matrices).  With nf4_dequantized_copy=False a matrix that has planes keeps no
+    # dequantized copy: its *_w field holds the same Nf4W.  quantization="fp8": the *_w fields hold Fp8W and there is no element-type
+    # copy of the matrices.
     nf4: Optional[Dict[str, Optional["Nf4W"]]] = None
 
 
@@ -110,6 +111,7 @@ class LlamaW:
     lm_head: torch.Tensor  # [V, H]
     layers: List[LlamaLayerW] = field(default_factory=list)
     quantization: Optional[str] = None  # None, "nf4" or "fp8" (the decoder-layer linears only)
+    nf4_dequantized_copy: bool = True  # quantization="nf4": False = the matrices with planes keep no element-type copy
 
 
 @dataclass
@@ -137,6 +139,10 @@ class Nf4W:
     uint8 codes in the GEMV's lane order, scale [N, K/64] fp32 resolved scales.  Built by ops.nf4_planes."""
     q: torch.Tensor
     scale: torch.Tensor
+
+    @property
+    def shape(self):
+        return (self.q.shape[0], self.q.shape[1] * 2)
 
     def nbytes(self) -> int:
         return self.q.numel() + self.scale.numel() * 4
@@ -219,19 +225,24 @@ def interleave_rows(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
 
 
 def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], device, n_tower_layers: Optional[int] = None,
-                     dtype: torch.dtype = BF16, quantization: Optional[str] = None) -> ModelWeights:
+                     dtype: torch.dtype = BF16, quantization: Optional[str] = None, nf4_dequantized_copy: bool = True) -> ModelWeights:
     """sd = {"vision_tower": ..., "region_extractor": ..., "mm_projector": ..., "llm": ...} with the
     reference's key names; tensors may live on the CPU in any float dtype.  ``dtype``: torch.bfloat16 or torch.float16.
     ``quantization="nf4"``: every decoder-layer linear (q/k/v/o/gate/up/down_proj) is NF4-quantized on the device as its own [out, in]
     matrix, before qkv is fused and gate/up interleaved (the reference's load_4bit, llava/model/builder.py:51-60); the layer keeps the
     dequantized matrices for every path and the NF4 planes for the batch-1 decode step.  Embeddings, lm_head, norms, towers, projector
     and region extractor stay unquantized.
+    ``nf4_dequantized_copy=False`` (only with ``quantization="nf4"``): a fused matrix with planes (K a multiple of 1024) drops its
+    dequantized copy once the planes are checked against it, and every path reads the planes (the NF4 GEMM, the one-token and multi-token
+    NF4 GEMVs), bit-identical to the copy.  Layer matrices take 4.5 bits per weight instead of 16 + 4.5.
     ``quantization="fp8"``: W8A8 with E4M3 codes (DESIGN.md §3): every decoder-layer linear is quantized on the device per output row, one
     matrix at a time, and the layer holds only the codes and row scales; every path (prefill, batched decode, beams, the one-token step)
     quantizes each activation row the same way before the FP8 GEMM.  Embeddings, lm_head, norms, towers, projector and region extractor
     stay unquantized."""
     if quantization not in (None, "nf4", "fp8"):
         raise ValueError(f"quantization={quantization!r}: supported are None, 'nf4' and 'fp8'")
+    if not nf4_dequantized_copy and quantization != "nf4":
+        raise ValueError(f"nf4_dequantized_copy=False needs quantization='nf4', not {quantization!r}")
     dev = torch.device(device)
 
     def g(d, k):
@@ -296,11 +307,12 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
 
     l, lc = sd["llm"], cfg.llama
     llama = LlamaW(embed=g(l, "model.embed_tokens.weight").contiguous(), norm=g(l, "model.norm.weight"),
-                   lm_head=g(l, "lm_head.weight" if "lm_head.weight" in l else "model.embed_tokens.weight").contiguous(), quantization=quantization)
+                   lm_head=g(l, "lm_head.weight" if "lm_head.weight" in l else "model.embed_tokens.weight").contiguous(), quantization=quantization,
+                   nf4_dequantized_copy=nf4_dequantized_copy)
     for i in range(lc.num_hidden_layers):
         p = f"model.layers.{i}."
         if quantization == "nf4":
-            llama.layers.append(_nf4_layer(l, p, g, dtype))
+            llama.layers.append(_nf4_layer(l, p, g, dtype, dequantized_copy=nf4_dequantized_copy))
             continue
         if quantization == "fp8":
             llama.layers.append(_fp8_layer(l, p, g, dtype))
@@ -315,9 +327,11 @@ def from_state_dicts(cfg: LlavaConfig, sd: Dict[str, Dict[str, torch.Tensor]], d
     return ModelWeights(vision, region, projector, llama)
 
 
-def _nf4_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> LlamaLayerW:
+def _nf4_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype, dequantized_copy: bool = True) -> LlamaLayerW:
     """One decoder layer with NF4 linears: each original matrix quantized and dequantized on its own, then the codes, scales and
-    dequantized matrices fused exactly as the plain layer's weights (q/k/v rows concatenated, gate/up rows interleaved)."""
+    dequantized matrices fused exactly as the plain layer's weights (q/k/v rows concatenated, gate/up rows interleaved).
+    dequantized_copy=False: a matrix with planes keeps only them (its *_w field holds the Nf4W); the layer's dequantized copies are
+    freed before it returns, so a load holds at most one layer's transient copies."""
     from . import ops
     with ops.elem_dtype(dtype):
         quant = {}
@@ -325,16 +339,22 @@ def _nf4_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> Lla
             key = p + ("self_attn." if n.endswith(("q_proj", "k_proj", "v_proj", "o_proj")) else "mlp.") + n + ".weight"
             codes, scale = ops.nf4_quantize(g(l, key).contiguous())
             quant[n] = (codes, scale, ops.nf4_dequantize(codes, scale))
-        fused = {
-            "qkv": [torch.cat([quant[n][k] for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous() for k in range(3)],
-            "o": list(quant["o_proj"]),
-            "gateup": [interleave_rows(quant["gate_proj"][k], quant["up_proj"][k]) for k in range(3)],
-            "down": list(quant["down_proj"]),
-        }
-        del quant
-        planes = {name: ops.nf4_planes(*f)[0] for name, f in fused.items()}
-    return LlamaLayerW(in_norm=g(l, p + "input_layernorm.weight"), qkv_w=fused["qkv"][2], o_w=fused["o"][2],
-                       post_norm=g(l, p + "post_attention_layernorm.weight"), gateup_w=fused["gateup"][2], down_w=fused["down"][2], nf4=planes)
+        # each original matrix is released as soon as its fused form exists (the load's transient stays about one layer)
+        fused = {"qkv": [torch.cat([quant[n][k] for n in ("q_proj", "k_proj", "v_proj")], 0).contiguous() for k in range(3)]}
+        for n in ("q_proj", "k_proj", "v_proj"):
+            del quant[n]
+        fused["o"] = list(quant.pop("o_proj"))
+        fused["gateup"] = [interleave_rows(quant["gate_proj"][k], quant["up_proj"][k]) for k in range(3)]
+        del quant["gate_proj"], quant["up_proj"]
+        fused["down"] = list(quant.pop("down_proj"))
+        planes, mats = {}, {}
+        for name in ("qkv", "o", "gateup", "down"):
+            codes, scale, deq = fused.pop(name)
+            planes[name] = ops.nf4_planes(codes, scale, deq)[0]
+            mats[name] = deq if dequantized_copy or planes[name] is None else planes[name]
+            del codes, scale, deq
+    return LlamaLayerW(in_norm=g(l, p + "input_layernorm.weight"), qkv_w=mats["qkv"], o_w=mats["o"],
+                       post_norm=g(l, p + "post_attention_layernorm.weight"), gateup_w=mats["gateup"], down_w=mats["down"], nf4=planes)
 
 
 def _fp8_layer(l: Dict[str, torch.Tensor], p: str, g, dtype: torch.dtype) -> LlamaLayerW:
