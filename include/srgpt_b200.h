@@ -275,6 +275,21 @@ int srgpt_argmax_bf16(const void* x, int ldx, int rows, int cols, long long* out
  * [n_beams, n_cand] (token -1 / score -inf when a row has fewer finite logits). */
 int srgpt_beam_candidates_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
                                float* cand_scores, int* cand_tokens, void* stream);
+/* Beam search over a batch of prompts (beam.cu): merges the candidates srgpt_beam_candidates_bf16 wrote for n_groups * k rows (prompt g
+ * owns rows g*k .. g*k+k-1).  Per prompt the n_cand best (score, beam within the prompt, token) in (score desc, beam asc, token asc)
+ * order, candidates with token < 0 dropped -> out_scores / out_beams / out_tokens [n_groups, n_cand] (score -inf, beam and token -1 where a
+ * prompt has fewer valid candidates).  One CTA per prompt; k * n_cand <= 4096. */
+int srgpt_beam_select(const float* cand_scores, const int* cand_tokens, int n_groups, int k, int n_cand, float* out_scores, int* out_beams,
+                      int* out_tokens, void* stream);
+/* Bytes of the workspace srgpt_kv_copy_pages needs for n_staged pairs (-1 on invalid arguments). */
+long long srgpt_kv_copy_workspace_bytes(int n_staged, int n_layers, int page_rows, int row_bytes);
+/* Copies rows of KV pages for K and V of every layer (beam.cu).  pages: [n_layers, n_pages, 2 (K, V), page_rows, row_bytes] bytes, the
+ * paged cache of the Llama decoder.  pairs: device int[n_pairs][4] = (src page, dst page, first row, rows); a pair outside the cache or
+ * the page is skipped.  The first n_staged pairs are staged through the workspace: one pass copies them there and every other pair
+ * straight to its destination, a second pass (a second launch, only when n_staged > 0) writes the staged ones.  So a pair whose
+ * destination is another pair's source must be staged; then any permutation is safe.  row_bytes a multiple of 16. */
+int srgpt_kv_copy_pages(void* pages, int n_layers, int n_pages, int page_rows, int row_bytes, const int* pairs, int n_pairs, int n_staged,
+                        void* workspace, long long workspace_bytes, void* stream);
 /* Temperature + nucleus (top-p) sampling of one token from fp32 logits [V] (sampling.cu): replaces HF's TemperatureLogitsWarper /
  * TopKLogitsWarper / TopPLogitsWarper / multinomial behind do_sample=True (llava/eval/eval_spatial.py:231-236, llava/eval/model_vqa.py:72-78).
  * params = device float[3] {temperature, top_p, top_k (0 = off)}; seed = device u64; the draw is a counter-based generator of

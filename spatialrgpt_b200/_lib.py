@@ -60,6 +60,9 @@ SIGNATURES = {
     "srgpt_argmax_f32": (ci, [vp, ci, ci, vp, vp]),
     "srgpt_argmax_bf16": (ci, [vp, ci, ci, ci, vp, vp]),
     "srgpt_beam_candidates_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp, vp]),
+    "srgpt_beam_select": (ci, [vp, vp, ci, ci, ci, vp, vp, vp, vp]),
+    "srgpt_kv_copy_workspace_bytes": (cll, [ci, ci, ci, ci]),
+    "srgpt_kv_copy_pages": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, vp, cll, vp]),
     "srgpt_sample_top_p_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp]),
     "srgpt_logits_process": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, ci, vp, ci, vp, vp, ci, vp, ci, vp, vp]),
     "srgpt_logits_pick_token": (ci, [vp, vp, ci, vp, vp, vp, ci, vp]),

@@ -1,0 +1,117 @@
+// Device side of beam search over a batch of prompts (llama_decoder.generate_beam_batch; DESIGN.md §7): the per-prompt merge of the
+// beam rows' candidates, and the KV page copies that replicate each prompt into its beams and make a beam's generated rows follow
+// its parent.
+#include "common.cuh"
+#include "srgpt_b200.h"
+
+namespace srgpt {
+
+constexpr int SELECT_THREADS = 256;
+constexpr int SELECT_MAX = 4096;  // k * n_cand candidates of one prompt, staged in shared memory
+
+// (score desc, beam asc, token asc): the flat-index order of HF's topk over a prompt's [num_beams x vocab] table on ties
+__device__ __forceinline__ bool select_before(float sa, int ba, int ta, float sb, int bb, int tb) {
+  return sa > sb || (sa == sb && (ba < bb || (ba == bb && ta < tb)));
+}
+
+// One CTA per prompt g: rows g*k .. g*k+k-1 of the candidates table.  Every valid candidate's rank is the number of valid candidates
+// before it in the merge order (the order is strict: a row holds each token once), so each lands in its slot with no sort state.
+__global__ void __launch_bounds__(SELECT_THREADS)
+beam_select_kernel(const float* __restrict__ cand_scores, const int* __restrict__ cand_tokens, int k, int n_cand, float* __restrict__ out_scores,
+                   int* __restrict__ out_beams, int* __restrict__ out_tokens) {
+  __shared__ float ss[SELECT_MAX];
+  __shared__ int st[SELECT_MAX];
+  __shared__ int n_valid;
+  const int N = k * n_cand;
+  const size_t in0 = (size_t)blockIdx.x * N, out0 = (size_t)blockIdx.x * n_cand;
+  if (threadIdx.x == 0) n_valid = 0;
+  int valid = 0;
+  for (int i = threadIdx.x; i < N; i += SELECT_THREADS) {
+    ss[i] = cand_scores[in0 + i];
+    st[i] = cand_tokens[in0 + i];
+    valid += st[i] >= 0;
+  }
+  __syncthreads();
+  atomicAdd(&n_valid, valid);
+  for (int i = threadIdx.x; i < N; i += SELECT_THREADS) {
+    const int t = st[i];
+    if (t < 0) continue;
+    const float s = ss[i];
+    const int b = i / n_cand;
+    int rank = 0;
+    for (int j = 0; j < N && rank < n_cand; ++j)
+      rank += st[j] >= 0 && select_before(ss[j], j / n_cand, st[j], s, b, t);
+    if (rank < n_cand) {
+      out_scores[out0 + rank] = s;
+      out_beams[out0 + rank] = b;
+      out_tokens[out0 + rank] = t;
+    }
+  }
+  __syncthreads();
+  for (int r = n_valid + threadIdx.x; r < n_cand; r += SELECT_THREADS) {  // fewer valid candidates than slots
+    out_scores[out0 + r] = -INFINITY;
+    out_beams[out0 + r] = -1;
+    out_tokens[out0 + r] = -1;
+  }
+}
+
+// KV page copies.  blockIdx.y = pair, blockIdx.x = layer * 2 + (0: K, 1: V); each unit is `rows` contiguous rows of one page half.
+// pass 0: pairs [0, n_staged) are copied into their workspace slot, the others straight to their destination page;
+// pass 1: the staged pairs go from the workspace to their destination.  A pair outside the cache or the page is skipped.
+constexpr int COPY_THREADS = 256;
+__global__ void __launch_bounds__(COPY_THREADS)
+kv_copy_kernel(uint8_t* __restrict__ pages, int n_pages, int page_rows, int row_bytes, const int4* __restrict__ pairs, int n_staged,
+               uint8_t* __restrict__ ws, int pass) {
+  const int p = blockIdx.y;
+  const int4 pr = pairs[p];  // (src page, dst page, first row, rows)
+  if (pr.x < 0 || pr.x >= n_pages || pr.y < 0 || pr.y >= n_pages || pr.z < 0 || pr.w < 0 || pr.z + pr.w > page_rows) return;
+  const int layer = blockIdx.x >> 1, half = blockIdx.x & 1;
+  const size_t half_bytes = (size_t)page_rows * row_bytes;
+  const size_t layer_bytes = (size_t)n_pages * 2 * half_bytes;
+  const size_t in_page = (size_t)half * half_bytes + (size_t)pr.z * row_bytes;
+  const size_t slot = ((size_t)p * gridDim.x + blockIdx.x) * half_bytes + (size_t)pr.z * row_bytes;  // this unit's rows in the workspace
+  const uint8_t* src = pass == 0 ? pages + layer * layer_bytes + (size_t)pr.x * 2 * half_bytes + in_page : ws + slot;
+  uint8_t* dst = pass == 0 && p < n_staged ? ws + slot : pages + layer * layer_bytes + (size_t)pr.y * 2 * half_bytes + in_page;
+  const int n16 = pr.w * row_bytes / 16;
+  for (int c = threadIdx.x; c < n16; c += COPY_THREADS) reinterpret_cast<uint4*>(dst)[c] = reinterpret_cast<const uint4*>(src)[c];
+}
+
+}  // namespace srgpt
+
+using namespace srgpt;
+
+extern "C" __attribute__((visibility("default"))) int srgpt_beam_select(const float* cand_scores, const int* cand_tokens, int n_groups, int k,
+                                                                        int n_cand, float* out_scores, int* out_beams, int* out_tokens, void* stream) {
+  SRGPT_CHECK_ARG(cand_scores && cand_tokens && out_scores && out_beams && out_tokens && n_groups > 0 && k > 0 && n_cand > 0);
+  SRGPT_CHECK_ARG((long long)k * n_cand <= SELECT_MAX);
+  beam_select_kernel<<<n_groups, SELECT_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(cand_scores, cand_tokens, k, n_cand, out_scores,
+                                                                                              out_beams, out_tokens);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) long long srgpt_kv_copy_workspace_bytes(int n_staged, int n_layers, int page_rows, int row_bytes) {
+  if (n_staged < 0 || n_layers <= 0 || page_rows <= 0 || row_bytes <= 0) return -1;
+  return (long long)n_staged * n_layers * 2 * page_rows * row_bytes;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_kv_copy_pages(void* pages, int n_layers, int n_pages, int page_rows, int row_bytes,
+                                                                          const int* pairs, int n_pairs, int n_staged, void* workspace,
+                                                                          long long workspace_bytes, void* stream) {
+  SRGPT_CHECK_ARG(pages && pairs && n_layers > 0 && n_pages > 0 && page_rows > 0 && row_bytes > 0 && (row_bytes % 16) == 0);
+  SRGPT_CHECK_ARG(n_pairs > 0 && n_pairs <= 65535 && n_staged >= 0 && n_staged <= n_pairs && 2 * n_layers <= 65535);
+  SRGPT_CHECK_ARG(((reinterpret_cast<uintptr_t>(pages) | reinterpret_cast<uintptr_t>(pairs) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0);
+  SRGPT_CHECK_ARG(n_staged == 0 || (workspace && workspace_bytes >= srgpt_kv_copy_workspace_bytes(n_staged, n_layers, page_rows, row_bytes)));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int4* pr = reinterpret_cast<const int4*>(pairs);
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  kv_copy_kernel<<<dim3(2 * n_layers, n_pairs), COPY_THREADS, 0, st>>>(reinterpret_cast<uint8_t*>(pages), n_pages, page_rows, row_bytes, pr,
+                                                                        n_staged, ws, 0);
+  SRGPT_CHECK_LAUNCH();
+  if (n_staged > 0) {
+    kv_copy_kernel<<<dim3(2 * n_layers, n_staged), COPY_THREADS, 0, st>>>(reinterpret_cast<uint8_t*>(pages), n_pages, page_rows, row_bytes, pr,
+                                                                           n_staged, ws, 1);
+    SRGPT_CHECK_LAUNCH();
+  }
+  return SRGPT_OK;
+}

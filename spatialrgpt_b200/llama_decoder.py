@@ -51,6 +51,73 @@ def first_stop(host_ids, lo: int, hi: int, eos, stopping_fn, limit: int) -> Opti
     return limit if hi >= limit else None
 
 
+class BeamHypotheses:
+    """The host bookkeeping of one prompt's beam search (HF BeamSearchScorer.process / finalize for one batch entry): the running beams'
+    tokens and scores, the kept hypotheses and the done flag.  ``advance`` takes the prompt's ranked candidates of one step."""
+
+    def __init__(self, k: int, eos, length_penalty: float, early_stopping: bool):
+        self.k, self.eos, self.length_penalty, self.early_stopping = k, eos, length_penalty, early_stopping
+        self.seqs: List[List[int]] = [[] for _ in range(k)]
+        self.scores = [0.0] + [-1e9] * (k - 1)
+        self.hyps: List = []  # (score, tokens) of finished hypotheses, at most k kept
+        self.worst, self.done = 1e9, False
+
+    def keep(self, score: float, toks: List[int]) -> None:
+        if len(self.hyps) < self.k or score > self.worst:
+            self.hyps.append((score, toks))
+            if len(self.hyps) > self.k:
+                self.hyps.remove(min(self.hyps, key=lambda x: x[0]))
+            self.worst = min(x[0] for x in self.hyps)
+
+    def advance(self, ranked, cur_len: int) -> List[int]:
+        """ranked: (score, beam, token) in (score desc, beam asc, token asc) order, at most 2k (or (1 + #EOS) k) of them.  An EOS of rank
+        < k closes a hypothesis; the other candidates become the next beams.  Returns each next beam's parent beam."""
+        nxt = []
+        for rank, (sc, b, t) in enumerate(ranked):
+            if t in self.eos:
+                if rank >= self.k:
+                    continue
+                self.keep(sc / (cur_len ** self.length_penalty), list(self.seqs[b]))
+            else:
+                nxt.append((sc, b, t))
+            if len(nxt) == self.k:
+                break
+        if len(nxt) < self.k:
+            raise RuntimeError("beam search ran out of non-EOS candidates")  # HF asserts the same
+        if len(self.hyps) >= self.k and (self.early_stopping or self.worst >= ranked[0][0] / (cur_len ** self.length_penalty)):
+            self.done = True
+        self.seqs = [self.seqs[b] + [t] for _, b, t in nxt]
+        self.scores = [sc for sc, _, _ in nxt]
+        return [b for _, b, _ in nxt]
+
+    def best(self, max_new_tokens: int) -> List[int]:
+        """finalize (beam_search.py): unless done, the running beams become hypotheses over their generated length; the best one, with the
+        first EOS appended when it is shorter than max_new_tokens."""
+        if not self.done:
+            for i in range(self.k):
+                self.keep(self.scores[i] / (len(self.seqs[i]) ** self.length_penalty), list(self.seqs[i]))
+        best = list(max(self.hyps, key=lambda x: x[0])[1])
+        if len(best) < max_new_tokens and self.eos:
+            best.append(self.eos[0])
+        return best
+
+
+def beam_page_pairs(tables: List[List[int]], parents: List[int], starts: List[int], n_gen: int, page_size: int = PAGE_SIZE):
+    """The KV copies that make every moved row (parents[r] != r) hold its parent's generated rows: positions [starts[r], starts[r] + n_gen)
+    of each, page by page, as (src page, dst page, first row, rows) over the page tables ``tables``.  Returns (pairs, n_staged): a pair
+    whose destination row is itself some row's parent is listed first and staged (kv_copy_pages), so cycles and chains are safe."""
+    sources = {p for r, p in enumerate(parents) if p != r}
+    staged, direct = [], []
+    for r, p in enumerate(parents):
+        if p == r or n_gen <= 0:
+            continue
+        s0, s1 = starts[r], starts[r] + n_gen
+        for j in range(s0 // page_size, (s1 - 1) // page_size + 1):
+            lo, hi = max(s0, j * page_size) - j * page_size, min(s1, (j + 1) * page_size) - j * page_size
+            (staged if r in sources else direct).append((tables[p][j], tables[r][j], lo, hi - lo))
+    return staged + direct, len(staged)
+
+
 class PagedKVCache:
     """KV pages for all layers: [layers, n_pages, 2 (k,v), PAGE_SIZE, n_kv_heads, head_dim] bf16, a free list
     and per-sequence page tables (int32, device) of fixed capacity so decode graphs stay valid."""
@@ -306,10 +373,11 @@ class LlamaDecoder:
                                         nf4_array=self._planes_array)
 
     @ops.in_own_dtype
-    def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int]) -> torch.Tensor:
-        """Prefill `len(seq_lens)` prompts packed back to back ([sum S_b, H]) into sequence slots 0..B-1 in ONE pass:
-        every GEMM runs over all rows, attention / RoPE / KV append per sequence (the unpadded varlen path of
-        modeling_llama.py:540-562).  The caller has reserved the pages.  Returns the final residual stream, packed."""
+    def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int], page_tables: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Prefill `len(seq_lens)` prompts packed back to back ([sum S_b, H]) into sequence slots 0..B-1 (or the rows of
+        ``page_tables``, a row-strided view of the cache's tables) in ONE pass: every GEMM runs over all rows, attention / RoPE / KV
+        append per sequence (the unpadded varlen path of modeling_llama.py:540-562).  The caller has reserved the pages.  Returns the
+        final residual stream, packed."""
         d = self.dims
         B = len(seq_lens)
         if packed_embeds.shape[0] != sum(seq_lens) or B < 1 or min(seq_lens) < 1:
@@ -320,7 +388,8 @@ class LlamaDecoder:
         cu = torch.tensor([0] + list(torch.tensor(seq_lens).cumsum(0).tolist()), dtype=torch.int32).to(self.device)
         sp = torch.zeros(B, dtype=torch.int32, device=self.device)
         x = packed_embeds.to(self.dtype).contiguous().clone()
-        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, self.cache.page_tables[:B],
+        pts = self.cache.page_tables[:B] if page_tables is None else page_tables
+        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pts,
                                         PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens), nf4_array=self._planes_array)
 
     @ops.in_own_dtype
@@ -803,27 +872,15 @@ class LlamaDecoder:
         st = self._batch_state(k)
         st["logits"][:, :V].copy_(lg)
         dev = self.device
-        beam_scores = torch.full((k,), -1e9, dtype=torch.float32)
-        beam_scores[0] = 0.0
-        d_scores = beam_scores.to(dev)
+        hyp = BeamHypotheses(k, eos, length_penalty, early_stopping)
+        d_scores = torch.tensor(hyp.scores, dtype=torch.float32).to(dev)
         cand_s = torch.empty((k, n_cand), dtype=torch.float32, device=dev)
         cand_t = torch.empty((k, n_cand), dtype=torch.int32, device=dev)
         h_s = torch.empty((k, n_cand), dtype=torch.float32, pin_memory=True)
         h_t = torch.empty((k, n_cand), dtype=torch.int32, pin_memory=True)
-        seqs: List[List[int]] = [[] for _ in range(k)]
-        hyps: List = []  # (score, tokens) of finished hypotheses, at most k kept
-        worst, done = 1e9, False
         zero = torch.zeros(k, dtype=torch.int32, device=dev)
         tables = [list(self.cache.owned[b]) for b in range(k)]  # page ids by position // PAGE_SIZE
         pages_all = self.cache.pages
-
-        def keep(score: float, toks: List[int]) -> None:
-            nonlocal worst
-            if len(hyps) < k or score > worst:
-                hyps.append((score, toks))
-                if len(hyps) > k:
-                    hyps.remove(min(hyps, key=lambda x: x[0]))
-                worst = min(x[0] for x in hyps)
 
         for step in range(max_new_tokens):
             ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t)
@@ -832,31 +889,13 @@ class LlamaDecoder:
             torch.cuda.current_stream().synchronize()
             # merge the per-beam candidates: (score desc, beam asc, token asc) = the flat-index order of HF's topk on ties
             flat = sorted(((-float(h_s[b, j]), b, int(h_t[b, j])) for b in range(k) for j in range(n_cand) if int(h_t[b, j]) >= 0))[:n_cand]
-            cur_len = step + 1
-            nxt = []
-            for rank, (neg, b, t) in enumerate(flat):
-                sc = -neg
-                if t in eos:
-                    if rank >= k:
-                        continue
-                    keep(sc / (cur_len ** length_penalty), list(seqs[b]))
-                else:
-                    nxt.append((sc, b, t))
-                if len(nxt) == k:
-                    break
-            if len(nxt) < k:
-                raise RuntimeError("beam search ran out of non-EOS candidates")  # HF asserts the same
-            if len(hyps) >= k and (early_stopping or worst >= (-flat[0][0]) / (cur_len ** length_penalty)):
-                done = True
-            seqs = [seqs[b] + [t] for _, b, t in nxt]
-            beam_scores = torch.tensor([sc for sc, _, _ in nxt], dtype=torch.float32)
-            if done or step == max_new_tokens - 1:
+            parents = hyp.advance([(-neg, b, t) for neg, b, t in flat], step + 1)
+            if hyp.done or step == max_new_tokens - 1:
                 break
-            if stopping_fn is not None and all(stopping_fn(torch.tensor(q, dtype=torch.int64)) for q in seqs):
+            if stopping_fn is not None and all(stopping_fn(torch.tensor(q, dtype=torch.int64)) for q in hyp.seqs):
                 break  # KeywordsStoppingCriteria.__call__ requires every row (beam) to have hit (mm_utils.py:616-617)
             # ---- device state of the next step: KV rows of the generated region follow their parents (HF _reorder_cache,
             #      modeling_llama.py:1151-1158, copies the WHOLE cache; here only the pages that hold generated tokens)
-            parents = [b for _, b, _ in nxt]
             if step > 0 and any(p != i for i, p in enumerate(parents)):
                 j0, j1 = S // PAGE_SIZE, (S + step - 1) // PAGE_SIZE
                 src = [tables[p][j] for i, p in enumerate(parents) if p != i for j in range(j0, j1 + 1)]
@@ -864,22 +903,99 @@ class LlamaDecoder:
                 src_t = torch.tensor(src, dtype=torch.int64).to(dev)
                 dst_t = torch.tensor(dst, dtype=torch.int64).to(dev)
                 pages_all[:, dst_t] = pages_all[:, src_t]  # gather into a temporary, then scatter: permutations are safe
-            ids = torch.tensor([t for _, _, t in nxt], dtype=torch.int32).to(dev)
+            ids = torch.tensor([q[-1] for q in hyp.seqs], dtype=torch.int32).to(dev)
             st["h"].copy_(ops.splice_rows(w.embed, None, None, None, zero, ids))
             st["pos"].fill_(S + step)
-            d_scores.copy_(beam_scores, non_blocking=True)
+            d_scores.copy_(torch.tensor(hyp.scores, dtype=torch.float32), non_blocking=True)
             if use_graph:  # the warm-up before the capture rewrites only this step's own KV rows
                 self._capture(("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), self._batch_kernels_per_layer * d.num_hidden_layers + 2)
                 self._replay(("beam", k))
             else:
                 self._batch_step_launch(st, logits_only=True)
-        if not done:  # finalize (beam_search.py): the running beams become hypotheses over their generated length
-            for i in range(k):
-                keep(float(beam_scores[i]) / (len(seqs[i]) ** length_penalty), list(seqs[i]))
-        best = list(max(hyps, key=lambda x: x[0])[1])
-        if len(best) < max_new_tokens and eos:
-            best.append(eos[0])
+        best = hyp.best(max_new_tokens)
         return torch.tensor(best, dtype=torch.int64, device=dev)
+
+    @torch.no_grad()
+    @ops.in_own_dtype
+    def generate_beam_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], num_beams: int, max_new_tokens: int, eos_token_ids=None,
+                            stopping_fn=None, length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True) -> List[torch.Tensor]:
+        """Beam search over B prompts packed back to back ([sum S_b, H]) at once (HF beam_search + BeamSearchScorer with batch_size = B).
+        Row g * k + i of every step is beam i of prompt g, so one batched decode step serves all B * k beams.  Device side: ONE packed
+        prefill of the B prompts, their pages copied into the other k - 1 beams of each (kv_copy_pages), then per step the candidates
+        kernel over all rows, the per-prompt merge (beam_select) whose B x n_cand results reach the host through pinned memory, and the
+        copy of the generated KV rows of every beam whose parent is another beam.  Host side: one BeamHypotheses per prompt.  A prompt
+        that is done keeps its rows in the step (the graph shape stays fixed) and its choices are ignored.  The loop ends when every
+        prompt is done, at max_new_tokens, or when ``stopping_fn`` holds for every beam of the prompts still running.  Returns a list
+        of B LongTensors of NEW ids, each prompt's best hypothesis."""
+        d, w, k, B = self.dims, self.w, int(num_beams), len(seq_lens)
+        V, R, dev = d.vocab_size, B * int(num_beams), self.device
+        seq_lens = [int(n) for n in seq_lens]
+        if k < 2:
+            raise ValueError("generate_beam_batch needs num_beams >= 2")
+        if B < 1 or packed_embeds.shape[0] != sum(seq_lens) or min(seq_lens) < 1:
+            raise RuntimeError("generate_beam_batch: rows do not match seq_lens")
+        if max_new_tokens < 1:
+            return [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
+        if max(seq_lens) + max_new_tokens > self.max_seq_len:
+            raise RuntimeError(f"{max(seq_lens)} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
+        eos = eos_list(eos_token_ids)
+        n_cand = max(2, 1 + len(eos)) * k
+        for b in range(len(self.cache.owned)):
+            self.cache.release(b)
+        self.ensure_capacity(R, max(seq_lens) + max_new_tokens)
+        starts = [n for n in seq_lens for _ in range(k)]  # row r = g * k + i: the first generated position of its prompt
+        self.cache.reserve_many([n + max_new_tokens for n in starts])
+        tables = [list(self.cache.owned[r]) for r in range(R)]
+        # the prompts are prefilled once, into beam 0 of each; the other beams get copies of its prompt rows
+        hidden = self.prefill_packed(packed_embeds, seq_lens, page_tables=self.cache.page_tables[:R:k])
+        ops.kv_copy_pages(self.cache.pages, [(tables[g * k][j], tables[g * k + i][j], 0, min(PAGE_SIZE, seq_lens[g] - j * PAGE_SIZE))
+                                             for g in range(B) for i in range(1, k) for j in range((seq_lens[g] + PAGE_SIZE - 1) // PAGE_SIZE)])
+        st = self._batch_state(R)
+        # every beam row starts from its prompt's last hidden row: final norm + lm_head over the R rows
+        last = torch.tensor([sum(seq_lens[:g + 1]) - 1 for g in range(B) for _ in range(k)], dtype=torch.int32).to(dev)
+        rows = ops.splice_rows(hidden, None, None, None, torch.zeros_like(last), last)
+        ops.rmsnorm(rows, w.norm, d.rms_norm_eps, out=st["xn"])
+        ops.gemm(st["xn"], w.lm_head, out=st["logits"][:, :V])
+        groups = [BeamHypotheses(k, eos, length_penalty, early_stopping) for _ in range(B)]
+        d_scores = torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32).to(dev)
+        cand_s = torch.empty((R, n_cand), dtype=torch.float32, device=dev)
+        cand_t = torch.empty((R, n_cand), dtype=torch.int32, device=dev)
+        sel = torch.empty((3, B, n_cand), dtype=torch.int32, device=dev)  # the merge's scores (as bits), beams, tokens: one copy to the host
+        h_sel = torch.empty((3, B, n_cand), dtype=torch.int32, pin_memory=True)
+        h_scores = h_sel[0].view(torch.float32)
+        zero = torch.zeros(R, dtype=torch.int32, device=dev)
+        tokens = [0] * R  # the token each row feeds to the next step (a done prompt's rows repeat theirs)
+        for step in range(max_new_tokens):
+            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t)
+            ops.beam_select(cand_s, cand_t, k, sel[0].view(torch.float32), sel[1], sel[2])
+            h_sel.copy_(sel, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+            scores, beams, toks = h_scores.tolist(), h_sel[1].tolist(), h_sel[2].tolist()
+            parents = list(range(R))
+            for g, grp in enumerate(groups):
+                if grp.done:
+                    continue
+                ranked = [(scores[g][j], beams[g][j], toks[g][j]) for j in range(n_cand) if toks[g][j] >= 0]
+                for i, b in enumerate(grp.advance(ranked, step + 1)):
+                    parents[g * k + i] = g * k + b
+                    tokens[g * k + i] = grp.seqs[i][-1]
+            if all(grp.done for grp in groups) or step == max_new_tokens - 1:
+                break
+            if stopping_fn is not None and all(stopping_fn(torch.tensor(q, dtype=torch.int64)) for grp in groups if not grp.done for q in grp.seqs):
+                break  # HF evaluates the criterion over the whole expanded batch; the rows of a finished prompt no longer matter
+            # the generated KV rows [S_g, S_g + step) follow their parents (the prompt rows are the same in every beam of a prompt)
+            pairs, n_staged = beam_page_pairs(tables, parents, starts, step)
+            ops.kv_copy_pages(self.cache.pages, pairs, n_staged)
+            st["h"].copy_(ops.splice_rows(w.embed, None, None, None, zero, torch.tensor(tokens, dtype=torch.int32).to(dev)))
+            st["pos"].copy_(torch.tensor([n + step for n in starts], dtype=torch.int32))
+            d_scores.copy_(torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32))
+            if use_graph:  # keyed by the row count, as generate_beam's graph: the same launch over the same buffers
+                self._capture(("beam", R), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],),
+                              self._batch_kernels_per_layer * d.num_hidden_layers + 2)
+                self._replay(("beam", R))
+            else:
+                self._batch_step_launch(st, logits_only=True)
+        return [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
 
     @torch.no_grad()
     @ops.in_own_dtype

@@ -457,6 +457,8 @@ class LlavaLlamaModel:
                 raise NotImplementedError("prompt_lookup_num_tokens with quantization='fp8' (the verify pass has no FP8 form)")
             if not getattr(self.llm, "supports_prompt_lookup", False):
                 raise NotImplementedError("prompt_lookup_num_tokens on the tensor-parallel decoder")
+        if num_beams != 1 and (not hasattr(self.llm, "generate_beam") or type(self.llm).__name__ == "TPLlamaDecoder"):
+            raise NotImplementedError("beam search on the tensor-parallel decoder")
         prefix = None
         if prefix_cache:
             if input_ids is None or input_ids.shape[0] != 1:
@@ -497,13 +499,9 @@ class LlavaLlamaModel:
         if lookup_k and B != 1:
             raise NotImplementedError("prompt_lookup_num_tokens serves batch-1 requests")
         left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
-        if num_beams != 1 and B != 1:
-            raise NotImplementedError("beam search over a batch of prompts (the reference's eval scripts run batch 1)")
         if B == 1 and num_beams != 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
-            if not hasattr(self.llm, "generate_beam") or type(self.llm).__name__ == "TPLlamaDecoder":
-                raise NotImplementedError("beam search on the tensor-parallel decoder")
             outs.append(self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                                length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph))
         elif B == 1:
@@ -535,16 +533,20 @@ class LlavaLlamaModel:
             outs.append(r)
         else:
             # batch > 1: one packed prefill over all prompts (llava_arch.py:549-611 pads, modeling_llama.py:540-562 unpads
-            # again; here the rows were never padded), then per-sequence decode
+            # again; here the rows were never padded), then per-sequence decode, or beam search with every prompt's beams in one step
             if packed is None:
                 T = inputs_embeds.shape[1]
                 packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
-            r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                        use_graph=use_graph, return_logits=return_logits, sampling=sampling, **proc)
-            if return_logits:
-                outs, all_logits = r
+            if num_beams != 1:
+                outs = self.llm.generate_beam_batch(packed, lens, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
+                                                    length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph)
             else:
-                outs = r
+                r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
+                                            use_graph=use_graph, return_logits=return_logits, sampling=sampling, **proc)
+                if return_logits:
+                    outs, all_logits = r
+                else:
+                    outs = r
         n_max = max(o.numel() for o in outs)
         seqs = torch.full((B, n_max), int(pad), dtype=torch.int64, device=self.device)
         for b, o in enumerate(outs):

@@ -901,6 +901,56 @@ def beam_candidates(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores
                                                  _p(cand_scores), _p(cand_tokens), _stream()), "srgpt_beam_candidates_bf16")
 
 
+def beam_select(cand_scores: torch.Tensor, cand_tokens: torch.Tensor, k: int, out_scores: torch.Tensor, out_beams: torch.Tensor,
+                out_tokens: torch.Tensor) -> None:
+    """Per prompt (k consecutive rows of the [G * k, n_cand] candidates of beam_candidates): its n_cand best (score, beam in the prompt,
+    token) in (score desc, beam asc, token asc) order, token < 0 dropped -> out_* [G, n_cand] (-inf / -1 / -1 past the valid ones)."""
+    _need(cand_scores, torch.float32, "beam_select.cand_scores"); _need(cand_tokens, torch.int32, "beam_select.cand_tokens")
+    _need(out_scores, torch.float32, "beam_select.out_scores"); _need(out_beams, torch.int32, "beam_select.out_beams")
+    _need(out_tokens, torch.int32, "beam_select.out_tokens")
+    rows, n_cand = cand_scores.shape
+    if k < 1 or rows % k or cand_tokens.shape != cand_scores.shape or not cand_scores.is_contiguous() or not cand_tokens.is_contiguous():
+        raise SrgptError("beam_select: candidates must be contiguous [n_groups * k, n_cand] scores and tokens")
+    G = rows // k
+    for o in (out_scores, out_beams, out_tokens):
+        if tuple(o.shape) != (G, n_cand) or not o.is_contiguous():
+            raise SrgptError(f"beam_select: outputs must be contiguous [{G}, {n_cand}]")
+    check(_lib.load().srgpt_beam_select(_p(cand_scores), _p(cand_tokens), G, k, n_cand, _p(out_scores), _p(out_beams), _p(out_tokens), _stream()),
+          "srgpt_beam_select")
+
+
+_KV_COPY_WS = {}  # device -> staging buffer of kv_copy_pages, grown on demand
+
+
+def kv_copy_pages(pages: torch.Tensor, pairs, n_staged: int = 0) -> None:
+    """Copies KV rows between pages of the paged cache pages [L, n_pages, 2, page_rows, n_kv_heads, head_dim] for K and V of every layer.
+    pairs: a host int list / tensor [n, 4] of (src page, dst page, first row, rows).  The first n_staged pairs go through a workspace, so
+    a pair whose destination is another pair's source must be among them (llama_decoder.beam_page_pairs orders them so)."""
+    if not pages.is_cuda or pages.dim() != 6 or not pages.is_contiguous():
+        raise SrgptError("kv_copy_pages: expected the contiguous CUDA KV cache [L, n_pages, 2, page_rows, n_kv_heads, head_dim]")
+    L, n_pages, _, page_rows = pages.shape[:4]
+    row_bytes = pages.shape[4] * pages.shape[5] * pages.element_size()
+    host = torch.as_tensor(pairs, dtype=torch.int32).reshape(-1, 4)
+    n = host.shape[0]
+    if n == 0:
+        return
+    if not 0 <= n_staged <= n:
+        raise SrgptError(f"kv_copy_pages: n_staged {n_staged} outside [0, {n}]")
+    src, dst, lo, cnt = host.unbind(1)
+    if bool(((src < 0) | (src >= n_pages) | (dst < 0) | (dst >= n_pages) | (lo < 0) | (cnt < 0) | (lo + cnt > page_rows)).any()):
+        raise SrgptError(f"kv_copy_pages: a pair lies outside the {n_pages} pages of {page_rows} rows")
+    lib = _lib.load()
+    ws_bytes = int(lib.srgpt_kv_copy_workspace_bytes(n_staged, L, page_rows, row_bytes))
+    ws = _KV_COPY_WS.get(pages.device)
+    if n_staged and (ws is None or ws.numel() < ws_bytes):
+        ws = _KV_COPY_WS[pages.device] = torch.empty(ws_bytes, dtype=torch.uint8, device=pages.device)
+    d_pairs = host.to(pages.device, non_blocking=False)
+    check(lib.srgpt_kv_copy_pages(_p(pages), L, n_pages, page_rows, row_bytes, _p(d_pairs), n, n_staged, _p(ws) if n_staged else None,
+                                  ws_bytes if n_staged else 0, _stream()), "srgpt_kv_copy_pages")
+    if n_staged:
+        _count(1)
+
+
 def argmax_f32(x: torch.Tensor) -> torch.Tensor:
     _need(x, torch.float32, "argmax_f32.x")
     rows, cols = x.shape
