@@ -298,6 +298,12 @@ int srgpt_kv_copy_pages(void* pages, int n_layers, int n_pages, int page_rows, i
  * srgpt_lm_head_argmax_bf16 / srgpt_llama_decode_step_bf16 (which advanced *step) with step_offset = -1. */
 int srgpt_sample_top_p_f32(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step, int step_offset,
                            long long* out_ids, const void* embed_table, void* next_x, int K, void* stream);
+/* The same draw for R rows in one launch (sampling.cu, one 1024-thread CTA per row): logits [R, ld], fp32 (logits_f32 = 1) or the element
+ * type (the rows of the batched lm_head GEMM).  Row r draws with seeds[r] (device u64[R]) at counter *step + step_offset and writes
+ * ids[r] (int64); no embedding row is written (srgpt_decode_batch_advance does that).  Row r's token equals what srgpt_sample_top_p_f32
+ * draws from that row converted to fp32 with seed seeds[r] and the same counter.  R <= 65535, ld >= V. */
+int srgpt_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
+                      const int* step, int step_offset, long long* ids, void* stream);
 /* HF's logits processors on the device (logits_process.cu): replaces RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
  * NoBadWordsLogitsProcessor, MinLengthLogitsProcessor and MinNewTokensLengthLogitsProcessor (transformers generation/logits_process.py),
  * which HF runs on the host behind generate(repetition_penalty=, no_repeat_ngram_size=, bad_words_ids=, min_length=, min_new_tokens=)

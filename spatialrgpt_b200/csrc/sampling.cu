@@ -11,6 +11,8 @@
 // The draw uses a counter-based generator (splitmix64 of seed and step), so a request is reproducible given its seed; it is
 // NOT torch's Philox stream, so sampled ids are comparable with the reference in distribution only (tests check the support and
 // the frequencies against the torch nucleus).  Greedy decoding (the graded mode) never runs this kernel.
+// A batch of sequences draws in one launch of sample_rows_kernel: one such CTA per row, the same arithmetic (sample_row) over fp32 rows or
+// the element-type rows of the batched lm_head, each row with its own seed.
 #include "common.cuh"
 #include "srgpt_b200.h"
 
@@ -45,10 +47,14 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
   return x ^ (x >> 31);
 }
 
-// params = {temperature, top_p, top_k (0 = off)} and the seed live in device memory, so one captured CUDA graph serves any request
-__global__ void __launch_bounds__(THREADS)
-sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step,
-                    int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table, bf16* __restrict__ next_x, int K) {
+__device__ __forceinline__ float logit(const float* __restrict__ x, int i) { return x[i]; }
+__device__ __forceinline__ float logit(const bf16* __restrict__ x, int i) { return e2f(x[i]); }  // exact: torch's .float() of the row
+
+// The draw of one row of V logits (fp32 or the element type) by the whole 1024-thread CTA; every thread returns the token.
+// params = {temperature, top_p, top_k (0 = off)} and the seed live in device memory, so one captured CUDA graph serves any request.
+template <typename T>
+__device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, const float* __restrict__ params,
+                                          const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step, int step_offset) {
   __shared__ float red[32];
   __shared__ float s_scan[THREADS];
   __shared__ int s_tok;
@@ -61,10 +67,10 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
   const int lo = min(V, tid * per), hi = min(V, lo + per);
 
   float m = -INFINITY;
-  for (int i = lo; i < hi; ++i) m = fmaxf(m, logits[i]);
+  for (int i = lo; i < hi; ++i) m = fmaxf(m, logit(logits, i));
   m = block_reduce_max(m, red);
   float z = 0.f;
-  for (int i = lo; i < hi; ++i) z += __expf((logits[i] - m) * inv_t);
+  for (int i = lo; i < hi; ++i) z += __expf((logit(logits, i) - m) * inv_t);
   z = block_reduce_sum(z, red);
   const float inv_z = 1.0f / z;
 
@@ -76,14 +82,14 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
     for (int it = 0; it < 26; ++it) {
       const float mid = 0.5f * (lo_t + hi_t);
       float c = 0.f;
-      for (int i = lo; i < hi; ++i) c += (__expf((logits[i] - m) * inv_t) * inv_z >= mid) ? 1.f : 0.f;
+      for (int i = lo; i < hi; ++i) c += (__expf((logit(logits, i) - m) * inv_t) * inv_z >= mid) ? 1.f : 0.f;
       c = block_reduce_sum(c, red);
       if (c >= (float)top_k) lo_t = mid; else hi_t = mid;
     }
     t_floor = lo_t;
     float s = 0.f;
     for (int i = lo; i < hi; ++i) {
-      const float p = __expf((logits[i] - m) * inv_t) * inv_z;
+      const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
       s += (p >= t_floor) ? p : 0.f;
     }
     mass_floor = block_reduce_sum(s, red);
@@ -99,7 +105,7 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
       const float mid = 0.5f * (lo_t + hi_t);
       float s = 0.f;
       for (int i = lo; i < hi; ++i) {
-        const float p = __expf((logits[i] - m) * inv_t) * inv_z;
+        const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
         s += (p >= mid) ? p : 0.f;
       }
       s = block_reduce_sum(s, red);
@@ -115,7 +121,7 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
   const float u = ((float)(r >> 40) + 0.5f) * (1.0f / 16777216.0f) * mass;  // (0, mass)
   float local = 0.f;
   for (int i = lo; i < hi; ++i) {
-    const float p = __expf((logits[i] - m) * inv_t) * inv_z;
+    const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
     local += (p >= t_keep) ? p : 0.f;
   }
   s_scan[tid] = local;
@@ -136,7 +142,7 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
     float acc = before;
     int pick = -1, last_kept = -1;
     for (int i = lo; i < hi; ++i) {
-      const float p = __expf((logits[i] - m) * inv_t) * inv_z;
+      const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
       if (p >= t_keep) {
         last_kept = i;
         acc += p;
@@ -151,7 +157,7 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = lo; i < hi; ++i)
-      if (logits[i] > best) { best = logits[i]; bi = i; }
+      if (logit(logits, i) > best) { best = logit(logits, i); bi = i; }
     __shared__ float sb[THREADS];
     __shared__ int si[THREADS];
     sb[tid] = best; si[tid] = bi;
@@ -164,11 +170,29 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
     __syncthreads();
     tok = s_tok;
   }
-  if (tid == 0) out_ids[*step + step_offset] = (long long)tok;
+  return tok;
+}
+
+__global__ void __launch_bounds__(THREADS)
+sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step,
+                    int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table, bf16* __restrict__ next_x, int K) {
+  const int tok = sample_row(logits, V, params, seed_ptr, step, step_offset);
+  if (threadIdx.x == 0) out_ids[*step + step_offset] = (long long)tok;
   if (embed_table != nullptr && next_x != nullptr) {
     const uint4* src = reinterpret_cast<const uint4*>(embed_table + (size_t)tok * K);
-    for (int c = tid; c < (K >> 3); c += THREADS) reinterpret_cast<uint4*>(next_x)[c] = src[c];
+    for (int c = threadIdx.x; c < (K >> 3); c += THREADS) reinterpret_cast<uint4*>(next_x)[c] = src[c];
   }
+}
+
+// R rows at once, one CTA per row: row r = logits + r * ld draws with seeds[r] at counter *step + step_offset -> ids[r].
+// Each row's token is the one sample_top_p_kernel draws from that row in fp32 with the same seed and counter.
+template <typename T>
+__global__ void __launch_bounds__(THREADS)
+sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seeds,
+                   const int* __restrict__ step, int step_offset, long long* __restrict__ ids) {
+  const int r = blockIdx.x;
+  const int tok = sample_row(logits + (size_t)r * ld, V, params, seeds + r, step, step_offset);
+  if (threadIdx.x == 0) ids[r] = (long long)tok;
 }
 
 }  // namespace sampling
@@ -189,6 +213,24 @@ extern "C" __attribute__((visibility("default"))) int srgpt_sample_top_p_f32(con
                                              (reinterpret_cast<uintptr_t>(next_x) & 15) == 0));
   sampling::sample_top_p_kernel<<<1, sampling::THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, V, params, seed, step, step_offset, out_ids, reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(next_x), K);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+// Draws one token per row for R rows of logits [R, ld] (fp32 when logits_f32, else the element type) -> ids[R].  Row r draws with
+// seeds[r] at counter *step + step_offset, exactly as srgpt_sample_top_p_f32 draws from that row converted to fp32.
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params,
+                                                                        const unsigned long long* seeds, const int* step, int step_offset,
+                                                                        long long* ids, void* stream) {
+  SRGPT_CHECK_ARG(logits && params && seeds && step && ids && R > 0 && R <= 65535 && V > 0 && ld >= V);
+  SRGPT_CHECK_ARG(logits_f32 == 0 || logits_f32 == 1);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (logits_f32)
+    sampling::sample_rows_kernel<float><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const float*>(logits), ld, V, params, seeds, step,
+                                                                         step_offset, ids);
+  else
+    sampling::sample_rows_kernel<bf16><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const bf16*>(logits), ld, V, params, seeds, step,
+                                                                        step_offset, ids);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }

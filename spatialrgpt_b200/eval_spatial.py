@@ -10,7 +10,9 @@ Same command line, same annotation format (``id``, ``image_info``, ``rle`` | ``b
 * depth: the monocular depth network (DepthAnything) is an external model and out of scope (SURVEY.md §8a row a0); the
   driver takes any ``depth_predictor(rgb uint8 [H, W, 3]) -> float tensor [h', w']`` and does the reference's post-processing
   (bilinear resize, min-max to 0..255, uint8, x3; eval_spatial.py:99-105) with the ``srgpt_depth_to_u8x3`` kernel;
-* generation is greedy (the benchmark script passes ``--temperature 0``); sampling raises ``NotImplementedError`` in the model.
+* the benchmark script passes ``--temperature 0``, so its generation is greedy; a positive ``--temperature`` samples with the
+  device sampler (temperature, ``--top_p`` and HF's default top-k of 50), seeded from ``torch.initial_seed()``: the same
+  distribution as HF's sampling, not the same random stream.
 """
 from __future__ import annotations
 

@@ -118,6 +118,28 @@ def beam_page_pairs(tables: List[List[int]], parents: List[int], starts: List[in
     return staged + direct, len(staged)
 
 
+def prompt_page_pairs(tables: List[List[int]], seq_lens: List[int], n: int, page_size: int = PAGE_SIZE):
+    """The KV copies that give rows g * n + 1 .. g * n + n - 1 the prompt rows [0, seq_lens[g]) of row g * n, which the prefill wrote:
+    (src page, dst page, first row, rows) over the page tables ``tables``, page by page.  No destination is a source, so none is staged."""
+    return [(tables[g * n][j], tables[g * n + i][j], 0, min(page_size, seq_lens[g] - j * page_size))
+            for g in range(len(seq_lens)) for i in range(1, n) for j in range((seq_lens[g] + page_size - 1) // page_size)]
+
+
+SEED_STRIDE = 0x9E3779B97F4A7C15  # the golden-ratio increment of splitmix64
+SEED_MASK = 0x7FFFFFFFFFFFFFFF
+
+
+def sequence_seeds(seed: int, n: int) -> List[int]:
+    """The sampling seeds of the n sequences of a sampled batch: sequence b's seed is sequence b - 1's plus SEED_STRIDE * (b + 1) (sequence
+    -1's is ``seed``), mod 2^63, i.e. seed + SEED_STRIDE * (b + 1) (b + 2) / 2.  The batched and the one-after-the-other paths both use it,
+    so a sequence draws with the same seed on either."""
+    out, s = [], int(seed) & SEED_MASK
+    for b in range(n):
+        s = (s + SEED_STRIDE * (b + 1)) & SEED_MASK
+        out.append(s)
+    return out
+
+
 class PagedKVCache:
     """KV pages for all layers: [layers, n_pages, 2 (k,v), PAGE_SIZE, n_kv_heads, head_dim] bf16, a free list
     and per-sequence page tables (int32, device) of fixed capacity so decode graphs stay valid."""
@@ -211,7 +233,7 @@ class LlamaDecoder:
                              "nf4_dequantized_copy=False does not keep")
         self._layer_array = self._make_layer_array()
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
-        # ("verify", T, ngram), ("batch", B, proc) and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
+        # ("verify", T, ngram), ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
         # dropped whenever one of them is replaced: the KV cache and layer array (ensure_capacity), the processor spec (_set_processors)
         # and the batched-decode buffers (_batch_state).
         self._graphs = {}
@@ -253,6 +275,7 @@ class LlamaDecoder:
     supports_prefix_reuse = True
     supports_prompt_lookup = True
     supports_logits_processors = True
+    supports_batch_sampling = True  # sampled batches run in the batched step (generate_batch), num_return_sequences included
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
@@ -393,10 +416,11 @@ class LlamaDecoder:
                                         PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens), nf4_array=self._planes_array)
 
     @ops.in_own_dtype
-    def first_tokens(self, hidden_packed: torch.Tensor, seq_lens: List[int], return_logits: bool = False):
+    def first_tokens(self, hidden_packed: torch.Tensor, seq_lens: List[int], return_logits: bool = False, repeat: int = 1):
         """Greedy first token of every packed sequence: final norm + lm_head over the B last rows as one GEMM
-        (bf16 logits, modeling_llama.py:1044-1045), argmax with the lowest index on ties."""
-        last = (torch.tensor(seq_lens).cumsum(0) - 1).to(torch.int32).to(self.device)
+        (bf16 logits, modeling_llama.py:1044-1045), argmax with the lowest index on ties.  ``repeat=n``: each last row n times
+        (B * n rows, row b * n + j from sequence b)."""
+        last = (torch.tensor(seq_lens).cumsum(0) - 1).repeat_interleave(repeat).to(torch.int32).to(self.device)
         rows = ops.splice_rows(hidden_packed, None, None, None, torch.zeros_like(last), last)
         hn = ops.rmsnorm(rows, self.w.norm, self.dims.rms_norm_eps)
         lg = ops.gemm(hn, self.w.lm_head, out=self._logits_buffer(hn.shape[0]))
@@ -467,7 +491,7 @@ class LlamaDecoder:
             while cap < ints.size:
                 cap *= 2
             self.proc_spec = torch.zeros(cap, dtype=torch.int32, device=self.device)
-            self._drop_graphs(lambda key: key[0] in ("step", "batch") and key[-1])  # the graphs with processing on read the old buffer
+            self._drop_graphs(lambda key: key[0] in ("step", "batch") and key[2])  # the graphs with processing on read the old buffer
         self.proc_spec[: ints.size].copy_(torch.from_numpy(ints))
         self.proc_fparams.copy_(torch.from_numpy(fparams))
         return True
@@ -759,15 +783,16 @@ class LlamaDecoder:
         st = dict(B=B, h=z(B, H), xn=z(B, H), qkv=z(B, (nh + 2 * nkv) * hd), attn=z(B, nh * hd), act=z(B, I),
                   logits=z(B, (V + 7) // 8 * 8), pos=z(B, dtype=torch.int32), step=z(1, dtype=torch.int32), ids=z(B, dtype=torch.int64),
                   out=z(self.out_ids.numel() * B, dtype=torch.int64), ticket=z(1, dtype=torch.int32),
-                  cu=torch.arange(B + 1, dtype=torch.int32, device=dev))
+                  cu=torch.arange(B + 1, dtype=torch.int32, device=dev), seeds=z(B, dtype=torch.int64), proc_rows=None)
         if self.fp8:  # the activation quantizer's codes and row scales
             st.update(q8=z(B, max(H, nh * hd, I), dtype=torch.uint8), s8=z(B, dtype=torch.float32))
         self._bstate = st
         return st
 
-    def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False) -> None:
+    def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False, sample: bool = False) -> None:
         """One decode step of all B sequences (llava_arch.py:549-611 + modeling_llama.py:540-562 semantics without padding): the
-        projections are wgmma GEMMs over the B rows (tall stream-K configuration), RoPE / KV append and attention per sequence."""
+        projections are wgmma GEMMs over the B rows (tall stream-K configuration), RoPE / KV append and attention per sequence.
+        ``sample``: row b draws its token with st["seeds"][b] at counter step (the counter the one-token loop uses for that token)."""
         d, w, B = self.dims, self.w, st["B"]
         nh, nkv, hd, V = d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.vocab_size
         qd = nh * hd
@@ -796,25 +821,39 @@ class LlamaDecoder:
         ops.gemm(xn, w.lm_head, out=lg)  # bf16 logits (modeling_llama.py:1044), arg max with the lowest index on ties
         if logits_only:  # beam search: the host picks the next tokens from the candidates of these logits
             return
-        if proc:  # the processors over each sequence's bf16 row and its history st["out"][t * B + b], t < step; then the arg max
+        if sample:  # from the bf16 rows, or from the processed fp32 rows
+            if proc:
+                ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, out=st["proc_rows"])
+            ops.sample_rows(st["proc_rows"] if proc else lg, self.sample_params, st["seeds"], st["step"], 0, st["ids"])
+        elif proc:  # the processors over each sequence's bf16 row and its history st["out"][t * B + b], t < step; then the arg max
             ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, ids=st["ids"])
         else:
             ops.argmax_bf16(lg, out=st["ids"])
         ops.decode_batch_advance(st["ids"], w.embed, h, st["out"], st["step"], st["pos"], st["ticket"])
 
     def _decode_batched(self, first: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos, stopping_fn, use_graph: bool,
-                        proc: bool = False):
-        """Greedy decode of B prefilled sequences together.  Returns a list of LongTensor [n_b] (each cut at its own stop)."""
+                        proc: bool = False, sample_from: Optional[torch.Tensor] = None, seeds: Optional[List[int]] = None):
+        """Decode of B prefilled sequences together: greedy, or sampled when ``sample_from`` holds the B first-token rows to draw from
+        ([B, V], the bf16 lm_head rows or the processed fp32 rows) and ``seeds`` the B row seeds.  Returns a list of LongTensor [n_b]
+        (each cut at its own stop)."""
         B = len(seq_lens)
         st = self._batch_state(B)
+        sample = sample_from is not None
+        if sample:  # the first tokens in one launch, at counter 0
+            st["seeds"].copy_(torch.tensor(seeds, dtype=torch.int64))
+            if proc and st["proc_rows"] is None:
+                st["proc_rows"] = torch.empty((B, self.dims.vocab_size), dtype=torch.float32, device=self.device)
+            st["step"].zero_()
+            ops.sample_rows(sample_from, self.sample_params, st["seeds"], st["step"], 0, st["ids"])
+            first = st["ids"]
         zero = torch.zeros(B, dtype=torch.int32, device=self.device)
         st["out"][:B].copy_(first)
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        key = ("batch", B, proc)
-        if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max
-            self._capture(key, lambda: self._batch_step_launch(st, proc=proc), (st["h"], st["pos"], st["step"], st["out"]),
+        key = ("batch", B, proc, True) if sample else ("batch", B, proc)
+        if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max (sampling: processing + draw)
+            self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample), (st["h"], st["pos"], st["step"], st["out"]),
                           self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4))
         need_check = bool(eos) or stopping_fn is not None
         out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
@@ -828,7 +867,7 @@ class LlamaDecoder:
             if use_graph:
                 self._replay(key)
             else:
-                self._batch_step_launch(st, proc=proc)
+                self._batch_step_launch(st, proc=proc, sample=sample)
             if need_check:  # same pipelining as the single-sequence loop: inspect row n-1 while row n is being computed
                 nxt = self._to_host((out2d[n], host[n]))
                 copied.synchronize()
@@ -948,8 +987,7 @@ class LlamaDecoder:
         tables = [list(self.cache.owned[r]) for r in range(R)]
         # the prompts are prefilled once, into beam 0 of each; the other beams get copies of its prompt rows
         hidden = self.prefill_packed(packed_embeds, seq_lens, page_tables=self.cache.page_tables[:R:k])
-        ops.kv_copy_pages(self.cache.pages, [(tables[g * k][j], tables[g * k + i][j], 0, min(PAGE_SIZE, seq_lens[g] - j * PAGE_SIZE))
-                                             for g in range(B) for i in range(1, k) for j in range((seq_lens[g] + PAGE_SIZE - 1) // PAGE_SIZE)])
+        ops.kv_copy_pages(self.cache.pages, prompt_page_pairs(tables, seq_lens, k))
         st = self._batch_state(R)
         # every beam row starts from its prompt's last hidden row: final norm + lm_head over the R rows
         last = torch.tensor([sum(seq_lens[:g + 1]) - 1 for g in range(B) for _ in range(k)], dtype=torch.int32).to(dev)
@@ -1000,14 +1038,29 @@ class LlamaDecoder:
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos_token_ids=None,
-                       stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None, processors=None):
+                       stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None, processors=None,
+                       num_return_sequences: int = 1):
         """Decoding of B prompts: ONE packed prefill pass (tensor-core bound, all prompts share every GEMM), one lm_head GEMM for the
         B first tokens, then BATCHED decode: every step advances all B sequences, each weight streamed once per step for the
-        whole batch (_decode_batched).  With ``return_logits`` or sampling the sequences are decoded one after the other with the
-        single-sequence weight-streaming step.  Returns a list of LongTensor [n_b] (and a list of fp32 logits).
-        ``processors``: the logits processors of generate_from_embeds, on every path (the first tokens included)."""
+        whole batch (_decode_batched), greedy or sampled (``sampling``: sequence b draws with sequence_seeds(seed, B)[b]).  With
+        ``return_logits`` the sequences are decoded one after the other with the single-sequence weight-streaming step.  Returns a
+        list of LongTensor [n_b] (and a list of fp32 logits).
+        ``processors``: the logits processors of generate_from_embeds, on every path (the first tokens included).
+        ``num_return_sequences=n`` (sampling only): n answers per prompt.  Each prompt is prefilled once, into row b * n; its prompt
+        pages are copied into rows b * n + 1 .. b * n + n - 1, and the B * n rows decode in the batched sampled step, row r with
+        sequence_seeds(seed, B * n)[r].  Returns B * n lists, row b * n + j being answer j of prompt b."""
+        n_ret = int(num_return_sequences)
+        if n_ret < 1:
+            raise ValueError(f"num_return_sequences must be >= 1, got {n_ret}")
+        if n_ret > 1:
+            if not sampling:
+                raise ValueError("num_return_sequences > 1 needs sampling: greedy decoding has one answer per prompt")
+            if return_logits:
+                raise NotImplementedError("num_return_sequences > 1 with output_logits")
+            if not self.supports_batch_sampling:
+                raise NotImplementedError("num_return_sequences > 1 on the tensor-parallel decoder (it does not sample)")
         d, w = self.dims, self.w
-        B = len(seq_lens)
+        B = len(seq_lens) * n_ret
         if max_new_tokens < 1:
             return [torch.empty(0, dtype=torch.int64, device=self.device) for _ in range(B)]
         if max_new_tokens > self.out_ids.numel():
@@ -1019,9 +1072,16 @@ class LlamaDecoder:
         for b in range(len(self.cache.owned)):
             self.cache.release(b)
         self.ensure_capacity(B, max(seq_lens) + max_new_tokens)
-        self.cache.reserve_many([n + max_new_tokens for n in seq_lens])
-        hidden = self.prefill_packed(packed_embeds, seq_lens)
-        first, lg = self.first_tokens(hidden, seq_lens, return_logits=True)
+        row_lens = [int(n) for n in seq_lens for _ in range(n_ret)]  # row b * n_ret + j continues prompt b
+        self.cache.reserve_many([n + max_new_tokens for n in row_lens])
+        if n_ret == 1:
+            hidden = self.prefill_packed(packed_embeds, seq_lens)
+        else:  # each prompt once, into the first of its rows; the other rows get copies of its prompt pages
+            tables = [list(self.cache.owned[r]) for r in range(B)]
+            hidden = self.prefill_packed(packed_embeds, seq_lens, page_tables=self.cache.page_tables[:B:n_ret])
+            ops.kv_copy_pages(self.cache.pages, prompt_page_pairs(tables, [int(n) for n in seq_lens], n_ret))
+        first, lg = self.first_tokens(hidden, seq_lens, return_logits=True, repeat=n_ret)
+        seq_lens = row_lens
         outs, all_logits = [], []
         sample = self._set_sampling(sampling)
         first_rows = None  # the processed first-token rows a sampled sequence draws from
@@ -1030,8 +1090,10 @@ class LlamaDecoder:
             ops.logits_process(lg, None, 0, 1, None, 0, self.proc_fparams, self.proc_spec, out=first_rows, ids=first)
         if max_new_tokens == 1 and not return_logits and not sample:
             return [first[b:b + 1] for b in range(B)]
-        if not return_logits and not sample and B > 1:
-            return self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc)
+        seeds = sequence_seeds(self.sample_seed, B) if sample else None
+        if not return_logits and B > 1 and (not sample or self.supports_batch_sampling):
+            return self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc,
+                                        sample_from=(first_rows if proc else lg) if sample else None, seeds=seeds)
         zero = torch.zeros(1, dtype=torch.int32, device=self.device)
         for b in range(B):
             logits = None
@@ -1044,7 +1106,7 @@ class LlamaDecoder:
             self.pos.fill_(seq_lens[b])
             self.step.fill_(1)
             if sample:  # re-draw the first token of this sequence from its logits row (a different draw per sequence: the seed moves)
-                self._set_seed(self.sample_seed + 0x9E3779B97F4A7C15 * (b + 1))
+                self._set_seed(seeds[b])
                 row = first_rows[b] if proc else lg[b].float().contiguous()
                 ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
             r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc)

@@ -427,6 +427,25 @@ class LlavaLlamaModel:
         sampling = None
         if do_sample and temperature not in (0, 0.0):
             sampling = dict(temperature=1.0 if temperature is None else float(temperature), top_p=top_p, top_k=top_k, seed=seed)
+        # num_return_sequences=n (sampling): n answers per prompt, rows b * n .. b * n + n - 1 of the result (HF's repeat_interleave
+        # order); each prompt is prefilled once and its n rows decode together in the batched sampled step
+        n_ret = generation_kwargs.pop("num_return_sequences", None)
+        n_ret = 1 if n_ret is None else int(n_ret)
+        if n_ret < 1:
+            raise ValueError(f"num_return_sequences must be >= 1, got {n_ret}")
+        if n_ret > 1:
+            if num_beams != 1:
+                raise NotImplementedError("num_return_sequences > 1 with beam search (the n best hypotheses are not returned)")
+            if sampling is None:
+                raise ValueError("num_return_sequences > 1 needs do_sample=True with temperature > 0: greedy decoding has one answer per prompt")
+            if prefix_cache:
+                raise NotImplementedError("num_return_sequences > 1 with prefix_cache=True")
+            if lookup_k:
+                raise NotImplementedError("num_return_sequences > 1 with prompt_lookup_num_tokens")
+            if return_logits:
+                raise NotImplementedError("num_return_sequences > 1 with output_logits")
+            if not getattr(type(self.llm), "supports_batch_sampling", False):
+                raise NotImplementedError("num_return_sequences > 1 on the tensor-parallel decoder (it does not sample)")
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
         # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
@@ -504,7 +523,7 @@ class LlavaLlamaModel:
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
             outs.append(self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                                length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph))
-        elif B == 1:
+        elif B == 1 and n_ret == 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
             reuse = 0
@@ -533,7 +552,8 @@ class LlavaLlamaModel:
             outs.append(r)
         else:
             # batch > 1: one packed prefill over all prompts (llava_arch.py:549-611 pads, modeling_llama.py:540-562 unpads
-            # again; here the rows were never padded), then per-sequence decode, or beam search with every prompt's beams in one step
+            # again; here the rows were never padded), then batched decode (n_ret rows per prompt), or beam search with every prompt's
+            # beams in one step
             if packed is None:
                 T = inputs_embeds.shape[1]
                 packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
@@ -542,13 +562,14 @@ class LlavaLlamaModel:
                                                     length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph)
             else:
                 r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                            use_graph=use_graph, return_logits=return_logits, sampling=sampling, **proc)
+                                            use_graph=use_graph, return_logits=return_logits, sampling=sampling, num_return_sequences=n_ret,
+                                            **proc)
                 if return_logits:
                     outs, all_logits = r
                 else:
                     outs = r
         n_max = max(o.numel() for o in outs)
-        seqs = torch.full((B, n_max), int(pad), dtype=torch.int64, device=self.device)
+        seqs = torch.full((len(outs), n_max), int(pad), dtype=torch.int64, device=self.device)
         for b, o in enumerate(outs):
             seqs[b, : o.numel()] = o
         if return_logits:

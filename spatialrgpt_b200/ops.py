@@ -841,6 +841,31 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
                                              _p(out_ids), _p(embed_table), _p(next_x), K, _stream()), "srgpt_sample_top_p_f32")
 
 
+def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor, step: torch.Tensor, step_offset: int,
+                ids: torch.Tensor) -> None:
+    """One token per row of ``logits`` ([R, V] fp32 or the element type, unit inner stride, e.g. the batched lm_head's rows) in one
+    launch -> ids int64 [R].  Row r draws with seeds[r] (device int64 [R]) at counter step + step_offset, the token sample_top_p draws
+    from that row in fp32 with that seed and counter.  ``params`` and ``step`` as for sample_top_p."""
+    _need(params, torch.float32, "sample_rows.params"); _need(seeds, torch.int64, "sample_rows.seeds")
+    _need(step, torch.int32, "sample_rows.step"); _need(ids, torch.int64, "sample_rows.ids")
+    if not logits.is_cuda:
+        raise SrgptError("sample_rows.logits: expected a CUDA tensor (the sm_90a kernels have no CPU fallback)")
+    f32 = logits.dtype == torch.float32
+    _need(logits, torch.float32 if f32 else ELEM(), "sample_rows.logits")
+    if logits.dim() != 2:
+        raise SrgptError(f"sample_rows: logits must be [R, V], got shape {tuple(logits.shape)}")
+    ld = _rowmajor2d(logits, "sample_rows.logits")
+    R, V = logits.shape
+    if params.numel() < 3 or step.numel() < 1:
+        raise SrgptError("sample_rows: params must be [temperature, top_p, top_k] and step a device int32 [1]")
+    if seeds.dim() != 1 or seeds.numel() != R or not seeds.is_contiguous():
+        raise SrgptError(f"sample_rows: seeds must be a contiguous int64 vector of {R} entries, got shape {tuple(seeds.shape)}")
+    if ids.dim() != 1 or ids.numel() != R or not ids.is_contiguous():
+        raise SrgptError(f"sample_rows: ids must be a contiguous int64 vector of {R} entries, got shape {tuple(ids.shape)}")
+    check(_lib.load().srgpt_sample_rows(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids), _stream()),
+          "srgpt_sample_rows")
+
+
 def logits_process(logits: torch.Tensor, hist: Optional[torch.Tensor], hist_row_stride: int, hist_tok_stride: int, step: Optional[torch.Tensor],
                    step_offset: int, fparams: torch.Tensor, spec: torch.Tensor, out: Optional[torch.Tensor] = None,
                    ids: Optional[torch.Tensor] = None) -> None:

@@ -65,6 +65,7 @@ class TPLlamaDecoder(LlamaDecoder):
     packs_decode_weights = False   # the ranks stream their bf16 shards
     supports_prompt_lookup = False  # the verify pass is a single-GPU kernel sequence
     supports_logits_processors = False  # the logits are vocabulary-parallel: no rank holds a whole row
+    supports_batch_sampling = False  # the decoder implements greedy decoding only
 
     def __init__(self, dims: LlamaDims, w: LlamaW, rank: int, world: int, group=None, max_seq_len: int = 4096, comm: Optional[str] = None, **kw):
         if getattr(w, "quantization", None) is not None:
