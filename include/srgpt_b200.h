@@ -290,6 +290,15 @@ long long srgpt_kv_copy_workspace_bytes(int n_staged, int n_layers, int page_row
  * destination is another pair's source must be staged; then any permutation is safe.  row_bytes a multiple of 16. */
 int srgpt_kv_copy_pages(void* pages, int n_layers, int n_pages, int page_rows, int row_bytes, const int* pairs, int n_pairs, int n_staged,
                         void* workspace, long long workspace_bytes, void* stream);
+/* Row log-softmax at target tokens (logprob.cu): replaces the .float() + CrossEntropyLoss of LlamaForCausalLM.forward
+ * (modeling_llama.py:1044-1058) and the per-token log-probabilities of likelihood scoring.  logits: [rows, ld] in the element type (the
+ * rounded lm_head output), ld >= V.  lse[rows] (fp32) = m + log sum exp(x - m) over each row, every element widened to fp32 exactly; a NaN
+ * in a row makes its lse NaN.  n pairs (pair_rows[i], pair_targets[i]) given in HOST memory: logprob[i] (fp32, device) = logits[row, target]
+ * - lse[row], 0 for target -100 (ignored).  loss (device float, optional) = the mean of -logprob over the pairs that are not ignored, NaN
+ * when every pair is.  A row outside [0, rows) or a target outside [0, V) that is not -100 is rejected (-1) before anything is read or
+ * launched.  workspace: device memory of at least 8 n bytes, 8-byte aligned.  Fixed reduction orders: repeated calls are bit-identical. */
+int srgpt_token_logprobs(const void* logits, long long ld, int rows, int V, const int* pair_rows, const long long* pair_targets, int n,
+                         void* workspace, long long workspace_bytes, float* lse, float* logprob, float* loss, void* stream);
 /* Temperature + nucleus (top-p) sampling of one token from fp32 logits [V] (sampling.cu): replaces HF's TemperatureLogitsWarper /
  * TopKLogitsWarper / TopPLogitsWarper / multinomial behind do_sample=True (llava/eval/eval_spatial.py:231-236, llava/eval/model_vqa.py:72-78).
  * params = device float[3] {temperature, top_p, top_k (0 = off)}; seed = device u64; the draw is a counter-based generator of

@@ -63,6 +63,7 @@ SIGNATURES = {
     "srgpt_beam_select": (ci, [vp, vp, ci, ci, ci, vp, vp, vp, vp]),
     "srgpt_kv_copy_workspace_bytes": (cll, [ci, ci, ci, ci]),
     "srgpt_kv_copy_pages": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, vp, cll, vp]),
+    "srgpt_token_logprobs": (ci, [vp, cll, ci, ci, vp, vp, ci, vp, cll, vp, vp, vp, vp]),
     "srgpt_sample_top_p_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp]),
     "srgpt_sample_rows": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, ci, vp, vp]),
     "srgpt_logits_process": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, ci, vp, ci, vp, vp, ci, vp, ci, vp, vp]),

@@ -105,8 +105,9 @@ def segmentation_to_mask(segmentation, height: int, width: int) -> np.ndarray:
 
 
 def build_sample(line: Dict[str, Any], tokenizer, image_processor, model_config, conv_mode: str, dataset: str, prompt_type: str,
-                 image_folder: str, rng: random.Random, open_image=None):
-    """CustomDataset.__getitem__ (eval_region_cls.py:169-250) -> (input_ids [T], images [1, 3, R, R], masks [n, R, R])."""
+                 image_folder: str, rng: random.Random, open_image=None, return_conv: bool = False):
+    """CustomDataset.__getitem__ (eval_region_cls.py:169-250) -> (input_ids [T], images [1, 3, R, R], masks [n, R, R]), and the
+    conversation whose prompt the ids are when ``return_conv``."""
     from PIL import Image
     bboxes, info = line["bbox"], line["image_info"]
     assert len(bboxes) == 1, "one box per sample (eval_region_cls.py:177)"
@@ -140,7 +141,29 @@ def build_sample(line: Dict[str, Any], tokenizer, image_processor, model_config,
     image = (open_image or (lambda p: Image.open(p)))(os.path.join(image_folder, line["image"])).convert("RGB").crop(tuple(crop))
     images = process_images([image], image_processor, model_config)
     input_ids = tokenizer_image_token(conv.get_prompt(), tokenizer, IMAGE_TOKEN_INDEX, return_tensors="pt")
-    return input_ids, images, masks
+    return (input_ids, images, masks, conv) if return_conv else (input_ids, images, masks)
+
+
+def category_names(annotation_file: str) -> List[str]:
+    """The annotation file's category names, lower-cased as the records' gt_name, in the file's order."""
+    with open(annotation_file) as f:
+        return [c["name"].lower() for c in json.load(f).get("categories", [])]
+
+
+def candidate_ids(conv, names: List[str], tokenizer, prompt_ids) -> List[List[int]]:
+    """Each name as the template renders a final assistant turn (the conversation's open last turn answered with it), tokenised like
+    the prompt: the ids after the prompt's, so each answer carries the template's own end-of-turn separator and a name that is a
+    prefix of another is not favoured.  Raises ValueError when the prompt's ids are not a prefix of the answered prompt's."""
+    prompt = [int(t) for t in prompt_ids.tolist()]
+    out = []
+    for name in names:
+        c = conv.copy()
+        c.messages[-1][1] = name
+        full = tokenizer_image_token(c.get_prompt(), tokenizer, IMAGE_TOKEN_INDEX)
+        if full[:len(prompt)] != prompt or len(full) == len(prompt):
+            raise ValueError(f"the prompt's tokens are not a prefix of the tokens of the prompt answered with {name!r}")
+        out.append(full[len(prompt):])
+    return out
 
 
 def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
@@ -161,17 +184,28 @@ def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
     rng = random.Random(seed)
     stop = stop_string(args.conv_mode)
     dev = model.device
+    # --score-categories: rank the annotation file's category names by likelihood (model.score) instead of generating an answer
+    names = category_names(args.annotation_file) if getattr(args, "score_categories", False) else None
+    tails = {}  # prompt text -> the names' candidate ids
     n = 0
     with open(answers_file, "w") as out:
         for line in data:
-            input_ids, images, masks = build_sample(line, tokenizer, image_processor, model.config, args.conv_mode, args.dataset, args.prompt_type,
-                                                    args.image_folder, rng)
+            input_ids, images, masks, conv = build_sample(line, tokenizer, image_processor, model.config, args.conv_mode, args.dataset,
+                                                          args.prompt_type, args.image_folder, rng, return_conv=True)
             # fp16 end to end, as the reference runs this script (builder.py:62 load, inputs cast at 316-317)
-            output_ids = model.generate(input_ids.unsqueeze(0).to(dev), images=images.to(dev, dtype=model.dtype),
-                                        masks=[masks.to(dev, dtype=model.dtype)], do_sample=args.temperature > 0, temperature=args.temperature,
-                                        top_p=args.top_p, num_beams=args.num_beams, max_new_tokens=64, use_cache=True,
-                                        pad_token_id=getattr(tokenizer, "pad_token_id", None))
-            text = clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop)
+            if names is not None:
+                key = conv.get_prompt()
+                if key not in tails:
+                    tails[key] = candidate_ids(conv, names, tokenizer, input_ids)
+                res = model.score(input_ids.unsqueeze(0).to(dev), images=images.to(dev, dtype=model.dtype),
+                                  masks=[masks.to(dev, dtype=model.dtype)], candidates=tails[key])
+                text = names[int(res.sequence_logprobs[0].argmax())]
+            else:
+                output_ids = model.generate(input_ids.unsqueeze(0).to(dev), images=images.to(dev, dtype=model.dtype),
+                                            masks=[masks.to(dev, dtype=model.dtype)], do_sample=args.temperature > 0,
+                                            temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams, max_new_tokens=64,
+                                            use_cache=True, pad_token_id=getattr(tokenizer, "pad_token_id", None))
+                text = clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop)
             out.write(json.dumps({"question_id": line["image"], "text": text, "gt_name": line["category_name"], "score": line["score"],
                                   "bbox": line["bbox"], "image_id": line["image_id"], "model_id": model_name, "metadata": {}}) + "\n")
             out.flush()
@@ -199,6 +233,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
                    help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
     p.add_argument("--nf4-planes-only", action="store_true",
                    help="with --quantization nf4: keep only the 4-bit planes of the layer matrices, no dequantized copy (same answers)")
+    p.add_argument("--score-categories", action="store_true",
+                   help="answer with the category name of the highest likelihood under the prompt (model.score) instead of generating")
     return p
 
 

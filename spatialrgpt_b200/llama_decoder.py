@@ -125,6 +125,44 @@ def prompt_page_pairs(tables: List[List[int]], seq_lens: List[int], n: int, page
             for g in range(len(seq_lens)) for i in range(1, n) for j in range((seq_lens[g] + page_size - 1) // page_size)]
 
 
+def candidate_pages(S: int, n_rows: int, page_size: int = PAGE_SIZE):
+    """A candidate that continues a prompt of S rows with n_rows >= 1 rows (positions [S, S + n_rows)): (shared, own) page counts.  Its
+    first S // page_size pages are the prompt's full pages, shared; it owns the pages from the prompt's partial last page (a copy) or
+    the first page past the prompt, up to the page of its last row."""
+    shared = S // page_size
+    return shared, (S + n_rows + page_size - 1) // page_size - shared
+
+
+def plan_score_passes(seq_lens: List[int], cand_lens: List[int], row_budget: int, free_pages: int, max_chunks: int = 65535,
+                      page_size: int = PAGE_SIZE):
+    """The passes of LlamaDecoder.score_candidates.  Candidate c of prompt b needs cand_lens[c] - 1 rows (its tokens but the last, at
+    positions S_b ..), so a one-token candidate needs none and is in no pass.  Returns a list of passes, each a list of (b, c, first row,
+    rows, own pages) in (b, c) order, filled greedily: a pass holds at most ``row_budget`` rows, ``free_pages`` owned pages (the pages
+    left after the prompts') and ``max_chunks`` candidates.  Raises when one candidate alone does not fit."""
+    passes, cur, rows, pages = [], [], 0, 0
+    for b, S in enumerate(seq_lens):
+        for c, L in enumerate(cand_lens):
+            n = int(L) - 1
+            if n < 1:
+                continue
+            shared, own = candidate_pages(int(S), n, page_size)
+            # the rows [S, S + n) land in table entries shared .. shared + own - 1, never in one of the prompt's full (shared) pages
+            first, last = int(S) // page_size, (int(S) + n - 1) // page_size
+            assert shared <= first and last < shared + own, "a candidate's K/V would land in a shared page"
+            if n > row_budget or own > free_pages:
+                raise RuntimeError(f"candidate {c} of prompt {b} needs {n} rows and {own} KV pages; a pass has {row_budget} rows and "
+                                   f"{free_pages} free pages")
+            if cur and (rows + n > row_budget or pages + own > free_pages or len(cur) >= max_chunks):
+                passes.append(cur)
+                cur, rows, pages = [], 0, 0
+            cur.append((b, c, rows, n, own))
+            rows += n
+            pages += own
+    if cur:
+        passes.append(cur)
+    return passes
+
+
 SEED_STRIDE = 0x9E3779B97F4A7C15  # the golden-ratio increment of splitmix64
 SEED_MASK = 0x7FFFFFFFFFFFFFFF
 
@@ -154,6 +192,11 @@ class PagedKVCache:
         self.page_tables = torch.zeros((max_seqs, max_pages_per_seq + 1), dtype=torch.int32, device=device)
         self.free: List[int] = list(range(n_pages - 1, -1, -1))
         self.owned: List[List[int]] = [[] for _ in range(max_seqs)]
+        # forked sequences (fork): id -> (source sequence, shared pages, owned pages); lent: source sequence -> number of live forks.
+        # Fork ids start past every slot, so they never name a slot of `owned`.
+        self.forks = {}
+        self.lent = {}
+        self._next_fork = max_seqs
 
     def reserve(self, seq: int, n_tokens: int) -> None:
         """Make sure sequence `seq` owns pages for positions [0, n_tokens)."""
@@ -187,8 +230,41 @@ class PagedKVCache:
         self.page_tables[:len(n_tokens)].copy_(host, non_blocking=True)
 
     def release(self, seq: int) -> None:
+        """Return the pages sequence `seq` owns to the free list (a fork's shared pages stay with their owner)."""
+        if seq in self.forks:
+            src, _, own = self.forks.pop(seq)
+            self.free.extend(reversed(own))
+            self.lent[src] -= 1
+            return
+        if self.lent.get(seq, 0):
+            raise RuntimeError(f"sequence {seq} still lends its pages to {self.lent[seq]} forked sequences")
         self.free.extend(reversed(self.owned[seq]))
         self.owned[seq] = []
+
+    def fork(self, src: int, shared_pages: int, n_tokens: int) -> int:
+        """A host-side sequence whose first `shared_pages` pages ARE sequence `src`'s (shared, never written or freed by the fork) and
+        which owns new pages for the rest of positions [0, n_tokens).  Returns its id (``table`` gives its page table; the caller builds
+        device tables from it).  ``release`` frees only the pages it owns; `src` cannot be released while forks share its pages."""
+        if not 0 <= shared_pages <= len(self.owned[src]):
+            raise RuntimeError(f"sequence {src} has {len(self.owned[src])} pages, cannot share {shared_pages}")
+        need = (n_tokens + PAGE_SIZE - 1) // PAGE_SIZE
+        if need > self.max_pages_per_seq:
+            raise RuntimeError(f"sequence needs {need} KV pages > capacity {self.max_pages_per_seq}")
+        add = max(0, need - shared_pages)
+        if add > len(self.free):
+            raise RuntimeError("KV cache exhausted")
+        fid = self._next_fork
+        self._next_fork += 1
+        self.forks[fid] = (src, list(self.owned[src][:shared_pages]), [self.free.pop() for _ in range(add)])
+        self.lent[src] = self.lent.get(src, 0) + 1
+        return fid
+
+    def table(self, seq: int) -> List[int]:
+        """Page ids of sequence `seq` by position // PAGE_SIZE (shared pages first for a fork)."""
+        if seq in self.forks:
+            _, shared, own = self.forks[seq]
+            return shared + own
+        return list(self.owned[seq])
 
     def layer(self, l: int) -> torch.Tensor:
         return self.pages[l]
@@ -345,16 +421,24 @@ class LlamaDecoder:
     def ensure_capacity(self, n_seqs: int, tokens_per_seq: int) -> None:
         """Grow the paged cache so `n_seqs` sequences of `tokens_per_seq` tokens fit at once (batched prefill).
         Re-allocation drops all cached sequences and the captured graphs (page addresses change)."""
-        c = self.cache
         need_pages = n_seqs * ((tokens_per_seq + PAGE_SIZE - 1) // PAGE_SIZE)
+        self._grow_cache(n_seqs, need_pages, f"{n_seqs} x {tokens_per_seq} tokens")
+
+    def _page_bytes(self) -> int:
+        d = self.dims
+        return 2 * PAGE_SIZE * d.num_key_value_heads * d.head_dim * 2 * d.num_hidden_layers
+
+    def _grow_cache(self, n_seqs: int, need_pages: int, what: str) -> None:
+        """Re-allocate the paged cache when it has fewer than `n_seqs` slots or `need_pages` pages (ensure_capacity)."""
+        c = self.cache
         if n_seqs <= len(c.owned) and need_pages <= c.n_pages:
             return
         d = self.dims
-        per_page = 2 * PAGE_SIZE * d.num_key_value_heads * d.head_dim * 2 * d.num_hidden_layers
+        per_page = self._page_bytes()
         free_b, _ = torch.cuda.mem_get_info(self.device)
         cur_b = c.pages.numel() * 2
         if need_pages * per_page > free_b + cur_b - (2 << 30):
-            raise RuntimeError(f"KV cache for {n_seqs} x {tokens_per_seq} tokens needs {need_pages * per_page >> 20} MiB, not available")
+            raise RuntimeError(f"KV cache for {what} needs {need_pages * per_page >> 20} MiB, not available")
         self._drop_graphs()
         self._record_prefix(0)
         n_pages_old, n_seqs_old = c.n_pages, len(c.owned)
@@ -435,9 +519,14 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def logits_all(self, hidden: torch.Tensor) -> torch.Tensor:
         """lm_head over every row -> fp32 logits [S, V] (LlamaForCausalLM.forward semantics, 1044-1045)."""
+        return self.lm_head_rows(hidden).float()  # bf16 rounding first, then .float()
+
+    @ops.in_own_dtype
+    def lm_head_rows(self, hidden: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Final norm + lm_head over every row of ``hidden`` -> element-type logits [S, V] (into ``out``, default a fresh
+        _logits_buffer)."""
         hn = ops.rmsnorm(hidden, self.w.norm, self.dims.rms_norm_eps)
-        lg = ops.gemm(hn, self.w.lm_head, out=self._logits_buffer(hn.shape[0]))  # bf16 rounding first, then .float()
-        return lg.float()
+        return ops.gemm(hn, self.w.lm_head, out=self._logits_buffer(hn.shape[0]) if out is None else out)
 
     # ---------------------------------------------------------------------------------------------
     def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False) -> None:
@@ -1115,3 +1204,105 @@ class LlamaDecoder:
             else:
                 outs.append(r)
         return (outs, all_logits) if return_logits else outs
+
+    # ---- likelihood scoring: every candidate continues its prompt from the prompt's own KV pages ------------------------------------
+    supports_scoring = True
+
+    @torch.no_grad()
+    @ops.in_own_dtype
+    def score_candidates(self, packed_embeds: torch.Tensor, seq_lens: List[int], candidates, row_budget: int) -> torch.Tensor:
+        """log p(cand_c[j] | prompt_b ++ cand_c[:j]) for B prompts packed back to back ([sum S_b, H]) and N candidate token lists shared by
+        every prompt -> fp32 [B, N, L_max], 0 past each candidate's length.
+        1. ONE packed prefill of the prompts into slots 0..B-1; final norm + lm_head over their B last rows, and token_logprobs gives
+           every log p(cand_c[0]).
+        2. Candidates run in passes (plan_score_passes: at most ``row_budget`` rows and the free KV pages each).  Candidate c of prompt b
+           is a fork of slot b (PagedKVCache.fork): its table points at the prompt's full pages, the prompt's partial last page is copied
+           into a page it owns (kv_copy_pages, rows [0, S_b % PAGE_SIZE)), and its rows cand_c[:-1] run at start_pos S_b.  A pass is one
+           llama_prefill_chunk_layers over all its chunks, one lm_head GEMM into a bounded logits buffer and one token_logprobs launch.
+        Every page is back on the free list afterwards."""
+        d, dev = self.dims, self.device
+        seq_lens = [int(n) for n in seq_lens]
+        cands = check_candidates(candidates, d.vocab_size)
+        B, N = len(seq_lens), len(cands)
+        lens = [len(c) for c in cands]
+        if B < 1 or packed_embeds.shape[0] != sum(seq_lens) or min(seq_lens) < 1:
+            raise RuntimeError("score_candidates: rows do not match seq_lens")
+        if max(seq_lens) + max(lens) > self.max_seq_len:
+            raise ValueError(f"a prompt of {max(seq_lens)} rows and a candidate of {max(lens)} tokens exceed max_seq_len {self.max_seq_len}")
+        if int(row_budget) < max(lens) - 1 or int(row_budget) < 1:
+            raise ValueError(f"row_budget {row_budget} is smaller than the longest candidate's {max(lens) - 1} rows")
+        L_max = max(lens)
+        # pages: the prompts', then as many candidate pages as memory allows (at least the largest single candidate's)
+        prompt_pages = sum((S + PAGE_SIZE - 1) // PAGE_SIZE for S in seq_lens)
+        tails = [candidate_pages(S, L - 1)[1] for S in seq_lens for L in lens if L > 1]
+        for b in range(len(self.cache.owned)):
+            self.cache.release(b)
+        free_b, _ = torch.cuda.mem_get_info(dev)
+        afford = self.cache.n_pages + max(0, free_b - (2 << 30)) // 2 // self._page_bytes()
+        self._grow_cache(B, min(prompt_pages + sum(tails), max(afford, prompt_pages + max(tails, default=0))), "scoring")
+        self.cache.reserve_many(seq_lens)
+        hidden = self.prefill_packed(packed_embeds, seq_lens)
+        out = torch.zeros((B, N, L_max), dtype=torch.float32, device=dev)
+        last = (torch.tensor(seq_lens).cumsum(0) - 1).to(torch.int32).to(dev)
+        lg = self.lm_head_rows(ops.splice_rows(hidden, None, None, None, torch.zeros_like(last), last))
+        _, lp, _ = ops.token_logprobs(lg, [b for b in range(B) for _ in range(N)], [c[0] for _ in range(B) for c in cands])
+        out[:, :, 0] = lp.view(B, N)
+        del hidden, lg
+        plan = plan_score_passes(seq_lens, lens, int(row_budget), len(self.cache.free))
+        buf = self._logits_buffer(max(sum(it[3] for it in p) for p in plan)) if plan else None
+        prompt_tables = [self.cache.table(b) for b in range(B)]
+        cap = self.cache.page_tables.shape[1]
+        forks = []
+        try:
+            for items in plan:
+                tables, copies, ids, targets, dst = [], [], [], [], []
+                for b, c, _, n, _ in items:
+                    S = seq_lens[b]
+                    shared = S // PAGE_SIZE
+                    f = self.cache.fork(b, shared, S + n)
+                    forks.append(f)
+                    t = self.cache.table(f)
+                    assert not set(t[shared:]) & set(prompt_tables[b]), "a candidate's K/V appends would land in a shared page"
+                    if S % PAGE_SIZE:
+                        copies.append((prompt_tables[b][shared], t[shared], 0, S % PAGE_SIZE))
+                    tables.append(t + [0] * (cap - len(t)))
+                    ids.extend(cands[c][:-1])
+                    targets.extend(cands[c][1:])
+                    dst.extend((b * N + c) * L_max + j for j in range(1, n + 1))
+                if copies:
+                    ops.kv_copy_pages(self.cache.pages, copies)
+                R = len(ids)
+                cu = torch.tensor([0] + [it[2] + it[3] for it in items], dtype=torch.int32).to(dev)
+                sp = torch.tensor([seq_lens[it[0]] for it in items], dtype=torch.int32).to(dev)
+                pts = torch.tensor(tables, dtype=torch.int32).to(dev)
+                x = self.embed_tokens(torch.tensor(ids, dtype=torch.int64))
+                h = ops.llama_prefill_chunk_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pts, PAGE_SIZE,
+                                                   self.cache.n_pages, cu, max(it[3] for it in items), nf4_array=self._planes_array)
+                lg = self.lm_head_rows(h, out=buf[:R])
+                _, lp, _ = ops.token_logprobs(lg, list(range(R)), targets)
+                out.view(-1)[torch.tensor(dst, dtype=torch.int64).to(dev)] = lp
+                while forks:
+                    self.cache.release(forks.pop())
+        finally:
+            while forks:
+                self.cache.release(forks.pop())
+            for b in range(B):
+                self.cache.release(b)
+        return out
+
+
+def check_candidates(candidates, vocab_size: int) -> List[List[int]]:
+    """The candidate token lists of a scoring request as lists of ints; raises ValueError on an empty list, an empty candidate or an id
+    outside [0, vocab_size)."""
+    if candidates is None or len(candidates) == 0:
+        raise ValueError("candidates must be a non-empty list of token-id lists")
+    out = []
+    for i, c in enumerate(candidates):
+        ids = [int(t) for t in (c.reshape(-1).tolist() if isinstance(c, torch.Tensor) else c)]
+        if not ids:
+            raise ValueError(f"candidate {i} is empty")
+        bad = [t for t in ids if t < 0 or t >= vocab_size]
+        if bad:
+            raise ValueError(f"candidate {i} holds token {bad[0]}, outside the vocabulary [0, {vocab_size})")
+        out.append(ids)
+    return out

@@ -14,7 +14,7 @@ import torch
 from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
-from .llama_decoder import LlamaDecoder
+from .llama_decoder import LlamaDecoder, check_candidates
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
@@ -29,6 +29,15 @@ class CausalLMOutputWithPast:
     past_key_values: Any = None
     hidden_states: Any = None
     attentions: Any = None
+
+
+@dataclass
+class ScoreOutput:
+    """LlavaLlamaModel.score: sequence_logprobs fp32 [B, N] (the sum over each candidate's tokens), token_logprobs fp32 [B, N, L_max]
+    (0 past a candidate's length) and lengths int64 [N]."""
+    sequence_logprobs: torch.Tensor
+    token_logprobs: torch.Tensor
+    lengths: torch.Tensor
 
 
 class LlavaLlamaModel:
@@ -369,14 +378,86 @@ class LlavaLlamaModel:
             llm.ensure_capacity(B, max(lens))
             llm.cache.reserve_many(lens)
             hid = llm.prefill_packed(torch.cat([inputs_embeds[b, valid[b]] for b in range(B)], 0), lens)
-        lg = llm.logits_all(hid)
+        loss = None
+        if labels is None:
+            lg = llm.logits_all(hid)
+        else:  # the element-type rows the lm_head GEMM writes, plus one zero row: the logits this call returns at padding positions
+            total = hid.shape[0]
+            buf = llm._logits_buffer(total + 1)
+            lg = llm.lm_head_rows(hid, out=buf[:total]).float()
+            buf[total].zero_()
+            loss = self._labels_loss(buf, labels, valid, lens, S)
         o = 0
         for b in range(B):
             logits[b, valid[b]] = lg[o:o + lens[b]]
             o += lens[b]
-        return CausalLMOutputWithPast(logits=logits)
+        return CausalLMOutputWithPast(logits=logits, loss=loss)
+
+    @staticmethod
+    def _labels_loss(elem_logits: torch.Tensor, labels: torch.Tensor, valid, lens, S: int) -> torch.Tensor:
+        """LlamaForCausalLM.forward's loss (modeling_llama.py:1044-1058): CrossEntropyLoss over logits[:, :-1] against labels[:, 1:],
+        IGNORE_INDEX skipped, mean over the batch.  ``elem_logits``: the packed element-type rows of the B sequences' valid positions and
+        one zero row after them, which stands for every padding position.  One token_logprobs launch; the mean is taken on the device."""
+        B = len(lens)
+        lab = labels.detach().to("cpu", torch.int64)
+        if tuple(lab.shape) != (B, S):
+            raise ValueError(f"labels {tuple(lab.shape)} do not match the inputs [{B}, {S}]")
+        rowmap = torch.full((B, S), sum(lens), dtype=torch.int32)  # the zero row
+        o = 0
+        for b in range(B):
+            rowmap[b, valid[b]] = torch.arange(o, o + lens[b], dtype=torch.int32)
+            o += lens[b]
+        rows, targets = rowmap[:, :-1].reshape(-1), lab[:, 1:].reshape(-1)
+        keep = targets != IGNORE_INDEX
+        _, _, loss = ops.token_logprobs(elem_logits, rows[keep], targets[keep], loss=True)
+        return loss
 
     __call__ = forward
+
+    # ---- likelihood scoring of answer candidates ------------------------------------------------------------------------------------
+    @torch.no_grad()
+    @ops.in_own_dtype
+    def score(self, input_ids: torch.Tensor, images=None, depths=None, masks=None, attention_mask=None, candidates=None) -> "ScoreOutput":
+        """Rank answer candidates by likelihood: ``candidates`` is a list of N non-empty token-id lists shared by the B prompts.
+        token_logprobs[b, c, j] = log p(cand_c[j] | prompt_b ++ cand_c[:j]), what forward() on the concatenation gives at those rows
+        up to rounding, but each prompt is prefilled once and every candidate continues from its KV pages (LlamaDecoder.
+        score_candidates).  Padding may be on either side of ``attention_mask``.  Raises ValueError on an empty candidate list or
+        candidate, an id outside the vocabulary, or a prompt + candidate longer than the decoder's max_seq_len."""
+        if not getattr(self.llm, "supports_scoring", False):
+            raise NotImplementedError("likelihood scoring (score()) on the tensor-parallel decoder")
+        cands = check_candidates(candidates, self.llm.dims.vocab_size)
+        lengths = [len(c) for c in cands]
+        if images is not None:
+            self.prepare_inputs_labels_for_multimodal(input_ids, None, attention_mask, None, None, images, masks, depths, _packed_only=True)
+            packed, lens = self._last_packed
+            lens = [int(n) for n in lens]
+        else:
+            B, T = input_ids.shape
+            rows = [slice(0, T)] * B
+            if attention_mask is not None:
+                am = attention_mask.bool().cpu()
+                rows = []
+                for b in range(B):
+                    idx = torch.nonzero(am[b]).flatten()
+                    if idx.numel() == 0 or int(idx[-1]) - int(idx[0]) + 1 != idx.numel():
+                        raise ValueError("score() needs every prompt's attention mask to be one non-empty run of ones")
+                    rows.append(slice(int(idx[0]), int(idx[-1]) + 1))
+            lens = [r.stop - r.start for r in rows]
+            if max(lens) + max(lengths) > self.llm.max_seq_len:
+                raise ValueError(f"a prompt of {max(lens)} rows and a candidate of {max(lengths)} tokens exceed max_seq_len {self.llm.max_seq_len}")
+            emb = self.llm.embed_tokens(input_ids)
+            packed = torch.cat([emb[b * T + r.start:b * T + r.stop] for b, r in enumerate(rows)], 0)
+        tok = self.llm.score_candidates(packed, lens, cands, self._score_row_budget(max(lengths)))
+        return ScoreOutput(sequence_logprobs=tok.sum(-1), token_logprobs=tok, lengths=torch.tensor(lengths, dtype=torch.int64))
+
+    def _score_row_budget(self, longest: int) -> int:
+        """Rows of one scoring pass: a quarter of the free device memory over what a row costs (its element-type logits row and the
+        chunked prefill's activations), between the longest candidate's rows and 8192."""
+        d = self.llm.dims
+        per_row = 2 * ((d.vocab_size + 7) // 8 * 8 + 3 * d.hidden_size + (2 * d.num_attention_heads + 2 * d.num_key_value_heads) * d.head_dim
+                       + d.intermediate_size)
+        free_b, _ = torch.cuda.mem_get_info(self.device)
+        return int(max(longest - 1, 1, min(8192, free_b // 4 // per_row)))
 
     def _lookup_history(self, input_ids, attention_mask, multimodal: bool) -> torch.Tensor:
         """The prompt rows of a batch-1 request as prompt-lookup history: the token id of a text row, -1 (never matches) for a row

@@ -866,6 +866,34 @@ def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor,
           "srgpt_sample_rows")
 
 
+def token_logprobs(logits: torch.Tensor, rows, targets, loss: bool = False):
+    """Log-softmax of each row of ``logits`` ([R, V] in the element type, unit inner stride, e.g. the lm_head GEMM's padded rows) at
+    target tokens, without an fp32 copy of the logits.  ``rows`` / ``targets``: host int sequences or CPU tensors of n pairs; target -100
+    is ignored.  Returns (lse fp32 [R], logprob fp32 [n], loss): logprob[i] = float(logits[rows[i], targets[i]]) - lse[rows[i]] (0 when
+    ignored); loss (a 0-dim fp32 tensor when ``loss``, else None) = the mean of -logprob over the pairs not ignored (NaN when none is).
+    Out-of-range pairs raise before anything is launched."""
+    _need(logits, ELEM(), "token_logprobs.logits")
+    if logits.dim() != 2:
+        raise SrgptError(f"token_logprobs: logits must be [rows, V], got shape {tuple(logits.shape)}")
+    ld = _rowmajor2d(logits, "token_logprobs.logits")
+    R, V = logits.shape
+    r = torch.as_tensor(rows, dtype=torch.int32).reshape(-1).contiguous()
+    t = torch.as_tensor(targets, dtype=torch.int64).reshape(-1).contiguous()
+    if r.device.type != "cpu" or t.device.type != "cpu" or r.numel() != t.numel():
+        raise SrgptError("token_logprobs: rows and targets must be host sequences of the same length")
+    n = r.numel()
+    dev = logits.device
+    lse = torch.empty(R, dtype=torch.float32, device=dev)
+    lp = torch.empty(n, dtype=torch.float32, device=dev)
+    out = torch.empty((), dtype=torch.float32, device=dev) if loss else None
+    ws = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    check(_lib.load().srgpt_token_logprobs(_p(logits), ld, R, V, _p(r) if n else None, _p(t) if n else None, n, _p(ws), ws.numel() * 8,
+                                           _p(lse), _p(lp) if n else None, _p(out), _stream()), "srgpt_token_logprobs")
+    if n or loss:
+        _count(1)
+    return lse, lp, out
+
+
 def logits_process(logits: torch.Tensor, hist: Optional[torch.Tensor], hist_row_stride: int, hist_tok_stride: int, step: Optional[torch.Tensor],
                    step_offset: int, fparams: torch.Tensor, spec: torch.Tensor, out: Optional[torch.Tensor] = None,
                    ids: Optional[torch.Tensor] = None) -> None:

@@ -66,6 +66,10 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_prompt_lookup = False  # the verify pass is a single-GPU kernel sequence
     supports_logits_processors = False  # the logits are vocabulary-parallel: no rank holds a whole row
     supports_batch_sampling = False  # the decoder implements greedy decoding only
+    supports_scoring = False  # likelihood scoring (score_candidates) is a single-GPU path
+
+    def score_candidates(self, *args, **kwargs):
+        raise NotImplementedError("likelihood scoring (score()) on the tensor-parallel decoder")
 
     def __init__(self, dims: LlamaDims, w: LlamaW, rank: int, world: int, group=None, max_seq_len: int = 4096, comm: Optional[str] = None, **kw):
         if getattr(w, "quantization", None) is not None:
