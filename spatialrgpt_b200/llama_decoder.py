@@ -18,7 +18,7 @@ import torch
 
 from . import logits_processors, ops
 from .config import LlamaDims
-from .weights import LlamaW, Nf4W
+from .weights import LlamaW
 
 PAGE_SIZE = 16
 
@@ -307,15 +307,11 @@ class LlamaDecoder:
         if self.nf4_planes_only and os.environ.get("SRGPT_DECODE_NF4", "1") == "0":
             raise ValueError("SRGPT_DECODE_NF4=0 runs the decode step over the dequantized copies, which a model loaded with "
                              "nf4_dequantized_copy=False does not keep")
-        self._layer_array = self._make_layer_array()
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
         # ("verify", T, ngram), ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
-        # dropped whenever one of them is replaced: the KV cache and layer array (ensure_capacity), the processor spec (_set_processors)
+        # dropped whenever one of them is replaced: the KV cache and the layer stack's array (ensure_capacity), the processor spec (_set_processors)
         # and the batched-decode buffers (_batch_state).
         self._graphs = {}
-        self.kernels_per_decode_step = 5 * dims.num_hidden_layers + 2
-        # batched decode step: 8 kernels per layer, 12 with the FP8 activation quantizers
-        self._batch_kernels_per_layer = 12 if self.fp8 else 8
         # sampling mode (do_sample=True): temperature / top_p live in device memory so one captured graph serves any setting
         self.sample_params = torch.tensor([1.0, 1.0, 0.0], dtype=torch.float32, device=dev)
         self.sample_logits: Optional[torch.Tensor] = None
@@ -341,12 +337,9 @@ class LlamaDecoder:
         # and the batch-1 decode step streams the NF4 planes instead (bit-identical).  decode_quant: matrix -> "nf4" or why the step reads
         # its dequantized copy.  SRGPT_DECODE_NF4=0 runs the usual step over the dequantized copies.
         self.decode_quant = {}
-        if self.fp8:
-            self._fp8_decode_weights()
-        elif getattr(w, "quantization", None) == "nf4" and os.environ.get("SRGPT_DECODE_NF4", "1") != "0":
-            self._nf4_decode_weights()
-        elif self.packs_decode_weights and self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
-            self._pack_decode_weights()
+        self._build_stack()
+        self.kernels_per_decode_step = self.stack.step_kernels
+        self._batch_kernels_per_layer = self.stack.kernels_per_layer  # batched decode step: as a prefill layer
 
     supports_prefix_reuse = True
     supports_prompt_lookup = True
@@ -358,59 +351,50 @@ class LlamaDecoder:
     _host_ids = None  # pinned host copy of generated ids for the stop checks, and the stream that fills it (_pinned_ids)
     _copy_stream = None
     last_speculation = (0, 0, 0)
-    _packed_array = None  # srgpt_llama_layer_packed[] of the decode step, None: the bf16 step
-    _lm_packed = None
-    _nf4_array = None  # srgpt_llama_layer_nf4[] of the decode step
     nf4_planes_only = False
+    stack: Optional[ops.LlamaStack] = None  # the layers as the composite entry points take them (_build_stack)
 
     @property
-    def _planes_array(self):
-        """The srgpt_llama_layer_nf4[] the prefill stacks and the verify pass take (planes-only NF4 models), else None."""
-        return self._nf4_array if self.nf4_planes_only else None
+    def _packed_array(self):
+        """The srgpt_llama_layer_packed[] the decode step streams, None when it streams no packed matrix."""
+        return self.stack.packed
 
-    def _make_layer_array(self):
-        """The layer descriptors of the prefill stacks and the decode step over the current KV cache."""
+    @property
+    def _nf4_array(self):
+        """The srgpt_llama_layer_nf4[] the decode step streams, None when it streams no NF4 planes."""
+        return self.stack.nf4
+
+    @ops.in_own_dtype
+    def _build_stack(self) -> None:
+        """The layers as the composite entry points take them (ops.LlamaStack), and the reports of what the decode step streams.  FP8 and
+        NF4 layers stream their codes or planes; lm_head stays unquantized and is packed in the bf16 build (SRGPT_DECODE_PACK=0: plain).
+        Unquantized bf16 layers stream their 12-bit packings, where a matrix has one."""
+        w, quant = self.w, getattr(self.w, "quantization", None)
+        pack = self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0"
+        packed, lm_packed = None, None
+        if quant == "fp8" or (quant == "nf4" and os.environ.get("SRGPT_DECODE_NF4", "1") != "0"):
+            for l, lw in enumerate(w.layers):
+                for name in ("qkv", "o", "gateup", "down"):
+                    K = getattr(lw, name + "_w").shape[1]
+                    self.decode_quant[f"layers.{l}.{name}"] = ("fp8" if quant == "fp8" else "nf4" if lw.nf4[name] is not None else
+                                                               f"K = {K} is not a multiple of {ops.NF4_BATCH}")
+            if pack:
+                lm_packed, why = ops.pack12(w.lm_head)
+                self.decode_pack["lm_head"] = why or "packed"
+        elif self.packs_decode_weights and pack:
+            packed = []
+            for l, lw in enumerate(w.layers):
+                packed.append({})
+                for name in ("qkv", "o", "gateup", "down"):
+                    packed[l][name], why = ops.pack12(getattr(lw, name + "_w"))
+                    self.decode_pack[f"layers.{l}.{name}"] = why or "packed"
+            lm_packed, why = ops.pack12(w.lm_head)
+            self.decode_pack["lm_head"] = why or "packed"
+            if "packed" not in self.decode_pack.values():
+                packed = None
         pages = [self.cache.layer(l) for l in range(self.dims.num_hidden_layers)]
-        return ops.make_llama_fp8_array(self.w.layers, pages) if self.fp8 else ops.make_llama_layer_array(self.w.layers, pages)
-
-    @ops.in_own_dtype
-    def _fp8_decode_weights(self) -> None:
-        """The FP8 step streams every layer matrix through the FP8 GEMV; lm_head stays unquantized and is packed in the bf16 build
-        (SRGPT_DECODE_PACK=0: plain)."""
-        for l in range(self.dims.num_hidden_layers):
-            for name in ("qkv", "o", "gateup", "down"):
-                self.decode_quant[f"layers.{l}.{name}"] = "fp8"
-        if self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
-            self._lm_packed, why = ops.pack12(self.w.lm_head)
-            self.decode_pack["lm_head"] = why or "packed"
-
-    @ops.in_own_dtype
-    def _nf4_decode_weights(self) -> None:
-        """The NF4 step's layer array; lm_head stays unquantized and is packed in the bf16 build (SRGPT_DECODE_PACK=0: plain)."""
-        for l, lw in enumerate(self.w.layers):
-            for name in ("qkv", "o", "gateup", "down"):
-                K = getattr(lw, name + "_w").shape[1]
-                self.decode_quant[f"layers.{l}.{name}"] = "nf4" if lw.nf4[name] is not None else f"K = {K} is not a multiple of {ops.NF4_BATCH}"
-        if self.dtype == torch.bfloat16 and os.environ.get("SRGPT_DECODE_PACK", "1") != "0":
-            self._lm_packed, why = ops.pack12(self.w.lm_head)
-            self.decode_pack["lm_head"] = why or "packed"
-        if any(v == "nf4" for v in self.decode_quant.values()):
-            self._nf4_array = ops.make_llama_nf4_array([lw.nf4 for lw in self.w.layers])
-
-    @ops.in_own_dtype
-    def _pack_decode_weights(self) -> None:
-        packed_layers = []
-        for l, lw in enumerate(self.w.layers):
-            pl = {}
-            for name in ("qkv", "o", "gateup", "down"):
-                pl[name], why = ops.pack12(getattr(lw, name + "_w"))
-                self.decode_pack[f"layers.{l}.{name}"] = why or "packed"
-            packed_layers.append(pl)
-        self._lm_packed, why = ops.pack12(self.w.lm_head)
-        self.decode_pack["lm_head"] = why or "packed"
-        if any(v == "packed" for v in self.decode_pack.values()):
-            self._packed_layers = packed_layers  # keeps the tensors behind the descriptors alive
-            self._packed_array = ops.make_llama_packed_array(packed_layers)
+        self.stack = ops.LlamaStack(w.layers, pages, packed=packed, nf4="nf4" in self.decode_quant.values(), planes_only=self.nf4_planes_only,
+                                    lm_packed=lm_packed)
 
     def _record_prefix(self, rows: int) -> None:
         self.prefix_rows = rows
@@ -445,7 +429,7 @@ class LlamaDecoder:
         self.cache = None
         del c
         self.cache = PagedKVCache(d, max(need_pages, n_pages_old), max(n_seqs, n_seqs_old), (self.max_seq_len + PAGE_SIZE - 1) // PAGE_SIZE, self.device, self.dtype)
-        self._layer_array = self._make_layer_array()
+        self.stack.set_pages([self.cache.layer(l) for l in range(d.num_hidden_layers)])
 
     @ops.in_own_dtype
     def embed_tokens(self, ids: torch.Tensor) -> torch.Tensor:
@@ -472,12 +456,9 @@ class LlamaDecoder:
         x = inputs_embeds.to(self.dtype).contiguous().clone()
         if start_pos != 0:
             cu = torch.tensor([0, S], dtype=torch.int32, device=self.device)
-            return ops.llama_prefill_chunk_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp,
-                                                  self.cache.page_tables[seq:seq + 1], PAGE_SIZE, self.cache.n_pages, cu, S,
-                                                  nf4_array=self._planes_array)
-        pt = self.cache.page_tables[seq]
-        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pt, PAGE_SIZE,
-                                        nf4_array=self._planes_array)
+            return ops.llama_prefill_chunk_layers(x, self.stack, d, self.cos, self.sin, sp, self.cache.page_tables[seq:seq + 1], PAGE_SIZE,
+                                                  self.cache.n_pages, cu, S)
+        return ops.llama_prefill_layers(x, self.stack, d, self.cos, self.sin, sp, self.cache.page_tables[seq], PAGE_SIZE)
 
     @ops.in_own_dtype
     def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int], page_tables: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -496,8 +477,7 @@ class LlamaDecoder:
         sp = torch.zeros(B, dtype=torch.int32, device=self.device)
         x = packed_embeds.to(self.dtype).contiguous().clone()
         pts = self.cache.page_tables[:B] if page_tables is None else page_tables
-        return ops.llama_prefill_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pts,
-                                        PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens), nf4_array=self._planes_array)
+        return ops.llama_prefill_layers(x, self.stack, d, self.cos, self.sin, sp, pts, PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens))
 
     @ops.in_own_dtype
     def first_tokens(self, hidden_packed: torch.Tensor, seq_lens: List[int], return_logits: bool = False, repeat: int = 1):
@@ -533,22 +513,8 @@ class LlamaDecoder:
         d, w = self.dims, self.w
         if (sample or proc) and logits_out is None:
             logits_out = self._sample_buffer()
-        if self.fp8:
-            ops.llama_decode_step_fp8(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos, self.sin,
-                                      self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed, self.lm_ws, self.out_ids,
-                                      self.step, logits_out)
-        elif self._nf4_array is not None:
-            ops.llama_decode_step_nf4(self.h, self._layer_array, self._nf4_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
-                                      d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
-                                      self.lm_ws, self.out_ids, self.step, logits_out)
-        elif self._packed_array is not None:
-            ops.llama_decode_step_packed(self.h, self._layer_array, self._packed_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf,
-                                         d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed, w.embed,
-                                         self.lm_ws, self.out_ids, self.step, logits_out)
-        else:
-            ops.llama_decode_step(self.h, self._layer_array, d.num_hidden_layers, self.q_buf, self.attn_buf, self.act_buf, d, self.cos,
-                                  self.sin, self.pos, self.active_pt, PAGE_SIZE, w.norm, w.lm_head, w.embed, self.lm_ws,
-                                  self.out_ids, self.step, logits_out)
+        ops.llama_decode_step(self.h, self.stack, self.q_buf, self.attn_buf, self.act_buf, d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE,
+                              w.norm, w.lm_head, w.embed, self.lm_ws, self.out_ids, self.step, logits_out)
         if proc:
             self._process_row(logits_out, sample)
         elif sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
@@ -765,15 +731,14 @@ class LlamaDecoder:
         d, w, st = self.dims, self.w, self._vstate
         if logits_all is not None and st["logits"] is None:
             st["logits"] = torch.empty((ops.SPEC_T_MAX, d.vocab_size), dtype=torch.float32, device=self.device)
-        ops.llama_verify_step(st["h"], self._layer_array, self._packed_array, d.num_hidden_layers, st["q"], st["attn"], st["act"], T, d,
-                              self.cos, self.sin, self.pos, st["pos_rows"], self.active_pt, PAGE_SIZE, w.norm, w.lm_head, self._lm_packed,
-                              w.embed, st["ws"], st["logits"] if logits_all is not None else None, logits_all, st["prompt"], st["prompt_len"],
-                              ngram, st["draft"], self.out_ids, self.step, st["state"], nf4_array=self._planes_array)
+        ops.llama_verify_step(st["h"], self.stack, st["q"], st["attn"], st["act"], T, d, self.cos, self.sin, self.pos, st["pos_rows"], self.active_pt,
+                              PAGE_SIZE, w.norm, w.lm_head, w.embed, st["ws"], st["logits"] if logits_all is not None else None, logits_all,
+                              st["prompt"], st["prompt_len"], ngram, st["draft"], self.out_ids, self.step, st["state"])
 
     def _verify_graph(self, T: int, ngram: int) -> torch.cuda.CUDAGraph:
         """The captured verify pass of this (T, n-gram size); its warm-up writes only this sequence's slack."""
         return self._capture(("verify", T, ngram), lambda: self._verify_launch(T, ngram),
-                             (self.pos, self.step, self.out_ids, self._vstate["state"]), 5 * self.dims.num_hidden_layers + 3)
+                             (self.pos, self.step, self.out_ids, self._vstate["state"]), self.stack.verify_kernels)
 
     def _verify_loop(self, T: int, ngram: int, lookup_ids, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits):
         """Tokens 1.. of sequence 0 by verify passes; pos / step / out_ids[:1] are set by the first token.  After each pass its state
@@ -873,7 +838,7 @@ class LlamaDecoder:
                   logits=z(B, (V + 7) // 8 * 8), pos=z(B, dtype=torch.int32), step=z(1, dtype=torch.int32), ids=z(B, dtype=torch.int64),
                   out=z(self.out_ids.numel() * B, dtype=torch.int64), ticket=z(1, dtype=torch.int32),
                   cu=torch.arange(B + 1, dtype=torch.int32, device=dev), seeds=z(B, dtype=torch.int64), proc_rows=None)
-        if self.fp8:  # the activation quantizer's codes and row scales
+        if self.stack.quantizes_activations:  # the activation quantizer's codes and row scales
             st.update(q8=z(B, max(H, nh * hd, I), dtype=torch.uint8), s8=z(B, dtype=torch.float32))
         self._bstate = st
         return st
@@ -887,14 +852,9 @@ class LlamaDecoder:
         qd = nh * hd
         h, xn, qkv, attn, act = st["h"], st["xn"], st["qkv"], st["attn"], st["act"]
         pts = self.cache.page_tables
-        if self.fp8:  # every linear as the activation quantizer + the FP8 GEMM
-            def linear(x, wt, **kw):
-                return ops.linear_fp8(x, wt, q=st["q8"][:, :x.shape[1]], scale=st["s8"], **kw)
-        elif self.nf4_planes_only:  # the NF4 GEMM where a matrix is held as planes
-            def linear(x, wt, **kw):
-                return ops.gemm_nf4(x, wt, **kw) if isinstance(wt, Nf4W) else ops.gemm(x, wt, **kw)
-        else:
-            linear = ops.gemm
+
+        def linear(x, wt, **kw):
+            return ops.linear(x, wt, st.get("q8"), st.get("s8"), **kw)
         for l, lw in enumerate(w.layers):
             pages = self.cache.layer(l)
             ops.rmsnorm(h, lw.in_norm, d.rms_norm_eps, out=xn)
@@ -1276,8 +1236,8 @@ class LlamaDecoder:
                 sp = torch.tensor([seq_lens[it[0]] for it in items], dtype=torch.int32).to(dev)
                 pts = torch.tensor(tables, dtype=torch.int32).to(dev)
                 x = self.embed_tokens(torch.tensor(ids, dtype=torch.int64))
-                h = ops.llama_prefill_chunk_layers(x, self._layer_array, d.num_hidden_layers, d, self.cos, self.sin, sp, pts, PAGE_SIZE,
-                                                   self.cache.n_pages, cu, max(it[3] for it in items), nf4_array=self._planes_array)
+                h = ops.llama_prefill_chunk_layers(x, self.stack, d, self.cos, self.sin, sp, pts, PAGE_SIZE, self.cache.n_pages, cu,
+                                                   max(it[3] for it in items))
                 lg = self.lm_head_rows(h, out=buf[:R])
                 _, lp, _ = ops.token_logprobs(lg, list(range(R)), targets)
                 out.view(-1)[torch.tensor(dst, dtype=torch.int64).to(dev)] = lp

@@ -13,6 +13,7 @@ import torch
 from . import _lib
 from ._lib import SrgptError
 from ._lib import check as _check_rc
+from .weights import Fp8W, Nf4W, Packed12W
 
 _KERNELS_PER_CALL = {"srgpt_lm_head_local_best_bf16": 2, "srgpt_mask_pool_bf16": 2, "srgpt_mask_weights": 2, "srgpt_lm_head_argmax_bf16": 2, "srgpt_depth_to_u8x3": 3,
                      "srgpt_lm_head_argmax_packed_bf16": 2, "srgpt_nf4_double_quant": 2}
@@ -421,7 +422,6 @@ def pack12(w: torch.Tensor, verify: bool = True):
     """Pack a bf16 matrix [N, K] for the decode GEMV.  Returns (Packed12W, None), or (None, reason) when the matrix must stay
     plain: K not a multiple of 1024, Inf / NaN, more than 1 % exceptions or more than 32 in one row.  With ``verify`` the packed
     matrix is unpacked on the device and compared bit for bit with ``w``; a difference raises SrgptError."""
-    from .weights import Packed12W
     _need(w, torch.bfloat16, "pack12.w")
     ldw = _rowmajor2d(w, "pack12.w")
     N, K = w.shape
@@ -541,7 +541,6 @@ def _nf4_desc(p) -> "_lib.Nf4":
 def nf4_planes(codes: torch.Tensor, scale: torch.Tensor, deq: torch.Tensor):
     """The decode GEMV's planes of a (fused) matrix: (Nf4W, None), or (None, reason) when K is not a multiple of 1024 and the decode
     step reads the dequantized matrix instead.  The lane-ordered planes must dequantize to exactly ``deq``; SrgptError otherwise."""
-    from .weights import Nf4W
     N, K = codes.shape[0], codes.shape[1] * 2
     if K % NF4_BATCH:
         return None, f"K = {K} is not a multiple of {NF4_BATCH}"
@@ -1037,45 +1036,76 @@ def make_siglip_layer_array(layers):
     return arr
 
 
-def make_llama_layer_array(layers, kv_pages_per_layer):
-    """ctypes array of srgpt_llama_layer_weights; a matrix held only as NF4 planes (an Nf4W in its *_w field) gets NULL, and the NF4
-    entry points take it from the srgpt_llama_layer_nf4 array instead."""
-    arr = (_lib.LlamaLayerWeights * len(layers))()
-    for i, lw in enumerate(layers):
-        for name in ("in_norm", "qkv_w", "o_w", "post_norm", "gateup_w", "down_w"):
-            t = getattr(lw, name)
-            setattr(arr[i], name, t.data_ptr() if isinstance(t, torch.Tensor) else None)
-        arr[i].kv_pages = kv_pages_per_layer[i].data_ptr()
+_MATS = ("qkv", "o", "gateup", "down")
+
+
+def _matrix_array(struct, desc, per_layer):
+    """ctypes array of `struct` (srgpt_llama_layer_packed / _nf4) over per-layer dicts {"qkv", "o", "gateup", "down"} -> weight or None."""
+    arr = (struct * len(per_layer))()
+    for i, pl in enumerate(per_layer):
+        for name in _MATS:
+            setattr(arr[i], name, desc(pl[name]))
     return arr
 
 
-def make_llama_packed_array(packed_layers):
-    """ctypes array of srgpt_llama_layer_packed over per-layer dicts {"qkv", "o", "gateup", "down"} -> Packed12W or None (plain)."""
-    arr = (_lib.LlamaLayerPacked * len(packed_layers))()
-    for i, pl in enumerate(packed_layers):
-        for name in ("qkv", "o", "gateup", "down"):
-            setattr(arr[i], name, _packed_desc(pl[name]))
-    return arr
+class LlamaStack:
+    """The Llama decoder's layers as the composite entry points (layers.cu) take them, and which family of those entry points each
+    call uses.  Holds the layer array over the current KV pages (srgpt_llama_layer_fp8 when the layers' matrices are Fp8W, else
+    srgpt_llama_layer_weights), the decode step's 12-bit packed matrices (``packed``: per-layer dicts of Packed12W or None) or NF4
+    planes (``nf4``: from the layers' ``nf4`` dicts; ``planes_only``: the matrices keep no element-type copy, so prefill and the verify
+    pass read the planes too), and lm_head's packing (``lm_packed``), with the tensors behind them."""
 
+    def __init__(self, layers, kv_pages, packed=None, nf4: bool = False, planes_only: bool = False, lm_packed=None):
+        self.src, self.n = layers, len(layers)
+        self.quantizes_activations = any(isinstance(lw.qkv_w, Fp8W) for lw in layers)  # FP8: prefill / batched linears quantize x
+        self.packed_layers, self.lm_packed = packed, lm_packed
+        self.packed = None if packed is None else _matrix_array(_lib.LlamaLayerPacked, _packed_desc, packed)
+        self.nf4 = _matrix_array(_lib.LlamaLayerNf4, _nf4_desc, [lw.nf4 for lw in layers]) if nf4 else None
+        self.planes = self.nf4 if planes_only else None
+        self._lm_desc = _packed_desc(lm_packed)
+        # kernels per layer of the prefill stacks and the batched step (FP8: + 4 activation quantizers); of a decode step; of a verify pass
+        self.kernels_per_layer = 12 if self.quantizes_activations else 8
+        self.step_kernels = 5 * self.n + 2
+        self.verify_kernels = 5 * self.n + 3
+        self.set_pages(kv_pages)
 
-def make_llama_nf4_array(nf4_layers):
-    """ctypes array of srgpt_llama_layer_nf4 over per-layer dicts {"qkv", "o", "gateup", "down"} -> Nf4W or None (dequantized weight)."""
-    arr = (_lib.LlamaLayerNf4 * len(nf4_layers))()
-    for i, pl in enumerate(nf4_layers):
-        for name in ("qkv", "o", "gateup", "down"):
-            setattr(arr[i], name, _nf4_desc(pl[name]))
-    return arr
+    def set_pages(self, kv_pages) -> None:
+        """Rebuild the layer array over new per-layer KV pages (the packed and NF4 arrays point at no page).  A matrix held only as NF4
+        planes (an Nf4W in its *_w field) gets NULL: the NF4 entry points take it from the planes."""
+        if self.quantizes_activations:
+            arr = (_lib.LlamaLayerFp8 * self.n)()
+            for i, lw in enumerate(self.src):
+                arr[i].in_norm, arr[i].post_norm = lw.in_norm.data_ptr(), lw.post_norm.data_ptr()
+                for name in _MATS:
+                    setattr(arr[i], name, _fp8_desc(getattr(lw, name + "_w")))
+                arr[i].kv_pages = kv_pages[i].data_ptr()
+        else:
+            arr = (_lib.LlamaLayerWeights * self.n)()
+            for i, lw in enumerate(self.src):
+                for name in ("in_norm", "qkv_w", "o_w", "post_norm", "gateup_w", "down_w"):
+                    t = getattr(lw, name)
+                    setattr(arr[i], name, t.data_ptr() if isinstance(t, torch.Tensor) else None)
+                arr[i].kv_pages = kv_pages[i].data_ptr()
+        self.layers = arr
 
-
-def make_llama_fp8_array(layers, kv_pages_per_layer):
-    """ctypes array of srgpt_llama_layer_fp8 over FP8 LlamaLayerW (their *_w fields hold Fp8W)."""
-    arr = (_lib.LlamaLayerFp8 * len(layers))()
-    for i, lw in enumerate(layers):
-        arr[i].in_norm, arr[i].post_norm = lw.in_norm.data_ptr(), lw.post_norm.data_ptr()
-        for name in ("qkv", "o", "gateup", "down"):
-            setattr(arr[i], name, _fp8_desc(getattr(lw, name + "_w")))
-        arr[i].kv_pages = kv_pages_per_layer[i].data_ptr()
-    return arr
+    def entry(self, op: str):
+        """(symbol, layer array arguments, lm_head packing arguments) of srgpt_llama_<op>_*, op = "prefill_layers",
+        "prefill_chunk_layers", "decode_step" or "verify_step".  Prefill takes the FP8 or, planes-only, the NF4 stack; the decode step
+        streams FP8, NF4 or packed matrices when there are some; the verify pass NF4 planes-only or packed ones."""
+        step = op in ("decode_step", "verify_step")
+        nf4 = self.nf4 if op == "decode_step" else self.planes
+        if self.quantizes_activations:
+            if op == "verify_step":
+                raise SrgptError("the verify pass of prompt-lookup decoding has no FP8 form")
+            fmt, arrays = "fp8_", (self.layers,)
+        elif nf4 is not None:
+            fmt, arrays = "nf4_", (self.layers, nf4)
+        elif step and self.packed is not None:
+            fmt, arrays = "packed_", (self.layers, self.packed)
+        else:
+            fmt, arrays = "", (self.layers,)
+        lm = (C.byref(self._lm_desc),) if step and fmt else ()
+        return f"srgpt_llama_{op}_{fmt}bf16", tuple(C.cast(a, C.c_void_p) for a in arrays), lm
 
 
 def clip_embed(patch_embeds: torch.Tensor, class_embedding: torch.Tensor, position_embedding: torch.Tensor, n_img: int, T: int) -> torch.Tensor:
@@ -1108,23 +1138,35 @@ def siglip_layers(x: torch.Tensor, layer_array, n_layers: int, n_img: int, T: in
     return x
 
 
-def _is_fp8_array(layer_array) -> bool:
-    return getattr(layer_array, "_type_", None) is _lib.LlamaLayerFp8
-
-
 def _fp8_workspaces(S: int, dims, dev):
     """The activation quantizer's codes [S, max(H, nh hd, I)] and scales [S] of the FP8 layer stacks."""
     K = max(dims.hidden_size, dims.num_attention_heads * dims.head_dim, dims.intermediate_size)
     return torch.empty(S * K, dtype=torch.uint8, device=dev), torch.empty(S, dtype=torch.float32, device=dev)
 
 
-def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_table, page_size: int,
-                         cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0, nf4_array=None) -> torch.Tensor:
+def _prefill(op: str, x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, rows) -> torch.Tensor:
+    """srgpt_llama_<op>_* of the stack over x [S, H] in place; ``rows`` = the entry point's arguments between sin and the stream."""
+    _ensure_gemm_workspace(x.device)
+    S, H = x.shape
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    dev = x.device
+    ws = (torch.empty((S, H), dtype=ELEM(), device=dev), torch.empty((S, (nh + 2 * nkv) * hd), dtype=ELEM(), device=dev),
+          torch.empty((S, nh * hd), dtype=ELEM(), device=dev), torch.empty((S, I), dtype=ELEM(), device=dev))
+    if stack.quantizes_activations:
+        ws += _fp8_workspaces(S, dims, dev)
+    name, arrays, _ = stack.entry(op)
+    check(getattr(_lib.load(), name)(_p(x), *arrays, stack.n, *(_p(t) for t in ws), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
+                                     _p(start_pos), *rows, _stream()), name)
+    _count(stack.kernels_per_layer * stack.n)
+    return x
+
+
+def llama_prefill_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, page_table, page_size: int,
+                         cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0) -> torch.Tensor:
     """All decoder layers over the prompt rows x [S, H] in place (K/V appended to the paged cache).  One prompt
     (page_table [cap], start_pos [1]) or, with cu_seqlens [n_seqs+1], n_seqs prompts packed back to back
-    (page_table [n_seqs, cap], start_pos [n_seqs]).  ``nf4_array`` (make_llama_nf4_array): every matrix with planes through gemm_nf4."""
+    (page_table [n_seqs, cap], start_pos [n_seqs])."""
     _need(x, ELEM(), "llama_prefill_layers.x")
-    _ensure_gemm_workspace(x.device)
     n_seqs, pt_stride = 1, 0
     if cu_seqlens is not None:
         _need(cu_seqlens, torch.int32, "llama_prefill_layers.cu_seqlens")
@@ -1132,132 +1174,42 @@ def llama_prefill_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos,
         if page_table.dim() != 2 or page_table.shape[0] < n_seqs or start_pos.numel() < n_seqs or page_table.stride(1) != 1:
             raise SrgptError("llama_prefill_layers: packed prompts need page_table [n_seqs, cap] and start_pos [n_seqs]")
         pt_stride = page_table.stride(0)
-    S, H = x.shape
-    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    dev = x.device
-    ws_h = torch.empty((S, H), dtype=ELEM(), device=dev)
-    ws_qkv = torch.empty((S, (nh + 2 * nkv) * hd), dtype=ELEM(), device=dev)
-    ws_attn = torch.empty((S, nh * hd), dtype=ELEM(), device=dev)
-    ws_act = torch.empty((S, I), dtype=ELEM(), device=dev)
-    import ctypes
-    if _is_fp8_array(layer_array):
-        ws_q8, ws_s = _fp8_workspaces(S, dims, dev)
-        check(_lib.load().srgpt_llama_prefill_layers_fp8_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
-                                                              _p(ws_attn), _p(ws_act), _p(ws_q8), _p(ws_s), S, H, nh, nkv, hd, I, dims.rms_norm_eps,
-                                                              _p(cos), _p(sin), _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens),
-                                                              max_seqlen, pt_stride, _stream()), "srgpt_llama_prefill_layers_fp8_bf16")
-        _count(12 * n_layers)
-        return x
-    if nf4_array is not None:
-        check(_lib.load().srgpt_llama_prefill_layers_nf4_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), ctypes.cast(nf4_array, ctypes.c_void_p),
-                                                              n_layers, _p(ws_h), _p(ws_qkv), _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I,
-                                                              dims.rms_norm_eps, _p(cos), _p(sin), _p(start_pos), _p(page_table), page_size, n_seqs,
-                                                              _p(cu_seqlens), max_seqlen, pt_stride, _stream()), "srgpt_llama_prefill_layers_nf4_bf16")
-        _count(8 * n_layers)
-        return x
-    check(_lib.load().srgpt_llama_prefill_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
-                                                      _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
-                                                      _p(start_pos), _p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride,
-                                                      _stream()), "srgpt_llama_prefill_layers_bf16")
-    _count(8 * n_layers)
-    return x
+    return _prefill("prefill_layers", x, stack, dims, cos, sin, start_pos,
+                    (_p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride))
 
 
-def llama_prefill_chunk_layers(x: torch.Tensor, layer_array, n_layers: int, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
-                               cu_seqlens: torch.Tensor, max_rows: int, nf4_array=None) -> torch.Tensor:
+def llama_prefill_chunk_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
+                               cu_seqlens: torch.Tensor, max_rows: int) -> torch.Tensor:
     """All decoder layers over x [S, H] in place: n_seqs chunks packed by cu_seqlens [n_seqs+1] that continue their sequences at
-    start_pos [n_seqs] (page_tables [n_seqs, cap]); attention reads every earlier position from the paged cache.  ``nf4_array``: as
-    llama_prefill_layers()."""
+    start_pos [n_seqs] (page_tables [n_seqs, cap]); attention reads every earlier position from the paged cache."""
     _need(x, ELEM(), "llama_prefill_chunk_layers.x")
     _need(cu_seqlens, torch.int32, "llama_prefill_chunk_layers.cu_seqlens")
-    _ensure_gemm_workspace(x.device)
     n_seqs = cu_seqlens.numel() - 1
     if page_tables.dim() != 2 or page_tables.shape[0] < n_seqs or start_pos.numel() < n_seqs or page_tables.stride(1) != 1:
         raise SrgptError("llama_prefill_chunk_layers: page_tables [n_seqs, cap] and start_pos [n_seqs] expected")
-    S, H = x.shape
-    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    dev = x.device
-    ws_h = torch.empty((S, H), dtype=ELEM(), device=dev)
-    ws_qkv = torch.empty((S, (nh + 2 * nkv) * hd), dtype=ELEM(), device=dev)
-    ws_attn = torch.empty((S, nh * hd), dtype=ELEM(), device=dev)
-    ws_act = torch.empty((S, I), dtype=ELEM(), device=dev)
-    import ctypes
-    if _is_fp8_array(layer_array):
-        ws_q8, ws_s = _fp8_workspaces(S, dims, dev)
-        check(_lib.load().srgpt_llama_prefill_chunk_layers_fp8_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
-                                                                    _p(ws_attn), _p(ws_act), _p(ws_q8), _p(ws_s), S, H, nh, nkv, hd, I,
-                                                                    dims.rms_norm_eps, _p(cos), _p(sin), _p(start_pos), _p(page_tables),
-                                                                    page_tables.stride(0), page_size, n_pages, n_seqs, _p(cu_seqlens), max_rows,
-                                                                    _stream()), "srgpt_llama_prefill_chunk_layers_fp8_bf16")
-        _count(12 * n_layers)
-        return x
-    if nf4_array is not None:
-        check(_lib.load().srgpt_llama_prefill_chunk_layers_nf4_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p),
-                                                                    ctypes.cast(nf4_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
-                                                                    _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
-                                                                    _p(start_pos), _p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs,
-                                                                    _p(cu_seqlens), max_rows, _stream()), "srgpt_llama_prefill_chunk_layers_nf4_bf16")
-        _count(8 * n_layers)
-        return x
-    check(_lib.load().srgpt_llama_prefill_chunk_layers_bf16(_p(x), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(ws_h), _p(ws_qkv),
-                                                            _p(ws_attn), _p(ws_act), S, H, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
-                                                            _p(start_pos), _p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs,
-                                                            _p(cu_seqlens), max_rows, _stream()), "srgpt_llama_prefill_chunk_layers_bf16")
-    _count(8 * n_layers)
-    return x
+    return _prefill("prefill_chunk_layers", x, stack, dims, cos, sin, start_pos,
+                    (_p(page_tables), page_tables.stride(0), page_size, n_pages, n_seqs, _p(cu_seqlens), max_rows))
 
 
-def llama_decode_step(h, layer_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table, page_size: int,
+def llama_decode_step(h, stack: LlamaStack, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table, page_size: int,
                       final_norm, lm_head, embed, lm_ws, out_ids, step, logits_out=None) -> None:
-    import ctypes
+    """One whole decode step (5 kernels per layer, lm_head + arg max) streaming the stack's decode weights."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    check(_lib.load().srgpt_llama_decode_step_bf16(_p(h), ctypes.cast(layer_array, ctypes.c_void_p), n_layers, _p(q_buf), _p(attn_buf),
-                                                   _p(act_buf), dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin),
-                                                   _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head), dims.vocab_size,
-                                                   _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), _stream()),
-          "srgpt_llama_decode_step_bf16")
+    name, arrays, lm = stack.entry("decode_step")
+    check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I,
+                                     dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head), *lm,
+                                     dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), _stream()), name)
+    _count(stack.step_kernels)
 
 
-def llama_decode_step_packed(h, layer_array, packed_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table,
-                             page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
-    """llama_decode_step() streaming the packed matrices of ``packed_array`` (make_llama_packed_array) and ``lm_packed``
-    (a Packed12W or None); bit-identical."""
-    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    lm_d = _packed_desc(lm_packed)
-    check(_lib.load().srgpt_llama_decode_step_packed_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(packed_array, C.c_void_p), n_layers,
-                                                          _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
-                                                          _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
-                                                          C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
-                                                          _stream()), "srgpt_llama_decode_step_packed_bf16")
-    _count(5 * n_layers + 2)
-
-
-def llama_decode_step_nf4(h, layer_array, nf4_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table,
-                          page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
-    """llama_decode_step() streaming the NF4 planes of ``nf4_array`` (make_llama_nf4_array) and lm_head from ``lm_packed`` (a
-    Packed12W or None); bit-identical to the plain step over the dequantized weights."""
-    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    lm_d = _packed_desc(lm_packed)
-    check(_lib.load().srgpt_llama_decode_step_nf4_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(nf4_array, C.c_void_p), n_layers,
-                                                       _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
-                                                       _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head),
-                                                       C.byref(lm_d), dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step),
-                                                       _stream()), "srgpt_llama_decode_step_nf4_bf16")
-    _count(5 * n_layers + 2)
-
-
-def llama_decode_step_fp8(h, fp8_array, n_layers: int, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table, page_size: int,
-                          final_norm, lm_head, lm_packed, embed, lm_ws, out_ids, step, logits_out=None) -> None:
-    """llama_decode_step() over FP8 layers (make_llama_fp8_array): every layer matrix streamed by the FP8 GEMV (gemv_fp8), lm_head from
-    ``lm_packed`` (a Packed12W or None) or lm_head."""
-    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    lm_d = _packed_desc(lm_packed)
-    check(_lib.load().srgpt_llama_decode_step_fp8_bf16(_p(h), C.cast(fp8_array, C.c_void_p), n_layers, _p(q_buf), _p(attn_buf), _p(act_buf),
-                                                       dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos),
-                                                       _p(page_table), page_size, _p(final_norm), _p(lm_head), C.byref(lm_d), dims.vocab_size,
-                                                       _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), _stream()),
-          "srgpt_llama_decode_step_fp8_bf16")
-    _count(5 * n_layers + 2)
+def linear(x: torch.Tensor, w, q8: Optional[torch.Tensor] = None, s8: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
+    """x · w^T (kw: gemm's residual / epilogue / out) by the kernel of w's format: gemm over an element-type matrix, gemm_nf4 over an
+    Nf4W, the activation quantizer into q8 [M, >= K] / s8 [M] + gemm_fp8 over an Fp8W."""
+    if isinstance(w, Nf4W):
+        return gemm_nf4(x, w, **kw)
+    if isinstance(w, Fp8W):
+        return linear_fp8(x, w, q=q8[:, :x.shape[1]], scale=s8, **kw)
+    return gemm(x, w, **kw)
 
 
 # ------------------------------------------------------------------------------------------------ prompt-lookup speculative decoding
@@ -1339,27 +1291,14 @@ def spec_accept(workspace: torch.Tensor, V: int, T: int, draft_ids: torch.Tensor
                                         _p(logits_rows), _p(logits_all), _stream()), "srgpt_spec_accept")
 
 
-def llama_verify_step(h, layer_array, packed_array, n_layers: int, q_buf, attn_buf, act_buf, T: int, dims, cos, sin, pos, pos_rows, page_table,
-                      page_size: int, final_norm, lm_head, lm_packed, embed, lm_ws, logits_rows, logits_all, prompt_ids, prompt_len, ngram: int, draft_ids,
-                      out_ids, step, state, nf4_array=None) -> None:
-    """One verify pass of T tokens (draft, layers, lm_head, accept); packed_array None = the bf16 weights.  ``nf4_array``
-    (make_llama_nf4_array): every matrix with planes streamed by gemv_multi_nf4, lm_head from ``lm_packed`` or lm_head."""
+def llama_verify_step(h, stack: LlamaStack, q_buf, attn_buf, act_buf, T: int, dims, cos, sin, pos, pos_rows, page_table, page_size: int,
+                      final_norm, lm_head, embed, lm_ws, logits_rows, logits_all, prompt_ids, prompt_len, ngram: int, draft_ids, out_ids, step,
+                      state) -> None:
+    """One verify pass of T tokens (draft, layers, lm_head, accept) streaming the stack's verify weights."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    common_a = (T, dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(pos_rows), _p(page_table), page_size,
-                _p(final_norm), _p(lm_head))
-    common_b = (dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(logits_all), _p(prompt_ids), _p(prompt_len), ngram, _p(draft_ids), _p(out_ids),
-                out_ids.numel(), _p(step), _p(state), _stream())
-    if nf4_array is not None:
-        lm_d = _packed_desc(lm_packed)
-        check(_lib.load().srgpt_llama_verify_step_nf4_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(nf4_array, C.c_void_p), n_layers,
-                                                           _p(q_buf), _p(attn_buf), _p(act_buf), *common_a, C.byref(lm_d), *common_b),
-              "srgpt_llama_verify_step_nf4_bf16")
-    elif packed_array is None:
-        check(_lib.load().srgpt_llama_verify_step_bf16(_p(h), C.cast(layer_array, C.c_void_p), n_layers, _p(q_buf), _p(attn_buf), _p(act_buf),
-                                                       *common_a, *common_b), "srgpt_llama_verify_step_bf16")
-    else:
-        lm_d = _packed_desc(lm_packed)
-        check(_lib.load().srgpt_llama_verify_step_packed_bf16(_p(h), C.cast(layer_array, C.c_void_p), C.cast(packed_array, C.c_void_p), n_layers,
-                                                              _p(q_buf), _p(attn_buf), _p(act_buf), *common_a, C.byref(lm_d), *common_b),
-              "srgpt_llama_verify_step_packed_bf16")
-    _count(5 * n_layers + 3 + (1 if logits_all is not None else 0))
+    name, arrays, lm = stack.entry("verify_step")
+    check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), T, dims.hidden_size, nh, nkv, hd, I,
+                                     dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(pos_rows), _p(page_table), page_size, _p(final_norm),
+                                     _p(lm_head), *lm, dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(logits_all), _p(prompt_ids),
+                                     _p(prompt_len), ngram, _p(draft_ids), _p(out_ids), out_ids.numel(), _p(step), _p(state), _stream()), name)
+    _count(stack.verify_kernels + (1 if logits_all is not None else 0))

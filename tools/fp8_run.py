@@ -90,7 +90,7 @@ def main():
     decs["packed"] = LlamaDecoder(d, w_plain, max_seq_len=1024)
     decs["nf4"] = LlamaDecoder(d, w_nf4, max_seq_len=1024)
     decs["fp8"] = LlamaDecoder(d, w_fp8, max_seq_len=1024)
-    assert decs["packed"]._packed_array is not None and decs["nf4"]._nf4_array is not None and decs["fp8"].fp8
+    assert "packed" in decs["packed"].decode_pack.values() and "nf4" in decs["nf4"].decode_quant.values() and decs["fp8"].fp8
     x = (torch.randn(64, d.hidden_size, generator=torch.Generator().manual_seed(1)) * 0.3).to(torch.bfloat16).to(dev)
     n = args.tokens
     ids = {k: dec.generate_from_embeds(x, n) for k, dec in decs.items()}  # warm-up: graphs captured

@@ -75,7 +75,7 @@ def main():
             runs[mode].append((tn - t1) * 1e3)
             ids[mode] = r
     med = {m: statistics.median(v[1:]) for m, v in runs.items()}
-    out = {"card": card(), "decode_pack": "packed" if dec._packed_array is not None else "bf16", "prompt_rows": PROMPT_ROWS, "new_tokens": N,
+    out = {"card": card(), "decode_pack": "packed" if any(v == "packed" for v in dec.decode_pack.values()) else "bf16", "prompt_rows": PROMPT_ROWS, "new_tokens": N,
            "processors": PROCESSORS, "decode_tokens_per_s": {m: round((N - 1) / (t / 1e3), 1) for m, t in med.items()},
            "ids_differ": bool(not torch.equal(ids["off"], ids["on"]))}
     dec.generate_from_embeds(x, N, processors=spec)

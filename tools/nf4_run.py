@@ -97,14 +97,14 @@ def stream_bytes(dec) -> int:
     total = 0
     for l, lw in enumerate(dec.w.layers):
         for i, m in enumerate(MATS):
-            if dec._nf4_array is not None and lw.nf4[m] is not None:
+            if dec.decode_quant.get(f"layers.{l}.{m}") == "nf4":
                 total += lw.nf4[m].nbytes()
-            elif dec._packed_array is not None and dec._packed_layers[l][m] is not None:
-                total += dec._packed_layers[l][m].nbytes()
+            elif dec.decode_pack.get(f"layers.{l}.{m}") == "packed":
+                total += dec.stack.packed_layers[l][m].nbytes()
             else:
                 t = getattr(lw, m + "_w")
                 total += t.numel() * t.element_size()
-    return total + (dec._lm_packed.nbytes() if dec._lm_packed is not None else dec.w.lm_head.numel() * dec.w.lm_head.element_size())
+    return total + (dec.stack.lm_packed.nbytes() if dec.stack.lm_packed is not None else dec.w.lm_head.numel() * dec.w.lm_head.element_size())
 
 
 def main():
@@ -123,7 +123,7 @@ def main():
     decs["packed12"] = LlamaDecoder(d, w, max_seq_len=1024)
     t_q, wq = timed(lambda: nf4_weights(w, d))
     decs["nf4"] = LlamaDecoder(d, wq, max_seq_len=1024)
-    assert decs["packed12"]._packed_array is not None and decs["nf4"]._nf4_array is not None
+    assert "packed" in decs["packed12"].decode_pack.values() and "nf4" in decs["nf4"].decode_quant.values()
     prompt_ids = torch.randint(1000, 30000, (PROMPT_ROWS,), generator=torch.Generator().manual_seed(7))
     x = decs["bf16"].embed_tokens(prompt_ids)
     N = args.new_tokens
@@ -144,7 +144,7 @@ def main():
     out["nf4_ids_equal_bf16"] = int((ids["nf4"] == ids["bf16"]).long().cumprod(0).sum())  # leading tokens in common (lossy weights)
     # per-GEMV: layer 0 of each arm, L2 flushed before each launch
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-    pk, nf = decs["packed12"]._packed_layers[0], wq.layers[0].nf4
+    pk, nf = decs["packed12"].stack.packed_layers[0], wq.layers[0].nf4
     H, I, nh, nkv, hd = d.hidden_size, d.intermediate_size, d.num_attention_heads, d.num_key_value_heads, d.head_dim
     dec = decs["nf4"]
     xh = torch.randn(H, device="cuda").to(w.embed.dtype)

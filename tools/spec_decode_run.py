@@ -99,7 +99,7 @@ def main():
             tn, r = timed(lambda: dec.generate_from_embeds(x, N, lookup_ids=hist, lookup_k=k))
             runs[c].append((tn - t1) * 1e3)
             spec[c] = dict(ids_identical=bool(torch.equal(r, ref)), last_speculation=list(dec.last_speculation))
-    out = {"card": card(), "decode_pack": "packed" if dec._packed_array is not None else "bf16", "prompt_rows": PROMPT_ROWS, "new_tokens": N,
+    out = {"card": card(), "decode_pack": "packed" if any(v == "packed" for v in dec.decode_pack.values()) else "bf16", "prompt_rows": PROMPT_ROWS, "new_tokens": N,
            "k": k}
     med = {c: statistics.median(v[1:]) for c, v in runs.items()}
     out["decode_tokens_per_s"] = {c: round((N - 1) / (m / 1e3), 1) for c, m in med.items()}
