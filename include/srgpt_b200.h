@@ -275,6 +275,15 @@ int srgpt_argmax_bf16(const void* x, int ldx, int rows, int cols, long long* out
  * [n_beams, n_cand] (token -1 / score -inf when a row has fewer finite logits). */
 int srgpt_beam_candidates_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
                                float* cand_scores, int* cand_tokens, void* stream);
+/* The same candidates and, when logprobs is given, every row's whole log_softmax (fp32, before the beam score is added) -> logprobs
+ * [n_beams, ldo], ldo >= V: HF's output_scores of a beam step (next_token_scores_processed). */
+int srgpt_beam_candidates_scores_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
+                                      float* cand_scores, int* cand_tokens, float* logprobs, long long ldo, void* stream);
+/* Score rows of a decode step (rowops.cu): HF's output_scores of a greedy step.  Row r of rows [R, ld] (fp32 when rows_f32, else the
+ * element type widened exactly, as .float()) -> scores + (*step + step_offset) * step_stride + r * row_stride, for r < R.  The index is
+ * read at run time, so one captured decode graph writes every step's rows.  R <= 65535, ld >= V, row_stride >= V. */
+int srgpt_step_scores(const void* rows, int rows_f32, long long ld, int R, int V, const int* step, int step_offset, float* scores,
+                      long long step_stride, long long row_stride, void* stream);
 /* Beam search over a batch of prompts (beam.cu): merges the candidates srgpt_beam_candidates_bf16 wrote for n_groups * k rows (prompt g
  * owns rows g*k .. g*k+k-1).  Per prompt the n_cand best (score, beam within the prompt, token) in (score desc, beam asc, token asc)
  * order, candidates with token < 0 dropped -> out_scores / out_beams / out_tokens [n_groups, n_cand] (score -inf, beam and token -1 where a
@@ -313,6 +322,15 @@ int srgpt_sample_top_p_f32(const float* logits, int V, const float* params, cons
  * draws from that row converted to fp32 with seed seeds[r] and the same counter.  R <= 65535, ld >= V. */
 int srgpt_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
                       const int* step, int step_offset, long long* ids, void* stream);
+/* srgpt_sample_top_p_f32 / srgpt_sample_rows, and the warped row each draw picks from (HF's output_scores of a sampled step):
+ * logits / temperature (an IEEE fp32 division) for every token the top-k cut and the nucleus keep, -inf for every other token.  The
+ * draws are those of the calls without scores.  The one-row form writes scores + (*step + step_offset) * step_stride (step_stride >= V);
+ * the R-row form writes row r to scores + (*step + step_offset) * step_stride + r * V (step_stride >= R * V). */
+int srgpt_sample_top_p_scores_f32(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step,
+                                  int step_offset, long long* out_ids, const void* embed_table, void* next_x, int K, float* scores,
+                                  long long step_stride, void* stream);
+int srgpt_sample_rows_scores(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
+                             const int* step, int step_offset, long long* ids, float* scores, long long step_stride, void* stream);
 /* HF's logits processors on the device (logits_process.cu): replaces RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
  * NoBadWordsLogitsProcessor, MinLengthLogitsProcessor and MinNewTokensLengthLogitsProcessor (transformers generation/logits_process.py),
  * which HF runs on the host behind generate(repetition_penalty=, no_repeat_ngram_size=, bad_words_ids=, min_length=, min_new_tokens=)

@@ -331,7 +331,7 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
 }
 __global__ void __launch_bounds__(BEAM_THREADS)
 beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const float* __restrict__ beam_scores, int n_cand, float* __restrict__ cand_scores,
-                       int* __restrict__ cand_tokens) {
+                       int* __restrict__ cand_tokens, float* __restrict__ logprobs, long long ldo) {
   __shared__ unsigned long long sk[32];
   __shared__ float sred[32];
   const bf16* row = logits + (size_t)blockIdx.x * ldx;
@@ -353,6 +353,10 @@ beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const fl
   }
   z = block_sum(z, sred);
   const float lse = logf(z);
+  if (logprobs != nullptr) {  // the whole log_softmax row (HF's output_scores of a beam step), before the beam score is added
+    float* orow = logprobs + (size_t)blockIdx.x * ldo;
+    for (int c = tid; c < V; c += BEAM_THREADS) orow[c] = (e2f(row[c]) - m) - lse;
+  }
   const float bs = beam_scores[blockIdx.x];
   // key = (order-preserving bits of the logit, ~token): the maximum key below the previous one is the next candidate
   unsigned long long prev = ~0ull;
@@ -529,9 +533,46 @@ extern "C" __attribute__((visibility("default"))) int srgpt_argmax_bf16(const vo
 // num_beams x n_cand pairs (the global top-2k is a subset of the per-row top-2k).
 extern "C" __attribute__((visibility("default"))) int srgpt_beam_candidates_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
                                                                                   float* cand_scores, int* cand_tokens, void* stream) {
+  return srgpt_beam_candidates_scores_bf16(logits, ldx, n_beams, V, beam_scores, n_cand, cand_scores, cand_tokens, nullptr, 0, stream);
+}
+
+// The same candidates, and (when logprobs is given) every row's whole log_softmax -> logprobs [n_beams, ldo] fp32.
+extern "C" __attribute__((visibility("default"))) int srgpt_beam_candidates_scores_bf16(const void* logits, int ldx, int n_beams, int V,
+                                                                                         const float* beam_scores, int n_cand, float* cand_scores,
+                                                                                         int* cand_tokens, float* logprobs, long long ldo, void* stream) {
   SRGPT_CHECK_ARG(logits && beam_scores && cand_scores && cand_tokens && n_beams > 0 && V > 0 && ldx >= V && n_cand > 0 && n_cand <= V);
+  SRGPT_CHECK_ARG(logprobs == nullptr || ldo >= V);
   beam_candidates_kernel<<<n_beams, BEAM_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const bf16*>(logits), ldx, V, beam_scores, n_cand,
-                                                                                             cand_scores, cand_tokens);
+                                                                                             cand_scores, cand_tokens, logprobs, ldo);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+// A decode step's score rows (HF's output_scores of a greedy step): row r of rows [R, ld] (fp32, or the element type widened exactly, as
+// .float() widens it) -> scores + (*step + step_offset) * step_stride + r * row_stride.  The index is read at run time, so one captured
+// decode graph writes every step's rows.  grid = (column blocks, R).
+__device__ __forceinline__ float widen(float x) { return x; }
+__device__ __forceinline__ float widen(bf16 x) { return e2f(x); }
+template <typename T>
+__global__ void __launch_bounds__(256)
+step_scores_kernel(const T* __restrict__ rows, long long ld, int V, const int* __restrict__ step, int step_offset, float* __restrict__ scores,
+                   long long step_stride, long long row_stride) {
+  const T* src = rows + (size_t)blockIdx.y * ld;
+  float* dst = scores + (long long)(*step + step_offset) * step_stride + (long long)blockIdx.y * row_stride;
+  for (int c = blockIdx.x * 256 + threadIdx.x; c < V; c += gridDim.x * 256) dst[c] = widen(src[c]);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_step_scores(const void* rows, int rows_f32, long long ld, int R, int V, const int* step,
+                                                                        int step_offset, float* scores, long long step_stride, long long row_stride,
+                                                                        void* stream) {
+  SRGPT_CHECK_ARG(rows && step && scores && R > 0 && R <= 65535 && V > 0 && ld >= V && row_stride >= V && step_stride >= 0);
+  SRGPT_CHECK_ARG(rows_f32 == 0 || rows_f32 == 1);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(ceil_div(V, 256 * 16), R);
+  if (rows_f32)
+    step_scores_kernel<float><<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(rows), ld, V, step, step_offset, scores, step_stride, row_stride);
+  else
+    step_scores_kernel<bf16><<<grid, 256, 0, st>>>(reinterpret_cast<const bf16*>(rows), ld, V, step, step_offset, scores, step_stride, row_stride);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }

@@ -54,7 +54,8 @@ __device__ __forceinline__ float logit(const bf16* __restrict__ x, int i) { retu
 // params = {temperature, top_p, top_k (0 = off)} and the seed live in device memory, so one captured CUDA graph serves any request.
 template <typename T>
 __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, const float* __restrict__ params,
-                                          const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step, int step_offset) {
+                                          const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step, int step_offset,
+                                          float* __restrict__ warped) {
   __shared__ float red[32];
   __shared__ float s_scan[THREADS];
   __shared__ int s_tok;
@@ -113,6 +114,16 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
     }
     t_keep = lo_t;
     mass = mass_lo;
+  }
+
+  // the warped row (HF's output_scores of a sampled step): logits / T for the tokens the draw can pick (p >= t_keep, the set the top-k
+  // cut and the nucleus bisection kept), -inf for every other token.  A true fp32 division, as TemperatureLogitsWarper divides.
+  if (warped != nullptr) {
+    const float t = params[0];
+    for (int i = tid; i < V; i += THREADS) {
+      const float x = logit(logits, i);
+      warped[i] = __expf((x - m) * inv_t) * inv_z >= t_keep ? __fdiv_rn(x, t) : -INFINITY;
+    }
   }
 
   // draw
@@ -175,8 +186,10 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
 
 __global__ void __launch_bounds__(THREADS)
 sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step,
-                    int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table, bf16* __restrict__ next_x, int K) {
-  const int tok = sample_row(logits, V, params, seed_ptr, step, step_offset);
+                    int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table, bf16* __restrict__ next_x, int K,
+                    float* __restrict__ scores, long long step_stride) {
+  float* warped = scores != nullptr ? scores + (long long)(*step + step_offset) * step_stride : nullptr;
+  const int tok = sample_row(logits, V, params, seed_ptr, step, step_offset, warped);
   if (threadIdx.x == 0) out_ids[*step + step_offset] = (long long)tok;
   if (embed_table != nullptr && next_x != nullptr) {
     const uint4* src = reinterpret_cast<const uint4*>(embed_table + (size_t)tok * K);
@@ -189,9 +202,10 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
 template <typename T>
 __global__ void __launch_bounds__(THREADS)
 sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seeds,
-                   const int* __restrict__ step, int step_offset, long long* __restrict__ ids) {
+                   const int* __restrict__ step, int step_offset, long long* __restrict__ ids, float* __restrict__ scores, long long step_stride) {
   const int r = blockIdx.x;
-  const int tok = sample_row(logits + (size_t)r * ld, V, params, seeds + r, step, step_offset);
+  float* warped = scores != nullptr ? scores + (long long)(*step + step_offset) * step_stride + (long long)r * V : nullptr;
+  const int tok = sample_row(logits + (size_t)r * ld, V, params, seeds + r, step, step_offset, warped);
   if (threadIdx.x == 0) ids[r] = (long long)tok;
 }
 
@@ -200,6 +214,38 @@ sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const floa
 
 using namespace srgpt;
 
+namespace {
+int launch_sample_top_p(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step, int step_offset,
+                        long long* out_ids, const void* embed_table, void* next_x, int K, float* scores, long long step_stride, void* stream) {
+  SRGPT_CHECK_ARG(logits && params && seed && step && out_ids && V > 0);
+  SRGPT_CHECK_ARG((embed_table == nullptr) == (next_x == nullptr));
+  SRGPT_CHECK_ARG(embed_table == nullptr || ((K % 8) == 0 && K > 0 && (reinterpret_cast<uintptr_t>(embed_table) & 15) == 0 &&
+                                             (reinterpret_cast<uintptr_t>(next_x) & 15) == 0));
+  SRGPT_CHECK_ARG(scores == nullptr || step_stride >= V);
+  sampling::sample_top_p_kernel<<<1, sampling::THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      logits, V, params, seed, step, step_offset, out_ids, reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(next_x), K,
+      scores, step_stride);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+int launch_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
+                       const int* step, int step_offset, long long* ids, float* scores, long long step_stride, void* stream) {
+  SRGPT_CHECK_ARG(logits && params && seeds && step && ids && R > 0 && R <= 65535 && V > 0 && ld >= V);
+  SRGPT_CHECK_ARG(logits_f32 == 0 || logits_f32 == 1);
+  SRGPT_CHECK_ARG(scores == nullptr || step_stride >= (long long)R * V);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (logits_f32)
+    sampling::sample_rows_kernel<float><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const float*>(logits), ld, V, params, seeds, step,
+                                                                         step_offset, ids, scores, step_stride);
+  else
+    sampling::sample_rows_kernel<bf16><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const bf16*>(logits), ld, V, params, seeds, step,
+                                                                        step_offset, ids, scores, step_stride);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+}  // namespace
+
 // Overwrites out_ids[*step + step_offset] (and, when given, next_x = embed_table[token]) with a token sampled from
 // softmax(logits / temperature) restricted to its top-p nucleus.  `params` = device float[3] {temperature, top_p, top_k (0 = off)},
 // `seed` = device u64 (read at run time: a captured graph must not freeze the seed of the request it was captured under).
@@ -207,14 +253,16 @@ using namespace srgpt;
 extern "C" __attribute__((visibility("default"))) int srgpt_sample_top_p_f32(const float* logits, int V, const float* params, const unsigned long long* seed,
                                                                              const int* step, int step_offset, long long* out_ids,
                                                                              const void* embed_table, void* next_x, int K, void* stream) {
-  SRGPT_CHECK_ARG(logits && params && seed && step && out_ids && V > 0);
-  SRGPT_CHECK_ARG((embed_table == nullptr) == (next_x == nullptr));
-  SRGPT_CHECK_ARG(embed_table == nullptr || ((K % 8) == 0 && K > 0 && (reinterpret_cast<uintptr_t>(embed_table) & 15) == 0 &&
-                                             (reinterpret_cast<uintptr_t>(next_x) & 15) == 0));
-  sampling::sample_top_p_kernel<<<1, sampling::THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      logits, V, params, seed, step, step_offset, out_ids, reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(next_x), K);
-  SRGPT_CHECK_LAUNCH();
-  return SRGPT_OK;
+  return launch_sample_top_p(logits, V, params, seed, step, step_offset, out_ids, embed_table, next_x, K, nullptr, 0, stream);
+}
+
+// The same draw, and the warped row it drew from -> scores + (*step + step_offset) * step_stride.
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_top_p_scores_f32(const float* logits, int V, const float* params,
+                                                                                    const unsigned long long* seed, const int* step, int step_offset,
+                                                                                    long long* out_ids, const void* embed_table, void* next_x, int K,
+                                                                                    float* scores, long long step_stride, void* stream) {
+  SRGPT_CHECK_ARG(scores != nullptr);
+  return launch_sample_top_p(logits, V, params, seed, step, step_offset, out_ids, embed_table, next_x, K, scores, step_stride, stream);
 }
 
 // Draws one token per row for R rows of logits [R, ld] (fp32 when logits_f32, else the element type) -> ids[R].  Row r draws with
@@ -222,15 +270,14 @@ extern "C" __attribute__((visibility("default"))) int srgpt_sample_top_p_f32(con
 extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params,
                                                                         const unsigned long long* seeds, const int* step, int step_offset,
                                                                         long long* ids, void* stream) {
-  SRGPT_CHECK_ARG(logits && params && seeds && step && ids && R > 0 && R <= 65535 && V > 0 && ld >= V);
-  SRGPT_CHECK_ARG(logits_f32 == 0 || logits_f32 == 1);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (logits_f32)
-    sampling::sample_rows_kernel<float><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const float*>(logits), ld, V, params, seeds, step,
-                                                                         step_offset, ids);
-  else
-    sampling::sample_rows_kernel<bf16><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const bf16*>(logits), ld, V, params, seeds, step,
-                                                                        step_offset, ids);
-  SRGPT_CHECK_LAUNCH();
-  return SRGPT_OK;
+  return launch_sample_rows(logits, logits_f32, ld, R, V, params, seeds, step, step_offset, ids, nullptr, 0, stream);
+}
+
+// The same draws, and row r's warped row -> scores + (*step + step_offset) * step_stride + r * V.
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows_scores(const void* logits, int logits_f32, int ld, int R, int V,
+                                                                               const float* params, const unsigned long long* seeds, const int* step,
+                                                                               int step_offset, long long* ids, float* scores, long long step_stride,
+                                                                               void* stream) {
+  SRGPT_CHECK_ARG(scores != nullptr);
+  return launch_sample_rows(logits, logits_f32, ld, R, V, params, seeds, step, step_offset, ids, scores, step_stride, stream);
 }

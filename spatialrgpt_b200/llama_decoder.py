@@ -53,20 +53,27 @@ def first_stop(host_ids, lo: int, hi: int, eos, stopping_fn, limit: int) -> Opti
 
 class BeamHypotheses:
     """The host bookkeeping of one prompt's beam search (HF BeamSearchScorer.process / finalize for one batch entry): the running beams'
-    tokens and scores, the kept hypotheses and the done flag.  ``advance`` takes the prompt's ranked candidates of one step."""
+    tokens and scores, the kept hypotheses and the done flag.  ``advance`` takes the prompt's ranked candidates of one step.
+    It also records the beam row every token was chosen from (HF's beam_indices: row0 + the beam, row0 being the prompt's first row of
+    the step), and ``best`` leaves the chosen hypothesis' score and rows in ``best_score`` / ``best_beams``."""
 
-    def __init__(self, k: int, eos, length_penalty: float, early_stopping: bool):
-        self.k, self.eos, self.length_penalty, self.early_stopping = k, eos, length_penalty, early_stopping
+    def __init__(self, k: int, eos, length_penalty: float, early_stopping: bool, row0: int = 0):
+        self.k, self.eos, self.length_penalty, self.early_stopping, self.row0 = k, eos, length_penalty, early_stopping, row0
         self.seqs: List[List[int]] = [[] for _ in range(k)]
+        self.beams: List[List[int]] = [[] for _ in range(k)]  # the row of every token of each running beam
         self.scores = [0.0] + [-1e9] * (k - 1)
         self.hyps: List = []  # (score, tokens) of finished hypotheses, at most k kept
+        self.hyp_beams: List[List[int]] = []  # the rows of each kept hypothesis, in the order of hyps
         self.worst, self.done = 1e9, False
+        self.best_score, self.best_beams = None, None
 
-    def keep(self, score: float, toks: List[int]) -> None:
+    def keep(self, score: float, toks: List[int], beams: Optional[List[int]] = None) -> None:
         if len(self.hyps) < self.k or score > self.worst:
             self.hyps.append((score, toks))
+            self.hyp_beams.append([] if beams is None else beams)
             if len(self.hyps) > self.k:
-                self.hyps.remove(min(self.hyps, key=lambda x: x[0]))
+                i = min(range(len(self.hyps)), key=lambda j: self.hyps[j][0])
+                del self.hyps[i], self.hyp_beams[i]
             self.worst = min(x[0] for x in self.hyps)
 
     def advance(self, ranked, cur_len: int) -> List[int]:
@@ -77,7 +84,7 @@ class BeamHypotheses:
             if t in self.eos:
                 if rank >= self.k:
                     continue
-                self.keep(sc / (cur_len ** self.length_penalty), list(self.seqs[b]))
+                self.keep(sc / (cur_len ** self.length_penalty), list(self.seqs[b]), self.beams[b] + [self.row0 + b])
             else:
                 nxt.append((sc, b, t))
             if len(nxt) == self.k:
@@ -87,6 +94,7 @@ class BeamHypotheses:
         if len(self.hyps) >= self.k and (self.early_stopping or self.worst >= ranked[0][0] / (cur_len ** self.length_penalty)):
             self.done = True
         self.seqs = [self.seqs[b] + [t] for _, b, t in nxt]
+        self.beams = [self.beams[b] + [self.row0 + b] for _, b, _ in nxt]
         self.scores = [sc for sc, _, _ in nxt]
         return [b for _, b, _ in nxt]
 
@@ -95,8 +103,10 @@ class BeamHypotheses:
         first EOS appended when it is shorter than max_new_tokens."""
         if not self.done:
             for i in range(self.k):
-                self.keep(self.scores[i] / (len(self.seqs[i]) ** self.length_penalty), list(self.seqs[i]))
-        best = list(max(self.hyps, key=lambda x: x[0])[1])
+                self.keep(self.scores[i] / (len(self.seqs[i]) ** self.length_penalty), list(self.seqs[i]), list(self.beams[i]))
+        i = max(range(len(self.hyps)), key=lambda j: self.hyps[j][0])
+        self.best_score, self.best_beams = self.hyps[i][0], list(self.hyp_beams[i])
+        best = list(self.hyps[i][1])
         if len(best) < max_new_tokens and self.eos:
             best.append(self.eos[0])
         return best
@@ -308,7 +318,8 @@ class LlamaDecoder:
             raise ValueError("SRGPT_DECODE_NF4=0 runs the decode step over the dequantized copies, which a model loaded with "
                              "nf4_dequantized_copy=False does not keep")
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
-        # ("verify", T, ngram), ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B).  A graph holds the addresses of every buffer it reads, so it is
+        # ("verify", T, ngram), ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B); the
+        # graphs that write output_scores rows end in ("scores", buffer address, step stride) (_scores_key).  A graph holds the addresses of every buffer it reads, so it is
         # dropped whenever one of them is replaced: the KV cache and the layer stack's array (ensure_capacity), the processor spec (_set_processors)
         # and the batched-decode buffers (_batch_state).
         self._graphs = {}
@@ -345,9 +356,11 @@ class LlamaDecoder:
     supports_prompt_lookup = True
     supports_logits_processors = True
     supports_batch_sampling = True  # sampled batches run in the batched step (generate_batch), num_return_sequences included
+    supports_output_scores = True  # generate(output_scores=True): the decode steps write each token's score row on the device
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
+    _scores = None  # the score buffer of output_scores (_scores_view), allocated on first use
     _host_ids = None  # pinned host copy of generated ids for the stop checks, and the stream that fills it (_pinned_ids)
     _copy_stream = None
     last_speculation = (0, 0, 0)
@@ -509,29 +522,43 @@ class LlamaDecoder:
         return ops.gemm(hn, self.w.lm_head, out=self._logits_buffer(hn.shape[0]) if out is None else out)
 
     # ---------------------------------------------------------------------------------------------
-    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False) -> None:
+    def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False,
+                            scores: Optional[torch.Tensor] = None) -> None:
         d, w = self.dims, self.w
-        if (sample or proc) and logits_out is None:
+        if (sample or proc or scores is not None) and logits_out is None:
             logits_out = self._sample_buffer()
         ops.llama_decode_step(self.h, self.stack, self.q_buf, self.attn_buf, self.act_buf, d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE,
                               w.norm, w.lm_head, w.embed, self.lm_ws, self.out_ids, self.step, logits_out)
-        if proc:
-            self._process_row(logits_out, sample)
-        elif sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
-            ops.sample_top_p(logits_out, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+        self._choose(logits_out, sample, proc, scores)
 
-    def _process_row(self, raw: torch.Tensor, sample: bool) -> None:
+    def _choose(self, raw: Optional[torch.Tensor], sample: bool, proc: bool, scores: Optional[torch.Tensor]) -> None:
+        """After an lm_head that advanced the step and wrote the greedy choice: the processors and / or the draw replace that choice, and
+        with ``scores`` ([T, 1, V] fp32) the row the token was chosen from goes to scores[step - 1] (the raw row when greedy without
+        processors, the processed row when greedy with them, the warped row when sampled)."""
+        if proc:
+            self._process_row(raw, sample, scores)
+        elif sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
+            ops.sample_top_p(raw, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, self.w.embed, self.h,
+                             **self._scores_kw(scores, True))
+        elif scores is not None:
+            ops.step_scores(raw, self.step, -1, scores)
+
+    def _process_row(self, raw: torch.Tensor, sample: bool, scores: Optional[torch.Tensor] = None) -> None:
         """After an lm_head that advanced the step: the processors over the raw fp32 row (history = out_ids[:step - 1]), then the
         processed greedy choice, or a draw from the processed row, replaces out_ids[step - 1] and the next embedding row."""
         w = self.w
+        if (sample or scores is not None) and self.proc_logits is None:
+            self.proc_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
         if sample:
-            if self.proc_logits is None:
-                self.proc_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
             ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, out=self.proc_logits)
-            ops.sample_top_p(self.proc_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+            ops.sample_top_p(self.proc_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
+                             **self._scores_kw(scores, True))
         else:
-            ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, ids=self.proc_ids)
+            ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, ids=self.proc_ids,
+                               **({} if scores is None else {"out": self.proc_logits}))
             ops.logits_pick_token(self.proc_ids, self.step, -1, self.out_ids, w.embed, self.h)
+            if scores is not None:
+                ops.step_scores(self.proc_logits, self.step, -1, scores)
 
     def _set_processors(self, processors) -> bool:
         """processors = None or a spec of logits_processors.parse / resolve_min_length.  Writes its device encoding; True when on."""
@@ -555,6 +582,28 @@ class LlamaDecoder:
         if self.sample_logits is None:
             self.sample_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
         return self.sample_logits
+
+    def _scores_view(self, steps: int, rows: int) -> torch.Tensor:
+        """fp32 [steps, rows, V] over the decoder's score buffer (output_scores): the captured graphs that write scores hold its address,
+        so it lives across requests and grows (dropping those graphs) when a request needs more."""
+        need = steps * rows * self.dims.vocab_size
+        if self._scores is None or self._scores.numel() < need:
+            self._drop_graphs(lambda key: isinstance(key[-1], tuple) and key[-1][0] == "scores")
+            self._scores = None
+            self._scores = torch.empty(need, dtype=torch.float32, device=self.device)
+        return self._scores[:need].view(steps, rows, self.dims.vocab_size)
+
+    @staticmethod
+    def _scores_kw(scores: Optional[torch.Tensor], strided: bool = False) -> dict:
+        """The sampler's keywords for a score buffer view; none without one, so the call is today's call."""
+        if scores is None:
+            return {}
+        return {"scores": scores, "step_stride": scores.stride(0)} if strided else {"scores": scores}
+
+    @staticmethod
+    def _scores_key(scores: Optional[torch.Tensor]):
+        """The graph-key suffix of a score buffer view: a graph holds the address and the step stride it writes to."""
+        return () if scores is None else (("scores", scores.data_ptr(), scores.stride(0)),)
 
     # ---- captured graphs ---------------------------------------------------------------------------------------------------------
     def _capture(self, key, launch, restore, kernels: int) -> torch.cuda.CUDAGraph:
@@ -593,11 +642,13 @@ class LlamaDecoder:
         entry = self._graphs.get(("step", False, False))
         return None if entry is None else entry[0]
 
-    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False) -> torch.cuda.CUDAGraph:
+    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False, scores: Optional[torch.Tensor] = None) -> torch.cuda.CUDAGraph:
         """The one-token step graph of this mode.  Sampling adds its kernel; processing adds 1 more when sampling, 3 when greedy
-        (processing, key unpack and pick)."""
-        kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0)
-        return self._capture(("step", sample, proc), lambda: self._decode_step_launch(seq, sample=sample, proc=proc),
+        (processing, key unpack and pick); greedy score rows add their copy (the sampler writes its own)."""
+        kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0) + (
+            1 if scores is not None and not sample else 0)
+        return self._capture(("step", sample, proc) + self._scores_key(scores),
+                             lambda: self._decode_step_launch(seq, sample=sample, proc=proc, **self._scores_kw(scores)),
                              (self.pos, self.step, self.h, self.out_ids), kernels)
 
     # ---- stop checks: generated ids reach the host through pinned memory while the next step runs --------------------------------
@@ -648,7 +699,8 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def generate_from_embeds(self, inputs_embeds: torch.Tensor, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
                              use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0,
-                             lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2, processors=None):
+                             lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2, processors=None,
+                             output_scores: bool = False):
         """Greedy (or, with ``sampling=dict(temperature, top_p, seed)``, nucleus-sampled) decoding started from prompt
         embeddings [S, H].  Returns LongTensor [n_new] (and fp32 logits [n_new, V] when return_logits).
         ``stopping_fn(ids_so_far: LongTensor) -> bool``.
@@ -663,7 +715,11 @@ class LlamaDecoder:
         request whose verify slack does not fit max_seq_len or the decoder's token cap runs the one-token loop and reports (0, 0, 0).
         ``processors`` (a spec of logits_processors.resolve_min_length, or None): HF's repetition penalty / no-repeat n-gram / bad words /
         minimum length over every token's logits, the first one included, before the greedy choice or the sampling warpers; the history
-        is the generated tokens.  Returned logits stay raw, as HF's output_logits."""
+        is the generated tokens.  Returned logits stay raw, as HF's output_logits.
+        ``output_scores``: returns (what it returns without, {"scores": fp32 [n_new, 1, V]}), row t being the row token t was chosen from
+        (HF's output_scores): the raw row when greedy, the processed row with processors, the warped row (logits / T, -inf where top-k /
+        top-p removed the token) when sampled.  The decode graphs write them on the device; prompt-lookup decoding takes them from its
+        verify passes' logit rows (greedy without processors: the raw rows)."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
         n_reuse = int(reuse_rows)
@@ -671,7 +727,8 @@ class LlamaDecoder:
             raise ValueError(f"reuse_rows={n_reuse} is not a reusable prefix here: sequence {seq}, {self.prefix_rows} recorded prefill rows, "
                              f"{S} prompt rows (at most S - 1 may be reused)")
         if max_new_tokens < 1:
-            return torch.empty(0, dtype=torch.int64, device=self.device)
+            empty = torch.empty(0, dtype=torch.int64, device=self.device)
+            return (empty, {"scores": torch.empty((0, 1, d.vocab_size), dtype=torch.float32, device=self.device)}) if output_scores else empty
         if max_new_tokens > self.out_ids.numel():
             raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
         if S + max_new_tokens > self.max_seq_len:
@@ -696,21 +753,28 @@ class LlamaDecoder:
         if seq == 0 and self.supports_prefix_reuse:
             self._record_prefix(S)
         n_rows = max_new_tokens + (slack if k > 0 else 0)  # verify passes write accepted logit rows past the budget too
-        logits = torch.empty((n_rows, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits else None
+        # prompt lookup's scores are its logit rows (greedy without processors), which the verify passes write on the logits_all route
+        lookup_scores = output_scores and k > 0 and max_new_tokens > 1
+        logits = torch.empty((n_rows, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits or lookup_scores else None
+        scores = self._scores_view(max_new_tokens, 1) if output_scores and not lookup_scores else None
         # first token: final norm + lm_head + argmax on the last prompt row; afterwards pos == S
         self.pos.fill_(S - 1)
         self.step.zero_()
         sample = self._set_sampling(sampling)
-        first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample or proc else None)
+        first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample or proc or scores is not None else None)
         ops.lm_head_argmax(hidden[S - 1 - n_reuse], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
                            embed_table=w.embed, next_x=self.h, logits_out=first_logits)
-        if proc:
-            self._process_row(first_logits, sample)
-        elif sample:
-            ops.sample_top_p(first_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
+        self._choose(first_logits, sample, proc, scores)
         if k > 0 and max_new_tokens > 1:
-            return self._verify_loop(k + 1, int(lookup_ngram), lookup_ids, max_new_tokens, eos, stopping_fn, use_graph, logits)
-        return self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc)
+            r = self._verify_loop(k + 1, int(lookup_ngram), lookup_ids, max_new_tokens, eos, stopping_fn, use_graph, logits)
+            if not output_scores:
+                return r
+            out, lg = r
+            return (r, {"scores": lg.unsqueeze(1).clone()}) if return_logits else (out, {"scores": lg.unsqueeze(1)})
+        r = self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, scores)
+        if not output_scores:
+            return r
+        return r, {"scores": scores[:(r[0] if return_logits else r).numel()].clone()}
 
     # ---- prompt-lookup speculative decoding: verify passes of T = k + 1 tokens, every weight streamed once per pass ---------------
     def _verify_buffers(self):
@@ -783,19 +847,19 @@ class LlamaDecoder:
         return out
 
     def _decode_loop(self, seq: int, n: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False,
-                     proc: bool = False):
+                     proc: bool = False, scores: Optional[torch.Tensor] = None):
         """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
-        out_ids[:n] are already set."""
+        out_ids[:n] are already set.  ``scores`` ([T, 1, V] fp32): each step's score row goes to scores[step]."""
         self.active_pt.copy_(self.cache.page_tables[seq])
-        key = ("step", sample, proc) if use_graph and logits is None else None
+        key = ("step", sample, proc) + self._scores_key(scores) if use_graph and logits is None else None
         if key is not None:
-            self._ensure_graph(seq, sample, proc)
+            self._ensure_graph(seq, sample, proc, scores)
 
         def launch_step(k: int) -> None:
             if key is not None:
                 self._replay(key)
             else:
-                self._decode_step_launch(seq, None if logits is None else logits[k], sample, proc)
+                self._decode_step_launch(seq, None if logits is None else logits[k], sample, proc, **self._scores_kw(scores))
 
         if not eos and stopping_fn is None:
             while n < max_new_tokens:
@@ -843,10 +907,13 @@ class LlamaDecoder:
         self._bstate = st
         return st
 
-    def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False, sample: bool = False) -> None:
+    def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False, sample: bool = False,
+                           scores: Optional[torch.Tensor] = None) -> None:
         """One decode step of all B sequences (llava_arch.py:549-611 + modeling_llama.py:540-562 semantics without padding): the
         projections are wgmma GEMMs over the B rows (tall stream-K configuration), RoPE / KV append and attention per sequence.
-        ``sample``: row b draws its token with st["seeds"][b] at counter step (the counter the one-token loop uses for that token)."""
+        ``sample``: row b draws its token with st["seeds"][b] at counter step (the counter the one-token loop uses for that token).
+        ``scores`` ([T, B, V] fp32): the rows the tokens were chosen from go to scores[step] (the bf16 rows widened, the processed rows,
+        or the sampler's warped rows)."""
         d, w, B = self.dims, self.w, st["B"]
         nh, nkv, hd, V = d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.vocab_size
         qd = nh * hd
@@ -873,37 +940,49 @@ class LlamaDecoder:
         if sample:  # from the bf16 rows, or from the processed fp32 rows
             if proc:
                 ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, out=st["proc_rows"])
-            ops.sample_rows(st["proc_rows"] if proc else lg, self.sample_params, st["seeds"], st["step"], 0, st["ids"])
+            ops.sample_rows(st["proc_rows"] if proc else lg, self.sample_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
         elif proc:  # the processors over each sequence's bf16 row and its history st["out"][t * B + b], t < step; then the arg max
-            ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, ids=st["ids"])
+            ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, ids=st["ids"],
+                               **({} if scores is None else {"out": st["proc_rows"]}))
+            if scores is not None:
+                ops.step_scores(st["proc_rows"], st["step"], 0, scores)
         else:
             ops.argmax_bf16(lg, out=st["ids"])
+            if scores is not None:
+                ops.step_scores(lg, st["step"], 0, scores)
         ops.decode_batch_advance(st["ids"], w.embed, h, st["out"], st["step"], st["pos"], st["ticket"])
 
     def _decode_batched(self, first: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos, stopping_fn, use_graph: bool,
-                        proc: bool = False, sample_from: Optional[torch.Tensor] = None, seeds: Optional[List[int]] = None):
+                        proc: bool = False, sample_from: Optional[torch.Tensor] = None, seeds: Optional[List[int]] = None,
+                        scores: Optional[torch.Tensor] = None):
         """Decode of B prefilled sequences together: greedy, or sampled when ``sample_from`` holds the B first-token rows to draw from
         ([B, V], the bf16 lm_head rows or the processed fp32 rows) and ``seeds`` the B row seeds.  Returns a list of LongTensor [n_b]
-        (each cut at its own stop)."""
+        (each cut at its own stop).  ``scores`` ([T, B, V] fp32; a greedy caller has written row 0): every step's rows go to scores[step].
+        A sequence that has stopped stays in the step, so its rows of the later steps hold what the step computed for it."""
         B = len(seq_lens)
         st = self._batch_state(B)
         sample = sample_from is not None
+        if proc and st["proc_rows"] is None and (sample or scores is not None):
+            st["proc_rows"] = torch.empty((B, self.dims.vocab_size), dtype=torch.float32, device=self.device)
         if sample:  # the first tokens in one launch, at counter 0
             st["seeds"].copy_(torch.tensor(seeds, dtype=torch.int64))
-            if proc and st["proc_rows"] is None:
-                st["proc_rows"] = torch.empty((B, self.dims.vocab_size), dtype=torch.float32, device=self.device)
             st["step"].zero_()
-            ops.sample_rows(sample_from, self.sample_params, st["seeds"], st["step"], 0, st["ids"])
+            ops.sample_rows(sample_from, self.sample_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
             first = st["ids"]
         zero = torch.zeros(B, dtype=torch.int32, device=self.device)
         st["out"][:B].copy_(first)
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        key = ("batch", B, proc, True) if sample else ("batch", B, proc)
+        if scores is not None:  # the graphs that write scores hold the buffer's address
+            key = ("batch", B, proc, sample) + self._scores_key(scores)
+        else:
+            key = ("batch", B, proc, True) if sample else ("batch", B, proc)
         if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max (sampling: processing + draw)
-            self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample), (st["h"], st["pos"], st["step"], st["out"]),
-                          self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4))
+            self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample, scores=scores),
+                          (st["h"], st["pos"], st["step"], st["out"]),
+                          self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4) + (
+                              1 if scores is not None and not sample else 0))
         need_check = bool(eos) or stopping_fn is not None
         out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
         if need_check:
@@ -916,7 +995,7 @@ class LlamaDecoder:
             if use_graph:
                 self._replay(key)
             else:
-                self._batch_step_launch(st, proc=proc, sample=sample)
+                self._batch_step_launch(st, proc=proc, sample=sample, scores=scores)
             if need_check:  # same pipelining as the single-sequence loop: inspect row n-1 while row n is being computed
                 nxt = self._to_host((out2d[n], host[n]))
                 copied.synchronize()
@@ -934,19 +1013,23 @@ class LlamaDecoder:
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_beam(self, inputs_embeds: torch.Tensor, num_beams: int, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
-                      length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True) -> torch.Tensor:
+                      length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True, output_scores: bool = False):
         """Beam search from prompt embeddings [S, H] (HF GenerationMixin.beam_search + BeamSearchScorer behind llava_llama.py:212 when
         the eval scripts pass --num_beams > 1; restated by the CPU checker of the test suite (beam_search_generate), which is pinned to HF's own
         generate()).  Device side: the prompt is prefilled once per beam as one packed batch (HF expands the inputs the same way), every
         step runs the batched decode layers over the num_beams rows, a kernel reduces each row's logits to its 2 x num_beams best
         (log-prob + beam score, token) pairs, and the surviving beams' KV rows are re-ordered page-wise.  Host side: the hypothesis
-        bookkeeping on the num_beams x 2 num_beams candidates - the same control logic HF runs in Python.  Returns the NEW ids."""
+        bookkeeping on the num_beams x 2 num_beams candidates - the same control logic HF runs in Python.  Returns the NEW ids.
+        ``output_scores``: returns (ids, extra) with extra = _beam_extra's dict: every step's log_softmax rows [steps, num_beams, V]
+        (HF's output_scores of beam search, written by the candidates kernel), the best hypothesis' score and the beam row of each of
+        its tokens."""
         d, w, k = self.dims, self.w, int(num_beams)
         S, V = inputs_embeds.shape[0], d.vocab_size
         if k < 2:
             raise ValueError("generate_beam needs num_beams >= 2")
         if max_new_tokens < 1:
-            return torch.empty(0, dtype=torch.int64, device=self.device)
+            empty = torch.empty(0, dtype=torch.int64, device=self.device)
+            return (empty, self._beam_extra(None, 0, [])) if output_scores else empty
         if S + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
@@ -969,9 +1052,10 @@ class LlamaDecoder:
         zero = torch.zeros(k, dtype=torch.int32, device=dev)
         tables = [list(self.cache.owned[b]) for b in range(k)]  # page ids by position // PAGE_SIZE
         pages_all = self.cache.pages
+        rows_out = self._scores_view(max_new_tokens, k) if output_scores else None
 
         for step in range(max_new_tokens):
-            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t)
+            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t, **self._logprobs_kw(rows_out, step))
             h_s.copy_(cand_s, non_blocking=True)
             h_t.copy_(cand_t, non_blocking=True)
             torch.cuda.current_stream().synchronize()
@@ -1000,13 +1084,26 @@ class LlamaDecoder:
                 self._replay(("beam", k))
             else:
                 self._batch_step_launch(st, logits_only=True)
-        best = hyp.best(max_new_tokens)
-        return torch.tensor(best, dtype=torch.int64, device=dev)
+        best = torch.tensor(hyp.best(max_new_tokens), dtype=torch.int64, device=dev)
+        return (best, self._beam_extra(rows_out, step + 1, [hyp])) if output_scores else best
+
+    @staticmethod
+    def _logprobs_kw(rows_out: Optional[torch.Tensor], step: int) -> dict:
+        """beam_candidates' keyword for the step's log_softmax rows; none without output_scores, so the call is today's."""
+        return {} if rows_out is None else {"logprobs": rows_out[step]}
+
+    def _beam_extra(self, scores: Optional[torch.Tensor], steps: int, groups: List[BeamHypotheses]) -> dict:
+        """What a beam search returns with output_scores: scores fp32 [steps, rows, V] (each step's log_softmax rows), and per prompt
+        sequence_score (its best hypothesis' score, HF's sequences_scores) and beam_indices (the beam row, counted over all prompts'
+        rows, of each token of that hypothesis; HF's beam_indices before padding)."""
+        sc = torch.empty((0, 0, self.dims.vocab_size), dtype=torch.float32, device=self.device) if scores is None else scores[:steps].clone()
+        return {"scores": sc, "sequence_scores": [g.best_score for g in groups], "beam_indices": [g.best_beams for g in groups]}
 
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_beam_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], num_beams: int, max_new_tokens: int, eos_token_ids=None,
-                            stopping_fn=None, length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True) -> List[torch.Tensor]:
+                            stopping_fn=None, length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True,
+                            output_scores: bool = False):
         """Beam search over B prompts packed back to back ([sum S_b, H]) at once (HF beam_search + BeamSearchScorer with batch_size = B).
         Row g * k + i of every step is beam i of prompt g, so one batched decode step serves all B * k beams.  Device side: ONE packed
         prefill of the B prompts, their pages copied into the other k - 1 beams of each (kv_copy_pages), then per step the candidates
@@ -1014,7 +1111,9 @@ class LlamaDecoder:
         copy of the generated KV rows of every beam whose parent is another beam.  Host side: one BeamHypotheses per prompt.  A prompt
         that is done keeps its rows in the step (the graph shape stays fixed) and its choices are ignored.  The loop ends when every
         prompt is done, at max_new_tokens, or when ``stopping_fn`` holds for every beam of the prompts still running.  Returns a list
-        of B LongTensors of NEW ids, each prompt's best hypothesis."""
+        of B LongTensors of NEW ids, each prompt's best hypothesis.  ``output_scores``: returns (ids, extra) as generate_beam, the score
+        rows [steps, B * k, V] in the step's row order (row g * k + i = beam i of prompt g).  A prompt that is done keeps its rows in the
+        step, so its rows of the later steps hold what the step computed for them."""
         d, w, k, B = self.dims, self.w, int(num_beams), len(seq_lens)
         V, R, dev = d.vocab_size, B * int(num_beams), self.device
         seq_lens = [int(n) for n in seq_lens]
@@ -1023,7 +1122,8 @@ class LlamaDecoder:
         if B < 1 or packed_embeds.shape[0] != sum(seq_lens) or min(seq_lens) < 1:
             raise RuntimeError("generate_beam_batch: rows do not match seq_lens")
         if max_new_tokens < 1:
-            return [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
+            empty = [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
+            return (empty, self._beam_extra(None, 0, [])) if output_scores else empty
         if max(seq_lens) + max_new_tokens > self.max_seq_len:
             raise RuntimeError(f"{max(seq_lens)} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
@@ -1043,7 +1143,8 @@ class LlamaDecoder:
         rows = ops.splice_rows(hidden, None, None, None, torch.zeros_like(last), last)
         ops.rmsnorm(rows, w.norm, d.rms_norm_eps, out=st["xn"])
         ops.gemm(st["xn"], w.lm_head, out=st["logits"][:, :V])
-        groups = [BeamHypotheses(k, eos, length_penalty, early_stopping) for _ in range(B)]
+        groups = [BeamHypotheses(k, eos, length_penalty, early_stopping, row0=g * k) for g in range(B)]
+        rows_out = self._scores_view(max_new_tokens, R) if output_scores else None
         d_scores = torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32).to(dev)
         cand_s = torch.empty((R, n_cand), dtype=torch.float32, device=dev)
         cand_t = torch.empty((R, n_cand), dtype=torch.int32, device=dev)
@@ -1053,7 +1154,7 @@ class LlamaDecoder:
         zero = torch.zeros(R, dtype=torch.int32, device=dev)
         tokens = [0] * R  # the token each row feeds to the next step (a done prompt's rows repeat theirs)
         for step in range(max_new_tokens):
-            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t)
+            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t, **self._logprobs_kw(rows_out, step))
             ops.beam_select(cand_s, cand_t, k, sel[0].view(torch.float32), sel[1], sel[2])
             h_sel.copy_(sel, non_blocking=True)
             torch.cuda.current_stream().synchronize()
@@ -1082,13 +1183,14 @@ class LlamaDecoder:
                 self._replay(("beam", R))
             else:
                 self._batch_step_launch(st, logits_only=True)
-        return [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
+        outs = [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
+        return (outs, self._beam_extra(rows_out, step + 1, groups)) if output_scores else outs
 
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos_token_ids=None,
                        stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None, processors=None,
-                       num_return_sequences: int = 1):
+                       num_return_sequences: int = 1, output_scores: bool = False):
         """Decoding of B prompts: ONE packed prefill pass (tensor-core bound, all prompts share every GEMM), one lm_head GEMM for the
         B first tokens, then BATCHED decode: every step advances all B sequences, each weight streamed once per step for the
         whole batch (_decode_batched), greedy or sampled (``sampling``: sequence b draws with sequence_seeds(seed, B)[b]).  With
@@ -1097,7 +1199,11 @@ class LlamaDecoder:
         ``processors``: the logits processors of generate_from_embeds, on every path (the first tokens included).
         ``num_return_sequences=n`` (sampling only): n answers per prompt.  Each prompt is prefilled once, into row b * n; its prompt
         pages are copied into rows b * n + 1 .. b * n + n - 1, and the B * n rows decode in the batched sampled step, row r with
-        sequence_seeds(seed, B * n)[r].  Returns B * n lists, row b * n + j being answer j of prompt b."""
+        sequence_seeds(seed, B * n)[r].  Returns B * n lists, row b * n + j being answer j of prompt b.
+        ``output_scores``: returns (what it returns without, {"scores": fp32 [n_max, B * n, V]}), scores[t, r] being the row token t of
+        row r was chosen from (generate_from_embeds) and n_max the longest row's length.  In the batched step a row that has stopped
+        keeps its place, so its later steps hold what the step computed for it; the one-after-the-other path (return_logits) leaves
+        them 0."""
         n_ret = int(num_return_sequences)
         if n_ret < 1:
             raise ValueError(f"num_return_sequences must be >= 1, got {n_ret}")
@@ -1111,7 +1217,8 @@ class LlamaDecoder:
         d, w = self.dims, self.w
         B = len(seq_lens) * n_ret
         if max_new_tokens < 1:
-            return [torch.empty(0, dtype=torch.int64, device=self.device) for _ in range(B)]
+            empty = [torch.empty(0, dtype=torch.int64, device=self.device) for _ in range(B)]
+            return (empty, {"scores": torch.empty((0, B, d.vocab_size), dtype=torch.float32, device=self.device)}) if output_scores else empty
         if max_new_tokens > self.out_ids.numel():
             raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
         if max(seq_lens) + max_new_tokens > self.max_seq_len:
@@ -1133,18 +1240,26 @@ class LlamaDecoder:
         seq_lens = row_lens
         outs, all_logits = [], []
         sample = self._set_sampling(sampling)
+        scores = self._scores_view(max_new_tokens, B) if output_scores else None
+        zero = torch.zeros(1, dtype=torch.int32, device=self.device)
         first_rows = None  # the processed first-token rows a sampled sequence draws from
         if proc:  # the first tokens with an empty history: only the minimum length and single-token bad words act
-            first_rows = torch.empty((B, d.vocab_size), dtype=torch.float32, device=self.device) if sample else None
+            first_rows = torch.empty((B, d.vocab_size), dtype=torch.float32, device=self.device) if sample or output_scores else None
             ops.logits_process(lg, None, 0, 1, None, 0, self.proc_fparams, self.proc_spec, out=first_rows, ids=first)
+        if scores is not None and not sample:  # the rows the greedy first tokens were chosen from (a sampler writes its own)
+            ops.step_scores(first_rows if proc else lg, zero, 0, scores)
         if max_new_tokens == 1 and not return_logits and not sample:
-            return [first[b:b + 1] for b in range(B)]
+            outs = [first[b:b + 1] for b in range(B)]
+            return (outs, {"scores": scores[:1].clone()}) if output_scores else outs
         seeds = sequence_seeds(self.sample_seed, B) if sample else None
         if not return_logits and B > 1 and (not sample or self.supports_batch_sampling):
-            return self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc,
-                                        sample_from=(first_rows if proc else lg) if sample else None, seeds=seeds)
-        zero = torch.zeros(1, dtype=torch.int32, device=self.device)
+            outs = self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc,
+                                        sample_from=(first_rows if proc else lg) if sample else None, seeds=seeds, scores=scores)
+            return (outs, {"scores": scores[:max(o.numel() for o in outs)].clone()}) if output_scores else outs
+        if scores is not None and B > 1:  # one row after the other: a row's steps past its stop are never written
+            scores.view(max_new_tokens, B * d.vocab_size)[1 if not sample else 0:].zero_()
         for b in range(B):
+            col = None if scores is None else scores[:, b:b + 1]  # sequence b's rows: [T, 1, V] with a step stride of B * V
             logits = None
             if return_logits:
                 logits = torch.empty((max_new_tokens, d.vocab_size), dtype=torch.float32, device=self.device)
@@ -1157,13 +1272,15 @@ class LlamaDecoder:
             if sample:  # re-draw the first token of this sequence from its logits row (a different draw per sequence: the seed moves)
                 self._set_seed(seeds[b])
                 row = first_rows[b] if proc else lg[b].float().contiguous()
-                ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h)
-            r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc)
+                ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
+                                 **self._scores_kw(col, True))
+            r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, col)
             if return_logits:
                 outs.append(r[0]); all_logits.append(r[1])
             else:
                 outs.append(r)
-        return (outs, all_logits) if return_logits else outs
+        r = (outs, all_logits) if return_logits else outs
+        return (r, {"scores": scores[:max(o.numel() for o in outs)].clone()}) if output_scores else r
 
     # ---- likelihood scoring: every candidate continues its prompt from the prompt's own KV pages ------------------------------------
     supports_scoring = True

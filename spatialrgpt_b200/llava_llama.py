@@ -40,6 +40,59 @@ class ScoreOutput:
     lengths: torch.Tensor
 
 
+@dataclass
+class GenerateDecoderOnlyOutput:
+    """generate(return_dict_in_generate=True) of greedy and sampled decoding, with HF's field names.  sequences: the int64 [rows, L]
+    generate() returns without the flag.  scores (output_scores=True): one fp32 [rows, V] tensor per step, the row the step's token was
+    chosen from (the raw row when greedy, after the logits processors when they are on, after the temperature / top-k / top-p warpers
+    when sampled).  logits (output_logits=True): what generate(output_logits=True) returns beside the ids, one fp32 [n_b, V] per row."""
+    sequences: torch.Tensor
+    scores: Optional[Tuple[torch.Tensor, ...]] = None
+    logits: Any = None
+    attentions: Any = None
+    hidden_states: Any = None
+    past_key_values: Any = None
+
+
+@dataclass
+class GenerateBeamDecoderOnlyOutput:
+    """generate(num_beams > 1, return_dict_in_generate=True), with HF's field names.  With output_scores=True: sequences_scores fp32 [B]
+    (each prompt's best hypothesis' score, its summed log-probabilities over length ** length_penalty), scores (one fp32 [B * num_beams,
+    V] log_softmax per step, before the beam score is added) and beam_indices int64 [B, L] (the row of each token of the hypothesis,
+    -1 past its end)."""
+    sequences: torch.Tensor
+    sequences_scores: Optional[torch.Tensor] = None
+    scores: Optional[Tuple[torch.Tensor, ...]] = None
+    logits: Any = None
+    beam_indices: Optional[torch.Tensor] = None
+    attentions: Any = None
+    hidden_states: Any = None
+    past_key_values: Any = None
+
+
+def compute_transition_scores(sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None, normalize_logits: bool = False,
+                              vocab_size: Optional[int] = None) -> torch.Tensor:
+    """HF's GenerationMixin.compute_transition_scores: the score of every generated token, fp32 [rows, steps] (beams: [B, L], 0 where
+    beam_indices is -1).  ``scores`` = generate()'s per-step tuple of [rows, V]; ``normalize_logits`` log-softmaxes each row first;
+    ``beam_indices`` picks the row of each step for beam search.  Post-processing of returned tensors, in torch."""
+    V = scores[0].shape[-1] if vocab_size is None else int(vocab_size)
+    if beam_indices is None:
+        beam_indices = torch.arange(scores[0].shape[0], device=sequences.device).view(-1, 1).expand(-1, len(scores))
+    sc = torch.stack(scores).reshape(len(scores), -1).transpose(0, 1)  # [rows * V, steps]
+    if normalize_logits:
+        sc = torch.nn.functional.log_softmax(sc.reshape(-1, V, sc.shape[-1]), dim=1).reshape(-1, sc.shape[-1])
+    mask = beam_indices < 0
+    max_len = int((1 - mask.long()).sum(-1).max())
+    beam_indices = beam_indices.clone()[:, :max_len]
+    mask = mask[:, :max_len]
+    beam_indices[mask] = 0
+    cut = sequences.shape[-1] - max_len
+    indices = sequences[:, cut:] + beam_indices * V
+    out = sc.gather(0, indices)
+    out[mask] = 0
+    return out
+
+
 class LlavaLlamaModel:
     config_class = LlavaConfig
     main_input_name = "input_embeds"
@@ -489,6 +542,11 @@ class LlavaLlamaModel:
         pad_token_id = generation_kwargs.pop("pad_token_id", None)
         eos_token_id = generation_kwargs.pop("eos_token_id", self.config.llama.eos_token_id)
         return_logits = bool(generation_kwargs.pop("output_logits", False))
+        # return_dict_in_generate=True: an output object with HF's field names (GenerateDecoderOnlyOutput / GenerateBeamDecoderOnlyOutput);
+        # with output_scores=True it carries the row each token was chosen from, written on the device by the decode step.  Without the
+        # dict, output_scores is ignored, as HF ignores it.
+        return_dict = bool(generation_kwargs.pop("return_dict_in_generate", False))
+        output_scores = bool(generation_kwargs.pop("output_scores", False)) and return_dict
         use_graph = bool(generation_kwargs.pop("use_cuda_graph", True))
         # prefix_cache=True (batch 1, opt-in): keep the previous such request's encoder outputs and the K/V of its prompt rows, and
         # prefill only the rows after the longest unchanged prefix (a follow-up turn of a conversation).  The new rows run through
@@ -559,6 +617,8 @@ class LlavaLlamaModel:
                 raise NotImplementedError("prompt_lookup_num_tokens on the tensor-parallel decoder")
         if num_beams != 1 and (not hasattr(self.llm, "generate_beam") or type(self.llm).__name__ == "TPLlamaDecoder"):
             raise NotImplementedError("beam search on the tensor-parallel decoder")
+        if output_scores and not getattr(self.llm, "supports_output_scores", False):
+            raise NotImplementedError("output_scores on the tensor-parallel decoder (its logits are vocabulary-parallel: no rank holds a whole row)")
         prefix = None
         if prefix_cache:
             if input_ids is None or input_ids.shape[0] != 1:
@@ -589,6 +649,8 @@ class LlavaLlamaModel:
         pad = pad_token_id if pad_token_id is not None else (self.config.llama.pad_token_id or 0)
 
         outs, all_logits = [], []
+        extra = None  # the decoder's output_scores results
+        sc_kw = {"output_scores": True} if output_scores else {}
         stop_fn = None
         if stopping_criteria:
             def stop_fn(ids, _sc=stopping_criteria):
@@ -602,8 +664,11 @@ class LlavaLlamaModel:
         if B == 1 and num_beams != 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
-            outs.append(self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                               length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph))
+            r = self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
+                                       length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph, **sc_kw)
+            if output_scores:
+                r, extra = r
+            outs.append(r)
         elif B == 1 and n_ret == 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
@@ -620,7 +685,9 @@ class LlavaLlamaModel:
                             lookup_ngram=lookup_ngram)
             r = self.llm.generate_from_embeds(emb, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                               use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse, **spec,
-                                              **proc)
+                                              **proc, **sc_kw)
+            if output_scores:
+                r, extra = r
             if lookup_k:
                 self.last_speculation = tuple(self.llm.last_speculation)
             if prefix is not None:
@@ -640,11 +707,15 @@ class LlavaLlamaModel:
                 packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
             if num_beams != 1:
                 outs = self.llm.generate_beam_batch(packed, lens, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                                    length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph)
+                                                    length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph, **sc_kw)
+                if output_scores:
+                    outs, extra = outs
             else:
                 r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                             use_graph=use_graph, return_logits=return_logits, sampling=sampling, num_return_sequences=n_ret,
-                                            **proc)
+                                            **proc, **sc_kw)
+                if output_scores:
+                    r, extra = r
                 if return_logits:
                     outs, all_logits = r
                 else:
@@ -653,9 +724,32 @@ class LlavaLlamaModel:
         seqs = torch.full((len(outs), n_max), int(pad), dtype=torch.int64, device=self.device)
         for b, o in enumerate(outs):
             seqs[b, : o.numel()] = o
+        if return_dict:
+            return self._generate_output(seqs, extra, all_logits if return_logits else None, num_beams != 1)
         if return_logits:
             return seqs, all_logits
         return seqs
+
+    def _generate_output(self, seqs: torch.Tensor, extra, logits, beams: bool):
+        """The return_dict_in_generate object of a request whose padded sequences are ``seqs`` and whose decoder returned ``extra``
+        (None without output_scores)."""
+        scores = None if extra is None else tuple(extra["scores"].unbind(0))
+        if not beams:
+            return GenerateDecoderOnlyOutput(sequences=seqs, scores=scores, logits=logits)
+        if extra is None:  # HF returns sequences_scores and beam_indices with output_scores only
+            return GenerateBeamDecoderOnlyOutput(sequences=seqs)
+        idx = torch.full(seqs.shape, -1, dtype=torch.int64)
+        for b, bi in enumerate(extra["beam_indices"]):
+            idx[b, : len(bi)] = torch.tensor(bi, dtype=torch.int64)
+        return GenerateBeamDecoderOnlyOutput(sequences=seqs, sequences_scores=torch.tensor(extra["sequence_scores"], dtype=torch.float32,
+                                                                                           device=self.device),
+                                             scores=scores, beam_indices=idx.to(self.device))
+
+    def compute_transition_scores(self, sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None,
+                                  normalize_logits: bool = False) -> torch.Tensor:
+        """HF's compute_transition_scores over generate(return_dict_in_generate=True, output_scores=True)'s sequences / scores /
+        beam_indices: the score of every generated token (module-level compute_transition_scores)."""
+        return compute_transition_scores(sequences, scores, beam_indices, normalize_logits, self.llm.dims.vocab_size)
 
 
 LlavaLlamaForCausalLM = LlavaLlamaModel

@@ -824,10 +824,13 @@ def lm_head_argmax_packed(x: torch.Tensor, p, norm_weight: Optional[torch.Tensor
 
 
 def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.Tensor, step_offset: int, out_ids: torch.Tensor,
-                 embed_table: Optional[torch.Tensor] = None, next_x: Optional[torch.Tensor] = None) -> None:
+                 embed_table: Optional[torch.Tensor] = None, next_x: Optional[torch.Tensor] = None, scores: Optional[torch.Tensor] = None,
+                 step_stride: int = 0) -> None:
     """One token from softmax(logits / T) restricted to its top-p nucleus -> out_ids[step + step_offset] (and next_x = embed row).
     ``params`` = device float32 [temperature, top_p, top_k (0 = off)]; ``step`` = device int32 [1]; ``seed`` = device int64 [1]
-    (read by the kernel at run time - graph-capturable), or a Python int for one-off eager calls."""
+    (read by the kernel at run time - graph-capturable), or a Python int for one-off eager calls.
+    ``scores`` (fp32, optional): the warped row the draw picked from (logits / T where kept, -inf elsewhere) goes to
+    scores.view(-1)[(step + step_offset) * step_stride:][:V]."""
     if not isinstance(seed, torch.Tensor):
         seed = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF], dtype=torch.int64, device=logits.device)
     _need(seed, torch.int64, "sample_top_p.seed")
@@ -836,15 +839,22 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
     if logits.dim() != 1 or not logits.is_contiguous() or params.numel() < 3:
         raise SrgptError("sample_top_p: logits must be a contiguous fp32 vector [V] and params [temperature, top_p, top_k]")
     K = 0 if embed_table is None else embed_table.shape[1]
+    if scores is not None:
+        _need(scores, torch.float32, "sample_top_p.scores")
+        check(_lib.load().srgpt_sample_top_p_scores_f32(_p(logits), logits.numel(), _p(params), _p(seed), _p(step), step_offset, _p(out_ids),
+                                                        _p(embed_table), _p(next_x), K, _p(scores), int(step_stride), _stream()),
+              "srgpt_sample_top_p_scores_f32")
+        return
     check(_lib.load().srgpt_sample_top_p_f32(_p(logits), logits.numel(), _p(params), _p(seed), _p(step), step_offset,
                                              _p(out_ids), _p(embed_table), _p(next_x), K, _stream()), "srgpt_sample_top_p_f32")
 
 
 def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor, step: torch.Tensor, step_offset: int,
-                ids: torch.Tensor) -> None:
+                ids: torch.Tensor, scores: Optional[torch.Tensor] = None) -> None:
     """One token per row of ``logits`` ([R, V] fp32 or the element type, unit inner stride, e.g. the batched lm_head's rows) in one
     launch -> ids int64 [R].  Row r draws with seeds[r] (device int64 [R]) at counter step + step_offset, the token sample_top_p draws
-    from that row in fp32 with that seed and counter.  ``params`` and ``step`` as for sample_top_p."""
+    from that row in fp32 with that seed and counter.  ``params`` and ``step`` as for sample_top_p.
+    ``scores`` (contiguous fp32 [T, R, V], optional): row r's warped row goes to scores[step + step_offset, r]."""
     _need(params, torch.float32, "sample_rows.params"); _need(seeds, torch.int64, "sample_rows.seeds")
     _need(step, torch.int32, "sample_rows.step"); _need(ids, torch.int64, "sample_rows.ids")
     if not logits.is_cuda:
@@ -861,8 +871,30 @@ def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor,
         raise SrgptError(f"sample_rows: seeds must be a contiguous int64 vector of {R} entries, got shape {tuple(seeds.shape)}")
     if ids.dim() != 1 or ids.numel() != R or not ids.is_contiguous():
         raise SrgptError(f"sample_rows: ids must be a contiguous int64 vector of {R} entries, got shape {tuple(ids.shape)}")
+    if scores is not None:
+        _need(scores, torch.float32, "sample_rows.scores")
+        if scores.dim() != 3 or scores.shape[1:] != (R, V) or not scores.is_contiguous():
+            raise SrgptError(f"sample_rows: scores must be contiguous fp32 [T, {R}, {V}], got shape {tuple(scores.shape)}")
+        check(_lib.load().srgpt_sample_rows_scores(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids),
+                                                   _p(scores), R * V, _stream()), "srgpt_sample_rows_scores")
+        return
     check(_lib.load().srgpt_sample_rows(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids), _stream()),
           "srgpt_sample_rows")
+
+
+def step_scores(rows: torch.Tensor, step: torch.Tensor, step_offset: int, scores: torch.Tensor) -> None:
+    """A decode step's score rows: rows ([R, V] fp32 or the element type, unit inner stride; a 1-D row counts as one) widened to fp32
+    -> scores[step + step_offset] (``scores`` a [T, R, V] fp32 view whose last dimension is contiguous, e.g. a column of a wider
+    [T, B, V] buffer; ``step`` = device int32 [1], read at run time)."""
+    x = rows if rows.dim() == 2 else rows.view(1, -1)
+    R, V = x.shape
+    f32 = x.dtype == torch.float32
+    _need(x, torch.float32 if f32 else ELEM(), "step_scores.rows"); _need(step, torch.int32, "step_scores.step")
+    _need(scores, torch.float32, "step_scores.scores")
+    if scores.dim() != 3 or scores.shape[1:] != (R, V) or scores.stride(2) != 1:
+        raise SrgptError(f"step_scores: scores must be fp32 [T, {R}, {V}] with a unit inner stride, got shape {tuple(scores.shape)}")
+    check(_lib.load().srgpt_step_scores(_p(x), int(f32), _rowmajor2d(x, "step_scores.rows"), R, V, _p(step), step_offset, _p(scores),
+                                        scores.stride(0), scores.stride(1), _stream()), "srgpt_step_scores")
 
 
 def token_logprobs(logits: torch.Tensor, rows, targets, loss: bool = False):
@@ -942,13 +974,24 @@ def logits_pick_token(ids: torch.Tensor, step: torch.Tensor, step_offset: int, o
           "srgpt_logits_pick_token")
 
 
-def beam_candidates(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores: torch.Tensor, cand_tokens: torch.Tensor) -> None:
-    """Per beam row: the n_cand best (log_softmax(logits)[token] + beam_scores[row], token) -> cand_scores / cand_tokens [k, n_cand]."""
+def beam_candidates(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores: torch.Tensor, cand_tokens: torch.Tensor,
+                    logprobs: Optional[torch.Tensor] = None) -> None:
+    """Per beam row: the n_cand best (log_softmax(logits)[token] + beam_scores[row], token) -> cand_scores / cand_tokens [k, n_cand].
+    ``logprobs`` (fp32 [k, V], unit inner stride, optional): every row's whole log_softmax."""
     _need(logits, ELEM(), "beam_candidates.logits"); _need(beam_scores, torch.float32, "beam_candidates.beam_scores")
     _need(cand_scores, torch.float32, "beam_candidates.cand_scores"); _need(cand_tokens, torch.int32, "beam_candidates.cand_tokens")
     k, V = logits.shape
     if cand_scores.shape != cand_tokens.shape or cand_scores.shape[0] != k or not cand_scores.is_contiguous() or not cand_tokens.is_contiguous():
         raise SrgptError("beam_candidates: cand_scores / cand_tokens must be contiguous [n_beams, n_cand]")
+    if logprobs is not None:
+        _need(logprobs, torch.float32, "beam_candidates.logprobs")
+        if logprobs.shape != (k, V):
+            raise SrgptError(f"beam_candidates: logprobs must be fp32 [{k}, {V}], got shape {tuple(logprobs.shape)}")
+        check(_lib.load().srgpt_beam_candidates_scores_bf16(_p(logits), _rowmajor2d(logits, "beam_candidates.logits"), k, V, _p(beam_scores),
+                                                            cand_scores.shape[1], _p(cand_scores), _p(cand_tokens), _p(logprobs),
+                                                            _rowmajor2d(logprobs, "beam_candidates.logprobs"), _stream()),
+              "srgpt_beam_candidates_scores_bf16")
+        return
     check(_lib.load().srgpt_beam_candidates_bf16(_p(logits), _rowmajor2d(logits, "beam_candidates.logits"), k, V, _p(beam_scores), cand_scores.shape[1],
                                                  _p(cand_scores), _p(cand_tokens), _stream()), "srgpt_beam_candidates_bf16")
 

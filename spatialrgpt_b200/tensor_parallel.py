@@ -66,6 +66,7 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_prompt_lookup = False  # the verify pass is a single-GPU kernel sequence
     supports_logits_processors = False  # the logits are vocabulary-parallel: no rank holds a whole row
     supports_batch_sampling = False  # the decoder implements greedy decoding only
+    supports_output_scores = False  # the logits are vocabulary-parallel: no rank holds a whole score row
     supports_scoring = False  # likelihood scoring (score_candidates) is a single-GPU path
 
     def score_candidates(self, *args, **kwargs):
