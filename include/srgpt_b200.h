@@ -600,6 +600,52 @@ int srgpt_llama_verify_step_nf4_bf16(void* h, const srgpt_llama_layer_weights* l
                                      void* lm_workspace, float* logits_rows, float* logits_all, const int* prompt_ids, const int* prompt_len, int ngram,
                                      int* draft_ids, long long* out_ids, int out_cap, int* step, int* state, void* stream);
 
+/* ---- batch-invariant decoding: B <= SRGPT_SPEC_T_MAX sequences in one weight pass, each row with the arithmetic of its one-token step.
+ * Row b is the newest token of the sequence at position pos_rows[b] (device int32 [B]) whose page table is page_tables + b * pt_stride,
+ * so every sequence's ids and logits are bit-identical to decoding it alone with srgpt_llama_decode_step_*. */
+/* srgpt_gemv_multi_bf16 in QKV_ROPE mode over rows of different sequences: row t is rotated at and appends K/V at position pos_rows[t]
+ * through page_tables + t * pt_stride (pt_stride = 0: one page table, the verify pass).  Row t equals srgpt_gemv_bf16 at that position. */
+int srgpt_gemv_rows_bf16(const void* x, int ldx, const void* W, int ldw, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
+                         int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows, void* kv_pages,
+                         const int* page_tables, int pt_stride, int page_size, void* stream);
+int srgpt_gemv_rows_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, void* y, int ldy, int T, int N, int K, const void* norm_weight,
+                                float eps, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows,
+                                void* kv_pages, const int* page_tables, int pt_stride, int page_size, void* stream);
+int srgpt_gemv_rows_nf4_bf16(const void* x, int ldx, const srgpt_nf4* nf4, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
+                             int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows, void* kv_pages,
+                             const int* page_tables, int pt_stride, int page_size, void* stream);
+/* Decode attention of T rows: row t (q row t, out row t) attends over kv rows 0 .. pos_rows[t] of the page table page_tables + t * pt_stride.
+ * The arithmetic of srgpt_attention_decode_bf16 per row.  srgpt_attention_decode_multi_bf16 is the pt_stride = 0 case. */
+int srgpt_attention_decode_rows_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages, const int* page_tables, int pt_stride,
+                                     int page_size, const int* pos_rows, int T, int n_heads, int n_kv_heads, int head_dim, float scale, void* stream);
+/* The end of a step of B rows (one CTA): row b's token is its arg max from the srgpt_lm_head_multi_* partials in `workspace` (lowest index
+ * on ties, as srgpt_lm_head_argmax_bf16), or ids[b] when ids != NULL.  out_ids[*step * B + b] = the token, x row b (x [B, H]) = its
+ * embedding row, ++pos_rows[b], then ++*step. */
+int srgpt_rows_advance(const void* workspace, int V, const long long* ids, int B, const void* embed_table, void* x, int H, long long* out_ids, int* step,
+                       int* pos_rows, void* stream);
+/* One decode step of B sequences: 5 kernels per layer (srgpt_gemv_rows_*, srgpt_attention_decode_rows_bf16, srgpt_gemv_multi_* for o /
+ * gate-up / down), lm_head over the B rows, then srgpt_rows_advance.  Sampled when seeds != NULL: row b draws from logits_rows row b with
+ * seeds[b] at counter *step (srgpt_sample_rows into ids [B], one more kernel).  Buffers: h [B, H], q_buf / attn_buf [B, nh*hd], act_buf
+ * [B, I], lm_workspace B * srgpt_lm_head_workspace(V) bytes, logits_rows fp32 [B, V] (optional when greedy).  pt_stride > 0.  The FP8
+ * layer format has no form of this step. */
+int srgpt_llama_decode_rows_bf16(void* h, const srgpt_llama_layer_weights* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int B, int H,
+                                 int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos_rows,
+                                 const int* page_tables, int pt_stride, int page_size, const void* final_norm, const void* lm_head, int V,
+                                 const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params,
+                                 const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, void* stream);
+int srgpt_llama_decode_rows_packed_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers,
+                                        void* q_buf, void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+                                        float eps, const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride,
+                                        int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+                                        const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params,
+                                        const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, void* stream);
+int srgpt_llama_decode_rows_nf4_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf,
+                                     void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                                     const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size,
+                                     const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table,
+                                     void* lm_workspace, float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
+                                     long long* out_ids, int* step, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -136,6 +136,17 @@ SIGNATURES = {
                                                        vp, ci, vp]),
     "srgpt_llama_verify_step_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp,
                                               vp, vp, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp]),
+    "srgpt_gemv_rows_bf16": (ci, [vp, ci, vp, ci, vp, ci, ci, ci, ci, vp, cf, ci, ci, ci, vp, vp, vp, vp, vp, ci, ci, vp]),
+    "srgpt_gemv_rows_packed_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, ci, ci, ci, vp, vp, vp, vp, vp, ci, ci, vp]),
+    "srgpt_gemv_rows_nf4_bf16": (ci, [vp, ci, vp, vp, ci, ci, ci, ci, vp, cf, ci, ci, ci, vp, vp, vp, vp, vp, ci, ci, vp]),
+    "srgpt_attention_decode_rows_bf16": (ci, [vp, ci, vp, ci, vp, vp, ci, ci, vp, ci, ci, ci, ci, cf, vp]),
+    "srgpt_rows_advance": (ci, [vp, ci, vp, ci, vp, vp, ci, vp, vp, vp, vp]),
+    "srgpt_llama_decode_rows_bf16": (ci, [vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, ci, vp, vp, vp, vp,
+                                          vp, vp, vp, vp, vp]),
+    "srgpt_llama_decode_rows_packed_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp, ci, vp,
+                                                 vp, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_llama_decode_rows_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp, ci, vp,
+                                              vp, vp, vp, vp, vp, vp, vp, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)

@@ -709,19 +709,21 @@ extern "C" __attribute__((visibility("default"))) int srgpt_attention_decode_tp_
   return SRGPT_OK;
 }
 
-// T consecutive tokens of one sequence (the verify pass of prompt-lookup speculative decoding): grid (q head, token), token t reads
-// q row t and the kv rows 0 .. pos_rows[t] through the one page table.  It is attn_decode_kernel itself, so every token gets the
+// T rows of decode attention in one launch: grid (q head, row), row t reads q row t and the kv rows 0 .. pos_rows[t] through the page table
+// at page_tables + t * pt_stride: T different sequences (pt_stride > 0, srgpt_llama_decode_rows_*), or T consecutive tokens of one sequence
+// (pt_stride = 0, the verify pass of prompt-lookup speculative decoding).  It is attn_decode_kernel itself, so every row gets the
 // one-token arithmetic (half-warp per kv row, rows in the same order, base-2 online softmax, the same merge) by construction.  The
-// prefetch before the dependency wait is off: rows at and after the pass's first position were written by an earlier pass with
-// drafts that may have been rejected, and this pass's qkv kernel overwrites them, so no position read before the wait is final.
-extern "C" __attribute__((visibility("default"))) int srgpt_attention_decode_multi_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages,
-                                                                                        const int* page_table, int page_size, const int* pos_rows, int T,
-                                                                                        int n_heads, int n_kv_heads, int head_dim, float scale, void* stream) {
-  SRGPT_CHECK_ARG(q && out && kv_pages && page_table && pos_rows && T >= 1 && T <= SRGPT_SPEC_T_MAX);
+// prefetch before the dependency wait is off: in a verify pass, rows at and after the pass's first position were written by an earlier
+// pass with drafts that may have been rejected, and this pass's qkv kernel overwrites them, so no position read before the wait is final.
+extern "C" __attribute__((visibility("default"))) int srgpt_attention_decode_rows_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages,
+                                                                                       const int* page_tables, int pt_stride, int page_size,
+                                                                                       const int* pos_rows, int T, int n_heads, int n_kv_heads, int head_dim,
+                                                                                       float scale, void* stream) {
+  SRGPT_CHECK_ARG(q && out && kv_pages && page_tables && pos_rows && T >= 1 && T <= SRGPT_SPEC_T_MAX && pt_stride >= 0);
   SRGPT_CHECK_ARG(n_heads > 0 && n_kv_heads > 0 && (n_heads % n_kv_heads) == 0 && page_size > 0);
   SRGPT_CHECK_ARG(aligned16(q) && aligned16(kv_pages) && (q_ld % 8) == 0 && q_ld >= n_heads * head_dim && o_ld >= n_heads * head_dim);
   if (head_dim != 128) {
-    set_last_error("srgpt_attention_decode_multi_bf16: head_dim %d unsupported (128 only)", head_dim);
+    set_last_error("srgpt_attention_decode_rows_bf16: head_dim %d unsupported (128 only)", head_dim);
     return SRGPT_ERR_UNSUPPORTED;
   }
   cudaLaunchConfig_t cfg = {};
@@ -734,7 +736,15 @@ extern "C" __attribute__((visibility("default"))) int srgpt_attention_decode_mul
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attn::attn_decode_kernel, reinterpret_cast<const bf16*>(q), reinterpret_cast<bf16*>(out),
-                                      reinterpret_cast<const bf16*>(kv_pages), page_table, page_size, pos_rows, n_kv_heads, n_heads / n_kv_heads,
-                                      scale * 1.4426950408889634f, (unsigned long long*)nullptr, 0, 0, q_ld, o_ld, 0));
+                                      reinterpret_cast<const bf16*>(kv_pages), page_tables, page_size, pos_rows, n_kv_heads, n_heads / n_kv_heads,
+                                      scale * 1.4426950408889634f, (unsigned long long*)nullptr, 0, 0, q_ld, o_ld, pt_stride));
   return SRGPT_OK;
+}
+
+// T consecutive tokens of one sequence (the verify pass of prompt-lookup speculative decoding): the rows attention over one page table.
+extern "C" __attribute__((visibility("default"))) int srgpt_attention_decode_multi_bf16(const void* q, int q_ld, void* out, int o_ld, const void* kv_pages,
+                                                                                        const int* page_table, int page_size, const int* pos_rows, int T,
+                                                                                        int n_heads, int n_kv_heads, int head_dim, float scale, void* stream) {
+  return srgpt_attention_decode_rows_bf16(q, q_ld, out, o_ld, kv_pages, page_table, 0, page_size, pos_rows, T, n_heads, n_kv_heads, head_dim, scale,
+                                          stream);
 }

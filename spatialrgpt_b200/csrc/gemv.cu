@@ -431,11 +431,11 @@ __device__ __forceinline__ void consume(Fmt& f, const typename Fmt::Raw& t, int 
 }
 
 // The stores of one token's results for a row pair: the fp32 sums a0 / a1 of rows r0 / r1 with the mode's rounding points (those of the
-// reference's torch ops, see the top of the file).  y and residual are the token's rows, pos its position (QKV + RoPE), logits its row of
-// fp32 logits (lm_head, may be null); lm_head returns the pair's best (value, row) in best / besti.
+// reference's torch ops, see the top of the file).  y and residual are the token's rows, pos its position and page_table its sequence's
+// page table (QKV + RoPE), logits its row of fp32 logits (lm_head, may be null); lm_head returns the pair's best (value, row) in best / besti.
 template <int MODE>
-__device__ __forceinline__ void store_pair(const Params& p, bf16* y, const bf16* residual, float* logits, int pos, int pi, int r0, int r1,
-                                           float a0, float a1, float& best, int& besti) {
+__device__ __forceinline__ void store_pair(const Params& p, bf16* y, const bf16* residual, float* logits, int pos, const int* page_table, int pi,
+                                           int r0, int r1, float a0, float a1, float& best, int& besti) {
   if (MODE == SRGPT_GEMV_PLAIN && p.y_f32 != nullptr) {
     // row-parallel linear of a tensor-parallel rank: the partial sums over this rank's K slice, reduced across ranks afterwards
     *reinterpret_cast<float2*>(p.y_f32 + r0) = make_float2(a0, a1);
@@ -465,7 +465,7 @@ __device__ __forceinline__ void store_pair(const Params& p, bf16* y, const bf16*
       y[r0] = f2e(v0);
       y[r1] = f2e(v1);
     } else {
-      const int page = p.page_table[pos / p.page_size], slot = pos % p.page_size;
+      const int page = page_table[pos / p.page_size], slot = pos % p.page_size;
       const bool is_v = head >= p.n_heads + p.n_kv_heads;
       const int kh = head - p.n_heads - (is_v ? p.n_kv_heads : 0) + p.kv_head_off;
       const int kv_row = (p.kv_heads_total > 0 ? p.kv_heads_total : p.n_kv_heads) * p.hd;
@@ -496,7 +496,7 @@ __device__ __forceinline__ void epilogue(const Params& p, bool active, int pi, i
   float best = -INFINITY;
   int besti = 0x7fffffff;
   if (active && lane == 0)
-    store_pair<MODE>(p, p.y, p.residual, p.logits_out, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos : 0, pi, r0, r1, a0, a1, best, besti);
+    store_pair<MODE>(p, p.y, p.residual, p.logits_out, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos : 0, p.page_table, pi, r0, r1, a0, a1, best, besti);
   if (MODE == MODE_LM) {
     if (lane == 0) { sv[warp] = best; si[warp] = besti; }
     __syncthreads();
@@ -710,8 +710,8 @@ __global__ void __launch_bounds__(THREADS, 2) fp8_gemv_kernel(const Params p, co
   if (active && lane == 0) {
     float best;
     int besti;
-    store_pair<MODE>(p, p.y, p.residual, nullptr, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos : 0, pi, r0, r1, a0 * (s_x * sw0), a1 * (s_x * sw1), best,
-                     besti);
+    store_pair<MODE>(p, p.y, p.residual, nullptr, MODE == SRGPT_GEMV_QKV_ROPE ? *p.pos : 0, p.page_table, pi, r0, r1, a0 * (s_x * sw0),
+                     a1 * (s_x * sw1), best, besti);
   }
   trace_mark(p.trace, 2);
 }
@@ -782,6 +782,9 @@ struct MParams {
   int T;        // tokens (rows of x / y)
   int ldx, ldy;  // row strides of x and y (residual) in elements
   int tile_ch;  // chunks of x per staged tile
+  // QKV_ROPE: row t is at position pos_rows[t] (NULL: *p.pos + t) and appends K / V through p.page_table + t * pt_stride (0: one sequence)
+  const int* pos_rows;
+  int pt_stride;
 };
 
 #define SRGPT_GEMV_MULTI_KERNEL decode_gemv_multi_kernel
@@ -886,6 +889,42 @@ spec_accept_kernel(const float* __restrict__ ws, int nparts, int T, const int* _
     *step = s0 + a + 1;
     *pos += a + 1;
   }
+}
+
+// One decode step of B sequences (srgpt_llama_decode_rows_*): row b's token is its arg max, reduced from its partials exactly as
+// lm_head_finalize_kernel does (lowest index on ties), or ids[b] when given (a draw).  It goes to out_ids[*step * B + b], row b of x
+// becomes its embedding, pos_rows[b] advances; then *step.
+__global__ void __launch_bounds__(256)
+rows_advance_kernel(const float* __restrict__ ws, int nparts, const long long* __restrict__ ids, int B, const bf16* __restrict__ embed_table,
+                    bf16* __restrict__ x, int H, long long* __restrict__ out_ids, int* step, int* pos_rows) {
+  __shared__ int s_tok[MT_MAX];
+  pdl_launch_dependents();
+  pdl_wait();
+  for (int b = 0; b < B; ++b) {
+    if (ids != nullptr) {
+      if (threadIdx.x == 0) s_tok[b] = (int)ids[b];
+      continue;
+    }
+    const float* part_val = ws + (size_t)b * 2 * nparts;
+    float best;
+    int bi;
+    block_argmax(part_val, reinterpret_cast<const int*>(part_val + nparts), nparts, best, bi);
+    if (threadIdx.x == 0) s_tok[b] = bi == 0x7fffffff ? 0 : bi;
+    __syncthreads();
+  }
+  __syncthreads();
+  const int s = *step;
+  if (threadIdx.x < B) {
+    out_ids[(size_t)s * B + threadIdx.x] = (long long)s_tok[threadIdx.x];
+    pos_rows[threadIdx.x] += 1;
+  }
+  for (int b = 0; b < B; ++b) {
+    const uint4* src = reinterpret_cast<const uint4*>(embed_table + (size_t)s_tok[b] * H);
+    uint4* dst = reinterpret_cast<uint4*>(x + (size_t)b * H);
+    for (int c = threadIdx.x; c < (H >> 3); c += blockDim.x) dst[c] = src[c];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *step = s + 1;
 }
 
 // output_logits: the accepted rows of the pass's logits [T, V] go to rows state[4] .. state[4] + state[5] - 1
@@ -1307,7 +1346,8 @@ static int multi_tile(int K, bool norm) { return norm ? (K >> 3) : ((K >> 3) < M
 template <class Fmt>
 static int gemv_multi_modes(gemv::MParams& mp, const void* x, int ldx, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
                             const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
-                            const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream) {
+                            const int* pos, void* kv_pages, const int* page_table, int page_size, void* stream, const int* pos_rows = nullptr,
+                            int pt_stride = 0) {
   SRGPT_CHECK_ARG(x && y && N > 0 && K > 0 && T >= 1 && T <= gemv::MT_MAX);
   SRGPT_CHECK_ARG((N % 2) == 0 && (K % 8) == 0 && (ldx % 8) == 0 && ldx >= K && (ldy % 2) == 0);
   SRGPT_CHECK_ARG(aligned16(x) && (reinterpret_cast<uintptr_t>(y) & 3) == 0);
@@ -1329,8 +1369,10 @@ static int gemv_multi_modes(gemv::MParams& mp, const void* x, int ldx, void* y, 
     case SRGPT_GEMV_QKV_ROPE:
       SRGPT_CHECK_ARG(residual == nullptr && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && (head_dim % 2) == 0);
       SRGPT_CHECK_ARG(N == (n_heads + 2 * n_kv_heads) * head_dim && ldy >= n_heads * head_dim);
-      SRGPT_CHECK_ARG(cos_tab && sin_tab && pos && kv_pages && page_table && page_size > 0);
+      SRGPT_CHECK_ARG(cos_tab && sin_tab && (pos || pos_rows) && kv_pages && page_table && page_size > 0 && pt_stride >= 0);
       set_rope(mp.p, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos, kv_pages, page_table, page_size);
+      mp.pos_rows = pos_rows;
+      mp.pt_stride = pt_stride;
       return gemv::launch_multi<SRGPT_GEMV_QKV_ROPE, Fmt>(mp, N / 2, st);
   }
   return SRGPT_ERR_INVALID;
@@ -1375,6 +1417,50 @@ extern "C" __attribute__((visibility("default"))) int srgpt_gemv_multi_nf4_bf16(
   mp.p.nf = *nf4;
   return gemv_multi_modes<gemv::Nf4>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
                                      kv_pages, page_table, page_size, stream);
+}
+
+// T rows of T different sequences in QKV_ROPE mode: row t rotates at pos_rows[t] and appends its K / V through page_tables + t * pt_stride.
+// The arithmetic of every row is that of the one-token srgpt_gemv_*_bf16 call at that position and page table.
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_rows_bf16(const void* x, int ldx, const void* W, int ldw, void* y, int ldy, int T, int N,
+                                                                           int K, const void* norm_weight, float eps, int n_heads, int n_kv_heads,
+                                                                           int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows,
+                                                                           void* kv_pages, const int* page_tables, int pt_stride, int page_size,
+                                                                           void* stream) {
+  SRGPT_CHECK_ARG(W && aligned16(W) && (ldw % 8) == 0 && ldw >= K && pos_rows != nullptr);
+  gemv::MParams mp = {};
+  mp.p.W = reinterpret_cast<const bf16*>(W);
+  mp.p.ldw = ldw;
+  return gemv_multi_modes<gemv::Bf16>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim,
+                                      cos_tab, sin_tab, nullptr, kv_pages, page_tables, page_size, stream, pos_rows, pt_stride);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_rows_packed_bf16(const void* x, int ldx, const srgpt_packed12* packed, void* y, int ldy,
+                                                                                  int T, int N, int K, const void* norm_weight, float eps, int n_heads,
+                                                                                  int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab,
+                                                                                  const int* pos_rows, void* kv_pages, const int* page_tables,
+                                                                                  int pt_stride, int page_size, void* stream) {
+  SRGPT_CHECK_ARG(packed_ok(packed, K) && pos_rows != nullptr);
+#ifdef SRGPT_ELEM_F16
+  return packed_needs_bf16("srgpt_gemv_rows_packed_bf16");
+#else
+  gemv::MParams mp = {};
+  mp.p.pk = *packed;
+  return gemv_multi_modes<gemv::Packed12>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim,
+                                          cos_tab, sin_tab, nullptr, kv_pages, page_tables, page_size, stream, pos_rows, pt_stride);
+#endif
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_gemv_rows_nf4_bf16(const void* x, int ldx, const srgpt_nf4* nf4, void* y, int ldy, int T, int N,
+                                                                               int K, const void* norm_weight, float eps, int n_heads, int n_kv_heads,
+                                                                               int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows,
+                                                                               void* kv_pages, const int* page_tables, int pt_stride, int page_size,
+                                                                               void* stream) {
+  SRGPT_CHECK_ARG(nf4 && nf4->q && nf4->scale && aligned16(nf4->q) && (reinterpret_cast<uintptr_t>(nf4->scale) & 3) == 0 && pos_rows != nullptr);
+  SRGPT_CHECK_ARG(K > 0 && (K % nf4::BATCH) == 0);
+  gemv::MParams mp = {};
+  mp.p.nf = *nf4;
+  return gemv_multi_modes<gemv::Nf4>(mp, x, ldx, y, ldy, T, N, K, norm_weight, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim,
+                                     cos_tab, sin_tab, nullptr, kv_pages, page_tables, page_size, stream, pos_rows, pt_stride);
 }
 
 template <class Fmt>
@@ -1441,5 +1527,20 @@ extern "C" __attribute__((visibility("default"))) int srgpt_spec_accept(const vo
     gemv::spec_copy_logits_kernel<<<dim3(ceil_div(V, 256 * 8), T), 256, 0, st>>>(logits_rows, logits_all, V, state, out_cap);
     SRGPT_CHECK_LAUNCH();
   }
+  return SRGPT_OK;
+}
+
+// The end of a decode step of B sequences: each row's arg max from its lm_head_multi partials in workspace (ids == NULL), or the drawn
+// ids [B]; then out_ids[*step * B + b], x row b = its embedding, ++pos_rows[b], ++*step.
+extern "C" __attribute__((visibility("default"))) int srgpt_rows_advance(const void* workspace, int V, const long long* ids, int B, const void* embed_table,
+                                                                         void* x, int H, long long* out_ids, int* step, int* pos_rows, void* stream) {
+  SRGPT_CHECK_ARG(B >= 1 && B <= gemv::MT_MAX && V > 0 && H > 0 && (H % 8) == 0);
+  SRGPT_CHECK_ARG((workspace || ids) && embed_table && x && out_ids && step && pos_rows && aligned16(embed_table) && aligned16(x));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  gemv::pdl_config(cfg, attr, 1, 256, 0, st);
+  SRGPT_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemv::rows_advance_kernel, reinterpret_cast<const float*>(workspace), gemv::grid_for((V + 1) / 2), ids, B,
+                                      reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(x), H, out_ids, step, pos_rows));
   return SRGPT_OK;
 }

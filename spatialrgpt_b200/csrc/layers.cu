@@ -273,21 +273,64 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_fp
                      page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
 }
 
-// ---- verify pass of prompt-lookup speculative decoding: T tokens through the layer stack, every weight streamed once -----------
+// ---- T-row passes: T rows through the layer stack, every weight streamed once, each row with the arithmetic of a one-token step ------
 // the T-row GEMV of W: over the NF4 planes, else the packing, else the element-type weight
 static int gemv_multi(const MatRef& W, const void* x, int ldx, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps,
-                      const void* residual, int mode, int n_heads, int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos,
-                      void* kv_pages, const int* page_table, int page_size, void* stream) {
+                      const void* residual, int mode, void* stream) {
   if (W.nf != nullptr)
-    return srgpt_gemv_multi_nf4_bf16(x, ldx, W.nf, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab,
-                                     pos, kv_pages, page_table, page_size, stream);
+    return srgpt_gemv_multi_nf4_bf16(x, ldx, W.nf, y, ldy, T, N, K, norm_weight, eps, residual, mode, 0, 0, 0, nullptr, nullptr, nullptr, nullptr,
+                                     nullptr, 0, stream);
   if (W.pk != nullptr)
-    return srgpt_gemv_multi_packed_bf16(x, ldx, W.pk, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab,
-                                        pos, kv_pages, page_table, page_size, stream);
-  return srgpt_gemv_multi_bf16(x, ldx, W.w, K, y, ldy, T, N, K, norm_weight, eps, residual, mode, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
-                               kv_pages, page_table, page_size, stream);
+    return srgpt_gemv_multi_packed_bf16(x, ldx, W.pk, y, ldy, T, N, K, norm_weight, eps, residual, mode, 0, 0, 0, nullptr, nullptr, nullptr, nullptr,
+                                        nullptr, 0, stream);
+  return srgpt_gemv_multi_bf16(x, ldx, W.w, K, y, ldy, T, N, K, norm_weight, eps, residual, mode, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                               stream);
 }
 
+// the T-row QKV + RoPE + KV-append GEMV of W: row t at pos_rows[t], through page_tables + t * pt_stride
+static int gemv_rows(const MatRef& W, const void* x, int ldx, void* y, int ldy, int T, int N, int K, const void* norm_weight, float eps, int n_heads,
+                     int n_kv_heads, int head_dim, const void* cos_tab, const void* sin_tab, const int* pos_rows, void* kv_pages, const int* page_tables,
+                     int pt_stride, int page_size, void* stream) {
+  if (W.nf != nullptr)
+    return srgpt_gemv_rows_nf4_bf16(x, ldx, W.nf, y, ldy, T, N, K, norm_weight, eps, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos_rows, kv_pages,
+                                    page_tables, pt_stride, page_size, stream);
+  if (W.pk != nullptr)
+    return srgpt_gemv_rows_packed_bf16(x, ldx, W.pk, y, ldy, T, N, K, norm_weight, eps, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos_rows,
+                                       kv_pages, page_tables, pt_stride, page_size, stream);
+  return srgpt_gemv_rows_bf16(x, ldx, W.w, K, y, ldy, T, N, K, norm_weight, eps, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos_rows, kv_pages,
+                              page_tables, pt_stride, page_size, stream);
+}
+
+// The layers over the T rows of h [T, H]: row t is at position pos_rows[t] of the sequence whose page table is page_tables + t * pt_stride
+// (pt_stride = 0: T consecutive positions of one sequence, the verify pass).  5 kernels per layer.
+static int rows_layers(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4,
+                       int n_layers, void* q_buf, void* attn_buf, void* act_buf, int T, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                       const void* cos_tab, const void* sin_tab, const int* pos_rows, const int* page_tables, int pt_stride, int page_size,
+                       void* stream) {
+  const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
+  const float scale = 1.0f / sqrtf((float)head_dim);
+  for (int l = 0; l < n_layers; ++l) {
+    const LayerRef w = layer_ref(l, layers, packed, nf4, nullptr);
+    SRGPT_TRY(gemv_rows(w.m[0], h, H, q_buf, qd, T, nqkv, H, w.in_norm, eps, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos_rows, w.kv_pages,
+                        page_tables, pt_stride, page_size, stream));
+    SRGPT_TRY(srgpt_attention_decode_rows_bf16(q_buf, qd, attn_buf, qd, w.kv_pages, page_tables, pt_stride, page_size, pos_rows, T, n_heads, n_kv_heads,
+                                               head_dim, scale, stream));
+    SRGPT_TRY(gemv_multi(w.m[1], attn_buf, qd, h, H, T, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, stream));
+    SRGPT_TRY(gemv_multi(w.m[2], h, H, act_buf, I, T, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, stream));
+    SRGPT_TRY(gemv_multi(w.m[3], act_buf, I, h, H, T, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, stream));
+  }
+  return SRGPT_OK;
+}
+
+// final norm + lm_head over the T rows: fp32 logits [T, V] (optional) and every row's arg max partials in lm_workspace
+static int lm_head_rows(const void* h, int T, int H, float eps, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+                        float* logits_rows, void* lm_workspace, void* stream) {
+  if (packed_or_null(lm_packed) != nullptr)
+    return srgpt_lm_head_multi_packed_bf16(h, H, lm_packed, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream);
+  return srgpt_lm_head_multi_bf16(h, H, lm_head, H, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream);
+}
+
+// verify pass of prompt-lookup speculative decoding: the draft writes pos_rows[t] = *pos + t, the rows pass runs over the one page table
 static int verify_step(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4,
                        int n_layers, void* q_buf, void* attn_buf, void* act_buf, int T, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
                        const void* cos_tab, const void* sin_tab, int* pos, int* pos_rows, const int* page_table, int page_size, const void* final_norm,
@@ -297,26 +340,10 @@ static int verify_step(void* h, const srgpt_llama_layer_weights* layers, const s
   SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos && pos_rows && page_table && final_norm && lm_head && lm_workspace && out_ids &&
                   step && state && draft_ids);
   SRGPT_CHECK_ARG(logits_all == nullptr || logits_rows != nullptr);
-  const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
-  const float scale = 1.0f / sqrtf((float)head_dim);
   SRGPT_TRY(srgpt_spec_draft(prompt_ids, prompt_len, out_ids, step, pos, pos_rows, T, ngram, embed_table, h, H, draft_ids, state, stream));
-  for (int l = 0; l < n_layers; ++l) {
-    const LayerRef w = layer_ref(l, layers, packed, nf4, nullptr);
-    SRGPT_TRY(gemv_multi(w.m[0], h, H, q_buf, qd, T, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab,
-                         pos, w.kv_pages, page_table, page_size, stream));
-    SRGPT_TRY(srgpt_attention_decode_multi_bf16(q_buf, qd, attn_buf, qd, w.kv_pages, page_table, page_size, pos_rows, T, n_heads, n_kv_heads, head_dim,
-                                                scale, stream));
-    SRGPT_TRY(gemv_multi(w.m[1], attn_buf, qd, h, H, T, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
-                         stream));
-    SRGPT_TRY(gemv_multi(w.m[2], h, H, act_buf, I, T, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, 0, 0, 0, nullptr, nullptr, nullptr, nullptr,
-                         nullptr, 0, stream));
-    SRGPT_TRY(gemv_multi(w.m[3], act_buf, I, h, H, T, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
-                         stream));
-  }
-  if (packed_or_null(lm_packed) != nullptr)
-    SRGPT_TRY(srgpt_lm_head_multi_packed_bf16(h, H, lm_packed, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream));
-  else
-    SRGPT_TRY(srgpt_lm_head_multi_bf16(h, H, lm_head, H, T, V, H, final_norm, eps, logits_rows, lm_workspace, stream));
+  SRGPT_TRY(rows_layers(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, T, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos_rows,
+                        page_table, 0, page_size, stream));
+  SRGPT_TRY(lm_head_rows(h, T, H, eps, final_norm, lm_head, lm_packed, V, logits_rows, lm_workspace, stream));
   return srgpt_spec_accept(lm_workspace, V, T, draft_ids, out_ids, out_cap, step, pos, state, logits_rows, logits_all, stream);
 }
 
@@ -352,4 +379,60 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_verify_step_nf
   return verify_step(h, layers, nullptr, nf4, n_layers, q_buf, attn_buf, act_buf, T, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
                      pos_rows, page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows, logits_all, prompt_ids,
                      prompt_len, ngram, draft_ids, out_ids, out_cap, step, state, stream);
+}
+
+// ---- decode step of B sequences, each with exactly the arithmetic of its one-token step ---------------------------------------------
+// Row b of h [B, H] is the newest token of the sequence at position pos_rows[b] with page table page_tables + b * pt_stride.  The rows
+// pass, then lm_head over the B rows and the advance: greedy (seeds == NULL) the arg max of each row; sampled, row b draws from its fp32
+// logits row with seeds[b] at counter *step (srgpt_sample_rows into ids [B]).  Token b goes to out_ids[*step * B + b], h row b becomes its
+// embedding, pos_rows[b] and then *step advance.
+static int decode_rows(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4,
+                       int n_layers, void* q_buf, void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                       const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size,
+                       const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
+                       float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids, long long* out_ids, int* step,
+                       void* stream) {
+  SRGPT_CHECK_ARG(B >= 1 && B <= SRGPT_SPEC_T_MAX && pt_stride > 0);
+  SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos_rows && page_tables && final_norm && lm_head && embed_table && lm_workspace &&
+                  out_ids && step);
+  SRGPT_CHECK_ARG(seeds == nullptr || (sample_params && ids && logits_rows));
+  SRGPT_TRY(rows_layers(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                        pos_rows, page_tables, pt_stride, page_size, stream));
+  SRGPT_TRY(lm_head_rows(h, B, H, eps, final_norm, lm_head, lm_packed, V, logits_rows, lm_workspace, stream));
+  if (seeds != nullptr) SRGPT_TRY(srgpt_sample_rows(logits_rows, 1, V, B, V, sample_params, seeds, step, 0, ids, stream));
+  return srgpt_rows_advance(lm_workspace, V, seeds != nullptr ? ids : nullptr, B, embed_table, h, H, out_ids, step, pos_rows, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads,
+    int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size,
+    const void* final_norm, const void* lm_head, int V, const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params,
+    const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, void* stream) {
+  return decode_rows(h, layers, nullptr, nullptr, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                     pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, nullptr, V, embed_table, lm_workspace, logits_rows, sample_params,
+                     seeds, ids, out_ids, step, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_packed_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, int n_layers, void* q_buf, void* attn_buf, void* act_buf,
+    int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos_rows,
+    const int* page_tables, int pt_stride, int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+    const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
+    long long* out_ids, int* step, void* stream) {
+  SRGPT_CHECK_ARG(packed != nullptr);
+  return decode_rows(h, layers, packed, nullptr, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                     pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
+                     sample_params, seeds, ids, out_ids, step, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_nf4_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf, void* attn_buf, void* act_buf,
+    int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos_rows,
+    const int* page_tables, int pt_stride, int page_size, const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V,
+    const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
+    long long* out_ids, int* step, void* stream) {
+  SRGPT_CHECK_ARG(nf4 != nullptr);
+  return decode_rows(h, layers, nullptr, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                     pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
+                     sample_params, seeds, ids, out_ids, step, stream);
 }

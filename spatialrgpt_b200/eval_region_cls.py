@@ -24,7 +24,7 @@ import torch
 
 from .constants import DEFAULT_IMAGE_TOKEN, IMAGE_TOKEN_INDEX
 from .conversation import conv_templates
-from .eval_spatial import clean_output, get_chunk, pad_to_square, rle_decode, stop_string
+from .eval_spatial import check_batch_size, clean_output, generate_invariant, get_chunk, pad_to_square, rle_decode, stop_string
 from .mm_utils import _mask_processor, get_model_name_from_path, process_images, tokenizer_image_token
 
 PROMPTS = [  # eval_region_cls.py:22-38 (data: the question pool of the benchmark)
@@ -168,6 +168,8 @@ def candidate_ids(conv, names: List[str], tokenizer, prompt_ids) -> List[List[in
 
 def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
     """eval_region_cls.py:277-349.  ``loader`` defaults to ``load_pretrained_model``."""
+    batch_size = int(getattr(args, "batch_size", 1) or 1)
+    check_batch_size(batch_size, **{"--num_beams > 1": args.num_beams > 1, "--score-categories": getattr(args, "score_categories", False)})
     if loader is None:
         from .builder import load_pretrained_model as loader
     model_path = os.path.expanduser(args.model_path)
@@ -188,7 +190,28 @@ def eval_model(args, loader=None, seed: Optional[int] = None) -> int:
     names = category_names(args.annotation_file) if getattr(args, "score_categories", False) else None
     tails = {}  # prompt text -> the names' candidate ids
     n = 0
+    gen_kw = dict(do_sample=args.temperature > 0, temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams, max_new_tokens=64,
+                  use_cache=True)
+
+    def record(line, text):
+        return {"question_id": line["image"], "text": text, "gt_name": line["category_name"], "score": line["score"], "bbox": line["bbox"],
+                "image_id": line["image_id"], "model_id": model_name, "metadata": {}}
+
     with open(answers_file, "w") as out:
+        if batch_size > 1:
+            # --batch-size N: N consecutive samples per generate(batch_invariant=True) call (the prompts drawn in the same order)
+            for g in range(0, len(data), batch_size):
+                lines = data[g:g + batch_size]
+                samples = [build_sample(line, tokenizer, image_processor, model.config, args.conv_mode, args.dataset, args.prompt_type,
+                                        args.image_folder, rng) for line in lines]
+                seed = {"seed": [torch.initial_seed()] * len(lines)} if args.temperature > 0 else {}  # batch 1 draws with the default seed
+                outs = generate_invariant(model, [ids.unsqueeze(0) for ids, _, _ in samples], torch.cat([im for _, im, _ in samples]).to(dev, dtype=model.dtype),
+                                          None, [m.to(dev, dtype=model.dtype) for _, _, m in samples], **gen_kw, **seed)
+                for line, output_ids in zip(lines, outs):
+                    out.write(json.dumps(record(line, clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop))) + "\n")
+                    n += 1
+                out.flush()
+            return n
         for line in data:
             input_ids, images, masks, conv = build_sample(line, tokenizer, image_processor, model.config, args.conv_mode, args.dataset,
                                                           args.prompt_type, args.image_folder, rng, return_conv=True)
@@ -235,6 +258,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
                    help="with --quantization nf4: keep only the 4-bit planes of the layer matrices, no dequantized copy (same answers)")
     p.add_argument("--score-categories", action="store_true",
                    help="answer with the category name of the highest likelihood under the prompt (model.score) instead of generating")
+    p.add_argument("--batch-size", type=int, default=1,
+                   help="answer this many consecutive samples in one generate(batch_invariant=True) call (same answers file)")
     return p
 
 

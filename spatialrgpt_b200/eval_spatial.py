@@ -251,10 +251,75 @@ def answer_questions(line: Dict[str, Any], model, tokenizer, image_processor, im
     return records
 
 
+def check_batch_size(batch_size: int, **refused) -> None:
+    """--batch-size N > 1 answers N annotations per generate(batch_invariant=True) call; the options in ``refused`` (flag name -> whether
+    it is on) have no batch-invariant form and are refused with it."""
+    if batch_size < 1:
+        raise ValueError(f"--batch-size must be at least 1, got {batch_size}")
+    on = [name for name, v in refused.items() if v]
+    if batch_size > 1 and on:
+        raise ValueError(f"--batch-size > 1 cannot be combined with {', '.join(on)}")
+
+
+def generate_invariant(model, prompts: Sequence[torch.Tensor], images: torch.Tensor, depths: Optional[torch.Tensor], masks, **kw) -> List[torch.Tensor]:
+    """generate(batch_invariant=True) over prompts [1, T_b] (one image each, the images [B, 3, R, R], depths the same or None, masks one
+    [n_b, R, R] or None per prompt): returns each prompt's ids [1, n_b], equal to a batch-1 generate() of it with the same kwargs.  The
+    prompts are right-padded under an attention mask; the result rows are padded with -1, which no token id is, and cut there."""
+    T = max(int(p.shape[1]) for p in prompts)
+    ids = torch.zeros((len(prompts), T), dtype=torch.int64)
+    am = torch.zeros((len(prompts), T), dtype=torch.int64)
+    for b, p in enumerate(prompts):
+        ids[b, :p.shape[1]] = p[0].cpu()
+        am[b, :p.shape[1]] = 1
+    mask_list = None if all(m is None for m in masks) else list(masks)
+    dev = model.device
+    out = model.generate(ids.to(dev), attention_mask=am.to(dev), images=images, depths=depths, masks=mask_list, batch_invariant=True,
+                         pad_token_id=-1, **kw)
+    return [row[row >= 0][None] for row in out]
+
+
+def answer_questions_batch(items: Sequence[Dict[str, Any]], model, tokenizer, image_processor, conv_mode: str, model_name: str,
+                           max_new_tokens: int = 128, temperature: float = 0.0, top_p=None) -> List[List[Dict[str, Any]]]:
+    """answer_questions for several annotations at once: turn i of every annotation that has one is answered by one
+    generate(batch_invariant=True) call, each annotation keeping its own conversation.  items: dicts with line, image, depth, masks and
+    image_file.  Returns each annotation's records, equal to what answer_questions writes for it."""
+    dev = model.device
+    imgs = [process_images([it["image"]], image_processor, model.config).to(dev, dtype=model.dtype) for it in items]
+    dps = [None if it["depth"] is None else process_images([it["depth"]], image_processor, model.config).to(dev, dtype=model.dtype) for it in items]
+    convs = [conv_templates[conv_mode].copy() for _ in items]
+    stop = stop_string(conv_mode)
+    records: List[List[Dict[str, Any]]] = [[] for _ in items]
+    turns = [len(it["line"]["conversations"]) // 2 for it in items]
+    kw = dict(do_sample=temperature > 0, temperature=temperature, top_p=top_p, num_beams=1, max_new_tokens=max_new_tokens, use_cache=True)
+    for i in range(max(turns, default=0)):
+        live = [b for b in range(len(items)) if turns[b] > i]
+        prompts = []
+        for b in live:
+            it, conv = items[b], convs[b]
+            q = it["line"]["conversations"][i * 2]["value"]
+            conv.append_message(conv.roles[0], question_with_depth_tokens(q) if it["depth"] is not None else q)
+            conv.append_message(conv.roles[1], None)
+            prompts.append(tokenizer_image_token(conv.get_prompt(), tokenizer, IMAGE_TOKEN_INDEX, return_tensors="pt").unsqueeze(0))
+        seed = {"seed": [torch.initial_seed()] * len(live)} if temperature > 0 else {}  # batch 1 draws with the default seed
+        outs = generate_invariant(model, prompts, torch.cat([imgs[b] for b in live]),
+                                  None if dps[live[0]] is None else torch.cat([dps[b] for b in live]),
+                                  [None if items[b]["masks"] is None else items[b]["masks"].to(dev, dtype=model.dtype) for b in live], **kw, **seed)
+        for b, output_ids in zip(live, outs):
+            line = items[b]["line"]
+            pred = clean_output(tokenizer.batch_decode(output_ids, skip_special_tokens=True)[0], stop)
+            records[b].append({"question_id": line["id"], "image": items[b]["image_file"], "question": line["text_q"], "pred": pred,
+                               "gt": line["conversations"][i * 2 + 1]["value"], "model_id": model_name, "qa_info": line["qa_info"]})
+    return records
+
+
 def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tensor]] = None, loader=None) -> int:
     """Reference ``eval_model`` (eval_spatial.py:109-260).  ``loader`` defaults to ``load_pretrained_model``;
     ``depth_predictor`` is the external depth network (None: the depth branch gets no input)."""
     from PIL import Image
+    batch_size = int(getattr(args, "batch_size", 1) or 1)
+    check_batch_size(batch_size, **{"--prefix-cache": getattr(args, "prefix_cache", False),
+                                    "--prompt-lookup-num-tokens": getattr(args, "prompt_lookup_num_tokens", 0),
+                                    "--num_beams > 1": args.num_beams > 1})
     if loader is None:
         from .builder import load_pretrained_model as loader
     model_path = os.path.expanduser(args.model_path)
@@ -284,20 +349,31 @@ def eval_model(args, depth_predictor: Optional[Callable[[np.ndarray], torch.Tens
     mask_proc = _mask_processor(image_processor)
     n = 0
     with open(answers_file, "w") as out:
-        for line in questions:
-            image_file = line["image_info"]["file_path"]
-            region_masks = regions_for_line(line, args.use_mask, pad)
-            # eval_spatial.py:183-190: the image processor without normalisation / rescaling, one [1, R, R] slice per region
-            masks = (torch.vstack([mask_proc.preprocess(m[None, ...], return_tensors="pt")["pixel_values"][0] for m in region_masks]).float()
-                     if region_masks else None)
-            image = Image.open(os.path.join(args.image_folder, image_file)).convert("RGB")
-            depth = depth_image(np.array(image), depth_predictor) if depth_predictor is not None else None
-            for rec in answer_questions(line, model, tokenizer, image_processor, image, depth, masks, args.conv_mode, model_name, image_file,
-                                        temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams,
-                                        prefix_cache=getattr(args, "prefix_cache", False),
-                                        prompt_lookup_num_tokens=getattr(args, "prompt_lookup_num_tokens", 0)):
-                out.write(json.dumps(rec) + "\n")
-                n += 1
+        # --batch-size N: N consecutive annotations at a time, their records written in the original order
+        for g in range(0, len(questions), batch_size):
+            items = []
+            for line in questions[g:g + batch_size]:
+                image_file = line["image_info"]["file_path"]
+                region_masks = regions_for_line(line, args.use_mask, pad)
+                # eval_spatial.py:183-190: the image processor without normalisation / rescaling, one [1, R, R] slice per region
+                masks = (torch.vstack([mask_proc.preprocess(m[None, ...], return_tensors="pt")["pixel_values"][0] for m in region_masks]).float()
+                         if region_masks else None)
+                image = Image.open(os.path.join(args.image_folder, image_file)).convert("RGB")
+                depth = depth_image(np.array(image), depth_predictor) if depth_predictor is not None else None
+                items.append(dict(line=line, image=image, depth=depth, masks=masks, image_file=image_file))
+            if batch_size == 1:
+                it = items[0]
+                groups = [answer_questions(it["line"], model, tokenizer, image_processor, it["image"], it["depth"], it["masks"], args.conv_mode,
+                                           model_name, it["image_file"], temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams,
+                                           prefix_cache=getattr(args, "prefix_cache", False),
+                                           prompt_lookup_num_tokens=getattr(args, "prompt_lookup_num_tokens", 0))]
+            else:
+                groups = answer_questions_batch(items, model, tokenizer, image_processor, args.conv_mode, model_name, temperature=args.temperature,
+                                                top_p=args.top_p)
+            for recs in groups:
+                for rec in recs:
+                    out.write(json.dumps(rec) + "\n")
+                    n += 1
     return n
 
 
@@ -322,6 +398,8 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--prompt-lookup-num-tokens", type=int, default=0,
                    help="greedy decoding by prompt lookup: draft up to this many tokens per verify pass (0 = off; same answers)")
     p.add_argument("--allow-no-depth", action="store_true", help="run an enable_depth checkpoint without a depth network (degraded answers)")
+    p.add_argument("--batch-size", type=int, default=1,
+                   help="answer turn i of this many consecutive annotations in one generate(batch_invariant=True) call (same answers file)")
     p.add_argument("--quantization", choices=["nf4", "fp8"], default=None,
                    help="quantization of the LLM's layer matrices: NF4 weight-only, or FP8 (E4M3) weights and activations")
     p.add_argument("--nf4-planes-only", action="store_true",

@@ -318,7 +318,7 @@ class LlamaDecoder:
             raise ValueError("SRGPT_DECODE_NF4=0 runs the decode step over the dequantized copies, which a model loaded with "
                              "nf4_dequantized_copy=False does not keep")
         # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
-        # ("verify", T, ngram), ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B); the
+        # ("verify", T, ngram), ("rows", B, sample) for the batch-invariant rows step, ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B); the
         # graphs that write output_scores rows end in ("scores", buffer address, step stride) (_scores_key).  A graph holds the addresses of every buffer it reads, so it is
         # dropped whenever one of them is replaced: the KV cache and the layer stack's array (ensure_capacity), the processor spec (_set_processors)
         # and the batched-decode buffers (_batch_state).
@@ -357,9 +357,11 @@ class LlamaDecoder:
     supports_logits_processors = True
     supports_batch_sampling = True  # sampled batches run in the batched step (generate_batch), num_return_sequences included
     supports_output_scores = True  # generate(output_scores=True): the decode steps write each token's score row on the device
+    supports_batch_invariant = True  # generate(batch_invariant=True): generate_rows, each row bit-identical to batch 1
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
+    _rstate = None  # buffers of the batch-invariant rows step (generate_rows), allocated on first use
     _scores = None  # the score buffer of output_scores (_scores_view), allocated on first use
     _host_ids = None  # pinned host copy of generated ids for the stop checks, and the stream that fills it (_pinned_ids)
     _copy_stream = None
@@ -1009,6 +1011,117 @@ class LlamaDecoder:
         n = min(n, max_new_tokens)
         res = out2d[:n].t().contiguous()
         return [res[b, : (stopped[b] if stopped[b] is not None else n)].clone() for b in range(B)]
+
+    # ---- batch-invariant decoding: up to SPEC_T_MAX sequences per weight pass, each bit-identical to its batch-1 generate_from_embeds --
+    def _rows_state(self):
+        """Buffers of the rows step (llama_decode_rows), sized for SPEC_T_MAX rows once, so a captured graph of B rows stays valid."""
+        st = self._rstate
+        if st is not None:
+            return st
+        d, dev, R = self.dims, self.device, ops.SPEC_T_MAX
+        H, qd, I = d.hidden_size, d.num_attention_heads * d.head_dim, d.intermediate_size
+        z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
+        st = dict(h=z(R, H), q=z(R, qd), attn=z(R, qd), act=z(R, I), ws=z(R * self.lm_ws.numel(), dtype=torch.uint8),
+                  logits=z(R, d.vocab_size, dtype=torch.float32), pos=z(R, dtype=torch.int32), step=z(1, dtype=torch.int32),
+                  out=z(self.out_ids.numel() * R, dtype=torch.int64), seeds=z(R, dtype=torch.int64), ids=z(R, dtype=torch.int64))
+        self._rstate = st
+        return st
+
+    def _rows_step_launch(self, B: int, sample: bool) -> None:
+        d, w, st = self.dims, self.w, self._rstate
+        ops.llama_decode_rows(st["h"][:B], self.stack, st["q"][:B], st["attn"][:B], st["act"][:B], B, d, self.cos, self.sin, st["pos"],
+                              self.cache.page_tables, PAGE_SIZE, w.norm, w.lm_head, w.embed, st["ws"], st["out"], st["step"], st["logits"],
+                              **(dict(sample_params=self.sample_params, seeds=st["seeds"], ids=st["ids"]) if sample else {}))
+
+    @torch.no_grad()
+    @ops.in_own_dtype
+    def generate_rows(self, embeds_list: List[torch.Tensor], max_new_tokens, eos_token_ids=None, stopping_fn=None, use_graph: bool = True,
+                      return_logits: bool = False, sampling=None, seeds: Optional[List[int]] = None):
+        """Decode B <= SPEC_T_MAX prompts (embeddings [S_b, H] each) together, row b bit-identical to ``generate_from_embeds(embeds_list[b],
+        max_new_tokens[b], ..., sampling=dict(sampling, seed=seeds[b]))``: each prompt is prefilled and gets its first token with the
+        calls batch 1 makes, then every step runs the rows step (llama_decode_rows), which streams each weight once for all rows and
+        gives each row the arithmetic of its one-token step.  ``max_new_tokens``: one budget, or one per row.  EOS and ``stopping_fn``
+        are checked per row; a row that has stopped stays in the step and its results are ignored.  Returns a list of B LongTensors
+        (and a list of B fp32 logits [n_b, V] when return_logits)."""
+        d, w, B = self.dims, self.w, len(embeds_list)
+        if self.fp8:
+            raise NotImplementedError("batch-invariant decoding has no FP8 form (the rows step is a 16-bit, packed or NF4 GEMV)")
+        if not 1 <= B <= ops.SPEC_T_MAX:
+            raise ValueError(f"generate_rows decodes 1 .. {ops.SPEC_T_MAX} prompts at once, got {B}")
+        budgets = [int(max_new_tokens)] * B if isinstance(max_new_tokens, int) else [int(m) for m in max_new_tokens]
+        if len(budgets) != B or min(budgets) < 1:
+            raise ValueError("generate_rows needs one budget of at least 1 token per prompt")
+        sample = bool(sampling)
+        if sample and (seeds is None or len(seeds) != B):
+            raise ValueError("sampled generate_rows needs one seed per prompt")
+        lens, mx = [int(e.shape[0]) for e in embeds_list], max(budgets)
+        if mx > self.out_ids.numel():
+            raise RuntimeError(f"max_new_tokens {mx} exceeds the decoder's cap {self.out_ids.numel()}")
+        if max(lens) + mx > self.max_seq_len:  # every row stays in the step until the last one stops
+            raise RuntimeError(f"{max(lens)} prompt + {mx} new tokens exceed max_seq_len {self.max_seq_len}")
+        eos = eos_list(eos_token_ids)
+        for b in range(len(self.cache.owned)):
+            self.cache.release(b)
+        self.ensure_capacity(B, max(lens) + mx)
+        self._set_sampling(sampling)
+        st = self._rows_state()
+        logits = [torch.empty((mx, d.vocab_size), dtype=torch.float32, device=self.device) for _ in range(B)] if return_logits else None
+        for b, emb in enumerate(embeds_list):  # generate_from_embeds' prefill and first token, into sequence b
+            S = lens[b]
+            self.cache.reserve(b, S + mx)
+            hidden = self.prefill_hidden(emb, b, 0)
+            self.pos.fill_(S - 1)
+            self.step.zero_()
+            if sample:
+                self._set_seed(int(seeds[b]))
+            first_logits = logits[b][0] if logits is not None else (self._sample_buffer() if sample else None)
+            ops.lm_head_argmax(hidden[S - 1], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
+                               embed_table=w.embed, next_x=self.h, logits_out=first_logits)
+            self._choose(first_logits, sample, False, None)
+            st["out"][b:b + 1].copy_(self.out_ids[:1])
+            st["h"][b].copy_(self.h)
+        st["pos"][:B].copy_(torch.tensor(lens, dtype=torch.int32))
+        st["step"].fill_(1)
+        if sample:
+            st["seeds"][:B].copy_(torch.tensor([int(s) & SEED_MASK for s in seeds], dtype=torch.int64))
+        key = ("rows", B, sample)
+        graph = use_graph and logits is None
+        if graph:
+            self._capture(key, lambda: self._rows_step_launch(B, sample), (st["h"], st["pos"], st["step"], st["out"]),
+                          self.stack.rows_kernels + (1 if sample else 0))
+        need_check = bool(eos) or stopping_fn is not None
+        out2d = st["out"][: mx * B].view(mx, B)
+        if need_check:
+            host = self._pinned_ids(mx * B).view(mx, B)
+            cols = [host[:, b] for b in range(B)]
+            copied = self._to_host((out2d[0], host[0]))
+        stopped = [None] * B
+        n = 1
+        while n < mx:
+            if graph:
+                self._replay(key)
+            else:
+                self._rows_step_launch(B, sample)
+                if logits is not None:
+                    for b in range(B):
+                        logits[b][n].copy_(st["logits"][b])
+            if need_check:  # inspect row n-1 of every sequence while row n is being computed
+                nxt = self._to_host((out2d[n], host[n]))
+                copied.synchronize()
+                for b in range(B):
+                    if stopped[b] is None:
+                        stopped[b] = first_stop(cols[b], n - 1, n, eos, stopping_fn, budgets[b])
+                copied = nxt
+                if all(s is not None for s in stopped):
+                    break
+            n += 1
+        n = min(n, mx)
+        res = out2d[:n].t().contiguous()
+        lens_out = [stopped[b] if stopped[b] is not None else min(n, budgets[b]) for b in range(B)]
+        outs = [res[b, :lens_out[b]].clone() for b in range(B)]
+        if logits is not None:
+            return outs, [logits[b][:lens_out[b]] for b in range(B)]
+        return outs
 
     @torch.no_grad()
     @ops.in_own_dtype

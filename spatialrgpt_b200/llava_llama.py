@@ -14,7 +14,7 @@ import torch
 from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
-from .llama_decoder import LlamaDecoder, check_candidates
+from .llama_decoder import LlamaDecoder, check_candidates, sequence_seeds
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
@@ -68,6 +68,32 @@ class GenerateBeamDecoderOnlyOutput:
     attentions: Any = None
     hidden_states: Any = None
     past_key_values: Any = None
+
+
+def refuse_batch_invariant(num_beams: int = 1, processors=None, lookup_k: int = 0, prefix_cache: bool = False, n_ret: int = 1,
+                           output_scores: bool = False, llm=None) -> None:
+    """The generate() options batch_invariant=True does not serve: raises NotImplementedError before any GPU work."""
+    if num_beams != 1:
+        raise NotImplementedError("batch_invariant=True with beam search")
+    if processors is not None:
+        raise NotImplementedError("batch_invariant=True with logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length)")
+    if lookup_k:
+        raise NotImplementedError("batch_invariant=True with prompt_lookup_num_tokens")
+    if prefix_cache:
+        raise NotImplementedError("batch_invariant=True with prefix_cache=True")
+    if n_ret != 1:
+        raise NotImplementedError("batch_invariant=True with num_return_sequences > 1")
+    if output_scores:
+        raise NotImplementedError("batch_invariant=True with output_scores")
+    if llm is not None and getattr(llm, "fp8", False):
+        raise NotImplementedError("batch_invariant=True with quantization='fp8' (the rows step has no FP8 form)")
+    if llm is not None and not getattr(llm, "supports_batch_invariant", False):
+        raise NotImplementedError("batch_invariant=True on the tensor-parallel decoder")
+
+
+def batch_invariant_groups(B: int, size: int):
+    """The (first, end) prompt ranges generate(batch_invariant=True) decodes one after another: groups of `size`, the last one shorter."""
+    return [(lo, min(lo + size, B)) for lo in range(0, B, size)]
 
 
 def compute_transition_scores(sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None, normalize_logits: bool = False,
@@ -585,6 +611,11 @@ class LlavaLlamaModel:
                 raise NotImplementedError("num_return_sequences > 1 with output_logits")
             if not getattr(type(self.llm), "supports_batch_sampling", False):
                 raise NotImplementedError("num_return_sequences > 1 on the tensor-parallel decoder (it does not sample)")
+        # batch_invariant=True (opt-in): row b of the result, ids and output_logits, equals bit for bit generate() of prompt b alone with the
+        # same kwargs.  Each prompt runs the encoders and the prefill batch 1 runs; then up to ops.SPEC_T_MAX prompts decode together in
+        # the rows step (LlamaDecoder.generate_rows), which streams each weight once and gives every row its one-token arithmetic.
+        # ``seed`` may be a list of one seed per prompt; a scalar seed gives prompt b the seed sequence_seeds(seed, B)[b].
+        batch_invariant = bool(generation_kwargs.pop("batch_invariant", False))
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
         # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
@@ -619,6 +650,20 @@ class LlavaLlamaModel:
             raise NotImplementedError("beam search on the tensor-parallel decoder")
         if output_scores and not getattr(self.llm, "supports_output_scores", False):
             raise NotImplementedError("output_scores on the tensor-parallel decoder (its logits are vocabulary-parallel: no rank holds a whole row)")
+        n_prompts = 1 if input_ids is None else int(input_ids.shape[0])
+        if isinstance(seed, (list, tuple)):
+            if not batch_invariant:
+                raise ValueError("a list of seeds needs batch_invariant=True")
+            if len(seed) != n_prompts:
+                raise ValueError(f"seed holds {len(seed)} seeds for {n_prompts} prompts")
+        if batch_invariant:
+            refuse_batch_invariant(num_beams=num_beams, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache, n_ret=n_ret,
+                                   output_scores=output_scores, llm=self.llm)
+            if isinstance(seed, (list, tuple)) and sampling is not None:
+                sampling["seed"] = int(seed[0]) if n_prompts == 1 else None
+            if n_prompts > 1:
+                return self._generate_batch_invariant(input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id,
+                                                      stopping_criteria, pad_token_id, use_graph, return_logits, return_dict, sampling, seed)
         prefix = None
         if prefix_cache:
             if input_ids is None or input_ids.shape[0] != 1:
@@ -726,6 +771,64 @@ class LlavaLlamaModel:
             seqs[b, : o.numel()] = o
         if return_dict:
             return self._generate_output(seqs, extra, all_logits if return_logits else None, num_beams != 1)
+        if return_logits:
+            return seqs, all_logits
+        return seqs
+
+    def _generate_batch_invariant(self, input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id, stopping_criteria,
+                                  pad_token_id, use_graph: bool, return_logits: bool, return_dict: bool, sampling, seed):
+        """generate(batch_invariant=True) over B > 1 prompts: every prompt's embeddings by the calls a batch-1 generate() of it makes (its
+        unpadded ids; its images, depth images and masks), then groups of at most ops.SPEC_T_MAX prompts through generate_rows."""
+        B, dev = int(input_ids.shape[0]), self.device
+        am = None if attention_mask is None else attention_mask.bool().cpu()
+        ids_rows = [input_ids[b] if am is None else input_ids[b][am[b].to(input_ids.device)] for b in range(B)]
+        if images is not None:
+            counts = [int((r == IMAGE_TOKEN_INDEX).sum()) for r in ids_rows]
+            all_images = self._stack_images(images)
+            all_depths = None if depths is None else self._stack_images(depths)
+            mask_list = (list(masks) if masks is not None else []) + [None] * all_images.shape[0]
+            embeds, off = [], 0
+            for b, ids in enumerate(ids_rows):
+                k = counts[b]
+                m = mask_list[off:off + k]
+                m = None if all(x is None for x in m) else m  # a prompt without regions is called as batch 1 calls it: masks=None
+                self.prepare_inputs_labels_for_multimodal(ids[None], None, None, None, None, all_images[off:off + k],
+                                                          m, None if all_depths is None else all_depths[off:off + k], _packed_only=True)
+                embeds.append(self._last_packed[0])
+                off += k
+        else:
+            embeds = [self.llm.embed_tokens(ids) for ids in ids_rows]  # [n_b, H]
+        lens = [int(e.shape[0]) for e in embeds]
+        if max_new_tokens is not None:
+            budgets = [int(max_new_tokens)] * B
+        else:
+            budgets = [20 if max_length is None else max(int(max_length) - n, 1) for n in lens]  # each row's own prompt length
+        seeds = None
+        if sampling is not None:
+            if isinstance(seed, (list, tuple)):
+                seeds = [int(s) for s in seed]
+            else:
+                seeds = sequence_seeds(torch.initial_seed() if seed is None else int(seed), B)
+            sampling = dict(sampling, seed=None)
+        stop_fn = None
+        if stopping_criteria:
+            def stop_fn(ids, _sc=stopping_criteria):
+                return any(bool(c(ids[None], None)) for c in _sc)
+        outs, all_logits = [], []
+        for lo, hi in batch_invariant_groups(B, ops.SPEC_T_MAX):
+            r = self.llm.generate_rows(embeds[lo:hi], budgets[lo:hi], eos_token_ids=eos_token_id, stopping_fn=stop_fn, use_graph=use_graph,
+                                       return_logits=return_logits, sampling=sampling, seeds=None if seeds is None else seeds[lo:hi])
+            if return_logits:
+                r, lg = r
+                all_logits.extend(lg)
+            outs.extend(r)
+        pad = pad_token_id if pad_token_id is not None else (self.config.llama.pad_token_id or 0)
+        n_max = max(o.numel() for o in outs)
+        seqs = torch.full((B, n_max), int(pad), dtype=torch.int64, device=dev)
+        for b, o in enumerate(outs):
+            seqs[b, : o.numel()] = o
+        if return_dict:
+            return self._generate_output(seqs, None, all_logits if return_logits else None, False)
         if return_logits:
             return seqs, all_logits
         return seqs

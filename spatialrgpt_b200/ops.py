@@ -1110,6 +1110,7 @@ class LlamaStack:
         self.kernels_per_layer = 12 if self.quantizes_activations else 8
         self.step_kernels = 5 * self.n + 2
         self.verify_kernels = 5 * self.n + 3
+        self.rows_kernels = 5 * self.n + 2  # + 1 when the rows are sampled
         self.set_pages(kv_pages)
 
     def set_pages(self, kv_pages) -> None:
@@ -1133,13 +1134,16 @@ class LlamaStack:
 
     def entry(self, op: str):
         """(symbol, layer array arguments, lm_head packing arguments) of srgpt_llama_<op>_*, op = "prefill_layers",
-        "prefill_chunk_layers", "decode_step" or "verify_step".  Prefill takes the FP8 or, planes-only, the NF4 stack; the decode step
-        streams FP8, NF4 or packed matrices when there are some; the verify pass NF4 planes-only or packed ones."""
-        step = op in ("decode_step", "verify_step")
-        nf4 = self.nf4 if op == "decode_step" else self.planes
+        "prefill_chunk_layers", "decode_step", "verify_step" or "decode_rows".  Prefill takes the FP8 or, planes-only, the NF4 stack; the
+        decode step and the rows step stream FP8 (the step only), NF4 or packed matrices when there are some; the verify pass NF4
+        planes-only or packed ones."""
+        step = op in ("decode_step", "verify_step", "decode_rows")
+        nf4 = self.nf4 if op in ("decode_step", "decode_rows") else self.planes
         if self.quantizes_activations:
             if op == "verify_step":
                 raise SrgptError("the verify pass of prompt-lookup decoding has no FP8 form")
+            if op == "decode_rows":
+                raise SrgptError("the batch-invariant decode step has no FP8 form")
             fmt, arrays = "fp8_", (self.layers,)
         elif nf4 is not None:
             fmt, arrays = "nf4_", (self.layers, nf4)
@@ -1345,3 +1349,62 @@ def llama_verify_step(h, stack: LlamaStack, q_buf, attn_buf, act_buf, T: int, di
                                      _p(lm_head), *lm, dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(logits_all), _p(prompt_ids),
                                      _p(prompt_len), ngram, _p(draft_ids), _p(out_ids), out_ids.numel(), _p(step), _p(state), _stream()), name)
     _count(stack.verify_kernels + (1 if logits_all is not None else 0))
+
+
+# ------------------------------------------------------------------------------------------------ batch-invariant decoding
+def gemv_rows(x: torch.Tensor, w, y: torch.Tensor, norm_weight: Optional[torch.Tensor], eps: float, n_heads: int, n_kv_heads: int,
+              head_dim: int, cos, sin, pos_rows: torch.Tensor, kv_pages, page_tables: torch.Tensor, page_size: int, packed=None) -> torch.Tensor:
+    """The QKV + RoPE + KV-append gemv of T rows of different sequences, x [T, K] -> y [T, >= nh*hd], every weight streamed once: row t
+    at position pos_rows[t] (int32 [T]) with the page table page_tables[t] (row t of a [T, cap] view).  ``w`` is the element-type matrix
+    or an Nf4W (its planes); ``packed`` = a Packed12W of ``w`` streams the 12-bit packing.  Row t equals a one-token gemv() there."""
+    _need(x, ELEM(), "gemv_rows.x")
+    _need(pos_rows, torch.int32, "gemv_rows.pos_rows")
+    T, K = x.shape
+    ldx, ldy, pt_ld = _rowmajor2d(x, "gemv_rows.x"), _rowmajor2d(y, "gemv_rows.y"), _rowmajor2d(page_tables, "gemv_rows.page_tables")
+    tail = (_p(norm_weight), eps, n_heads, n_kv_heads, head_dim, _p(cos), _p(sin), _p(pos_rows), _p(kv_pages), _p(page_tables), pt_ld, page_size,
+            _stream())
+    lib = _lib.load()
+    if isinstance(w, Nf4W):
+        check(lib.srgpt_gemv_rows_nf4_bf16(_p(x), ldx, C.byref(_nf4_desc(w)), _p(y), ldy, T, w.q.shape[0], K, *tail), "srgpt_gemv_rows_nf4_bf16")
+    elif packed is not None:
+        check(lib.srgpt_gemv_rows_packed_bf16(_p(x), ldx, C.byref(_packed_desc(packed)), _p(y), ldy, T, packed.sm.shape[0], K, *tail),
+              "srgpt_gemv_rows_packed_bf16")
+    else:
+        check(lib.srgpt_gemv_rows_bf16(_p(x), ldx, _p(w), w.stride(0), _p(y), ldy, T, w.shape[0], K, *tail), "srgpt_gemv_rows_bf16")
+    return y
+
+
+def attention_decode_rows(q: torch.Tensor, out: torch.Tensor, kv_pages: torch.Tensor, page_tables: torch.Tensor, page_size: int,
+                          pos_rows: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: int, scale: float) -> torch.Tensor:
+    """Decode attention of T rows of different sequences: row t of q [T, >= nh*hd] attends over kv rows 0 .. pos_rows[t] of the page table
+    page_tables[t] -> out row t, each row as attention_decode() computes it."""
+    _need(pos_rows, torch.int32, "attention_decode_rows.pos_rows")
+    T = q.shape[0]
+    check(_lib.load().srgpt_attention_decode_rows_bf16(_p(q), _rowmajor2d(q, "attention_decode_rows.q"), _p(out),
+                                                       _rowmajor2d(out, "attention_decode_rows.out"), _p(kv_pages), _p(page_tables),
+                                                       _rowmajor2d(page_tables, "attention_decode_rows.page_tables"), page_size, _p(pos_rows), T,
+                                                       n_heads, n_kv_heads, head_dim, scale, _stream()), "srgpt_attention_decode_rows_bf16")
+    return out
+
+
+def rows_advance(workspace: Optional[torch.Tensor], V: int, ids: Optional[torch.Tensor], B: int, embed_table: torch.Tensor, x: torch.Tensor,
+                 out_ids: torch.Tensor, step: torch.Tensor, pos_rows: torch.Tensor) -> None:
+    """The end of a step of B rows: each row's arg max from lm_head_multi's partials in ``workspace`` (or the ids [B] given) goes to
+    out_ids[step * B + b], x row b becomes its embedding, pos_rows[b] and then step advance."""
+    check(_lib.load().srgpt_rows_advance(_p(workspace), V, _p(ids), B, _p(embed_table), _p(x), embed_table.shape[1], _p(out_ids), _p(step),
+                                         _p(pos_rows), _stream()), "srgpt_rows_advance")
+
+
+def llama_decode_rows(h, stack: LlamaStack, q_buf, attn_buf, act_buf, B: int, dims, cos, sin, pos_rows, page_tables, page_size: int, final_norm,
+                      lm_head, embed, lm_ws, out_ids, step, logits_rows=None, sample_params=None, seeds=None, ids=None) -> None:
+    """One decode step of B sequences, each row bit-identical to that sequence's one-token step (llama_decode_step): the rows layers,
+    lm_head over the B rows, then the arg max (or, with ``seeds``, the draw from logits_rows) and the advance.  page_tables is a
+    [>= B, cap] row-major view; row b of h / pos_rows / page_tables is sequence b."""
+    nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    name, arrays, lm = stack.entry("decode_rows")
+    check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), B, dims.hidden_size, nh, nkv, hd, I,
+                                     dims.rms_norm_eps, _p(cos), _p(sin), _p(pos_rows), _p(page_tables),
+                                     _rowmajor2d(page_tables, "llama_decode_rows.page_tables"), page_size, _p(final_norm), _p(lm_head), *lm,
+                                     dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(sample_params), _p(seeds), _p(ids), _p(out_ids),
+                                     _p(step), _stream()), name)
+    _count(stack.rows_kernels + (1 if seeds is not None else 0))
