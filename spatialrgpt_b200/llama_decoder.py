@@ -12,7 +12,7 @@ with the position / step counters living in device memory.
 from __future__ import annotations
 
 import os
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import torch
 
@@ -49,6 +49,49 @@ def first_stop(host_ids, lo: int, hi: int, eos, stopping_fn, limit: int) -> Opti
         if int(host_ids[k]) in eos or (stopping_fn is not None and stopping_fn(host_ids[:k + 1])):
             return k + 1
     return limit if hi >= limit else None
+
+
+def decode_steps(launch, fetch, host, budgets: List[int], eos, stopping_fn) -> List[int]:
+    """The decode steps of B rows whose token 0 is already generated; returns each row's length.  ``launch(n)`` enqueues the step
+    that produces token n of every row; ``fetch(n)`` enqueues the copy of id row n into ``host`` ([T, B], T = max(budgets)) and
+    returns what to ``.synchronize()`` on.  With EOS ids or a criterion, step n is enqueued BEFORE row n - 1 is inspected, so the host
+    inspects while exactly one step runs, and no host round trip per token stalls the device (HF inspects after every token too, with
+    a blocking .item(); the result is the same).  Without either, the steps run back to back with no copy.  A row that has stopped
+    stays in the step and its later ids are ignored; the loop ends when every row has stopped or T - 1 steps have run.  A row's
+    length is its first stop (first_stop), else its budget: once the budget is spent the last token is returned whatever it is."""
+    T = max(budgets)
+    if not eos and stopping_fn is None:
+        for n in range(1, T):
+            launch(n)
+        return list(budgets)
+    cols = host.unbind(1)
+    stops = [None] * len(budgets)
+    copied = fetch(0)
+    n = 1
+    while n < T:
+        launch(n)
+        nxt = fetch(n)
+        copied.synchronize()
+        for b, m in enumerate(budgets):
+            if stops[b] is None:
+                stops[b] = first_stop(cols[b], n - 1, n, eos, stopping_fn, m)
+        if None not in stops:
+            break
+        copied = nxt
+        n += 1
+    return [m if s is None else s for s, m in zip(stops, budgets)]
+
+
+class GraphKey(NamedTuple):
+    """What a captured graph computes: its kind ("step", "batch", "rows", "beam" or "verify"), its rows (T for a verify pass), whether
+    it samples, whether the logits processors run, the (address, step stride) of the score rows it writes (output_scores), and the
+    n-gram size of a verify pass."""
+    kind: str
+    rows: int = 1
+    sample: bool = False
+    proc: bool = False
+    scores: Optional[tuple] = None
+    ngram: int = 0
 
 
 class BeamHypotheses:
@@ -251,6 +294,12 @@ class PagedKVCache:
         self.free.extend(reversed(self.owned[seq]))
         self.owned[seq] = []
 
+    def release_all(self, keep: Optional[int] = None) -> None:
+        """release() every slot but `keep`: a request starts from an empty cache (a batch leaves pages owned by slots 1..B-1)."""
+        for seq in range(len(self.owned)):
+            if seq != keep:
+                self.release(seq)
+
     def fork(self, src: int, shared_pages: int, n_tokens: int) -> int:
         """A host-side sequence whose first `shared_pages` pages ARE sequence `src`'s (shared, never written or freed by the fork) and
         which owns new pages for the rest of positions [0, n_tokens).  Returns its id (``table`` gives its page table; the caller builds
@@ -317,11 +366,9 @@ class LlamaDecoder:
         if self.nf4_planes_only and os.environ.get("SRGPT_DECODE_NF4", "1") == "0":
             raise ValueError("SRGPT_DECODE_NF4=0 runs the decode step over the dequantized copies, which a model loaded with "
                              "nf4_dequantized_copy=False does not keep")
-        # Captured CUDA graphs: key -> (graph, kernels one replay launches).  Keys: ("step", sample, proc) for the one-token step,
-        # ("verify", T, ngram), ("rows", B, sample) for the batch-invariant rows step, ("batch", B, proc) for the greedy batched step, ("batch", B, proc, True) for the sampled one and ("beam", B); the
-        # graphs that write output_scores rows end in ("scores", buffer address, step stride) (_scores_key).  A graph holds the addresses of every buffer it reads, so it is
-        # dropped whenever one of them is replaced: the KV cache and the layer stack's array (ensure_capacity), the processor spec (_set_processors)
-        # and the batched-decode buffers (_batch_state).
+        # Captured CUDA graphs: GraphKey -> (graph, kernels one replay launches).  A graph holds the addresses of every buffer it reads,
+        # so it is dropped whenever one of them is replaced: the KV cache and the layer stack's array (ensure_capacity), the processor
+        # spec (_set_processors), the score buffer (_scores_view) and the batched-decode buffers (_batch_state).
         self._graphs = {}
         # sampling mode (do_sample=True): temperature / top_p live in device memory so one captured graph serves any setting
         self.sample_params = torch.tensor([1.0, 1.0, 0.0], dtype=torch.float32, device=dev)
@@ -575,7 +622,7 @@ class LlamaDecoder:
             while cap < ints.size:
                 cap *= 2
             self.proc_spec = torch.zeros(cap, dtype=torch.int32, device=self.device)
-            self._drop_graphs(lambda key: key[0] in ("step", "batch") and key[2])  # the graphs with processing on read the old buffer
+            self._drop_graphs(lambda key: key.proc)  # the graphs with processing on read the old buffer
         self.proc_spec[: ints.size].copy_(torch.from_numpy(ints))
         self.proc_fparams.copy_(torch.from_numpy(fparams))
         return True
@@ -590,7 +637,7 @@ class LlamaDecoder:
         so it lives across requests and grows (dropping those graphs) when a request needs more."""
         need = steps * rows * self.dims.vocab_size
         if self._scores is None or self._scores.numel() < need:
-            self._drop_graphs(lambda key: isinstance(key[-1], tuple) and key[-1][0] == "scores")
+            self._drop_graphs(lambda key: key.scores is not None)
             self._scores = None
             self._scores = torch.empty(need, dtype=torch.float32, device=self.device)
         return self._scores[:need].view(steps, rows, self.dims.vocab_size)
@@ -603,9 +650,9 @@ class LlamaDecoder:
         return {"scores": scores, "step_stride": scores.stride(0)} if strided else {"scores": scores}
 
     @staticmethod
-    def _scores_key(scores: Optional[torch.Tensor]):
-        """The graph-key suffix of a score buffer view: a graph holds the address and the step stride it writes to."""
-        return () if scores is None else (("scores", scores.data_ptr(), scores.stride(0)),)
+    def _scores_key(scores: Optional[torch.Tensor]) -> Optional[tuple]:
+        """GraphKey.scores of a score buffer view: a graph holds the address and the step stride it writes to."""
+        return None if scores is None else (scores.data_ptr(), scores.stride(0))
 
     # ---- captured graphs ---------------------------------------------------------------------------------------------------------
     def _capture(self, key, launch, restore, kernels: int) -> torch.cuda.CUDAGraph:
@@ -641,7 +688,7 @@ class LlamaDecoder:
     @property
     def _graph(self) -> Optional[torch.cuda.CUDAGraph]:
         """The greedy one-token step graph, once _ensure_graph has captured it."""
-        entry = self._graphs.get(("step", False, False))
+        entry = self._graphs.get(GraphKey("step"))
         return None if entry is None else entry[0]
 
     def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False, scores: Optional[torch.Tensor] = None) -> torch.cuda.CUDAGraph:
@@ -649,7 +696,7 @@ class LlamaDecoder:
         (processing, key unpack and pick); greedy score rows add their copy (the sampler writes its own)."""
         kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0) + (
             1 if scores is not None and not sample else 0)
-        return self._capture(("step", sample, proc) + self._scores_key(scores),
+        return self._capture(GraphKey("step", 1, sample, proc, self._scores_key(scores)),
                              lambda: self._decode_step_launch(seq, sample=sample, proc=proc, **self._scores_kw(scores)),
                              (self.pos, self.step, self.h, self.out_ids), kernels)
 
@@ -676,6 +723,44 @@ class LlamaDecoder:
             done = torch.cuda.Event()
             done.record(side)
         return done
+
+    def _run_steps(self, launch, out2d: torch.Tensor, budgets: List[int], eos, stopping_fn) -> List[int]:
+        """decode_steps over the device ids ``out2d`` ([T, B]); the rows it inspects reach pinned memory on the copy stream."""
+        host = self._pinned_ids(out2d.numel()).view(out2d.shape) if eos or stopping_fn is not None else None
+        return decode_steps(launch, lambda n: self._to_host((out2d[n], host[n])), host, budgets, eos, stopping_fn)
+
+    def _start_request(self, prompt_lens: List[int], max_new_tokens: int, writes_ids: bool = True, keep: Optional[int] = None,
+                       slack: int = 0) -> None:
+        """The KV cache of a request whose slot b continues a prompt of prompt_lens[b] rows by up to max_new_tokens tokens: every
+        slot but ``keep`` (whose prompt prefix is reused) released, the cache grown to hold the rows, and each row's pages reserved
+        with ``slack`` more positions (prompt lookup's verify passes write past the budget).  ``writes_ids``: the ids go to out_ids,
+        whose length caps max_new_tokens; beam search keeps its ids on the host."""
+        if writes_ids and max_new_tokens > self.out_ids.numel():
+            raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
+        S = max(prompt_lens)
+        if S + max_new_tokens > self.max_seq_len:  # every row stays in the step until the last one stops
+            raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
+        self.cache.release_all(keep)
+        if keep is None:  # growing re-allocates the cache, which would lose the kept slot's K/V
+            self.ensure_capacity(len(prompt_lens), S + max_new_tokens + slack)
+        self.cache.reserve_many([n + max_new_tokens + slack for n in prompt_lens])
+
+    def _prefill_first_token(self, embeds: torch.Tensor, seq: int, reuse_rows: int, logits_row: Optional[torch.Tensor], sample: bool,
+                             proc: bool, scores: Optional[torch.Tensor]) -> None:
+        """Batch 1's prefill of the prompt ``embeds`` [S, H] into sequence `seq` (its first reuse_rows rows are in the pages already)
+        and its first token: final norm + lm_head + arg max on the last row, which writes out_ids[0], the token's embedding row (h)
+        and pos = S, step = 1; then _choose.  The fp32 logits go to ``logits_row``, or to the sample buffer when the choice reads
+        them.  generate_rows starts every row with it, so each row's first token is its batch-1 request's by construction."""
+        d, w = self.dims, self.w
+        S = embeds.shape[0]
+        hidden = self.prefill_hidden(embeds[reuse_rows:], seq, reuse_rows)
+        self.pos.fill_(S - 1)
+        self.step.zero_()
+        if logits_row is None and (sample or proc or scores is not None):
+            logits_row = self._sample_buffer()
+        ops.lm_head_argmax(hidden[S - 1 - reuse_rows], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
+                           embed_table=w.embed, next_x=self.h, logits_out=logits_row)
+        self._choose(logits_row, sample, proc, scores)
 
     def _set_sampling(self, sampling) -> bool:
         """sampling = None (greedy) or dict(temperature=, top_p=, top_k=, seed=).  Returns True when tokens are sampled."""
@@ -722,7 +807,7 @@ class LlamaDecoder:
         (HF's output_scores): the raw row when greedy, the processed row with processors, the warped row (logits / T, -inf where top-k /
         top-p removed the token) when sampled.  The decode graphs write them on the device; prompt-lookup decoding takes them from its
         verify passes' logit rows (greedy without processors: the raw rows)."""
-        d, w = self.dims, self.w
+        d = self.dims
         S = inputs_embeds.shape[0]
         n_reuse = int(reuse_rows)
         if n_reuse != 0 and (seq != 0 or n_reuse < 0 or n_reuse > self.prefix_rows or n_reuse > S - 1):
@@ -731,10 +816,6 @@ class LlamaDecoder:
         if max_new_tokens < 1:
             empty = torch.empty(0, dtype=torch.int64, device=self.device)
             return (empty, {"scores": torch.empty((0, 1, d.vocab_size), dtype=torch.float32, device=self.device)}) if output_scores else empty
-        if max_new_tokens > self.out_ids.numel():
-            raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
-        if S + max_new_tokens > self.max_seq_len:
-            raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         if lookup_k and self.fp8:
             raise NotImplementedError("prompt-lookup decoding (prompt_lookup_num_tokens) has no FP8 verify pass; decode FP8 weights without it")
         eos = eos_list(eos_token_ids)
@@ -743,37 +824,28 @@ class LlamaDecoder:
         if k > 0 and (seq != 0 or sampling or int(lookup_ngram) < 1 or processors):
             raise ValueError("prompt-lookup decoding serves greedy decoding of sequence 0 with lookup_ngram >= 1, without logits processors")
         proc = self._set_processors(processors)
+        sample = self._set_sampling(sampling)
         # a verify pass writes up to T positions past the last emitted token, and one pass is in flight after the stop is seen
-        slack = 2 * ops.SPEC_T_MAX
-        if k > 0 and (S + max_new_tokens + slack > self.max_seq_len or max_new_tokens + slack > self.out_ids.numel()):
-            k = 0
-        for b in range(len(self.cache.owned)):  # a previous batched generate leaves pages owned by sequences 1..B-1
-            if not (n_reuse and b == seq):
-                self.cache.release(b)
-        self.cache.reserve(seq, S + max_new_tokens + (slack if k > 0 else 0))
-        hidden = self.prefill_hidden(inputs_embeds[n_reuse:], seq, n_reuse)
-        if seq == 0 and self.supports_prefix_reuse:
-            self._record_prefix(S)
-        n_rows = max_new_tokens + (slack if k > 0 else 0)  # verify passes write accepted logit rows past the budget too
+        slack = 2 * ops.SPEC_T_MAX if k > 0 else 0
+        if slack and (S + max_new_tokens + slack > self.max_seq_len or max_new_tokens + slack > self.out_ids.numel()):
+            k, slack = 0, 0
+        # the prompt goes to slot `seq` (the slots before it are reserved alike and stay unused)
+        self._start_request([S] * (seq + 1), max_new_tokens, keep=seq if n_reuse else None, slack=slack)
+        n_rows = max_new_tokens + slack  # verify passes write accepted logit rows past the budget too
         # prompt lookup's scores are its logit rows (greedy without processors), which the verify passes write on the logits_all route
         lookup_scores = output_scores and k > 0 and max_new_tokens > 1
         logits = torch.empty((n_rows, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits or lookup_scores else None
         scores = self._scores_view(max_new_tokens, 1) if output_scores and not lookup_scores else None
-        # first token: final norm + lm_head + argmax on the last prompt row; afterwards pos == S
-        self.pos.fill_(S - 1)
-        self.step.zero_()
-        sample = self._set_sampling(sampling)
-        first_logits = logits[0] if logits is not None else (self._sample_buffer() if sample or proc or scores is not None else None)
-        ops.lm_head_argmax(hidden[S - 1 - n_reuse], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
-                           embed_table=w.embed, next_x=self.h, logits_out=first_logits)
-        self._choose(first_logits, sample, proc, scores)
+        self._prefill_first_token(inputs_embeds, seq, n_reuse, None if logits is None else logits[0], sample, proc, scores)
+        if seq == 0 and self.supports_prefix_reuse:
+            self._record_prefix(S)
         if k > 0 and max_new_tokens > 1:
             r = self._verify_loop(k + 1, int(lookup_ngram), lookup_ids, max_new_tokens, eos, stopping_fn, use_graph, logits)
             if not output_scores:
                 return r
             out, lg = r
             return (r, {"scores": lg.unsqueeze(1).clone()}) if return_logits else (out, {"scores": lg.unsqueeze(1)})
-        r = self._decode_loop(seq, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, scores)
+        r = self._decode_loop(seq, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, scores)
         if not output_scores:
             return r
         return r, {"scores": scores[:(r[0] if return_logits else r).numel()].clone()}
@@ -803,7 +875,7 @@ class LlamaDecoder:
 
     def _verify_graph(self, T: int, ngram: int) -> torch.cuda.CUDAGraph:
         """The captured verify pass of this (T, n-gram size); its warm-up writes only this sequence's slack."""
-        return self._capture(("verify", T, ngram), lambda: self._verify_launch(T, ngram),
+        return self._capture(GraphKey("verify", T, ngram=ngram), lambda: self._verify_launch(T, ngram),
                              (self.pos, self.step, self.out_ids, self._vstate["state"]), self.stack.verify_kernels)
 
     def _verify_loop(self, T: int, ngram: int, lookup_ids, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits):
@@ -829,7 +901,7 @@ class LlamaDecoder:
         stats, known, r, prev = (0, 0, 0), 1, 0, None
         while n is None:
             if graph:
-                self._replay(("verify", T, ngram))
+                self._replay(GraphKey("verify", T, ngram=ngram))
             else:
                 self._verify_launch(T, ngram, logits)
             # the state after pass r and out_ids[known, + 2T): pass r's tokens lie in [step after r-1, + T), inside [step after r-2, + 2T)
@@ -848,44 +920,24 @@ class LlamaDecoder:
             return out, logits[:n]
         return out
 
-    def _decode_loop(self, seq: int, n: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False,
+    def _decode_loop(self, seq: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False,
                      proc: bool = False, scores: Optional[torch.Tensor] = None):
-        """Steps n..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
-        out_ids[:n] are already set.  ``scores`` ([T, 1, V] fp32): each step's score row goes to scores[step]."""
+        """Steps 1..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
+        out_ids[0] are already set.  ``scores`` ([T, 1, V] fp32): each step's score row goes to scores[step].  On a stop, the step in
+        flight only touched this sequence's own KV slot and the step counters, which the next request resets."""
         self.active_pt.copy_(self.cache.page_tables[seq])
-        key = ("step", sample, proc) + self._scores_key(scores) if use_graph and logits is None else None
-        if key is not None:
+        graph = use_graph and logits is None
+        key = GraphKey("step", 1, sample, proc, self._scores_key(scores))
+        if graph:
             self._ensure_graph(seq, sample, proc, scores)
 
-        def launch_step(k: int) -> None:
-            if key is not None:
+        def launch(n: int) -> None:
+            if graph:
                 self._replay(key)
             else:
-                self._decode_step_launch(seq, None if logits is None else logits[k], sample, proc, **self._scores_kw(scores))
+                self._decode_step_launch(seq, None if logits is None else logits[n], sample, proc, **self._scores_kw(scores))
 
-        if not eos and stopping_fn is None:
-            while n < max_new_tokens:
-                launch_step(n)
-                n += 1
-        else:
-            # EOS / stopping criteria (the mode eval_spatial.py:223-237 runs) WITHOUT a host round trip per token: the step that
-            # produces token n is enqueued BEFORE token n-1 is inspected, token ids reach the host through a side stream into
-            # pinned memory, and the host inspects token n-1 while the GPU computes token n.  On a stop the one speculative
-            # step is discarded (it only touched this sequence's own KV slot and the step counters, which the next request
-            # resets).  HF inspects after every token too (a blocking .item()); the result is identical.
-            host = self._pinned_ids(self.out_ids.numel())
-            copied = self._to_host((self.out_ids[:n], host[:n]))
-            checked = 0
-            while n < max_new_tokens:  # once the budget is spent the last token is returned whatever it is (HF semantics)
-                launch_step(n)
-                nxt = self._to_host((self.out_ids[n:n + 1], host[n:n + 1]))
-                copied.synchronize()
-                stop = first_stop(host, checked, n, eos, stopping_fn, max_new_tokens)
-                if stop is not None:
-                    n = stop
-                    break
-                checked, copied = n, nxt
-                n += 1
+        n = self._run_steps(launch, self.out_ids[:max_new_tokens].view(max_new_tokens, 1), [max_new_tokens], eos, stopping_fn)[0]
         out = self.out_ids[:n].clone()
         if logits is not None:
             return out, logits[:n]
@@ -896,7 +948,7 @@ class LlamaDecoder:
         st = self._bstate
         if st is not None and st["B"] == B:
             return st
-        self._drop_graphs(lambda key: key[0] in ("batch", "beam"))  # they read the buffers replaced here
+        self._drop_graphs(lambda key: key.kind in ("batch", "beam"))  # they read the buffers replaced here
         d, dev = self.dims, self.device
         H, nh, nkv, hd, I, V = d.hidden_size, d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.intermediate_size, d.vocab_size
         z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
@@ -976,41 +1028,23 @@ class LlamaDecoder:
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        if scores is not None:  # the graphs that write scores hold the buffer's address
-            key = ("batch", B, proc, sample) + self._scores_key(scores)
-        else:
-            key = ("batch", B, proc, True) if sample else ("batch", B, proc)
+        key = GraphKey("batch", B, sample, proc, self._scores_key(scores))  # the graphs that write scores hold the buffer's address
         if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max (sampling: processing + draw)
             self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample, scores=scores),
                           (st["h"], st["pos"], st["step"], st["out"]),
                           self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4) + (
                               1 if scores is not None and not sample else 0))
-        need_check = bool(eos) or stopping_fn is not None
-        out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
-        if need_check:
-            host = self._pinned_ids(max_new_tokens * B).view(max_new_tokens, B)
-            cols = [host[:, b] for b in range(B)]
-            copied = self._to_host((out2d[0], host[0]))
-        stopped = [None] * B  # length at which sequence b stopped
-        n = 1
-        while n < max_new_tokens:
+
+        def launch(n: int) -> None:
             if use_graph:
                 self._replay(key)
             else:
                 self._batch_step_launch(st, proc=proc, sample=sample, scores=scores)
-            if need_check:  # same pipelining as the single-sequence loop: inspect row n-1 while row n is being computed
-                nxt = self._to_host((out2d[n], host[n]))
-                copied.synchronize()
-                for b in range(B):
-                    if stopped[b] is None:
-                        stopped[b] = first_stop(cols[b], n - 1, n, eos, stopping_fn, max_new_tokens)
-                copied = nxt
-                if all(s is not None for s in stopped):
-                    break
-            n += 1
-        n = min(n, max_new_tokens)
-        res = out2d[:n].t().contiguous()
-        return [res[b, : (stopped[b] if stopped[b] is not None else n)].clone() for b in range(B)]
+
+        out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
+        lens = self._run_steps(launch, out2d, [max_new_tokens] * B, eos, stopping_fn)
+        res = out2d[:max(lens)].t().contiguous()
+        return [res[b, :lens[b]].clone() for b in range(B)]
 
     # ---- batch-invariant decoding: up to SPEC_T_MAX sequences per weight pass, each bit-identical to its batch-1 generate_from_embeds --
     def _rows_state(self):
@@ -1043,7 +1077,7 @@ class LlamaDecoder:
         gives each row the arithmetic of its one-token step.  ``max_new_tokens``: one budget, or one per row.  EOS and ``stopping_fn``
         are checked per row; a row that has stopped stays in the step and its results are ignored.  Returns a list of B LongTensors
         (and a list of B fp32 logits [n_b, V] when return_logits)."""
-        d, w, B = self.dims, self.w, len(embeds_list)
+        d, B = self.dims, len(embeds_list)
         if self.fp8:
             raise NotImplementedError("batch-invariant decoding has no FP8 form (the rows step is a 16-bit, packed or NF4 GEMV)")
         if not 1 <= B <= ops.SPEC_T_MAX:
@@ -1055,69 +1089,39 @@ class LlamaDecoder:
         if sample and (seeds is None or len(seeds) != B):
             raise ValueError("sampled generate_rows needs one seed per prompt")
         lens, mx = [int(e.shape[0]) for e in embeds_list], max(budgets)
-        if mx > self.out_ids.numel():
-            raise RuntimeError(f"max_new_tokens {mx} exceeds the decoder's cap {self.out_ids.numel()}")
-        if max(lens) + mx > self.max_seq_len:  # every row stays in the step until the last one stops
-            raise RuntimeError(f"{max(lens)} prompt + {mx} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
-        for b in range(len(self.cache.owned)):
-            self.cache.release(b)
-        self.ensure_capacity(B, max(lens) + mx)
+        self._start_request(lens, mx)
         self._set_sampling(sampling)
         st = self._rows_state()
         logits = [torch.empty((mx, d.vocab_size), dtype=torch.float32, device=self.device) for _ in range(B)] if return_logits else None
         for b, emb in enumerate(embeds_list):  # generate_from_embeds' prefill and first token, into sequence b
-            S = lens[b]
-            self.cache.reserve(b, S + mx)
-            hidden = self.prefill_hidden(emb, b, 0)
-            self.pos.fill_(S - 1)
-            self.step.zero_()
             if sample:
                 self._set_seed(int(seeds[b]))
-            first_logits = logits[b][0] if logits is not None else (self._sample_buffer() if sample else None)
-            ops.lm_head_argmax(hidden[S - 1], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
-                               embed_table=w.embed, next_x=self.h, logits_out=first_logits)
-            self._choose(first_logits, sample, False, None)
+            self._prefill_first_token(emb, b, 0, None if logits is None else logits[b][0], sample, False, None)
             st["out"][b:b + 1].copy_(self.out_ids[:1])
             st["h"][b].copy_(self.h)
         st["pos"][:B].copy_(torch.tensor(lens, dtype=torch.int32))
         st["step"].fill_(1)
         if sample:
             st["seeds"][:B].copy_(torch.tensor([int(s) & SEED_MASK for s in seeds], dtype=torch.int64))
-        key = ("rows", B, sample)
+        key = GraphKey("rows", B, sample)
         graph = use_graph and logits is None
         if graph:
             self._capture(key, lambda: self._rows_step_launch(B, sample), (st["h"], st["pos"], st["step"], st["out"]),
                           self.stack.rows_kernels + (1 if sample else 0))
-        need_check = bool(eos) or stopping_fn is not None
-        out2d = st["out"][: mx * B].view(mx, B)
-        if need_check:
-            host = self._pinned_ids(mx * B).view(mx, B)
-            cols = [host[:, b] for b in range(B)]
-            copied = self._to_host((out2d[0], host[0]))
-        stopped = [None] * B
-        n = 1
-        while n < mx:
+
+        def launch(n: int) -> None:
             if graph:
                 self._replay(key)
-            else:
-                self._rows_step_launch(B, sample)
-                if logits is not None:
-                    for b in range(B):
-                        logits[b][n].copy_(st["logits"][b])
-            if need_check:  # inspect row n-1 of every sequence while row n is being computed
-                nxt = self._to_host((out2d[n], host[n]))
-                copied.synchronize()
+                return
+            self._rows_step_launch(B, sample)
+            if logits is not None:
                 for b in range(B):
-                    if stopped[b] is None:
-                        stopped[b] = first_stop(cols[b], n - 1, n, eos, stopping_fn, budgets[b])
-                copied = nxt
-                if all(s is not None for s in stopped):
-                    break
-            n += 1
-        n = min(n, mx)
-        res = out2d[:n].t().contiguous()
-        lens_out = [stopped[b] if stopped[b] is not None else min(n, budgets[b]) for b in range(B)]
+                    logits[b][n].copy_(st["logits"][b])
+
+        out2d = st["out"][: mx * B].view(mx, B)
+        lens_out = self._run_steps(launch, out2d, budgets, eos, stopping_fn)
+        res = out2d[:max(lens_out)].t().contiguous()
         outs = [res[b, :lens_out[b]].clone() for b in range(B)]
         if logits is not None:
             return outs, [logits[b][:lens_out[b]] for b in range(B)]
@@ -1143,14 +1147,9 @@ class LlamaDecoder:
         if max_new_tokens < 1:
             empty = torch.empty(0, dtype=torch.int64, device=self.device)
             return (empty, self._beam_extra(None, 0, [])) if output_scores else empty
-        if S + max_new_tokens > self.max_seq_len:
-            raise RuntimeError(f"{S} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
         n_cand = max(2, 1 + len(eos)) * k
-        for b in range(len(self.cache.owned)):
-            self.cache.release(b)
-        self.ensure_capacity(k, S + max_new_tokens)
-        self.cache.reserve_many([S + max_new_tokens] * k)
+        self._start_request([S] * k, max_new_tokens, writes_ids=False)
         hidden = self.prefill_packed(inputs_embeds.to(self.dtype).repeat(k, 1), [S] * k)
         _, lg = self.first_tokens(hidden, [S] * k, return_logits=True)
         st = self._batch_state(k)
@@ -1193,8 +1192,8 @@ class LlamaDecoder:
             st["pos"].fill_(S + step)
             d_scores.copy_(torch.tensor(hyp.scores, dtype=torch.float32), non_blocking=True)
             if use_graph:  # the warm-up before the capture rewrites only this step's own KV rows
-                self._capture(("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), self._batch_kernels_per_layer * d.num_hidden_layers + 2)
-                self._replay(("beam", k))
+                self._capture(GraphKey("beam", k), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],), self._batch_kernels_per_layer * d.num_hidden_layers + 2)
+                self._replay(GraphKey("beam", k))
             else:
                 self._batch_step_launch(st, logits_only=True)
         best = torch.tensor(hyp.best(max_new_tokens), dtype=torch.int64, device=dev)
@@ -1237,15 +1236,10 @@ class LlamaDecoder:
         if max_new_tokens < 1:
             empty = [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
             return (empty, self._beam_extra(None, 0, [])) if output_scores else empty
-        if max(seq_lens) + max_new_tokens > self.max_seq_len:
-            raise RuntimeError(f"{max(seq_lens)} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
         n_cand = max(2, 1 + len(eos)) * k
-        for b in range(len(self.cache.owned)):
-            self.cache.release(b)
-        self.ensure_capacity(R, max(seq_lens) + max_new_tokens)
         starts = [n for n in seq_lens for _ in range(k)]  # row r = g * k + i: the first generated position of its prompt
-        self.cache.reserve_many([n + max_new_tokens for n in starts])
+        self._start_request(starts, max_new_tokens, writes_ids=False)
         tables = [list(self.cache.owned[r]) for r in range(R)]
         # the prompts are prefilled once, into beam 0 of each; the other beams get copies of its prompt rows
         hidden = self.prefill_packed(packed_embeds, seq_lens, page_tables=self.cache.page_tables[:R:k])
@@ -1291,9 +1285,9 @@ class LlamaDecoder:
             st["pos"].copy_(torch.tensor([n + step for n in starts], dtype=torch.int32))
             d_scores.copy_(torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32))
             if use_graph:  # keyed by the row count, as generate_beam's graph: the same launch over the same buffers
-                self._capture(("beam", R), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],),
+                self._capture(GraphKey("beam", R), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],),
                               self._batch_kernels_per_layer * d.num_hidden_layers + 2)
-                self._replay(("beam", R))
+                self._replay(GraphKey("beam", R))
             else:
                 self._batch_step_launch(st, logits_only=True)
         outs = [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
@@ -1332,17 +1326,10 @@ class LlamaDecoder:
         if max_new_tokens < 1:
             empty = [torch.empty(0, dtype=torch.int64, device=self.device) for _ in range(B)]
             return (empty, {"scores": torch.empty((0, B, d.vocab_size), dtype=torch.float32, device=self.device)}) if output_scores else empty
-        if max_new_tokens > self.out_ids.numel():
-            raise RuntimeError(f"max_new_tokens {max_new_tokens} exceeds the decoder's cap {self.out_ids.numel()}")
-        if max(seq_lens) + max_new_tokens > self.max_seq_len:
-            raise RuntimeError(f"{max(seq_lens)} prompt + {max_new_tokens} new tokens exceed max_seq_len {self.max_seq_len}")
         eos = eos_list(eos_token_ids)
         proc = self._set_processors(processors)
-        for b in range(len(self.cache.owned)):
-            self.cache.release(b)
-        self.ensure_capacity(B, max(seq_lens) + max_new_tokens)
         row_lens = [int(n) for n in seq_lens for _ in range(n_ret)]  # row b * n_ret + j continues prompt b
-        self.cache.reserve_many([n + max_new_tokens for n in row_lens])
+        self._start_request(row_lens, max_new_tokens)
         if n_ret == 1:
             hidden = self.prefill_packed(packed_embeds, seq_lens)
         else:  # each prompt once, into the first of its rows; the other rows get copies of its prompt pages
@@ -1387,7 +1374,7 @@ class LlamaDecoder:
                 row = first_rows[b] if proc else lg[b].float().contiguous()
                 ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
                                  **self._scores_kw(col, True))
-            r = self._decode_loop(b, 1, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, col)
+            r = self._decode_loop(b, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, col)
             if return_logits:
                 outs.append(r[0]); all_logits.append(r[1])
             else:
@@ -1425,8 +1412,7 @@ class LlamaDecoder:
         # pages: the prompts', then as many candidate pages as memory allows (at least the largest single candidate's)
         prompt_pages = sum((S + PAGE_SIZE - 1) // PAGE_SIZE for S in seq_lens)
         tails = [candidate_pages(S, L - 1)[1] for S in seq_lens for L in lens if L > 1]
-        for b in range(len(self.cache.owned)):
-            self.cache.release(b)
+        self.cache.release_all()
         free_b, _ = torch.cuda.mem_get_info(dev)
         afford = self.cache.n_pages + max(0, free_b - (2 << 30)) // 2 // self._page_bytes()
         self._grow_cache(B, min(prompt_pages + sum(tails), max(afford, prompt_pages + max(tails, default=0))), "scoring")

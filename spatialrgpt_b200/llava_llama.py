@@ -96,6 +96,14 @@ def batch_invariant_groups(B: int, size: int):
     return [(lo, min(lo + size, B)) for lo in range(0, B, size)]
 
 
+def stopping_fn_of(stopping_criteria):
+    """generate()'s stopping_criteria as the decoders take it: a function of one row's ids so far that holds when any criterion
+    holds for them as a batch of one; None without criteria."""
+    if not stopping_criteria:
+        return None
+    return lambda ids: any(bool(c(ids[None], None)) for c in stopping_criteria)
+
+
 def compute_transition_scores(sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None, normalize_logits: bool = False,
                               vocab_size: Optional[int] = None) -> torch.Tensor:
     """HF's GenerationMixin.compute_transition_scores: the score of every generated token, fp32 [rows, steps] (beams: [B, L], 0 where
@@ -691,15 +699,11 @@ class LlavaLlamaModel:
                               image_equal=[], mask_equal=[], encoders_skipped=False)
         if max_new_tokens is None:
             max_new_tokens = 20 if max_length is None else max(int(max_length) - max(lens), 1)  # HF default max_length=20
-        pad = pad_token_id if pad_token_id is not None else (self.config.llama.pad_token_id or 0)
 
         outs, all_logits = [], []
         extra = None  # the decoder's output_scores results
         sc_kw = {"output_scores": True} if output_scores else {}
-        stop_fn = None
-        if stopping_criteria:
-            def stop_fn(ids, _sc=stopping_criteria):
-                return any(bool(c(ids[None], None)) for c in _sc)
+        stop_fn = stopping_fn_of(stopping_criteria)
         lens = [int(n) for n in lens]
         processors = logits_processors.resolve_min_length(processors, max(lens))  # HF subtracts the (padded) inputs_embeds length
         proc = {} if processors is None else {"processors": processors}
@@ -765,21 +769,13 @@ class LlavaLlamaModel:
                     outs, all_logits = r
                 else:
                     outs = r
-        n_max = max(o.numel() for o in outs)
-        seqs = torch.full((len(outs), n_max), int(pad), dtype=torch.int64, device=self.device)
-        for b, o in enumerate(outs):
-            seqs[b, : o.numel()] = o
-        if return_dict:
-            return self._generate_output(seqs, extra, all_logits if return_logits else None, num_beams != 1)
-        if return_logits:
-            return seqs, all_logits
-        return seqs
+        return self._generate_result(outs, pad_token_id, return_dict, all_logits if return_logits else None, extra, num_beams != 1)
 
     def _generate_batch_invariant(self, input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id, stopping_criteria,
                                   pad_token_id, use_graph: bool, return_logits: bool, return_dict: bool, sampling, seed):
         """generate(batch_invariant=True) over B > 1 prompts: every prompt's embeddings by the calls a batch-1 generate() of it makes (its
         unpadded ids; its images, depth images and masks), then groups of at most ops.SPEC_T_MAX prompts through generate_rows."""
-        B, dev = int(input_ids.shape[0]), self.device
+        B = int(input_ids.shape[0])
         am = None if attention_mask is None else attention_mask.bool().cpu()
         ids_rows = [input_ids[b] if am is None else input_ids[b][am[b].to(input_ids.device)] for b in range(B)]
         if images is not None:
@@ -810,10 +806,7 @@ class LlavaLlamaModel:
             else:
                 seeds = sequence_seeds(torch.initial_seed() if seed is None else int(seed), B)
             sampling = dict(sampling, seed=None)
-        stop_fn = None
-        if stopping_criteria:
-            def stop_fn(ids, _sc=stopping_criteria):
-                return any(bool(c(ids[None], None)) for c in _sc)
+        stop_fn = stopping_fn_of(stopping_criteria)
         outs, all_logits = [], []
         for lo, hi in batch_invariant_groups(B, ops.SPEC_T_MAX):
             r = self.llm.generate_rows(embeds[lo:hi], budgets[lo:hi], eos_token_ids=eos_token_id, stopping_fn=stop_fn, use_graph=use_graph,
@@ -822,20 +815,19 @@ class LlavaLlamaModel:
                 r, lg = r
                 all_logits.extend(lg)
             outs.extend(r)
+        return self._generate_result(outs, pad_token_id, return_dict, all_logits if return_logits else None)
+
+    def _generate_result(self, outs: List[torch.Tensor], pad_token_id, return_dict: bool, logits=None, extra=None, beams: bool = False):
+        """What generate() returns for the decoder's rows ``outs``: the ids [rows, longest] padded on the right with pad_token_id (the
+        config's, else 0), with the fp32 ``logits`` of each row when output_logits, or as the return_dict_in_generate object, which
+        also carries ``extra``, the decoder's output_scores results."""
         pad = pad_token_id if pad_token_id is not None else (self.config.llama.pad_token_id or 0)
         n_max = max(o.numel() for o in outs)
-        seqs = torch.full((B, n_max), int(pad), dtype=torch.int64, device=dev)
+        seqs = torch.full((len(outs), n_max), int(pad), dtype=torch.int64, device=self.device)
         for b, o in enumerate(outs):
             seqs[b, : o.numel()] = o
-        if return_dict:
-            return self._generate_output(seqs, None, all_logits if return_logits else None, False)
-        if return_logits:
-            return seqs, all_logits
-        return seqs
-
-    def _generate_output(self, seqs: torch.Tensor, extra, logits, beams: bool):
-        """The return_dict_in_generate object of a request whose padded sequences are ``seqs`` and whose decoder returned ``extra``
-        (None without output_scores)."""
+        if not return_dict:
+            return seqs if logits is None else (seqs, logits)
         scores = None if extra is None else tuple(extra["scores"].unbind(0))
         if not beams:
             return GenerateDecoderOnlyOutput(sequences=seqs, scores=scores, logits=logits)

@@ -136,7 +136,7 @@ class TPLlamaDecoder(LlamaDecoder):
     def _capture(self, key, launch, restore, kernels: int) -> torch.cuda.CUDAGraph:
         had = key in self._graphs
         g = super()._capture(key, launch, restore, kernels)
-        if not had and key[0] == "step":
+        if not had and key.kind == "step":
             # the warm-up step before the capture ran real collectives with the current (epoch, step): retire those flag values
             self.tp_epoch.add_(1)
         return g
