@@ -646,6 +646,37 @@ int srgpt_llama_decode_rows_nf4_bf16(void* h, const srgpt_llama_layer_weights* l
                                      void* lm_workspace, float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
                                      long long* out_ids, int* step, void* stream);
 
+/* ---- classifier-free guidance (guidance.cu): replaces HF UnbatchedClassifierFreeGuidanceLogitsProcessor (transformers
+ * generation/logits_process.py), which GenerationMixin puts first among the logits processors behind generate(guidance_scale=,
+ * negative_prompt_ids=) (call site llava_llama.py:212).  Prompt b decodes in row b of a rows step of 2P rows and its unconditional
+ * branch (its negative prompt, then the tokens chosen for prompt b) in row P + b.
+ * srgpt_guidance_rows: logits fp32 [2P, V] (the rows step's logits_rows), P <= SRGPT_SPEC_T_MAX / 2, scale = device float g.  Per pair:
+ * s = log_softmax(row b), u = log_softmax(row P + b), each (x - m) - log(sum exp(x - m)) in fp32; guided row b [V] (fp32 [P, V], not
+ * overlapping logits) = fl(fl(g * fl(s - u)) + u); logits and guided 16-byte aligned.  lse (optional, fp32 [2P][2]) = {m, log sum
+ * exp(x - m)} of every row.  ids (optional, int64 [2P]): ids[b] = ids[P + b] = the arg max of guided row b (lowest index on ties, NaN never wins, 0 for an all-NaN row).  One
+ * 512-thread CTA per pair, fixed reduction order. */
+int srgpt_guidance_rows(const float* logits, int V, int P, const float* scale, float* guided, float* lse, long long* ids, void* stream);
+/* ids[P + b] = ids[b] for b < P (a prompt's drawn token is its unconditional branch's next token). */
+int srgpt_guidance_pair_ids(long long* ids, int P, void* stream);
+typedef struct {
+  const float* scale;  /* device float: g */
+  float* guided_rows;  /* fp32 [B / 2, V]: the guided rows the choice is made from */
+} srgpt_guidance;
+/* srgpt_llama_decode_rows_* with guidance: B = 2P rows, row P + b the unconditional branch of row b.  After lm_head, srgpt_guidance_rows
+ * over logits_rows (needed); greedy: its arg max goes to ids (needed) for both rows of a pair; sampled (seeds != NULL, seeds [P]):
+ * srgpt_sample_rows draws row b from guided row b, then srgpt_guidance_pair_ids.  srgpt_rows_advance then takes ids for all B rows.
+ * guidance == NULL is the step of the format's own entry point.  packed and nf4 select the weight format (at most one non-NULL;
+ * lm_packed may be NULL); one more kernel than the unguided step when greedy, three more than the unguided sampled step's one.
+ * One entry point for every format, running the same layer body (decode_rows in layers.cu) as the three above, rather than a new
+ * argument on each of them: their argument lists stay as they are, so existing callers and bindings of the C ABI keep working. */
+int srgpt_llama_decode_rows_guided_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed,
+                                        const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int B, int H,
+                                        int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab,
+                                        int* pos_rows, const int* page_tables, int pt_stride, int page_size, const void* final_norm,
+                                        const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
+                                        float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
+                                        long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

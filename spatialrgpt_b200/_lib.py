@@ -147,6 +147,10 @@ SIGNATURES = {
                                                  vp, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_llama_decode_rows_nf4_bf16": (ci, [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp, ci, vp,
                                               vp, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_guidance_rows": (ci, [vp, ci, ci, vp, vp, vp, vp, vp]),
+    "srgpt_guidance_pair_ids": (ci, [vp, ci, vp]),
+    "srgpt_llama_decode_rows_guided_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp,
+                                                 ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)
@@ -176,6 +180,11 @@ class Nf4(C.Structure):
 
 class LlamaLayerNf4(C.Structure):
     _fields_ = [(n, Nf4) for n in ("qkv", "o", "gateup", "down")]
+
+
+class Guidance(C.Structure):
+    """srgpt_guidance: the device scale g and the guided rows [B / 2, V] of a guided rows step."""
+    _fields_ = [("scale", vp), ("guided_rows", vp)]
 
 
 class Fp8(C.Structure):

@@ -391,14 +391,24 @@ static int decode_rows(void* h, const srgpt_llama_layer_weights* layers, const s
                        const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size,
                        const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
                        float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids, long long* out_ids, int* step,
-                       void* stream) {
+                       const srgpt_guidance* guidance, void* stream) {
   SRGPT_CHECK_ARG(B >= 1 && B <= SRGPT_SPEC_T_MAX && pt_stride > 0);
+  SRGPT_CHECK_ARG(guidance == nullptr || ((B % 2) == 0 && guidance->scale && guidance->guided_rows && ids && logits_rows));
   SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos_rows && page_tables && final_norm && lm_head && embed_table && lm_workspace &&
                   out_ids && step);
   SRGPT_CHECK_ARG(seeds == nullptr || (sample_params && ids && logits_rows));
   SRGPT_TRY(rows_layers(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
                         pos_rows, page_tables, pt_stride, page_size, stream));
   SRGPT_TRY(lm_head_rows(h, B, H, eps, final_norm, lm_head, lm_packed, V, logits_rows, lm_workspace, stream));
+  if (guidance != nullptr) {  // rows B/2 .. B-1 are the unconditional branches of rows 0 .. B/2-1; each pair takes the guided choice
+    const int P = B / 2;
+    SRGPT_TRY(srgpt_guidance_rows(logits_rows, V, P, guidance->scale, guidance->guided_rows, nullptr, seeds == nullptr ? ids : nullptr, stream));
+    if (seeds != nullptr) {
+      SRGPT_TRY(srgpt_sample_rows(guidance->guided_rows, 1, V, P, V, sample_params, seeds, step, 0, ids, stream));
+      SRGPT_TRY(srgpt_guidance_pair_ids(ids, P, stream));
+    }
+    return srgpt_rows_advance(lm_workspace, V, ids, B, embed_table, h, H, out_ids, step, pos_rows, stream);
+  }
   if (seeds != nullptr) SRGPT_TRY(srgpt_sample_rows(logits_rows, 1, V, B, V, sample_params, seeds, step, 0, ids, stream));
   return srgpt_rows_advance(lm_workspace, V, seeds != nullptr ? ids : nullptr, B, embed_table, h, H, out_ids, step, pos_rows, stream);
 }
@@ -410,7 +420,7 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_bf
     const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, void* stream) {
   return decode_rows(h, layers, nullptr, nullptr, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
                      pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, nullptr, V, embed_table, lm_workspace, logits_rows, sample_params,
-                     seeds, ids, out_ids, step, stream);
+                     seeds, ids, out_ids, step, nullptr, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_packed_bf16(
@@ -422,7 +432,7 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_pa
   SRGPT_CHECK_ARG(packed != nullptr);
   return decode_rows(h, layers, packed, nullptr, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
                      pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
-                     sample_params, seeds, ids, out_ids, step, stream);
+                     sample_params, seeds, ids, out_ids, step, nullptr, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_nf4_bf16(
@@ -434,5 +444,19 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_nf
   SRGPT_CHECK_ARG(nf4 != nullptr);
   return decode_rows(h, layers, nullptr, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
                      pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
-                     sample_params, seeds, ids, out_ids, step, stream);
+                     sample_params, seeds, ids, out_ids, step, nullptr, stream);
+}
+
+// The rows step of B = 2P rows with classifier-free guidance: one entry point for every weight format of the step (packed / nf4 may be
+// NULL, not both given), the same layer body as the three above.
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_guided_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4, int n_layers,
+    void* q_buf, void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab,
+    const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size, const void* final_norm, const void* lm_head,
+    const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_rows, const float* sample_params,
+    const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream) {
+  SRGPT_CHECK_ARG(packed == nullptr || nf4 == nullptr);
+  return decode_rows(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                     pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
+                     sample_params, seeds, ids, out_ids, step, guidance, stream);
 }

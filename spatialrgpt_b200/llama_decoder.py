@@ -1061,25 +1061,49 @@ class LlamaDecoder:
         self._rstate = st
         return st
 
-    def _rows_step_launch(self, B: int, sample: bool) -> None:
+    def _guidance_state(self):
+        """The rows state's buffers of classifier-free guidance, added on first use: the device scale g and the guided rows of up to
+        SPEC_T_MAX / 2 prompts (a captured guided step holds their addresses)."""
+        st = self._rows_state()
+        if "guided" not in st:
+            st["scale"] = torch.ones(1, dtype=torch.float32, device=self.device)
+            st["guided"] = torch.empty((ops.SPEC_T_MAX // 2, self.dims.vocab_size), dtype=torch.float32, device=self.device)
+        return st
+
+    def _rows_step_launch(self, B: int, sample: bool, guided: bool = False) -> None:
+        """The rows step over B rows; ``guided``: B = 2P rows, row P + b the unconditional branch of row b (llama_decode_rows' guidance)."""
         d, w, st = self.dims, self.w, self._rstate
+        kw = dict(sample_params=self.sample_params, seeds=st["seeds"], ids=st["ids"]) if sample else {}
+        if guided:
+            kw.update(ids=st["ids"], guidance=(st["scale"], st["guided"]))
         ops.llama_decode_rows(st["h"][:B], self.stack, st["q"][:B], st["attn"][:B], st["act"][:B], B, d, self.cos, self.sin, st["pos"],
-                              self.cache.page_tables, PAGE_SIZE, w.norm, w.lm_head, w.embed, st["ws"], st["out"], st["step"], st["logits"],
-                              **(dict(sample_params=self.sample_params, seeds=st["seeds"], ids=st["ids"]) if sample else {}))
+                              self.cache.page_tables, PAGE_SIZE, w.norm, w.lm_head, w.embed, st["ws"], st["out"], st["step"], st["logits"], **kw)
 
     @torch.no_grad()
     @ops.in_own_dtype
     def generate_rows(self, embeds_list: List[torch.Tensor], max_new_tokens, eos_token_ids=None, stopping_fn=None, use_graph: bool = True,
-                      return_logits: bool = False, sampling=None, seeds: Optional[List[int]] = None):
+                      return_logits: bool = False, sampling=None, seeds: Optional[List[int]] = None, guidance_scale: Optional[float] = None,
+                      negative_embeds: Optional[List[torch.Tensor]] = None):
         """Decode B <= SPEC_T_MAX prompts (embeddings [S_b, H] each) together, row b bit-identical to ``generate_from_embeds(embeds_list[b],
         max_new_tokens[b], ..., sampling=dict(sampling, seed=seeds[b]))``: each prompt is prefilled and gets its first token with the
         calls batch 1 makes, then every step runs the rows step (llama_decode_rows), which streams each weight once for all rows and
         gives each row the arithmetic of its one-token step.  ``max_new_tokens``: one budget, or one per row.  EOS and ``stopping_fn``
         are checked per row; a row that has stopped stays in the step and its results are ignored.  Returns a list of B LongTensors
-        (and a list of B fp32 logits [n_b, V] when return_logits)."""
+        (and a list of B fp32 logits [n_b, V] when return_logits).
+        ``negative_embeds`` (B <= SPEC_T_MAX / 2 embeddings [T_b, H]) with ``guidance_scale`` g: classifier-free guidance (HF's
+        UnbatchedClassifierFreeGuidanceLogitsProcessor).  Prompt b's unconditional branch is its negative prompt, prefilled batch 1 into
+        sequence B + b at positions from 0 and continued by the tokens chosen for prompt b; the 2B rows run the rows step, and each token is
+        chosen (greedy arg max, or drawn with seeds[b]) from g * (log_softmax(c) - log_softmax(u)) + log_softmax(u) of the two rows'
+        fp32 logits c and u (ops.guidance_rows).  The conditional rows keep their one-token arithmetic, so prompt b's ids and logits equal
+        its guided call alone.  EOS and stopping_fn look at the conditional rows; the returned logits are their raw rows."""
         d, B = self.dims, len(embeds_list)
+        guided = negative_embeds is not None
         if self.fp8:
             raise NotImplementedError("batch-invariant decoding has no FP8 form (the rows step is a 16-bit, packed or NF4 GEMV)")
+        if guided and not 1 <= B <= ops.SPEC_T_MAX // 2:
+            raise ValueError(f"guided generate_rows decodes 1 .. {ops.SPEC_T_MAX // 2} prompts at once (each with its unconditional row), got {B}")
+        if guided and (len(negative_embeds) != B or guidance_scale is None or min(int(e.shape[0]) for e in negative_embeds) < 1):
+            raise ValueError("guided generate_rows needs guidance_scale and one non-empty negative prompt per prompt")
         if not 1 <= B <= ops.SPEC_T_MAX:
             raise ValueError(f"generate_rows decodes 1 .. {ops.SPEC_T_MAX} prompts at once, got {B}")
         budgets = [int(max_new_tokens)] * B if isinstance(max_new_tokens, int) else [int(m) for m in max_new_tokens]
@@ -1089,37 +1113,58 @@ class LlamaDecoder:
         if sample and (seeds is None or len(seeds) != B):
             raise ValueError("sampled generate_rows needs one seed per prompt")
         lens, mx = [int(e.shape[0]) for e in embeds_list], max(budgets)
+        R = 2 * B if guided else B  # rows of the step
         eos = eos_list(eos_token_ids)
-        self._start_request(lens, mx)
+        self._start_request(lens + ([int(e.shape[0]) for e in negative_embeds] if guided else []), mx)
         self._set_sampling(sampling)
-        st = self._rows_state()
+        st = self._guidance_state() if guided else self._rows_state()
         logits = [torch.empty((mx, d.vocab_size), dtype=torch.float32, device=self.device) for _ in range(B)] if return_logits else None
-        for b, emb in enumerate(embeds_list):  # generate_from_embeds' prefill and first token, into sequence b
+        if guided:  # each prompt and each negative prompt prefilled batch 1; the first token of a pair from its two last rows
+            for r, emb in enumerate(list(embeds_list) + list(negative_embeds)):
+                self._prefill_first_token(emb, r, 0, st["logits"][r], False, False, None)
+            if logits is not None:
+                for b in range(B):
+                    logits[b][0].copy_(st["logits"][b])
+            st["scale"].fill_(float(guidance_scale))
+            st["step"].zero_()  # a draw of the first token uses counter 0, as batch 1's
             if sample:
-                self._set_seed(int(seeds[b]))
-            self._prefill_first_token(emb, b, 0, None if logits is None else logits[b][0], sample, False, None)
-            st["out"][b:b + 1].copy_(self.out_ids[:1])
-            st["h"][b].copy_(self.h)
-        st["pos"][:B].copy_(torch.tensor(lens, dtype=torch.int32))
+                st["seeds"][:B].copy_(torch.tensor([int(s) & SEED_MASK for s in seeds], dtype=torch.int64))
+            ids = st["ids"][:R]
+            ops.guidance_rows(st["logits"][:R], st["scale"], st["guided"][:B], ids=None if sample else ids)
+            if sample:
+                ops.sample_rows(st["guided"][:B], self.sample_params, st["seeds"][:B], st["step"], 0, st["ids"][:B])
+                ops.guidance_pair_ids(ids, B)
+            st["out"][:R].copy_(ids)
+            st["h"][:R].copy_(ops.splice_rows(self.w.embed, None, None, None, torch.zeros(R, dtype=torch.int32, device=self.device),
+                                              ids.to(torch.int32)))
+            st["pos"][:R].copy_(torch.tensor(lens + [int(e.shape[0]) for e in negative_embeds], dtype=torch.int32))
+        else:
+            for b, emb in enumerate(embeds_list):  # generate_from_embeds' prefill and first token, into sequence b
+                if sample:
+                    self._set_seed(int(seeds[b]))
+                self._prefill_first_token(emb, b, 0, None if logits is None else logits[b][0], sample, False, None)
+                st["out"][b:b + 1].copy_(self.out_ids[:1])
+                st["h"][b].copy_(self.h)
+            st["pos"][:B].copy_(torch.tensor(lens, dtype=torch.int32))
         st["step"].fill_(1)
-        if sample:
+        if sample and not guided:
             st["seeds"][:B].copy_(torch.tensor([int(s) & SEED_MASK for s in seeds], dtype=torch.int64))
-        key = GraphKey("rows", B, sample)
+        key = GraphKey("guided" if guided else "rows", B, sample)
         graph = use_graph and logits is None
         if graph:
-            self._capture(key, lambda: self._rows_step_launch(B, sample), (st["h"], st["pos"], st["step"], st["out"]),
-                          self.stack.rows_kernels + (1 if sample else 0))
+            self._capture(key, lambda: self._rows_step_launch(R, sample, guided), (st["h"], st["pos"], st["step"], st["out"]),
+                          self.stack.rows_kernels + ((3 if sample else 1) if guided else (1 if sample else 0)))
 
         def launch(n: int) -> None:
             if graph:
                 self._replay(key)
                 return
-            self._rows_step_launch(B, sample)
+            self._rows_step_launch(R, sample, guided)
             if logits is not None:
                 for b in range(B):
                     logits[b][n].copy_(st["logits"][b])
 
-        out2d = st["out"][: mx * B].view(mx, B)
+        out2d = st["out"][: mx * R].view(mx, R)[:, :B]  # the conditional rows; an unconditional row repeats its prompt's tokens
         lens_out = self._run_steps(launch, out2d, budgets, eos, stopping_fn)
         res = out2d[:max(lens_out)].t().contiguous()
         outs = [res[b, :lens_out[b]].clone() for b in range(B)]

@@ -91,6 +91,55 @@ def refuse_batch_invariant(num_beams: int = 1, processors=None, lookup_k: int = 
         raise NotImplementedError("batch_invariant=True on the tensor-parallel decoder")
 
 
+def refuse_guidance(num_beams: int = 1, processors=None, lookup_k: int = 0, prefix_cache: bool = False, n_ret: int = 1,
+                    output_scores: bool = False, llm=None) -> None:
+    """The generate() options classifier-free guidance (guidance_scale != 1) does not serve: raises NotImplementedError before any GPU
+    work.  Guided decoding runs each prompt and its unconditional branch as two rows of the rows step (LlamaDecoder.generate_rows)."""
+    if num_beams != 1:
+        raise NotImplementedError("guidance_scale with beam search (HF never reorders the unconditional branch's cache with the beams)")
+    if processors is not None:
+        raise NotImplementedError("guidance_scale with logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length): "
+                                  "the rows step runs none")
+    if lookup_k:
+        raise NotImplementedError("guidance_scale with prompt_lookup_num_tokens (the verify pass has no unconditional row)")
+    if prefix_cache:
+        raise NotImplementedError("guidance_scale with prefix_cache=True (guided prompts are prefilled whole)")
+    if n_ret != 1:
+        raise NotImplementedError("guidance_scale with num_return_sequences > 1")
+    if output_scores:
+        raise NotImplementedError("guidance_scale with output_scores (the guided rows are not returned)")
+    if llm is not None and getattr(llm, "fp8", False):
+        raise NotImplementedError("guidance_scale with quantization='fp8' (the rows step has no FP8 form)")
+    if llm is not None and not getattr(llm, "supports_batch_invariant", False):
+        raise NotImplementedError("guidance_scale on the tensor-parallel decoder (the rows step is a single-GPU kernel sequence)")
+
+
+def negative_prompt_rows(negative_prompt_ids, negative_prompt_attention_mask, n_prompts: int, vocab_size: int) -> List[torch.Tensor]:
+    """generate()'s negative_prompt_ids [B, T] (and optional attention mask [B, T], padding on either side) -> the B unpadded id rows
+    (host int64).  Raises ValueError on a shape that does not match the B prompts, a mask that is not one non-empty run of ones per row,
+    or an id outside [0, vocab_size) (IMAGE_TOKEN_INDEX included: the unconditional branch sees no images)."""
+    ids = torch.as_tensor(negative_prompt_ids).detach().to("cpu")
+    if ids.dim() != 2 or ids.shape[0] != n_prompts or ids.shape[1] < 1 or ids.dtype.is_floating_point:
+        raise ValueError(f"negative_prompt_ids must be integer ids [{n_prompts}, T >= 1] (one row per prompt), got {tuple(ids.shape)}")
+    ids = ids.to(torch.int64)
+    lo, hi = int(ids.min()), int(ids.max())
+    if lo < 0 or hi >= vocab_size:
+        raise ValueError(f"negative_prompt_ids holds the id {lo if lo < 0 else hi}, outside the vocabulary [0, {vocab_size}) (image "
+                         f"placeholders such as IMAGE_TOKEN_INDEX = {IMAGE_TOKEN_INDEX} have no place in the unconditional branch)")
+    if negative_prompt_attention_mask is None:
+        return list(ids.unbind(0))
+    am = torch.as_tensor(negative_prompt_attention_mask).detach().to("cpu").bool()
+    if tuple(am.shape) != tuple(ids.shape):
+        raise ValueError(f"negative_prompt_attention_mask {tuple(am.shape)} does not match negative_prompt_ids {tuple(ids.shape)}")
+    rows = []
+    for b in range(n_prompts):
+        idx = torch.nonzero(am[b]).flatten()
+        if idx.numel() == 0 or int(idx[-1]) - int(idx[0]) + 1 != idx.numel():
+            raise ValueError("negative_prompt_attention_mask needs every row to be one non-empty run of ones")
+        rows.append(ids[b, int(idx[0]):int(idx[-1]) + 1])
+    return rows
+
+
 def batch_invariant_groups(B: int, size: int):
     """The (first, end) prompt ranges generate(batch_invariant=True) decodes one after another: groups of `size`, the last one shorter."""
     return [(lo, min(lo + size, B)) for lo in range(0, B, size)]
@@ -624,6 +673,15 @@ class LlavaLlamaModel:
         # the rows step (LlamaDecoder.generate_rows), which streams each weight once and gives every row its one-token arithmetic.
         # ``seed`` may be a list of one seed per prompt; a scalar seed gives prompt b the seed sequence_seeds(seed, B)[b].
         batch_invariant = bool(generation_kwargs.pop("batch_invariant", False))
+        # guidance_scale=g with negative_prompt_ids (opt-in; HF's UnbatchedClassifierFreeGuidanceLogitsProcessor): classifier-free guidance.
+        # Each prompt's unconditional branch is the text model over its negative prompt (no images, masks or depth), continued by the
+        # tokens chosen for the prompt; every token is chosen from g * (log_softmax(cond) - log_softmax(uncond)) + log_softmax(uncond).
+        # The prompt and its branch decode as two rows of the rows step, so row b of the result equals a guided call of prompt b alone.
+        # g = None or 1 is plain generate() (negative prompts ignored, as HF ignores them).
+        guidance_scale = generation_kwargs.pop("guidance_scale", None)
+        negative_prompt_ids = generation_kwargs.pop("negative_prompt_ids", None)
+        negative_prompt_attention_mask = generation_kwargs.pop("negative_prompt_attention_mask", None)
+        guided = guidance_scale is not None and float(guidance_scale) != 1.0
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
         # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
@@ -659,11 +717,23 @@ class LlavaLlamaModel:
         if output_scores and not getattr(self.llm, "supports_output_scores", False):
             raise NotImplementedError("output_scores on the tensor-parallel decoder (its logits are vocabulary-parallel: no rank holds a whole row)")
         n_prompts = 1 if input_ids is None else int(input_ids.shape[0])
+        neg_rows = None
+        if guided:
+            refuse_guidance(num_beams=num_beams, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache, n_ret=n_ret,
+                            output_scores=output_scores, llm=self.llm)
+            if negative_prompt_ids is None:
+                raise ValueError("guidance_scale != 1 needs negative_prompt_ids: the prompt is given as embeddings, so HF's fallback (the "
+                                 "last prompt id) does not exist here")
+            neg_rows = negative_prompt_rows(negative_prompt_ids, negative_prompt_attention_mask, n_prompts, self.llm.dims.vocab_size)
         if isinstance(seed, (list, tuple)):
-            if not batch_invariant:
+            if not batch_invariant and not guided:
                 raise ValueError("a list of seeds needs batch_invariant=True")
             if len(seed) != n_prompts:
                 raise ValueError(f"seed holds {len(seed)} seeds for {n_prompts} prompts")
+        if guided:  # with or without batch_invariant=True: guided rows already decode batch-invariantly
+            return self._generate_batch_invariant(input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id,
+                                                  stopping_criteria, pad_token_id, use_graph, return_logits, return_dict, sampling, seed,
+                                                  guidance=(float(guidance_scale), neg_rows))
         if batch_invariant:
             refuse_batch_invariant(num_beams=num_beams, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache, n_ret=n_ret,
                                    output_scores=output_scores, llm=self.llm)
@@ -772,9 +842,11 @@ class LlavaLlamaModel:
         return self._generate_result(outs, pad_token_id, return_dict, all_logits if return_logits else None, extra, num_beams != 1)
 
     def _generate_batch_invariant(self, input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id, stopping_criteria,
-                                  pad_token_id, use_graph: bool, return_logits: bool, return_dict: bool, sampling, seed):
+                                  pad_token_id, use_graph: bool, return_logits: bool, return_dict: bool, sampling, seed, guidance=None):
         """generate(batch_invariant=True) over B > 1 prompts: every prompt's embeddings by the calls a batch-1 generate() of it makes (its
-        unpadded ids; its images, depth images and masks), then groups of at most ops.SPEC_T_MAX prompts through generate_rows."""
+        unpadded ids; its images, depth images and masks), then groups of at most ops.SPEC_T_MAX prompts through generate_rows.
+        ``guidance`` = (g, the B unpadded negative prompt id rows): classifier-free guidance for any B >= 1, in groups of at most
+        ops.SPEC_T_MAX / 2 prompts (each with its unconditional row); a scalar seed of one prompt is its own seed, as in batch 1."""
         B = int(input_ids.shape[0])
         am = None if attention_mask is None else attention_mask.bool().cpu()
         ids_rows = [input_ids[b] if am is None else input_ids[b][am[b].to(input_ids.device)] for b in range(B)]
@@ -803,14 +875,22 @@ class LlavaLlamaModel:
         if sampling is not None:
             if isinstance(seed, (list, tuple)):
                 seeds = [int(s) for s in seed]
+            elif guidance is not None and B == 1:
+                seeds = [int(torch.initial_seed() if seed is None else seed)]
             else:
                 seeds = sequence_seeds(torch.initial_seed() if seed is None else int(seed), B)
             sampling = dict(sampling, seed=None)
         stop_fn = stopping_fn_of(stopping_criteria)
         outs, all_logits = [], []
-        for lo, hi in batch_invariant_groups(B, ops.SPEC_T_MAX):
+        guide, negs = {}, None
+        if guidance is not None:
+            negs = [self.llm.embed_tokens(r.to(self.device)) for r in guidance[1]]
+            guide = dict(guidance_scale=guidance[0])
+        for lo, hi in batch_invariant_groups(B, ops.SPEC_T_MAX // 2 if guidance is not None else ops.SPEC_T_MAX):
+            if negs is not None:
+                guide["negative_embeds"] = negs[lo:hi]
             r = self.llm.generate_rows(embeds[lo:hi], budgets[lo:hi], eos_token_ids=eos_token_id, stopping_fn=stop_fn, use_graph=use_graph,
-                                       return_logits=return_logits, sampling=sampling, seeds=None if seeds is None else seeds[lo:hi])
+                                       return_logits=return_logits, sampling=sampling, seeds=None if seeds is None else seeds[lo:hi], **guide)
             if return_logits:
                 r, lg = r
                 all_logits.extend(lg)

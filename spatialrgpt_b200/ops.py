@@ -1137,6 +1137,12 @@ class LlamaStack:
         "prefill_chunk_layers", "decode_step", "verify_step" or "decode_rows".  Prefill takes the FP8 or, planes-only, the NF4 stack; the
         decode step and the rows step stream FP8 (the step only), NF4 or packed matrices when there are some; the verify pass NF4
         planes-only or packed ones."""
+        fmt, arrays, lm = self.formats(op)
+        return f"srgpt_llama_{op}_{fmt + '_' if fmt else ''}bf16", arrays, lm
+
+    def formats(self, op: str):
+        """The weight format entry() picks for `op` ("" for the element-type matrices, "packed", "nf4" or "fp8"), the layer array
+        arguments of that format and its lm_head packing arguments."""
         step = op in ("decode_step", "verify_step", "decode_rows")
         nf4 = self.nf4 if op in ("decode_step", "decode_rows") else self.planes
         if self.quantizes_activations:
@@ -1144,15 +1150,15 @@ class LlamaStack:
                 raise SrgptError("the verify pass of prompt-lookup decoding has no FP8 form")
             if op == "decode_rows":
                 raise SrgptError("the batch-invariant decode step has no FP8 form")
-            fmt, arrays = "fp8_", (self.layers,)
+            fmt, arrays = "fp8", (self.layers,)
         elif nf4 is not None:
-            fmt, arrays = "nf4_", (self.layers, nf4)
+            fmt, arrays = "nf4", (self.layers, nf4)
         elif step and self.packed is not None:
-            fmt, arrays = "packed_", (self.layers, self.packed)
+            fmt, arrays = "packed", (self.layers, self.packed)
         else:
             fmt, arrays = "", (self.layers,)
         lm = (C.byref(self._lm_desc),) if step and fmt else ()
-        return f"srgpt_llama_{op}_{fmt}bf16", tuple(C.cast(a, C.c_void_p) for a in arrays), lm
+        return fmt, tuple(C.cast(a, C.c_void_p) for a in arrays), lm
 
 
 def clip_embed(patch_embeds: torch.Tensor, class_embedding: torch.Tensor, position_embedding: torch.Tensor, n_img: int, T: int) -> torch.Tensor:
@@ -1395,12 +1401,59 @@ def rows_advance(workspace: Optional[torch.Tensor], V: int, ids: Optional[torch.
                                          _p(pos_rows), _stream()), "srgpt_rows_advance")
 
 
+def guidance_rows(logits: torch.Tensor, scale: torch.Tensor, guided: torch.Tensor, lse: Optional[torch.Tensor] = None,
+                  ids: Optional[torch.Tensor] = None) -> None:
+    """Classifier-free guidance over the fp32 rows logits [2P, V]: guided [P, V] row b = g * (log_softmax(row b) - log_softmax(row P + b))
+    + log_softmax(row P + b) with g = scale[0] (device fp32), three separately rounded fp32 operations.  ``lse`` (fp32 [2P, 2]): each row's
+    {max, log sum exp(x - max)}.  ``ids`` (int64 [2P]): ids[b] = ids[P + b] = the arg max of guided row b (lowest index on ties, NaN never
+    wins)."""
+    _need(logits, torch.float32, "guidance_rows.logits"); _need(scale, torch.float32, "guidance_rows.scale")
+    _need(guided, torch.float32, "guidance_rows.guided")
+    if logits.dim() != 2 or logits.shape[0] % 2 or not logits.is_contiguous():
+        raise SrgptError(f"guidance_rows: logits must be contiguous fp32 [2P, V], got shape {tuple(logits.shape)}")
+    P, V = logits.shape[0] // 2, logits.shape[1]
+    if tuple(guided.shape) != (P, V) or not guided.is_contiguous():
+        raise SrgptError(f"guidance_rows: guided must be contiguous fp32 [{P}, {V}], got shape {tuple(guided.shape)}")
+    if lse is not None and (lse.dtype != torch.float32 or lse.numel() != 4 * P or not lse.is_contiguous()):
+        raise SrgptError(f"guidance_rows: lse must be contiguous fp32 [{2 * P}, 2]")
+    if ids is not None and (ids.dtype != torch.int64 or ids.numel() != 2 * P or not ids.is_contiguous()):
+        raise SrgptError(f"guidance_rows: ids must be a contiguous int64 vector of {2 * P} entries")
+    check(_lib.load().srgpt_guidance_rows(_p(logits), V, P, _p(scale), _p(guided), _p(lse), _p(ids), _stream()), "srgpt_guidance_rows")
+    _count(1)
+
+
+def guidance_pair_ids(ids: torch.Tensor, P: int) -> None:
+    """ids[P + b] = ids[b] for b < P (int64 [2P])."""
+    _need(ids, torch.int64, "guidance_pair_ids.ids")
+    if ids.numel() < 2 * P:
+        raise SrgptError(f"guidance_pair_ids: ids holds {ids.numel()} entries, needs {2 * P}")
+    check(_lib.load().srgpt_guidance_pair_ids(_p(ids), P, _stream()), "srgpt_guidance_pair_ids")
+    _count(1)
+
+
 def llama_decode_rows(h, stack: LlamaStack, q_buf, attn_buf, act_buf, B: int, dims, cos, sin, pos_rows, page_tables, page_size: int, final_norm,
-                      lm_head, embed, lm_ws, out_ids, step, logits_rows=None, sample_params=None, seeds=None, ids=None) -> None:
+                      lm_head, embed, lm_ws, out_ids, step, logits_rows=None, sample_params=None, seeds=None, ids=None, guidance=None) -> None:
     """One decode step of B sequences, each row bit-identical to that sequence's one-token step (llama_decode_step): the rows layers,
     lm_head over the B rows, then the arg max (or, with ``seeds``, the draw from logits_rows) and the advance.  page_tables is a
-    [>= B, cap] row-major view; row b of h / pos_rows / page_tables is sequence b."""
+    [>= B, cap] row-major view; row b of h / pos_rows / page_tables is sequence b.
+    ``guidance`` = (scale, guided): classifier-free guidance over B = 2P rows, row P + b the unconditional branch of row b
+    (srgpt_llama_decode_rows_guided_bf16): both rows of a pair take the arg max of guided row b, or with ``seeds`` ([P]) the draw from
+    it.  scale is the device fp32 g, guided the fp32 [P, V] rows; ids [B] and logits_rows are needed."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    if guidance is not None:  # one entry point for every format of the rows step: the format's array goes to its own argument
+        fmt, arrays, lm = stack.formats("decode_rows")
+        scale, guided = guidance
+        desc = _lib.Guidance(_p(scale), _p(guided))
+        layers = arrays[0]
+        packed = arrays[1] if fmt == "packed" else None
+        nf4 = arrays[1] if fmt == "nf4" else None
+        check(_lib.load().srgpt_llama_decode_rows_guided_bf16(
+            _p(h), layers, packed, nf4, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), B, dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
+            _p(cos), _p(sin), _p(pos_rows), _p(page_tables), _rowmajor2d(page_tables, "llama_decode_rows.page_tables"), page_size, _p(final_norm),
+            _p(lm_head), lm[0] if lm else None, dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(sample_params), _p(seeds), _p(ids),
+            _p(out_ids), _p(step), C.byref(desc), _stream()), "srgpt_llama_decode_rows_guided_bf16")
+        _count(stack.rows_kernels + (3 if seeds is not None else 1))
+        return
     name, arrays, lm = stack.entry("decode_rows")
     check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), B, dims.hidden_size, nh, nkv, hd, I,
                                      dims.rms_norm_eps, _p(cos), _p(sin), _p(pos_rows), _p(page_tables),
