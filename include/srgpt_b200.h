@@ -677,6 +677,35 @@ int srgpt_llama_decode_rows_guided_bf16(void* h, const srgpt_llama_layer_weights
                                         float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
                                         long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream);
 
+/* ---- contrastive search (contrastive.cu, beam.cu): replaces _ranking_fast and the candidate bookkeeping of HF
+ * GenerationMixin.contrastive_search (transformers 4.37.2 generation/utils.py), which generate() runs behind llava_llama.py:212 when
+ * num_beams == 1, do_sample is false, penalty_alpha > 0 and top_k > 1.  B prompts x k candidates decode as rows g * k + i of the
+ * batched step; every prompt keeps its context, the final-norm hidden rows of its positions so far (HF's last_hidden_states), in
+ * ctx [B, L_cap, H] (element type); prompt g's context length is pos[g * k], the position its candidates are processed at.
+ * srgpt_contrastive_partial_floats: the fp32 entries of the penalty's per-chunk maxima for (B, k, L_cap) (-1 on invalid arguments). */
+long long srgpt_contrastive_partial_floats(int B, int k, int L_cap);
+/* The degeneration penalty, first pass: cand [B * k, ldc] (the step's final-norm rows) against ctx[g, 0 .. pos[g * k]).  One CTA per
+ * (32 context rows, prompt); each context row's norm and its dot products with the candidates (staged in shared memory, 8 at a time)
+ * in one pass, fp32 accumulation.  partial [B, ceil(L_cap / 32), k] = each chunk's largest cosine per candidate (chunks past the
+ * context are not written).  1 <= k <= 64, H % 8 == 0, H <= 12800. */
+int srgpt_contrastive_penalty_bf16(const void* cand, int ldc, const void* ctx, int L_cap, int H, const int* pos, int B, int k, float* partial,
+                                   void* stream);
+/* The choice, one CTA per prompt g: pen[g * k + i] = the largest partial of candidate i over the chunks of the context (fixed order);
+ * score = fl(fl(alpha[0] * exp(cand_scores)) - fl(alpha[1] * pen)) with alpha = device fp32 {1 - penalty_alpha, penalty_alpha};
+ * cand_scores / cand_tokens [B * k] = srgpt_beam_candidates_bf16 over the next-logits rows with zero beam scores.  sel[g] = the
+ * largest score's index (the lowest on ties; a token < 0 never wins).  Then out_ids[*step * B + g] = its token, ctx[g, L] = xn row
+ * g * k + sel (when L < L_cap), next_logits[g] = logits row g * k + sel, pos[g * k + i] = L + 1 for every i, and the last CTA
+ * advances *step.  ticket: one zeroed device uint, returned to zero. */
+int srgpt_contrastive_select_bf16(const float* cand_scores, const int* cand_tokens, const float* partial, const float* alpha, const void* xn, int ldx,
+                                  int H, const void* logits, int ldl, int V, void* ctx, int L_cap, void* next_logits, int ldn, int* pos, int B, int k,
+                                  long long* out_ids, int* step, void* ticket, int* sel, float* pen, float* score, void* stream);
+/* The KV broadcast of a contrastive step (beam.cu): for each prompt g, the K and V of every layer at position pos[g * k + sel[g]] +
+ * pos_offset are copied from row g * k + sel[g] into the other k - 1 rows of the prompt, pages looked up in page_tables [rows, pt_stride]
+ * (the cache's tables, row r = sequence r).  pages as srgpt_kv_copy_pages.  HF keeps the chosen candidate's cache; here the k rows'
+ * histories stay identical, so one position per step is all that moves. */
+int srgpt_kv_broadcast_rows(void* pages, int n_layers, int n_pages, int page_rows, int row_bytes, const int* page_tables, int pt_stride,
+                            const int* pos, int pos_offset, const int* sel, int n_groups, int k, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -151,6 +151,10 @@ SIGNATURES = {
     "srgpt_guidance_pair_ids": (ci, [vp, ci, vp]),
     "srgpt_llama_decode_rows_guided_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp,
                                                  ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_contrastive_partial_floats": (cll, [ci, ci, ci]),
+    "srgpt_contrastive_penalty_bf16": (ci, [vp, ci, vp, ci, ci, vp, ci, ci, vp, vp]),
+    "srgpt_contrastive_select_bf16": (ci, [vp, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_kv_broadcast_rows": (ci, [vp, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci, ci, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)

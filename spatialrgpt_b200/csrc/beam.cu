@@ -1,6 +1,6 @@
 // Device side of beam search over a batch of prompts (llama_decoder.generate_beam_batch; DESIGN.md §7): the per-prompt merge of the
 // beam rows' candidates, and the KV page copies that replicate each prompt into its beams and make a beam's generated rows follow
-// its parent.
+// its parent.  Also the one-position KV broadcast of contrastive search (llama_decoder.generate_contrastive).
 #include "common.cuh"
 #include "srgpt_b200.h"
 
@@ -76,6 +76,37 @@ kv_copy_kernel(uint8_t* __restrict__ pages, int n_pages, int page_rows, int row_
   for (int c = threadIdx.x; c < n16; c += COPY_THREADS) reinterpret_cast<uint4*>(dst)[c] = reinterpret_cast<const uint4*>(src)[c];
 }
 
+// Contrastive search keeps the k rows of a prompt identical: after the choice, row g * k + sel[g] holds the only K / V of the position
+// just written that the prompt keeps.  blockIdx.x = layer * 2 + (0: K, 1: V), blockIdx.y = prompt g; each thread reads one 16-byte
+// piece of the chosen row once and writes it to the k - 1 siblings.  The position is pos[g * k + sel[g]] + pos_offset; a page id outside
+// the cache, a position outside the page table or a selection outside [0, k) leaves the prompt untouched.
+__global__ void __launch_bounds__(COPY_THREADS)
+kv_broadcast_kernel(uint8_t* __restrict__ pages, int n_pages, int page_rows, int row_bytes, const int* __restrict__ page_tables, int pt_stride,
+                    const int* __restrict__ pos, int pos_offset, const int* __restrict__ sel, int k) {
+  const int g = blockIdx.y, s = sel[g];
+  if (s < 0 || s >= k) return;
+  const int src_row = g * k + s;
+  const int p = pos[src_row] + pos_offset;
+  if (p < 0 || p / page_rows >= pt_stride) return;
+  const int j = p / page_rows;
+  const int src_page = page_tables[(size_t)src_row * pt_stride + j];
+  if (src_page < 0 || src_page >= n_pages) return;
+  const int layer = blockIdx.x >> 1, half = blockIdx.x & 1;
+  const size_t half_bytes = (size_t)page_rows * row_bytes;
+  const size_t in_page = (size_t)half * half_bytes + (size_t)(p - j * page_rows) * row_bytes;
+  uint8_t* base = pages + (size_t)layer * n_pages * 2 * half_bytes;
+  const uint4* src = reinterpret_cast<const uint4*>(base + (size_t)src_page * 2 * half_bytes + in_page);
+  const int n16 = row_bytes / 16;
+  for (int c = threadIdx.x; c < n16; c += COPY_THREADS) {
+    const uint4 v = src[c];
+    for (int i = 0; i < k; ++i) {
+      const int dst_page = page_tables[(size_t)(g * k + i) * pt_stride + j];
+      if (i == s || dst_page < 0 || dst_page >= n_pages) continue;
+      reinterpret_cast<uint4*>(base + (size_t)dst_page * 2 * half_bytes + in_page)[c] = v;
+    }
+  }
+}
+
 }  // namespace srgpt
 
 using namespace srgpt;
@@ -113,5 +144,17 @@ extern "C" __attribute__((visibility("default"))) int srgpt_kv_copy_pages(void* 
                                                                            n_staged, ws, 1);
     SRGPT_CHECK_LAUNCH();
   }
+  return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_kv_broadcast_rows(void* pages, int n_layers, int n_pages, int page_rows, int row_bytes,
+                                                                              const int* page_tables, int pt_stride, const int* pos, int pos_offset,
+                                                                              const int* sel, int n_groups, int k, void* stream) {
+  SRGPT_CHECK_ARG(pages && page_tables && pos && sel && n_layers > 0 && n_pages > 0 && page_rows > 0 && row_bytes > 0 && (row_bytes % 16) == 0);
+  SRGPT_CHECK_ARG(pt_stride > 0 && n_groups > 0 && n_groups <= 65535 && k >= 1 && 2 * n_layers <= 65535);
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(pages) & 15) == 0);
+  kv_broadcast_kernel<<<dim3(2 * n_layers, n_groups), COPY_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<uint8_t*>(pages), n_pages, page_rows, row_bytes, page_tables, pt_stride, pos, pos_offset, sel, k);
+  SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }

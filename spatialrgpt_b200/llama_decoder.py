@@ -83,15 +83,16 @@ def decode_steps(launch, fetch, host, budgets: List[int], eos, stopping_fn) -> L
 
 
 class GraphKey(NamedTuple):
-    """What a captured graph computes: its kind ("step", "batch", "rows", "beam" or "verify"), its rows (T for a verify pass), whether
-    it samples, whether the logits processors run, the (address, step stride) of the score rows it writes (output_scores), and the
-    n-gram size of a verify pass."""
+    """What a captured graph computes: its kind ("step", "batch", "rows", "beam", "verify" or "contrastive"), its rows (T for a verify
+    pass), whether it samples, whether the logits processors run, the (address, step stride) of the score rows it writes (output_scores),
+    the n-gram size of a verify pass, and the candidates per prompt of a contrastive step (B * k rows)."""
     kind: str
     rows: int = 1
     sample: bool = False
     proc: bool = False
     scores: Optional[tuple] = None
     ngram: int = 0
+    group: int = 0
 
 
 class BeamHypotheses:
@@ -405,6 +406,7 @@ class LlamaDecoder:
     supports_batch_sampling = True  # sampled batches run in the batched step (generate_batch), num_return_sequences included
     supports_output_scores = True  # generate(output_scores=True): the decode steps write each token's score row on the device
     supports_batch_invariant = True  # generate(batch_invariant=True): generate_rows, each row bit-identical to batch 1
+    supports_contrastive = True  # generate(penalty_alpha=, top_k=): generate_contrastive
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
@@ -746,11 +748,12 @@ class LlamaDecoder:
         self.cache.reserve_many([n + max_new_tokens + slack for n in prompt_lens])
 
     def _prefill_first_token(self, embeds: torch.Tensor, seq: int, reuse_rows: int, logits_row: Optional[torch.Tensor], sample: bool,
-                             proc: bool, scores: Optional[torch.Tensor]) -> None:
+                             proc: bool, scores: Optional[torch.Tensor]) -> torch.Tensor:
         """Batch 1's prefill of the prompt ``embeds`` [S, H] into sequence `seq` (its first reuse_rows rows are in the pages already)
         and its first token: final norm + lm_head + arg max on the last row, which writes out_ids[0], the token's embedding row (h)
         and pos = S, step = 1; then _choose.  The fp32 logits go to ``logits_row``, or to the sample buffer when the choice reads
-        them.  generate_rows starts every row with it, so each row's first token is its batch-1 request's by construction."""
+        them.  generate_rows starts every row with it, so each row's first token is its batch-1 request's by construction.  Returns
+        the prefill's final residual stream of rows reuse_rows .. S - 1."""
         d, w = self.dims, self.w
         S = embeds.shape[0]
         hidden = self.prefill_hidden(embeds[reuse_rows:], seq, reuse_rows)
@@ -761,6 +764,7 @@ class LlamaDecoder:
         ops.lm_head_argmax(hidden[S - 1 - reuse_rows], w.lm_head, w.norm, d.rms_norm_eps, self.lm_ws, self.out_ids, self.step, self.pos,
                            embed_table=w.embed, next_x=self.h, logits_out=logits_row)
         self._choose(logits_row, sample, proc, scores)
+        return hidden
 
     def _set_sampling(self, sampling) -> bool:
         """sampling = None (greedy) or dict(temperature=, top_p=, top_k=, seed=).  Returns True when tokens are sampled."""
@@ -948,7 +952,7 @@ class LlamaDecoder:
         st = self._bstate
         if st is not None and st["B"] == B:
             return st
-        self._drop_graphs(lambda key: key.kind in ("batch", "beam"))  # they read the buffers replaced here
+        self._drop_graphs(lambda key: key.kind in ("batch", "beam", "contrastive"))  # they read the buffers replaced here
         d, dev = self.dims, self.device
         H, nh, nkv, hd, I, V = d.hidden_size, d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.intermediate_size, d.vocab_size
         z = lambda *shape, dtype=self.dtype: torch.zeros(shape, dtype=dtype, device=dev)  # noqa: E731
@@ -1243,6 +1247,116 @@ class LlamaDecoder:
                 self._batch_step_launch(st, logits_only=True)
         best = torch.tensor(hyp.best(max_new_tokens), dtype=torch.int64, device=dev)
         return (best, self._beam_extra(rows_out, step + 1, [hyp])) if output_scores else best
+
+    # ---- contrastive search: B prompts x k candidates per step in the batched step, the choice made on the device ----------------
+    def _contrastive_state(self, B: int, k: int, L_cap: int):
+        """The batched step's buffers of B * k rows and contrastive search's own: each prompt's context rows ctx [B, L_cap, H], its
+        next-logits row, the candidates, the penalty's chunk maxima and the choice.  A captured step holds their addresses, so they are
+        replaced (and the contrastive graphs dropped) only when (B, k) changes or a request needs a longer context."""
+        st = self._batch_state(B * k)
+        cs = st.get("contrastive")
+        if cs is not None and (cs["B"], cs["k"]) == (B, k) and cs["L_cap"] >= L_cap:
+            return st, cs
+        self._drop_graphs(lambda key: key.kind == "contrastive")
+        st["contrastive"] = None
+        d, dev = self.dims, self.device
+        L_cap = min((L_cap + 127) // 128 * 128, self.max_seq_len)  # a little slack, so nearby request lengths share the graph
+        V = d.vocab_size
+        cs = dict(B=B, k=k, L_cap=L_cap, ctx=torch.zeros((B, L_cap, d.hidden_size), dtype=self.dtype, device=dev),
+                  next=torch.zeros((B, (V + 7) // 8 * 8), dtype=self.dtype, device=dev)[:, :V],
+                  zero=torch.zeros(B, dtype=torch.float32, device=dev), cand_s=torch.zeros((B, k), dtype=torch.float32, device=dev),
+                  cand_t=torch.zeros((B, k), dtype=torch.int32, device=dev), src_id=torch.zeros(B * k, dtype=torch.int32, device=dev),
+                  partial=ops.contrastive_partial(B, k, L_cap, dev), alpha=torch.zeros(2, dtype=torch.float32, device=dev),
+                  sel=torch.zeros(B, dtype=torch.int32, device=dev), pen=torch.zeros((B, k), dtype=torch.float32, device=dev),
+                  score=torch.zeros((B, k), dtype=torch.float32, device=dev))
+        st["contrastive"] = cs
+        return st, cs
+
+    def _contrastive_step_launch(self, st, cs, scores: Optional[torch.Tensor] = None) -> None:
+        """One contrastive step: (the next-logits rows to scores[step]), their k candidates each, the B * k candidate tokens through the
+        batched step, the degeneration penalty, the choice, and the chosen row's K / V at the new position copied into its siblings."""
+        k, V = cs["k"], self.dims.vocab_size
+        if scores is not None:
+            ops.step_scores(cs["next"], st["step"], 0, scores)
+        ops.beam_candidates(cs["next"], cs["zero"], cs["cand_s"], cs["cand_t"])
+        ops.splice_rows(self.w.embed, None, None, None, cs["src_id"], cs["cand_t"].view(-1), out=st["h"])
+        self._batch_step_launch(st, logits_only=True)
+        ops.contrastive_penalty(st["xn"], cs["ctx"], st["pos"], k, cs["partial"])
+        ops.contrastive_select(cs["cand_s"], cs["cand_t"], cs["partial"], cs["alpha"], st["xn"], st["logits"][:, :V], cs["ctx"], cs["next"],
+                               st["pos"], st["out"], st["step"], st["ticket"], cs["sel"], cs["pen"], cs["score"])
+        ops.kv_broadcast_rows(self.cache.pages, self.cache.page_tables, st["pos"], -1, cs["sel"], k)
+
+    @torch.no_grad()
+    @ops.in_own_dtype
+    def generate_contrastive(self, packed_embeds: torch.Tensor, seq_lens: List[int], top_k: int, penalty_alpha: float, max_new_tokens: int,
+                             eos_token_ids=None, stopping_fn=None, use_graph: bool = True, output_scores: bool = False):
+        """Contrastive search (HF GenerationMixin.contrastive_search + _ranking_fast, transformers 4.37.2) over B prompts packed back to
+        back ([sum S_b, H]).  Row g * k + i of every step is candidate i of prompt g: ONE packed prefill into row g * k (B = 1: batch 1's
+        prefill and lm_head, so the first logits row is greedy generate()'s), the prompt pages copied into the other k - 1 rows, every
+        prompt row's final norm into its context (HF's last_hidden_states), lm_head on the last row into its next-logits row.  Then each
+        token is one step (one graph replay): the k most probable tokens of the next-logits row (beam_candidates), all B * k of them
+        through the batched step, pen = the largest cosine of each candidate's final-norm row against the prompt's context, score =
+        (1 - alpha) * p - alpha * pen, the best candidate emitted (lowest index on ties), its row appended to the context, its logits
+        row the next one, and its K / V at the new position copied into its siblings, so the k rows' histories stay identical.
+        EOS and ``stopping_fn`` are checked per prompt; a prompt that has stopped keeps its rows in the step.  Returns a list of B
+        LongTensors of new ids; ``output_scores``: (ids, {"scores": fp32 [n_max, B, V]}), scores[t, g] the next-logits row token t of
+        prompt g was chosen from (widened exactly).  HF pads a batch on the left and its pad rows join the context; packed prompts have
+        no pad rows, so the context is the prompt's own rows (the same for batch 1 and unpadded batches)."""
+        d, w, k, B = self.dims, self.w, int(top_k), len(seq_lens)
+        V, R, dev = d.vocab_size, B * int(top_k), self.device
+        seq_lens = [int(n) for n in seq_lens]
+        alpha = float(penalty_alpha)
+        if not 2 <= k <= 64:
+            raise ValueError(f"generate_contrastive needs 2 <= top_k <= 64, got {k}")
+        if not 0.0 <= alpha <= 1.0:
+            raise ValueError(f"generate_contrastive needs 0 <= penalty_alpha <= 1, got {penalty_alpha}")
+        if B < 1 or packed_embeds.shape[0] != sum(seq_lens) or min(seq_lens) < 1:
+            raise RuntimeError("generate_contrastive: rows do not match seq_lens")
+        if max_new_tokens < 1:
+            empty = [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
+            return (empty, {"scores": torch.empty((0, B, V), dtype=torch.float32, device=dev)}) if output_scores else empty
+        eos = eos_list(eos_token_ids)
+        starts = [n for n in seq_lens for _ in range(k)]  # row g * k + i: the first generated position of prompt g
+        self._start_request(starts, max_new_tokens)
+        tables = [list(self.cache.owned[r]) for r in range(R)]
+        st, cs = self._contrastive_state(B, k, max(seq_lens) + max_new_tokens)
+        ctx, nxt = cs["ctx"], cs["next"]
+        if B == 1:
+            first = self._sample_buffer()
+            hidden = self._prefill_first_token(packed_embeds, 0, 0, first, False, False, None)
+            nxt[0].copy_(first)  # lm_head_argmax's fp32 row holds element-type values: exact
+        else:
+            hidden = self.prefill_packed(packed_embeds, seq_lens, page_tables=self.cache.page_tables[:R:k])
+        ops.kv_copy_pages(self.cache.pages, prompt_page_pairs(tables, seq_lens, k))
+        off = 0
+        for g, n in enumerate(seq_lens):
+            ops.rmsnorm(hidden[off:off + n], w.norm, d.rms_norm_eps, out=ctx[g, :n])
+            off += n
+        if B > 1:  # the last prompt rows' final norm is in the context already
+            last = torch.tensor([g * cs["L_cap"] + n - 1 for g, n in enumerate(seq_lens)], dtype=torch.int32).to(dev)
+            rows = ops.splice_rows(ctx.view(-1, d.hidden_size), None, None, None, torch.zeros_like(last), last)
+            ops.gemm(rows, w.lm_head, out=nxt)
+        cs["alpha"].copy_(torch.tensor([1.0 - alpha, alpha], dtype=torch.float64).float())
+        st["pos"].copy_(torch.tensor(starts, dtype=torch.int32))
+        st["step"].zero_()
+        scores = self._scores_view(max_new_tokens, B) if output_scores else None
+        key = GraphKey("contrastive", R, scores=self._scores_key(scores), group=k)
+        if use_graph:  # the warm-up before the capture writes only this step's own rows, which the first replay writes again
+            self._capture(key, lambda: self._contrastive_step_launch(st, cs, scores), (st["pos"], st["step"], nxt),
+                          self._batch_kernels_per_layer * d.num_hidden_layers + 7 + (1 if scores is not None else 0))
+
+        def launch(n: int) -> None:
+            if use_graph:
+                self._replay(key)
+            else:
+                self._contrastive_step_launch(st, cs, scores)
+
+        launch(0)  # token 0 needs a step of its own: the prefill gave only the row its candidates come from
+        out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
+        lens = self._run_steps(launch, out2d, [max_new_tokens] * B, eos, stopping_fn)
+        res = out2d[:max(lens)].t().contiguous()
+        outs = [res[b, :lens[b]].clone() for b in range(B)]
+        return (outs, {"scores": scores[:max(lens)].clone()}) if output_scores else outs
 
     @staticmethod
     def _logprobs_kw(rows_out: Optional[torch.Tensor], step: int) -> dict:

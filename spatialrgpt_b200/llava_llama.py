@@ -6,6 +6,7 @@
 star and llava/model/builder.py:138 use; the reference never defines it)."""
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Any, List, Optional, Sequence, Tuple, Union
 
@@ -112,6 +113,40 @@ def refuse_guidance(num_beams: int = 1, processors=None, lookup_k: int = 0, pref
         raise NotImplementedError("guidance_scale with quantization='fp8' (the rows step has no FP8 form)")
     if llm is not None and not getattr(llm, "supports_batch_invariant", False):
         raise NotImplementedError("guidance_scale on the tensor-parallel decoder (the rows step is a single-GPU kernel sequence)")
+
+
+def refuse_contrastive(top_k: int = 50, processors=None, lookup_k: int = 0, prefix_cache: bool = False, return_logits: bool = False,
+                       guided: bool = False, batch_invariant: bool = False, llm=None) -> None:
+    """The generate() options contrastive search (penalty_alpha > 0, top_k > 1, greedy, one beam) does not serve: raises
+    NotImplementedError before any GPU work.  Contrastive search runs every prompt's top_k candidates as rows of the batched step
+    (LlamaDecoder.generate_contrastive)."""
+    if top_k > 64:
+        raise NotImplementedError(f"contrastive search with top_k = {top_k} > 64 (the candidates of a prompt are ranked in one CTA)")
+    if processors is not None:
+        raise NotImplementedError("penalty_alpha with logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length)")
+    if lookup_k:
+        raise NotImplementedError("penalty_alpha with prompt_lookup_num_tokens (the verify pass checks greedy choices)")
+    if prefix_cache:
+        raise NotImplementedError("penalty_alpha with prefix_cache=True (the context needs every prompt row's hidden state)")
+    if return_logits:
+        raise NotImplementedError("penalty_alpha with output_logits")
+    if guided:
+        raise NotImplementedError("penalty_alpha with guidance_scale != 1")
+    if batch_invariant:
+        raise NotImplementedError("penalty_alpha with batch_invariant=True (the candidates run in the batched step)")
+    if llm is not None and not getattr(llm, "supports_contrastive", False):
+        raise NotImplementedError("penalty_alpha on the tensor-parallel decoder")
+
+
+def contrastive_alpha(penalty_alpha) -> float:
+    """generate()'s penalty_alpha as a float, ValueError unless it is a finite number in [0, 1]."""
+    try:
+        a = float(penalty_alpha)
+    except (TypeError, ValueError):
+        raise ValueError(f"penalty_alpha must be a number in [0, 1], got {penalty_alpha!r}") from None
+    if isinstance(penalty_alpha, bool) or not math.isfinite(a) or not 0.0 <= a <= 1.0:
+        raise ValueError(f"penalty_alpha must be a finite number in [0, 1], got {penalty_alpha!r}")
+    return a
 
 
 def negative_prompt_rows(negative_prompt_ids, negative_prompt_attention_mask, n_prompts: int, vocab_size: int) -> List[torch.Tensor]:
@@ -682,6 +717,13 @@ class LlavaLlamaModel:
         negative_prompt_ids = generation_kwargs.pop("negative_prompt_ids", None)
         negative_prompt_attention_mask = generation_kwargs.pop("negative_prompt_attention_mask", None)
         guided = guidance_scale is not None and float(guidance_scale) != 1.0
+        # penalty_alpha=a with top_k=k (HF's contrastive search): when num_beams == 1, do_sample is false, a > 0 and k > 1 (top_k defaults
+        # to 50, as HF's GenerationConfig), every token is chosen among the k most probable by (1 - a) * p - a * (the largest cosine of
+        # the candidate's hidden state against the sequence's earlier ones).  Otherwise penalty_alpha is ignored, as HF ignores it.
+        penalty_alpha = generation_kwargs.pop("penalty_alpha", None)
+        contrastive_k = 50 if top_k is None else int(top_k)
+        contrastive = (penalty_alpha is not None and contrastive_alpha(penalty_alpha) > 0.0 and contrastive_k > 1 and num_beams == 1
+                       and not do_sample)
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
         # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
@@ -717,6 +759,9 @@ class LlavaLlamaModel:
         if output_scores and not getattr(self.llm, "supports_output_scores", False):
             raise NotImplementedError("output_scores on the tensor-parallel decoder (its logits are vocabulary-parallel: no rank holds a whole row)")
         n_prompts = 1 if input_ids is None else int(input_ids.shape[0])
+        if contrastive:
+            refuse_contrastive(top_k=contrastive_k, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache,
+                               return_logits=return_logits, guided=guided, batch_invariant=batch_invariant, llm=self.llm)
         neg_rows = None
         if guided:
             refuse_guidance(num_beams=num_beams, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache, n_ret=n_ret,
@@ -780,7 +825,15 @@ class LlavaLlamaModel:
         if lookup_k and B != 1:
             raise NotImplementedError("prompt_lookup_num_tokens serves batch-1 requests")
         left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
-        if B == 1 and num_beams != 1:
+        if contrastive:  # any B: the prompts' unpadded rows, packed
+            if packed is None:
+                T = inputs_embeds.shape[1]
+                packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
+            outs = self.llm.generate_contrastive(packed, lens, contrastive_k, contrastive_alpha(penalty_alpha), int(max_new_tokens),
+                                                 eos_token_ids=eos_token_id, stopping_fn=stop_fn, use_graph=use_graph, **sc_kw)
+            if output_scores:
+                outs, extra = outs
+        elif B == 1 and num_beams != 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
             r = self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,

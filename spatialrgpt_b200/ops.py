@@ -200,7 +200,9 @@ def patchify(images: torch.Tensor, patch: int, ldk: int) -> torch.Tensor:
     return out
 
 
-def splice_rows(src0: torch.Tensor, src1, src2, src3, src_id: torch.Tensor, src_row: torch.Tensor) -> torch.Tensor:
+def splice_rows(src0: torch.Tensor, src1, src2, src3, src_id: torch.Tensor, src_row: torch.Tensor,
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[r] = row src_row[r] of source src_id[r] (a fresh [rows, cols] tensor, or ``out``, contiguous)."""
     _need(src0, ELEM(), "splice.src0"); _need(src_id, torch.int32, "splice.src_id"); _need(src_row, torch.int32, "splice.src_row")
     cols = src0.shape[-1]
     rows = src_id.numel()
@@ -209,7 +211,12 @@ def splice_rows(src0: torch.Tensor, src1, src2, src3, src_id: torch.Tensor, src_
             _need(s, ELEM(), "splice.src")
             if s.shape[-1] != cols or not s.is_contiguous():
                 raise SrgptError("splice: all sources must be contiguous with the same width")
-    out = torch.empty((rows, cols), dtype=ELEM(), device=src0.device)
+    if out is None:
+        out = torch.empty((rows, cols), dtype=ELEM(), device=src0.device)
+    else:
+        _need(out, ELEM(), "splice.out")
+        if tuple(out.shape) != (rows, cols) or not out.is_contiguous():
+            raise SrgptError(f"splice: out must be contiguous [{rows}, {cols}], got shape {tuple(out.shape)}")
     check(_lib.load().srgpt_splice_rows_bf16(_p(src0), _p(src1), _p(src2), _p(src3), _p(src_id), _p(src_row), _p(out), rows,
                                              cols, _stream()), "srgpt_splice_rows_bf16")
     return out
@@ -1044,6 +1051,87 @@ def kv_copy_pages(pages: torch.Tensor, pairs, n_staged: int = 0) -> None:
                                   ws_bytes if n_staged else 0, _stream()), "srgpt_kv_copy_pages")
     if n_staged:
         _count(1)
+
+
+def kv_broadcast_rows(pages: torch.Tensor, page_tables: torch.Tensor, pos: torch.Tensor, pos_offset: int, sel: torch.Tensor, k: int) -> None:
+    """Contrastive search's KV broadcast: for each prompt g (sel int32 [G]), the K / V of every layer at position pos[g * k + sel[g]] +
+    pos_offset of row g * k + sel[g] -> the same position of rows g * k + i, i != sel[g].  page_tables: the cache's int32 [rows, cap]
+    tables (row r = sequence r, G * k <= rows); pos: int32 [>= G * k]."""
+    if not pages.is_cuda or pages.dim() != 6 or not pages.is_contiguous():
+        raise SrgptError("kv_broadcast_rows: expected the contiguous CUDA KV cache [L, n_pages, 2, page_rows, n_kv_heads, head_dim]")
+    _need(page_tables, torch.int32, "kv_broadcast_rows.page_tables"); _need(pos, torch.int32, "kv_broadcast_rows.pos")
+    _need(sel, torch.int32, "kv_broadcast_rows.sel")
+    G = sel.numel()
+    if k < 1 or G < 1 or not sel.is_contiguous() or not pos.is_contiguous() or pos.numel() < G * k:
+        raise SrgptError(f"kv_broadcast_rows: needs k >= 1, a contiguous sel [G >= 1] and pos of at least G * k entries")
+    if page_tables.dim() != 2 or page_tables.shape[0] < G * k:
+        raise SrgptError(f"kv_broadcast_rows: page_tables must be [>= {G * k}, cap], got shape {tuple(page_tables.shape)}")
+    L, n_pages, _, page_rows = pages.shape[:4]
+    row_bytes = pages.shape[4] * pages.shape[5] * pages.element_size()
+    check(_lib.load().srgpt_kv_broadcast_rows(_p(pages), L, n_pages, page_rows, row_bytes, _p(page_tables),
+                                              _rowmajor2d(page_tables, "kv_broadcast_rows.page_tables"), _p(pos), pos_offset, _p(sel), G, k,
+                                              _stream()), "srgpt_kv_broadcast_rows")
+
+
+def contrastive_partial(B: int, k: int, L_cap: int, device) -> torch.Tensor:
+    """The fp32 buffer of contrastive_penalty's per-chunk maxima for B prompts of k candidates over contexts of at most L_cap rows."""
+    n = int(_lib.load().srgpt_contrastive_partial_floats(B, k, L_cap))
+    if n < 0:
+        raise SrgptError(f"contrastive_partial: invalid B={B}, k={k}, L_cap={L_cap}")
+    return torch.empty(n, dtype=torch.float32, device=device)
+
+
+def contrastive_penalty(cand: torch.Tensor, ctx: torch.Tensor, pos: torch.Tensor, k: int, partial: torch.Tensor) -> None:
+    """Degeneration penalty, first pass: the B * k rows of ``cand`` ([B * k, H], unit inner stride) against each prompt's context rows
+    ctx[g, 0 .. pos[g * k]) (ctx contiguous [B, L_cap, H]) -> partial (contrastive_partial(B, k, L_cap)) = each 32-row chunk's largest
+    cosine per candidate."""
+    _need(cand, ELEM(), "contrastive_penalty.cand"); _need(ctx, ELEM(), "contrastive_penalty.ctx")
+    _need(pos, torch.int32, "contrastive_penalty.pos"); _need(partial, torch.float32, "contrastive_penalty.partial")
+    if ctx.dim() != 3 or not ctx.is_contiguous():
+        raise SrgptError(f"contrastive_penalty: ctx must be contiguous [B, L_cap, H], got shape {tuple(ctx.shape)}")
+    B, L_cap, H = ctx.shape
+    if not 1 <= k <= 64 or tuple(cand.shape) != (B * k, H):
+        raise SrgptError(f"contrastive_penalty: needs 1 <= k <= 64 and cand [{B} * k, {H}], got k={k}, shape {tuple(cand.shape)}")
+    if pos.numel() < B * k or not pos.is_contiguous():
+        raise SrgptError(f"contrastive_penalty: pos must be a contiguous int32 vector of at least {B * k} entries")
+    if partial.numel() < _lib.load().srgpt_contrastive_partial_floats(B, k, L_cap) or not partial.is_contiguous():
+        raise SrgptError("contrastive_penalty: partial is smaller than contrastive_partial(B, k, L_cap)")
+    check(_lib.load().srgpt_contrastive_penalty_bf16(_p(cand), _rowmajor2d(cand, "contrastive_penalty.cand"), _p(ctx), L_cap, H, _p(pos), B, k,
+                                                     _p(partial), _stream()), "srgpt_contrastive_penalty_bf16")
+
+
+def contrastive_select(cand_scores: torch.Tensor, cand_tokens: torch.Tensor, partial: torch.Tensor, alpha: torch.Tensor, xn: torch.Tensor,
+                       logits: torch.Tensor, ctx: torch.Tensor, next_logits: torch.Tensor, pos: torch.Tensor, out_ids: torch.Tensor,
+                       step: torch.Tensor, ticket: torch.Tensor, sel: torch.Tensor, pen: torch.Tensor, score: torch.Tensor) -> None:
+    """Contrastive search's choice for B prompts of k candidates (cand_scores fp32 / cand_tokens int32 [B, k], beam_candidates' log-probs
+    over next_logits): pen = the penalty from ``partial``, score = (1 - a) * exp(log-prob) - a * pen with alpha = fp32 {1 - a, a}; the
+    best candidate (lowest index on ties) -> sel [B], its token -> out_ids[step * B + g], its xn row appended to ctx[g] at pos[g * k],
+    its logits row -> next_logits[g]; the k rows' positions and the step advance.  pen / score: fp32 [B, k]."""
+    _need(cand_scores, torch.float32, "contrastive_select.cand_scores"); _need(cand_tokens, torch.int32, "contrastive_select.cand_tokens")
+    _need(partial, torch.float32, "contrastive_select.partial"); _need(alpha, torch.float32, "contrastive_select.alpha")
+    for t, n in ((xn, "xn"), (logits, "logits"), (ctx, "ctx"), (next_logits, "next_logits")):
+        _need(t, ELEM(), "contrastive_select." + n)
+    _need(pos, torch.int32, "contrastive_select.pos"); _need(out_ids, torch.int64, "contrastive_select.out_ids")
+    _need(step, torch.int32, "contrastive_select.step"); _need(ticket, torch.int32, "contrastive_select.ticket")
+    _need(sel, torch.int32, "contrastive_select.sel"); _need(pen, torch.float32, "contrastive_select.pen")
+    _need(score, torch.float32, "contrastive_select.score")
+    if cand_scores.dim() != 2 or cand_tokens.shape != cand_scores.shape or not cand_scores.is_contiguous() or not cand_tokens.is_contiguous():
+        raise SrgptError("contrastive_select: candidates must be contiguous [B, k] scores and tokens")
+    B, k = cand_scores.shape
+    if not 1 <= k <= 64 or ctx.dim() != 3 or not ctx.is_contiguous() or ctx.shape[0] != B:
+        raise SrgptError(f"contrastive_select: needs 1 <= k <= 64 and a contiguous ctx [{B}, L_cap, H]")
+    _, L_cap, H = ctx.shape
+    V = logits.shape[1]
+    if tuple(xn.shape) != (B * k, H) or logits.shape[0] != B * k or tuple(next_logits.shape) != (B, V):
+        raise SrgptError(f"contrastive_select: xn must be [{B * k}, {H}], logits [{B * k}, V] and next_logits [{B}, V]")
+    if partial.numel() < _lib.load().srgpt_contrastive_partial_floats(B, k, L_cap) or alpha.numel() != 2:
+        raise SrgptError("contrastive_select: partial is smaller than contrastive_partial(B, k, L_cap), or alpha is not {1 - a, a}")
+    if pos.numel() < B * k or sel.numel() != B or pen.numel() != B * k or score.numel() != B * k or out_ids.numel() < B:
+        raise SrgptError(f"contrastive_select: pos needs {B * k} entries, sel {B}, pen and score {B * k}, out_ids at least {B}")
+    check(_lib.load().srgpt_contrastive_select_bf16(
+        _p(cand_scores), _p(cand_tokens), _p(partial), _p(alpha), _p(xn), _rowmajor2d(xn, "contrastive_select.xn"), H, _p(logits),
+        _rowmajor2d(logits, "contrastive_select.logits"), V, _p(ctx), L_cap, _p(next_logits), _rowmajor2d(next_logits, "contrastive_select.next_logits"),
+        _p(pos), B, k, _p(out_ids), _p(step), _p(ticket), _p(sel), _p(pen), _p(score), _stream()), "srgpt_contrastive_select_bf16")
 
 
 def argmax_f32(x: torch.Tensor) -> torch.Tensor:
