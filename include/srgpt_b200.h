@@ -168,6 +168,15 @@ int srgpt_attention_prefill_paged_bf16(const void* q, int q_ld, void* out, int o
                                        const int* page_tables, int page_table_stride, int page_size, const int* start_pos,
                                        const int* cu_seqlens, int n_seqs, int max_rows, int total_rows, int n_heads, int n_kv_heads,
                                        int head_dim, float scale, void* stream);
+/* Causal attention probabilities (attention_probs.cu; HF eager attention's softmax(Q K^T * scale + causal mask) in fp32, cast to the
+ * element type), the S x S matrix the kernels above never build.  q / k: the rotated q and k columns of n_seqs sequences packed back to
+ * back (cu_seqlens device int32 [n_seqs + 1]; NULL: one sequence of max_seqlen rows), row strides q_ld / k_ld; query head h reads kv head
+ * h / (n_heads / n_kv_heads).  Sequence b's probabilities go to out + b * seq_stride + h * head_stride, an out_rows x out_rows block with
+ * row stride ld (elements), its local row / column i at row / column row_off[b] + i (device int32 [n_seqs]; NULL: 0).  Every entry of the
+ * block is written: entries above the diagonal and at rows / columns outside the sequence are 0.  head_dim 128 only. */
+int srgpt_attention_probs_bf16(const void* q, int q_ld, const void* k, int k_ld, int n_seqs, const int* cu_seqlens, int max_seqlen, int n_heads,
+                               int n_kv_heads, int head_dim, float scale, void* out, long long seq_stride, long long head_stride, long long ld,
+                               int out_rows, const int* row_off, void* stream);
 /* flags[r] = 1 when rows r of a and b ([rows, row_bytes] bytes, rows contiguous) are bitwise equal, else 0 (rowops.cu).  The
  * prompt-prefix cache of generate(prefix_cache=True) compares a request's images / depths / masks with the previous ones. */
 int srgpt_rows_equal(const void* a, const void* b, int rows, long long row_bytes, int* flags, void* stream);
@@ -522,6 +531,29 @@ int srgpt_llama_prefill_chunk_layers_fp8_bf16(void* x, const srgpt_llama_layer_f
                                               int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
                                               const int* page_tables, int page_table_stride, int page_size, int n_pages, int n_seqs,
                                               const int* cu_seqlens, int max_rows, void* stream);
+/* What srgpt_llama_prefill_layers_probe_bf16 records (forward(output_hidden_states=, output_attentions=)).  Outputs are padded per
+ * sequence: sequence b's local row i is output row row_off[b] + i (device int32 [n_seqs]) of blocks of out_rows rows; strides in elements.
+ * hidden != NULL: before layer l the residual rows x go to hidden + l * hidden_layer_stride + b * hidden_seq_stride + row * hidden_ld
+ *   (slots 0 .. n_layers - 1: the embeddings, then the residual stream after each layer but the last).
+ * attn != NULL: layer l's probabilities (srgpt_attention_probs_bf16 over the rotated q / k of ws_qkv) go to attn + l * attn_layer_stride,
+ *   sequence b at + b * attn_seq_stride, head h at + h * attn_head_stride, rows attn_ld apart. */
+typedef struct {
+  void* hidden;
+  long long hidden_layer_stride, hidden_seq_stride, hidden_ld;
+  void* attn;
+  long long attn_layer_stride, attn_seq_stride, attn_head_stride, attn_ld;
+  int out_rows;
+  const int* row_off;
+} srgpt_prefill_probe;
+/* srgpt_llama_prefill_layers_bf16 (or its _nf4 / _fp8 forms: fp8 != NULL takes the FP8 layers, else nf4 != NULL the NF4 planes beside the
+ * element-type layers) with the probes of `probe` recorded; x, the KV cache and every bit of the arithmetic are those of the unprobed
+ * call.  ws_q8 / ws_scale are needed with fp8 only. */
+int srgpt_llama_prefill_layers_probe_bf16(void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4,
+                                          const srgpt_llama_layer_fp8* fp8, int n_layers, void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act,
+                                          void* ws_q8, float* ws_scale, int S, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+                                          const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables, int page_size,
+                                          int n_seqs, const int* cu_seqlens, int max_seqlen, int page_table_stride,
+                                          const srgpt_prefill_probe* probe, void* stream);
 /* srgpt_gemv_bf16 over FP8 planes (fp8_gemv_kernel, gemv.cu), every mode: x (RMS-normalised first when norm_weight is given) is quantized
  * in the kernel by the activation definition above, the weight codes are turned into their element-type values exactly, and a row's sum
  * acc of exact products (fp32) becomes acc * fl32(s_x * scale[row]) before the mode's stores and rounding points.  `w` is a host pointer;

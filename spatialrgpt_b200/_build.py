@@ -22,7 +22,7 @@ LIB_PATH_F16 = os.path.join(PKG_DIR, "libsrgpt_b200_f16.so")
 VARIANTS = {"bf16": (LIB_PATH, []), "f16": (LIB_PATH_F16, ["-DSRGPT_ELEM_F16"])}
 
 SOURCES = ["capi.cu", "gemm_wgmma.cu", "gemv.cu", "attention.cu", "attention_wgmma.cu", "attention_paged_wgmma.cu", "rowops.cu", "region.cu", "sampling.cu", "tp_comm.cu", "preprocess.cu", "layers.cu", "pack12.cu", "logits_process.cu", "nf4.cu", "fp8.cu", "beam.cu",
-           "logprob.cu", "guidance.cu", "contrastive.cu"]
+           "logprob.cu", "guidance.cu", "contrastive.cu", "attention_probs.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

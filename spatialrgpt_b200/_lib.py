@@ -155,6 +155,9 @@ SIGNATURES = {
     "srgpt_contrastive_penalty_bf16": (ci, [vp, ci, vp, ci, ci, vp, ci, ci, vp, vp]),
     "srgpt_contrastive_select_bf16": (ci, [vp, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_kv_broadcast_rows": (ci, [vp, ci, ci, ci, ci, vp, ci, vp, ci, vp, ci, ci, vp]),
+    "srgpt_attention_probs_bf16": (ci, [vp, ci, vp, ci, ci, vp, ci, ci, ci, ci, cf, vp, cll, cll, cll, ci, vp, vp]),
+    "srgpt_llama_prefill_layers_probe_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci,
+                                                   vp, ci, ci, vp, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)
@@ -189,6 +192,13 @@ class LlamaLayerNf4(C.Structure):
 class Guidance(C.Structure):
     """srgpt_guidance: the device scale g and the guided rows [B / 2, V] of a guided rows step."""
     _fields_ = [("scale", vp), ("guided_rows", vp)]
+
+
+class PrefillProbe(C.Structure):
+    """srgpt_prefill_probe: where a probed prefill stack stores its hidden states and attention probabilities (strides in elements)."""
+    _fields_ = [("hidden", vp), ("hidden_layer_stride", cll), ("hidden_seq_stride", cll), ("hidden_ld", cll), ("attn", vp),
+                ("attn_layer_stride", cll), ("attn_seq_stride", cll), ("attn_head_stride", cll), ("attn_ld", cll), ("out_rows", ci),
+                ("row_off", vp)]
 
 
 class Fp8(C.Structure):

@@ -16,6 +16,13 @@ using namespace srgpt;
 static inline const char* cptr(const void* p, size_t byte_off) { return reinterpret_cast<const char*>(p) + byte_off; }
 static inline char* mptr(void* p, size_t byte_off) { return reinterpret_cast<char*>(p) + byte_off; }
 
+namespace srgpt {
+namespace probs {  // attention_probs.cu
+int store_rows(const void* x, int rows, int H, int n_seqs, const int* cu_seqlens, void* dst, long long seq_stride, long long ld, const int* row_off,
+               void* stream);
+}
+}  // namespace srgpt
+
 extern "C" __attribute__((visibility("default"))) int srgpt_vit_layers_bf16(void* x, const srgpt_siglip_layer_weights* layers, int n_layers, void* ws_h, void* ws_qkv,
                                                                               void* ws_attn, void* ws_mlp, int n_img, int T, int D, int heads, int I, float eps,
                                                                               int fc1_epilogue, void* stream) {
@@ -104,15 +111,19 @@ static int prefill_layers(bool chunk, void* x, const srgpt_llama_layer_weights* 
                           int n_layers, void* ws_h, void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_s, int S, int H, int n_heads,
                           int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, const int* start_pos,
                           const int* page_table, int page_table_stride, int page_size, int n_pages, int n_seqs, const int* cu_seqlens, int max_rows,
-                          void* stream) {
+                          void* stream, const srgpt_prefill_probe* probe = nullptr) {
   SRGPT_CHECK_ARG(x && (layers || fp8) && ws_h && ws_qkv && ws_attn && ws_act && n_layers >= 0 && S > 0 && H > 0 && n_heads > 0 && n_kv_heads > 0 && head_dim > 0 && I > 0);
   SRGPT_CHECK_ARG(fp8 == nullptr || (ws_q8 && ws_s));
   SRGPT_CHECK_ARG(cu_seqlens != nullptr ? (n_seqs >= 1 && max_rows >= 1 && max_rows <= S && page_table_stride > 0) : (n_seqs == 1));
   SRGPT_CHECK_ARG(!chunk || (start_pos && page_table && cu_seqlens && n_pages > 0));
+  SRGPT_CHECK_ARG(probe == nullptr || (!chunk && probe->out_rows >= max(max_rows, cu_seqlens != nullptr ? 1 : S)));
   const int qd = n_heads * head_dim, kd = n_kv_heads * head_dim, nqkv = qd + 2 * kd;
   const float scale = 1.0f / sqrtf((float)head_dim);
   for (int l = 0; l < n_layers; ++l) {
     const LayerRef w = layer_ref(l, layers, nullptr, nf4, fp8);
+    if (probe != nullptr && probe->hidden != nullptr)  // hidden_states[l]: the rows layer l reads
+      SRGPT_TRY(probs::store_rows(x, S, H, n_seqs, cu_seqlens, mptr(probe->hidden, (size_t)l * probe->hidden_layer_stride * 2), probe->hidden_seq_stride,
+                                  probe->hidden_ld, probe->row_off, stream));
     SRGPT_TRY(srgpt_rmsnorm_bf16(x, H, w.in_norm, ws_h, H, S, H, eps, stream));
     SRGPT_TRY(linear(w.m[0], ws_h, H, ws_q8, ws_s, ws_qkv, nqkv, S, nqkv, H, nullptr, 0, SRGPT_EPI_NONE, stream));
     if (cu_seqlens != nullptr)
@@ -120,6 +131,10 @@ static int prefill_layers(bool chunk, void* x, const srgpt_llama_layer_weights* 
                                                  page_table_stride, page_size, n_seqs, cu_seqlens, stream));
     else
       SRGPT_TRY(srgpt_rope_kv_append_bf16(ws_qkv, S, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, start_pos, w.kv_pages, page_table, page_size, stream));
+    if (probe != nullptr && probe->attn != nullptr)  // RoPE rotated q and k in place in ws_qkv, where the attention below reads them
+      SRGPT_TRY(srgpt_attention_probs_bf16(ws_qkv, nqkv, cptr(ws_qkv, (size_t)qd * 2), nqkv, n_seqs, cu_seqlens, cu_seqlens != nullptr ? max_rows : S,
+                                           n_heads, n_kv_heads, head_dim, scale, mptr(probe->attn, (size_t)l * probe->attn_layer_stride * 2),
+                                           probe->attn_seq_stride, probe->attn_head_stride, probe->attn_ld, probe->out_rows, probe->row_off, stream));
     if (chunk)
       SRGPT_TRY(srgpt_attention_prefill_paged_bf16(ws_qkv, nqkv, ws_attn, qd, w.kv_pages, n_pages, page_table, page_table_stride, page_size, start_pos,
                                                    cu_seqlens, n_seqs, max_rows, S, n_heads, n_kv_heads, head_dim, scale, stream));
@@ -164,6 +179,16 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers
   SRGPT_CHECK_ARG(layers != nullptr && nf4 != nullptr);
   return prefill_layers(false, x, layers, nf4, nullptr, n_layers, ws_h, ws_qkv, ws_attn, ws_act, nullptr, nullptr, S, H, n_heads, n_kv_heads, head_dim, I, eps,
                         cos_tab, sin_tab, start_pos, page_table, page_table_stride, page_size, 0, n_seqs, cu_seqlens, max_seqlen, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_layers_probe_bf16(
+    void* x, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_nf4* nf4, const srgpt_llama_layer_fp8* fp8, int n_layers, void* ws_h,
+    void* ws_qkv, void* ws_attn, void* ws_act, void* ws_q8, float* ws_scale, int S, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps,
+    const void* cos_tab, const void* sin_tab, const int* start_pos, const int* page_tables, int page_size, int n_seqs, const int* cu_seqlens,
+    int max_seqlen, int page_table_stride, const srgpt_prefill_probe* probe, void* stream) {
+  SRGPT_CHECK_ARG(probe != nullptr);
+  return prefill_layers(false, x, layers, nf4, fp8, n_layers, ws_h, ws_qkv, ws_attn, ws_act, ws_q8, ws_scale, S, H, n_heads, n_kv_heads, head_dim, I, eps,
+                        cos_tab, sin_tab, start_pos, page_tables, page_table_stride, page_size, 0, n_seqs, cu_seqlens, max_seqlen, stream, probe);
 }
 
 extern "C" __attribute__((visibility("default"))) int srgpt_llama_prefill_chunk_layers_bf16(

@@ -12,6 +12,7 @@ with the position / step counters living in device memory.
 from __future__ import annotations
 
 import os
+from dataclasses import dataclass
 from typing import List, NamedTuple, Optional
 
 import torch
@@ -330,6 +331,16 @@ class PagedKVCache:
         return self.pages[l]
 
 
+@dataclass
+class PrefillProbe:
+    """What a probed prefill records (ops.llama_prefill_layers_probe): ``hidden`` [n_layers, B, R, H] receives the rows each layer reads,
+    ``attn`` [n_layers, B, n_heads, R, R] each layer's attention probabilities (either may be None); prompt b's rows start at output row
+    ``row_off[b]`` (device int32 [B])."""
+    row_off: torch.Tensor
+    hidden: Optional[torch.Tensor] = None
+    attn: Optional[torch.Tensor] = None
+
+
 class LlamaDecoder:
     def __init__(self, dims: LlamaDims, w: LlamaW, max_seq_len: int = 4096, max_new_tokens_cap: int = 4096, max_seqs: int = 1,
                  kv_pages: Optional[int] = None):
@@ -407,6 +418,7 @@ class LlamaDecoder:
     supports_output_scores = True  # generate(output_scores=True): the decode steps write each token's score row on the device
     supports_batch_invariant = True  # generate(batch_invariant=True): generate_rows, each row bit-identical to batch 1
     supports_contrastive = True  # generate(penalty_alpha=, top_k=): generate_contrastive
+    supports_forward_outputs = True  # forward(output_hidden_states=, output_attentions=): the probed prefill (PrefillProbe)
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
@@ -506,14 +518,17 @@ class LlamaDecoder:
         return ops.splice_rows(self.w.embed, None, None, None, torch.zeros_like(flat), flat)
 
     @ops.in_own_dtype
-    def prefill_hidden(self, inputs_embeds: torch.Tensor, seq: int = 0, start_pos: int = 0) -> torch.Tensor:
+    def prefill_hidden(self, inputs_embeds: torch.Tensor, seq: int = 0, start_pos: int = 0, probe: Optional[PrefillProbe] = None) -> torch.Tensor:
         """Run all layers over one sequence's prompt rows [S, H] at positions start_pos .. start_pos + S - 1; fills the KV cache;
         returns the final-layer residual stream [S, H] (before the final norm).  With start_pos > 0 the rows are a chunk that
-        continues the sequence: positions [0, start_pos) must already be in its pages, and attention reads them from there."""
+        continues the sequence: positions [0, start_pos) must already be in its pages, and attention reads them from there.
+        ``probe``: record the hidden states / attention probabilities (PrefillProbe; whole prompts only, start_pos 0)."""
         d, w = self.dims, self.w
         S = inputs_embeds.shape[0]
         if start_pos < 0 or start_pos + S > self.max_seq_len:
             raise RuntimeError(f"prompt of {S} tokens at {start_pos} exceeds max_seq_len {self.max_seq_len}")
+        if probe is not None and start_pos != 0:
+            raise NotImplementedError("hidden states and attentions of a chunked prefill")
         self._record_prefix(0)
         self.cache.reserve(seq, start_pos + S)
         sp = torch.tensor([start_pos], dtype=torch.int32, device=self.device)
@@ -522,14 +537,18 @@ class LlamaDecoder:
             cu = torch.tensor([0, S], dtype=torch.int32, device=self.device)
             return ops.llama_prefill_chunk_layers(x, self.stack, d, self.cos, self.sin, sp, self.cache.page_tables[seq:seq + 1], PAGE_SIZE,
                                                   self.cache.n_pages, cu, S)
+        if probe is not None:
+            return ops.llama_prefill_layers_probe(x, self.stack, d, self.cos, self.sin, sp, self.cache.page_tables[seq], PAGE_SIZE, probe.row_off,
+                                                  probe.hidden, probe.attn)
         return ops.llama_prefill_layers(x, self.stack, d, self.cos, self.sin, sp, self.cache.page_tables[seq], PAGE_SIZE)
 
     @ops.in_own_dtype
-    def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int], page_tables: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def prefill_packed(self, packed_embeds: torch.Tensor, seq_lens: List[int], page_tables: Optional[torch.Tensor] = None,
+                       probe: Optional[PrefillProbe] = None) -> torch.Tensor:
         """Prefill `len(seq_lens)` prompts packed back to back ([sum S_b, H]) into sequence slots 0..B-1 (or the rows of
         ``page_tables``, a row-strided view of the cache's tables) in ONE pass: every GEMM runs over all rows, attention / RoPE / KV
         append per sequence (the unpadded varlen path of modeling_llama.py:540-562).  The caller has reserved the pages.  Returns the
-        final residual stream, packed."""
+        final residual stream, packed.  ``probe``: record the hidden states / attention probabilities (PrefillProbe)."""
         d = self.dims
         B = len(seq_lens)
         if packed_embeds.shape[0] != sum(seq_lens) or B < 1 or min(seq_lens) < 1:
@@ -541,6 +560,9 @@ class LlamaDecoder:
         sp = torch.zeros(B, dtype=torch.int32, device=self.device)
         x = packed_embeds.to(self.dtype).contiguous().clone()
         pts = self.cache.page_tables[:B] if page_tables is None else page_tables
+        if probe is not None:
+            return ops.llama_prefill_layers_probe(x, self.stack, d, self.cos, self.sin, sp, pts, PAGE_SIZE, probe.row_off, probe.hidden, probe.attn,
+                                                  cu_seqlens=cu, max_seqlen=max(seq_lens))
         return ops.llama_prefill_layers(x, self.stack, d, self.cos, self.sin, sp, pts, PAGE_SIZE, cu_seqlens=cu, max_seqlen=max(seq_lens))
 
     @ops.in_own_dtype
@@ -561,15 +583,20 @@ class LlamaDecoder:
         return torch.empty((rows, (V + 7) // 8 * 8), dtype=self.dtype, device=self.device)[:, :V]
 
     @ops.in_own_dtype
-    def logits_all(self, hidden: torch.Tensor) -> torch.Tensor:
+    def logits_all(self, hidden: torch.Tensor, normed: Optional[torch.Tensor] = None) -> torch.Tensor:
         """lm_head over every row -> fp32 logits [S, V] (LlamaForCausalLM.forward semantics, 1044-1045)."""
-        return self.lm_head_rows(hidden).float()  # bf16 rounding first, then .float()
+        return self.lm_head_rows(hidden, normed=normed).float()  # bf16 rounding first, then .float()
 
     @ops.in_own_dtype
-    def lm_head_rows(self, hidden: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def final_norm(self, hidden: torch.Tensor) -> torch.Tensor:
+        """The final RMSNorm of every row of ``hidden``: the rows the lm_head GEMM reads."""
+        return ops.rmsnorm(hidden, self.w.norm, self.dims.rms_norm_eps)
+
+    @ops.in_own_dtype
+    def lm_head_rows(self, hidden: torch.Tensor, out: Optional[torch.Tensor] = None, normed: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Final norm + lm_head over every row of ``hidden`` -> element-type logits [S, V] (into ``out``, default a fresh
-        _logits_buffer)."""
-        hn = ops.rmsnorm(hidden, self.w.norm, self.dims.rms_norm_eps)
+        _logits_buffer).  ``normed``: final_norm(hidden) when the caller has it already."""
+        hn = self.final_norm(hidden) if normed is None else normed
         return ops.gemm(hn, self.w.lm_head, out=self._logits_buffer(hn.shape[0]) if out is None else out)
 
     # ---------------------------------------------------------------------------------------------

@@ -15,7 +15,7 @@ import torch
 from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
-from .llama_decoder import LlamaDecoder, check_candidates, sequence_seeds
+from .llama_decoder import LlamaDecoder, PrefillProbe, check_candidates, sequence_seeds
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
@@ -519,15 +519,29 @@ class LlavaLlamaModel:
     @torch.no_grad()
     @ops.in_own_dtype
     def forward(self, input_ids=None, images=None, masks=None, depths=None, attention_mask=None, position_ids=None,
-                past_key_values=None, seqlens_in_batch=None, inputs_embeds=None, labels=None, use_cache=None, **kwargs):
+                past_key_values=None, seqlens_in_batch=None, inputs_embeds=None, labels=None, use_cache=None, output_attentions=None,
+                output_hidden_states=None, **kwargs):
+        """Logits of every position (and the loss with ``labels``), as LlavaLlamaForCausalLM.forward.  ``output_hidden_states=True``:
+        ``hidden_states`` is a tuple of L + 1 element-type [B, S, H] tensors, the embeddings, the residual stream after each layer but the
+        last, and the final norm of the last (the rows lm_head reads).  ``output_attentions=True``: ``attentions`` is a tuple of L
+        element-type [B, num_heads, S, S] tensors, each layer's causal softmax in fp32, cast.  Both are views of one allocation each, and
+        are 0 at every padded position (query or key).  The logits and the loss are bit-identical with or without them."""
         if past_key_values is not None:
             raise NotImplementedError("external past_key_values are not supported; the KV cache is paged and internal")
+        want_h, want_a = bool(output_hidden_states), bool(output_attentions)
+        if want_h or want_a:
+            if not getattr(self.llm, "supports_forward_outputs", False):
+                raise NotImplementedError("output_hidden_states / output_attentions on the tensor-parallel decoder: no rank holds every attention head")
+            if inputs_embeds is not None or images is None:  # the row count is known before any device work
+                self._check_forward_outputs_fit(*(inputs_embeds.shape[:2] if inputs_embeds is not None else input_ids.shape), want_h, want_a)
         if inputs_embeds is None:
             if images is None:
                 inputs_embeds = self.llm.embed_tokens(input_ids).view(*input_ids.shape, -1)
             else:
                 (_, position_ids, attention_mask, _, inputs_embeds, labels) = self.prepare_inputs_labels_for_multimodal(
                     input_ids, position_ids, attention_mask, None, labels, images, masks, depths)
+                if want_h or want_a:  # the spliced row count
+                    self._check_forward_outputs_fit(*inputs_embeds.shape[:2], want_h, want_a)
         B, S, H = inputs_embeds.shape
         lens = [S] * B if attention_mask is None else attention_mask.bool().sum(-1).tolist()
         lens = [int(n) for n in lens]
@@ -543,26 +557,52 @@ class LlavaLlamaModel:
         llm = self.llm
         for b in range(len(llm.cache.owned)):
             llm.cache.release(b)
+        probe, hs, att = None, None, None
+        if want_h or want_a:
+            d = llm.dims
+            L = d.num_hidden_layers
+            if want_h:
+                hs = torch.empty((L + 1, B, S, H), dtype=self.dtype, device=self.device)
+                for b in range(B):  # the probed prefill writes the valid rows only
+                    hs[:, b, :valid[b].start].zero_()
+                    hs[:, b, valid[b].stop:].zero_()
+            if want_a:  # every entry is written by the probability kernel, padding included
+                att = torch.empty((L, B, d.num_attention_heads, S, S), dtype=self.dtype, device=self.device)
+            probe = PrefillProbe(torch.tensor([v.start for v in valid], dtype=torch.int32).to(self.device), None if hs is None else hs[:L], att)
         if B == 1:
-            hid = llm.prefill_hidden(inputs_embeds[0, valid[0]], 0, 0)
+            hid = llm.prefill_hidden(inputs_embeds[0, valid[0]], 0, 0, **({} if probe is None else dict(probe=probe)))
         else:  # one packed pass over all rows of the batch
             llm.ensure_capacity(B, max(lens))
             llm.cache.reserve_many(lens)
-            hid = llm.prefill_packed(torch.cat([inputs_embeds[b, valid[b]] for b in range(B)], 0), lens)
+            hid = llm.prefill_packed(torch.cat([inputs_embeds[b, valid[b]] for b in range(B)], 0), lens,
+                                     **({} if probe is None else dict(probe=probe)))
+        hn = None if hs is None else llm.final_norm(hid)  # hidden_states[L]: the very rows lm_head reads
         loss = None
         if labels is None:
-            lg = llm.logits_all(hid)
+            lg = llm.logits_all(hid, **({} if hn is None else dict(normed=hn)))
         else:  # the element-type rows the lm_head GEMM writes, plus one zero row: the logits this call returns at padding positions
             total = hid.shape[0]
             buf = llm._logits_buffer(total + 1)
-            lg = llm.lm_head_rows(hid, out=buf[:total]).float()
+            lg = llm.lm_head_rows(hid, out=buf[:total], **({} if hn is None else dict(normed=hn))).float()
             buf[total].zero_()
             loss = self._labels_loss(buf, labels, valid, lens, S)
         o = 0
         for b in range(B):
             logits[b, valid[b]] = lg[o:o + lens[b]]
+            if hs is not None:
+                hs[-1, b, valid[b]] = hn[o:o + lens[b]]
             o += lens[b]
-        return CausalLMOutputWithPast(logits=logits, loss=loss)
+        return CausalLMOutputWithPast(logits=logits, loss=loss, hidden_states=None if hs is None else tuple(hs.unbind(0)),
+                                      attentions=None if att is None else tuple(att.unbind(0)))
+
+    def _check_forward_outputs_fit(self, B: int, S: int, hidden: bool, attentions: bool) -> None:
+        """RuntimeError naming the bytes forward()'s hidden states / attentions need when they exceed the free device memory."""
+        d = self.llm.dims
+        need = 2 * ((d.num_hidden_layers + 1) * B * S * d.hidden_size * hidden + d.num_hidden_layers * B * d.num_attention_heads * S * S * attentions)
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need > free:
+            raise RuntimeError(f"forward(output_hidden_states={hidden}, output_attentions={attentions}) over {B} x {S} rows needs {need} bytes "
+                               f"({need / 2 ** 30:.1f} GiB) for its outputs; {free} bytes are free on {self.device}")
 
     @staticmethod
     def _labels_loss(elem_logits: torch.Tensor, labels: torch.Tensor, valid, lens, S: int) -> torch.Tensor:

@@ -1319,6 +1319,83 @@ def llama_prefill_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, sta
                     (_p(page_table), page_size, n_seqs, _p(cu_seqlens), max_seqlen, pt_stride))
 
 
+def llama_prefill_layers_probe(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, page_table, page_size: int, row_off: torch.Tensor,
+                               hidden: Optional[torch.Tensor] = None, attn: Optional[torch.Tensor] = None,
+                               cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0) -> torch.Tensor:
+    """llama_prefill_layers with the probes recorded: ``hidden`` [n_layers, n_seqs, R, H] gets the rows each layer reads (the
+    embeddings, then the residual stream after every layer but the last), ``attn`` [n_layers, n_seqs, n_heads, R, R] every layer's
+    attention probabilities; sequence b's rows start at output row row_off[b] (device int32 [n_seqs]).  Either may be None.  x, the KV
+    cache and every bit of the arithmetic are those of llama_prefill_layers."""
+    _need(x, ELEM(), "llama_prefill_layers_probe.x")
+    _need(row_off, torch.int32, "llama_prefill_layers_probe.row_off")
+    S, H = x.shape
+    L, nh = stack.n, dims.num_attention_heads
+    n_seqs, pt_stride = 1, 0
+    if cu_seqlens is not None:
+        _need(cu_seqlens, torch.int32, "llama_prefill_layers_probe.cu_seqlens")
+        n_seqs = cu_seqlens.numel() - 1
+        if page_table.dim() != 2 or page_table.shape[0] < n_seqs or start_pos.numel() < n_seqs or page_table.stride(1) != 1:
+            raise SrgptError("llama_prefill_layers_probe: packed prompts need page_table [n_seqs, cap] and start_pos [n_seqs]")
+        pt_stride = page_table.stride(0)
+    if row_off.numel() < n_seqs:
+        raise SrgptError("llama_prefill_layers_probe: row_off needs one offset per sequence")
+    probe = _lib.PrefillProbe()
+    R = None
+    if hidden is not None:
+        _need(hidden, ELEM(), "llama_prefill_layers_probe.hidden")
+        if hidden.dim() != 4 or tuple(hidden.shape[:2]) != (L, n_seqs) or hidden.shape[3] != H or hidden.stride(3) != 1:
+            raise SrgptError(f"llama_prefill_layers_probe: hidden must be [{L}, {n_seqs}, R, {H}] with unit inner stride, got {tuple(hidden.shape)}")
+        R = hidden.shape[2]
+        probe.hidden, probe.hidden_layer_stride, probe.hidden_seq_stride, probe.hidden_ld = hidden.data_ptr(), *hidden.stride()[:3]
+    if attn is not None:
+        _need(attn, ELEM(), "llama_prefill_layers_probe.attn")
+        if attn.dim() != 5 or tuple(attn.shape[:3]) != (L, n_seqs, nh) or attn.shape[3] != attn.shape[4] or attn.stride(4) != 1:
+            raise SrgptError(f"llama_prefill_layers_probe: attn must be [{L}, {n_seqs}, {nh}, R, R] with unit inner stride, got {tuple(attn.shape)}")
+        if R is not None and attn.shape[3] != R:
+            raise SrgptError("llama_prefill_layers_probe: hidden and attn must have the same rows per sequence")
+        R = attn.shape[3]
+        probe.attn, probe.attn_layer_stride, probe.attn_seq_stride, probe.attn_head_stride, probe.attn_ld = attn.data_ptr(), *attn.stride()[:4]
+    if R is None:
+        raise SrgptError("llama_prefill_layers_probe: nothing to record (hidden and attn are both None)")
+    probe.out_rows, probe.row_off = R, row_off.data_ptr()
+    _ensure_gemm_workspace(x.device)
+    nkv, hd, I = dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    dev = x.device
+    ws = (torch.empty((S, H), dtype=ELEM(), device=dev), torch.empty((S, (nh + 2 * nkv) * hd), dtype=ELEM(), device=dev),
+          torch.empty((S, nh * hd), dtype=ELEM(), device=dev), torch.empty((S, I), dtype=ELEM(), device=dev))
+    ws += _fp8_workspaces(S, dims, dev) if stack.quantizes_activations else (None, None)
+    fmt, arrays, _ = stack.formats("prefill_layers")
+    layers, nf4, fp8 = (None, None, arrays[0]) if fmt == "fp8" else (arrays[0], arrays[1] if fmt == "nf4" else None, None)
+    check(_lib.load().srgpt_llama_prefill_layers_probe_bf16(_p(x), layers, nf4, fp8, L, *(_p(t) for t in ws), S, H, nh, nkv, hd, I,
+                                                            dims.rms_norm_eps, _p(cos), _p(sin), _p(start_pos), _p(page_table), page_size, n_seqs,
+                                                            _p(cu_seqlens), max_seqlen, pt_stride, C.byref(probe), _stream()),
+          "srgpt_llama_prefill_layers_probe_bf16")
+    _count((stack.kernels_per_layer + (hidden is not None) + (attn is not None)) * L)
+    return x
+
+
+def attention_probs(q: torch.Tensor, k: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: int, scale: float, out: torch.Tensor,
+                    cu_seqlens: Optional[torch.Tensor] = None, max_seqlen: int = 0, row_off: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Causal attention probabilities in the element type into out [n_seqs, n_heads, R, R] (any strides, unit inner one): q / k are
+    row-major views [rows, heads * head_dim] (e.g. the rotated columns of a fused qkv buffer) of one sequence (cu_seqlens None) or of
+    sequences packed by cu_seqlens [n_seqs + 1] (max_seqlen = the longest); sequence b's block starts at row / column row_off[b].
+    Every entry of ``out`` is written."""
+    _need(q, ELEM(), "attention_probs.q"); _need(k, ELEM(), "attention_probs.k"); _need(out, ELEM(), "attention_probs.out")
+    n_seqs = 1 if cu_seqlens is None else cu_seqlens.numel() - 1
+    if cu_seqlens is None:
+        max_seqlen = q.shape[0]
+    else:
+        _need(cu_seqlens, torch.int32, "attention_probs.cu_seqlens")
+    if row_off is not None:
+        _need(row_off, torch.int32, "attention_probs.row_off")
+    if out.dim() != 4 or tuple(out.shape[:2]) != (n_seqs, n_heads) or out.shape[2] != out.shape[3] or out.stride(3) != 1:
+        raise SrgptError(f"attention_probs: out must be [{n_seqs}, {n_heads}, R, R] with unit inner stride, got {tuple(out.shape)}")
+    check(_lib.load().srgpt_attention_probs_bf16(_p(q), _rowmajor2d(q, "attention_probs.q"), _p(k), _rowmajor2d(k, "attention_probs.k"), n_seqs,
+                                                 _p(cu_seqlens), max_seqlen, n_heads, n_kv_heads, head_dim, scale, _p(out), out.stride(0),
+                                                 out.stride(1), out.stride(2), out.shape[2], _p(row_off), _stream()), "srgpt_attention_probs_bf16")
+    return out
+
+
 def llama_prefill_chunk_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
                                cu_seqlens: torch.Tensor, max_rows: int) -> torch.Tensor:
     """All decoder layers over x [S, H] in place: n_seqs chunks packed by cu_seqlens [n_seqs+1] that continue their sequences at

@@ -70,6 +70,7 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_scoring = False  # likelihood scoring (score_candidates) is a single-GPU path
     supports_batch_invariant = False  # the rows step (generate_rows) is a single-GPU kernel sequence
     supports_contrastive = False  # contrastive search runs the batched step and its choice on one GPU
+    supports_forward_outputs = False  # forward()'s attentions need every head, and no rank holds them all
 
     def score_candidates(self, *args, **kwargs):
         raise NotImplementedError("likelihood scoring (score()) on the tensor-parallel decoder")
