@@ -177,6 +177,23 @@ int srgpt_attention_prefill_paged_bf16(const void* q, int q_ld, void* out, int o
 int srgpt_attention_probs_bf16(const void* q, int q_ld, const void* k, int k_ld, int n_seqs, const int* cu_seqlens, int max_seqlen, int n_heads,
                                int n_kv_heads, int head_dim, float scale, void* out, long long seq_stride, long long head_stride, long long ld,
                                int out_rows, const int* row_off, void* stream);
+/* The attention probabilities of one-token decode steps over the paged cache (attention_probs.cu; HF generate(output_attentions=True)'s
+ * decode-step entries, eager attention: softmax(q K^T * scale) in fp32, cast to the element type), which the flash-decode kernels never
+ * build.  Row r: rotated q at q + r * q_ld (n_heads * 128 wide), keys 0 .. pos[r] in kv_pages through page_tables + r * pt_stride, query
+ * head h reading KV head h / (n_heads / n_kv_heads) (at most 8 query heads per KV head).  The logits are srgpt_attention_probs_bf16's
+ * (fp32 dot products, times scale * log2(e), exp2f, fp32 sum).  Row r, head h goes to out + (*step + step_offset) * step_stride
+ * + r * row_stride + h * head_stride, in generate()'s padded columns: prompt key p (p < n_prompt[r]) at column off[r] + p, generated key
+ * n_prompt[r] + j at column T + j.  Every column of [0, min(T + pos[r] + 1 - n_prompt[r], n_cols)) is written (0 where no key lands) and
+ * nothing past it.  step / pos / off / n_prompt: device int32, read at run time, so one captured graph serves every step.  ws: fp32
+ * workspace of 2 * rows * n_heads * ceil(n_cols / 128) floats.  Two launches.  head_dim 128 only. */
+int srgpt_attention_probs_decode_bf16(const void* q, int q_ld, const void* kv_pages, const int* page_tables, int pt_stride, int page_size,
+                                      const int* pos, int rows, int n_heads, int n_kv_heads, int head_dim, float scale, const int* off,
+                                      const int* n_prompt, int T, int n_cols, const int* step, int step_offset, void* out, long long step_stride,
+                                      long long row_stride, long long head_stride, float* ws, void* stream);
+/* Rows x [rows, H] (contiguous) -> dst + (*step + step_offset) * step_stride + r * row_stride (strides in elements; step device int32):
+ * generate(output_hidden_states=True)'s per-step hidden rows, written by the store kernel of the probed prefill. */
+int srgpt_store_step_rows_bf16(const void* x, int rows, int H, const int* step, int step_offset, void* dst, long long step_stride,
+                               long long row_stride, void* stream);
 /* flags[r] = 1 when rows r of a and b ([rows, row_bytes] bytes, rows contiguous) are bitwise equal, else 0 (rowops.cu).  The
  * prompt-prefix cache of generate(prefix_cache=True) compares a request's images / depths / masks with the previous ones. */
 int srgpt_rows_equal(const void* a, const void* b, int rows, long long row_bytes, int* flags, void* stream);
@@ -568,6 +585,31 @@ int srgpt_llama_decode_step_fp8_bf16(void* h, const srgpt_llama_layer_fp8* layer
                                      int* pos, const int* page_table, int page_size, const void* final_norm, const void* lm_head,
                                      const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out,
                                      long long* out_ids, int* step, void* stream);
+/* What srgpt_llama_decode_step_probe_bf16 records (generate(output_hidden_states=, output_attentions=) over the decode steps; strides in
+ * elements; the step's slot is *step + step_offset, read before the lm_head advances step).
+ * hidden != NULL: before layer l the residual row h goes to hidden + slot * hidden_step_stride + l * hidden_layer_stride (slot l), and
+ *   srgpt_rmsnorm_bf16 of the last layer's row to slot n_layers; hidden_row_stride is the row stride of a batched caller (unused here).
+ * attn != NULL: layer l's probabilities (srgpt_attention_probs_decode_bf16 with rows = 1, off / n_prompt / T / n_cols / ws) go to
+ *   attn + l * attn_layer_stride with step / row / head strides attn_step_stride / attn_row_stride / attn_head_stride. */
+typedef struct {
+  void* hidden;
+  long long hidden_step_stride, hidden_layer_stride, hidden_row_stride;
+  void* attn;
+  long long attn_step_stride, attn_layer_stride, attn_row_stride, attn_head_stride;
+  int step_offset, T, n_cols;
+  const int* off;
+  const int* n_prompt;
+  float* ws;
+} srgpt_decode_probe;
+/* srgpt_llama_decode_step_bf16 (or its _packed / _nf4 / _fp8 forms: the one of packed / nf4 / fp8 given, lm_packed may be NULL) with the
+ * probes of `probe` recorded; h, pos, step, the KV cache, the ids and the logits are those of the unprobed call.  The final norm row
+ * passes through act_buf, so I >= H when hidden is recorded. */
+int srgpt_llama_decode_step_probe_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed,
+                                       const srgpt_llama_layer_nf4* nf4, const srgpt_llama_layer_fp8* fp8, int n_layers, void* q_buf, void* attn_buf,
+                                       void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab,
+                                       const void* sin_tab, int* pos, const int* page_table, int page_size, const void* final_norm,
+                                       const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
+                                       float* logits_out, long long* out_ids, int* step, const srgpt_decode_probe* probe, void* stream);
 
 /* ---- prompt-lookup speculative decoding, batch 1, greedy (HF GenerationMixin._assisted_decoding with
  * PromptLookupCandidateGenerator, i.e. generate(prompt_lookup_num_tokens=k); call site llava_llama.py:212).

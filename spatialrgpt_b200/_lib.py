@@ -158,6 +158,10 @@ SIGNATURES = {
     "srgpt_attention_probs_bf16": (ci, [vp, ci, vp, ci, ci, vp, ci, ci, ci, ci, cf, vp, cll, cll, cll, ci, vp, vp]),
     "srgpt_llama_prefill_layers_probe_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci,
                                                    vp, ci, ci, vp, vp]),
+    "srgpt_attention_probs_decode_bf16": (ci, [vp, ci, vp, vp, ci, ci, vp, ci, ci, ci, ci, cf, vp, vp, ci, ci, vp, ci, vp, cll, cll, cll, vp, vp]),
+    "srgpt_store_step_rows_bf16": (ci, [vp, ci, ci, vp, ci, vp, cll, cll, vp]),
+    "srgpt_llama_decode_step_probe_bf16": (ci, [vp, vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, vp, vp, vp, ci, vp,
+                                                vp, vp, vp, vp, vp, vp]),
 }
 
 SPEC_T_MAX = 8  # SRGPT_SPEC_T_MAX: tokens per verify pass (the last emitted token + up to 7 drafts)
@@ -199,6 +203,13 @@ class PrefillProbe(C.Structure):
     _fields_ = [("hidden", vp), ("hidden_layer_stride", cll), ("hidden_seq_stride", cll), ("hidden_ld", cll), ("attn", vp),
                 ("attn_layer_stride", cll), ("attn_seq_stride", cll), ("attn_head_stride", cll), ("attn_ld", cll), ("out_rows", ci),
                 ("row_off", vp)]
+
+
+class DecodeProbe(C.Structure):
+    """srgpt_decode_probe: where a probed decode step stores its hidden rows and attention probabilities (strides in elements)."""
+    _fields_ = [("hidden", vp), ("hidden_step_stride", cll), ("hidden_layer_stride", cll), ("hidden_row_stride", cll), ("attn", vp),
+                ("attn_step_stride", cll), ("attn_layer_stride", cll), ("attn_row_stride", cll), ("attn_head_stride", cll), ("step_offset", ci),
+                ("T", ci), ("n_cols", ci), ("off", vp), ("n_prompt", vp), ("ws", vp)]
 
 
 class Fp8(C.Structure):

@@ -1,7 +1,10 @@
 // Kernels behind forward(output_attentions=True, output_hidden_states=True) (DESIGN.md §4, §7):
 //   * attn_probs_kernel : the causal attention probabilities softmax(Q K^T * scale) of one layer, written in the element type
 //     straight into the caller's [n_seqs, n_heads, out_rows, out_rows] blocks - the S x S matrix the flash kernels never build.
-//   * store_rows_kernel : copies the residual rows of packed sequences into a padded [n_seqs, out_rows, H] output.
+//   * store_rows_kernel : copies the residual rows of packed sequences into a padded [n_seqs, out_rows, H] output (optionally at the
+//     device step counter: generate()'s per-step hidden states).
+//   * decode_stats_kernel / decode_probs_kernel : the probabilities of one-token decode steps over the paged KV cache, written at the
+//     device step in generate()'s padded column layout (generate(output_attentions=True)).
 // Reference: HF eager_attention_forward (softmax in fp32, then cast to the query dtype) and LlamaModel's hidden-state capture.
 #include "common.cuh"
 #include "srgpt_b200.h"
@@ -198,11 +201,13 @@ attn_probs_kernel(const bf16* __restrict__ q, int q_ld, const bf16* __restrict__
   }
 }
 
-// Row r of x [rows, H] (sequence s of the packed rows, local row r - cu[s]) -> dst + s * seq_stride + (row_off[s] + local) * ld.
+// Row r of x [rows, H] (sequence s of the packed rows, local row r - cu[s]) -> dst + s * seq_stride + (row_off[s] + local) * ld, and
+// + (*step + step_offset) * step_stride when step != NULL.
 __global__ void __launch_bounds__(128)
 store_rows_kernel(const bf16* __restrict__ x, int H, int n_seqs, const int* __restrict__ cu_seqlens, bf16* __restrict__ dst, long long seq_stride,
-                  long long ld, const int* __restrict__ row_off) {
+                  long long ld, const int* __restrict__ row_off, const int* __restrict__ step, int step_offset, long long step_stride) {
   const int row = blockIdx.x;
+  if (step != nullptr) dst += (long long)(*step + step_offset) * step_stride;
   int seq = 0, local = row;
   if (cu_seqlens != nullptr) {  // largest s with cu_seqlens[s] <= row
     int lo = 0, hi = n_seqs - 1;
@@ -220,16 +225,194 @@ store_rows_kernel(const bf16* __restrict__ x, int H, int n_seqs, const int* __re
 }
 
 int store_rows(const void* x, int rows, int H, int n_seqs, const int* cu_seqlens, void* dst, long long seq_stride, long long ld, const int* row_off,
-               void* stream) {
+               void* stream, const int* step, int step_offset, long long step_stride) {
   SRGPT_CHECK_ARG(x && dst && rows > 0 && n_seqs >= 1 && (cu_seqlens != nullptr || n_seqs == 1));
-  SRGPT_CHECK_ARG((H % 8) == 0 && (ld % 8) == 0 && (seq_stride % 8) == 0 && ld >= H);
+  SRGPT_CHECK_ARG((H % 8) == 0 && (ld % 8) == 0 && (seq_stride % 8) == 0 && ld >= H && (step_stride % 8) == 0);
   SRGPT_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0);
   store_rows_kernel<<<rows, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const bf16*>(x), H, n_seqs, cu_seqlens,
-                                                                              reinterpret_cast<bf16*>(dst), seq_stride, ld, row_off);
+                                                                              reinterpret_cast<bf16*>(dst), seq_stride, ld, row_off, step,
+                                                                              step_offset, step_stride);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }
 
+
+// ---- one-token decode steps over the paged cache ---------------------------------------------------------------------------------
+// Query row r (position pos[r], so keys 0 .. pos[r]) of a step, heads kvh * G .. kvh * G + G - 1 of KV head kvh.  A quad of lanes takes
+// one key (each lane 32 of its 128 dimensions, 16-byte loads in four interleaved strips, so a quad reads 64 contiguous bytes per load),
+// and the quad's partial dot products meet by two xor shuffles: each K row is read once for the whole GQA group.  The logits are those
+// of attn_probs_kernel: fp32 dot products of the rotated q and k, times scale * log2(e); the softmax is exp2f(s - m) / sum in fp32.
+// Two launches over the same grid (128-key chunks of the key range, KV heads, rows), so that a long context spreads over many SMs:
+// decode_stats_kernel writes each chunk's (max, sum) per head to ws, decode_probs_kernel combines the chunks of its row in chunk order
+// and writes the probabilities of its chunk of output columns.
+constexpr int DCHUNK = 128, DTHREADS = 128, DMAX_GROUP = 8;
+
+struct DecodeArgs {
+  const bf16* q;
+  int q_ld;
+  const bf16* kv_pages;
+  const int* page_tables;
+  int pt_stride, page_size, n_kv_heads, group;
+  const int* pos;
+  float scale_log2;
+  const int* off;
+  const int* n_prompt;
+  int T, n_cols;
+  const int* step;
+  int step_offset;
+  bf16* out;
+  long long step_stride, row_stride, head_stride;
+  float2* ws;  // [rows][n_heads][ceil(n_cols / DCHUNK)]
+};
+
+// the group's query rows as fp32 in shared memory
+__device__ __forceinline__ void load_q_group(const DecodeArgs& a, float (*qs)[HD], int r, int kvh) {
+  const bf16* src = a.q + (size_t)r * a.q_ld + (size_t)kvh * a.group * HD;
+  for (int i = threadIdx.x; i < a.group * HD; i += DTHREADS) qs[i / HD][i % HD] = e2f(src[i]);
+}
+
+// the group's logits (base 2) of key j, in every lane of the quad
+__device__ __forceinline__ void key_logits(const DecodeArgs& a, const int* pt, int kvh, int j, const float (*qs)[HD], float* s) {
+  const int ql = threadIdx.x & 3;
+  const unsigned qmask = 0xfu << (threadIdx.x & 28);  // the quad: the other quads of the warp may be on another key or done
+  const int page = pt[j / a.page_size], slot = j % a.page_size;
+  const bf16* kp = a.kv_pages + (((size_t)page * 2 + 0) * a.page_size + slot) * (size_t)a.n_kv_heads * HD + kvh * HD;
+  float k[32];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint4 u = *reinterpret_cast<const uint4*>(kp + (i * 4 + ql) * 8);
+    const bf16* e = reinterpret_cast<const bf16*>(&u);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) k[i * 8 + t] = e2f(e[t]);
+  }
+#pragma unroll
+  for (int g = 0; g < DMAX_GROUP; ++g) {
+    if (g >= a.group) break;
+    float acc = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int t = 0; t < 8; ++t) acc = fmaf(k[i * 8 + t], qs[g][(i * 4 + ql) * 8 + t], acc);
+    acc += __shfl_xor_sync(qmask, acc, 1);
+    acc += __shfl_xor_sync(qmask, acc, 2);
+    s[g] = acc * a.scale_log2;
+  }
+}
+
+// (m, l) of two parts of a softmax sum merged: m the larger max, l the sums rescaled to it (an empty part has m = -inf, l = 0)
+__device__ __forceinline__ void merge_ml(float& m, float& l, float m2, float l2) {
+  const float mn = fmaxf(m, m2);
+  if (mn == -INFINITY) return;
+  l = l * exp2f(m - mn) + l2 * exp2f(m2 - mn);
+  m = mn;
+}
+
+__global__ void __launch_bounds__(DTHREADS) decode_stats_kernel(const DecodeArgs a) {
+  __shared__ float qs[DMAX_GROUP][HD];
+  __shared__ float2 part[DTHREADS / 32][DMAX_GROUP];
+  const int c = blockIdx.x, kvh = blockIdx.y, r = blockIdx.z;
+  const int P = a.pos[r] + 1, j0 = c * DCHUNK;
+  if (j0 >= P) return;  // decode_probs_kernel reads the chunks below P only
+  load_q_group(a, qs, r, kvh);
+  __syncthreads();
+  const int* pt = a.page_tables + (size_t)r * a.pt_stride;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float m[DMAX_GROUP], l[DMAX_GROUP], s[DMAX_GROUP];
+#pragma unroll
+  for (int g = 0; g < DMAX_GROUP; ++g) m[g] = -INFINITY, l[g] = 0.f;
+  const int j1 = min(P, j0 + DCHUNK);
+  for (int jb = j0; jb < j1; jb += DTHREADS / 4) {
+    const int j = jb + (threadIdx.x >> 2);
+    if (j >= j1) break;
+    key_logits(a, pt, kvh, j, qs, s);
+#pragma unroll
+    for (int g = 0; g < DMAX_GROUP; ++g) {
+      if (g >= a.group) break;
+      merge_ml(m[g], l[g], s[g], 1.f);
+    }
+  }
+  // quads -> warp (xor 4, 8, 16), warps -> CTA in warp order
+#pragma unroll
+  for (int g = 0; g < DMAX_GROUP; ++g) {
+    if (g >= a.group) break;
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, m[g], o), l2 = __shfl_xor_sync(0xffffffffu, l[g], o);
+      merge_ml(m[g], l[g], m2, l2);
+    }
+    if (lane == 0) part[warp][g] = make_float2(m[g], l[g]);
+  }
+  __syncthreads();
+  if (threadIdx.x < a.group) {
+    const int g = threadIdx.x;
+    float mm = -INFINITY, ll = 0.f;
+    for (int w = 0; w < DTHREADS / 32; ++w) merge_ml(mm, ll, part[w][g].x, part[w][g].y);
+    const int n_chunks = (a.n_cols + DCHUNK - 1) / DCHUNK;
+    a.ws[((size_t)r * a.n_kv_heads * a.group + kvh * a.group + g) * n_chunks + c] = make_float2(mm, ll);
+  }
+}
+
+__global__ void __launch_bounds__(DTHREADS) decode_probs_kernel(const DecodeArgs a) {
+  __shared__ float qs[DMAX_GROUP][HD];
+  __shared__ float2 stat[DMAX_GROUP];  // (max, 1 / sum) of each head of the group
+  const int c = blockIdx.x, kvh = blockIdx.y, r = blockIdx.z;
+  const int P = a.pos[r] + 1, n = a.n_prompt[r], off = a.off[r];
+  const int cols = min(a.T + P - n, a.n_cols);  // the row's view: T prompt columns, then the generated keys
+  const int c0 = c * DCHUNK, c1 = min(cols, c0 + DCHUNK);
+  if (c0 >= c1) return;
+  load_q_group(a, qs, r, kvh);
+  if (threadIdx.x < a.group) {
+    const int g = threadIdx.x, n_chunks = (a.n_cols + DCHUNK - 1) / DCHUNK;
+    const float2* w = a.ws + ((size_t)r * a.n_kv_heads * a.group + kvh * a.group + g) * n_chunks;
+    float mm = -INFINITY, ll = 0.f;
+    for (int k = 0; k * DCHUNK < P; ++k) merge_ml(mm, ll, w[k].x, w[k].y);
+    stat[g] = make_float2(mm, ll > 0.f ? 1.f / ll : 0.f);
+  }
+  __syncthreads();
+  const int* pt = a.page_tables + (size_t)r * a.pt_stride;
+  bf16* ob = a.out + (long long)(*a.step + a.step_offset) * a.step_stride + (long long)r * a.row_stride + (long long)kvh * a.group * a.head_stride;
+  const int ql = threadIdx.x & 3;
+  float s[DMAX_GROUP];
+  for (int cb = c0; cb < c1; cb += DTHREADS / 4) {
+    const int col = cb + (threadIdx.x >> 2);
+    if (col >= c1) break;
+    const int j = (col >= off && col < off + n) ? col - off : (col >= a.T ? n + col - a.T : -1);
+    if (j >= 0 && j < P) {  // every lane of the quad takes part in the shuffles
+      key_logits(a, pt, kvh, j, qs, s);
+#pragma unroll
+      for (int g = 0; g < DMAX_GROUP; ++g) {
+        if (g >= a.group) break;
+        if ((g & 3) == ql) ob[g * a.head_stride + col] = f2e(exp2f(s[g] - stat[g].x) * stat[g].y);
+      }
+    } else {
+      for (int g = ql; g < a.group; g += 4) ob[g * a.head_stride + col] = f2e(0.f);
+    }
+  }
+}
+
+int decode_probs(const void* q, int q_ld, const void* kv_pages, const int* page_tables, int pt_stride, int page_size, const int* pos, int rows,
+                 int n_heads, int n_kv_heads, int head_dim, float scale, const int* off, const int* n_prompt, int T, int n_cols, const int* step,
+                 int step_offset, void* out, long long step_stride, long long row_stride, long long head_stride, float* ws, void* stream) {
+  SRGPT_CHECK_ARG(q && kv_pages && page_tables && pos && off && n_prompt && step && out && ws);
+  SRGPT_CHECK_ARG(rows >= 1 && rows <= 65535 && n_heads > 0 && n_kv_heads > 0 && n_kv_heads <= 65535 && (n_heads % n_kv_heads) == 0);
+  SRGPT_CHECK_ARG(n_heads / n_kv_heads <= DMAX_GROUP && page_size > 0 && (pt_stride > 0 || rows == 1) && q_ld >= n_heads * head_dim);
+  SRGPT_CHECK_ARG(T >= 1 && n_cols >= T && head_stride >= n_cols && row_stride >= head_stride * n_heads);
+  SRGPT_CHECK_ARG(((q_ld % 8) == 0) && ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(kv_pages)) & 15) == 0);
+  if (head_dim != HD) {
+    set_last_error("srgpt_attention_probs_decode_bf16: head_dim %d unsupported (128 only)", head_dim);
+    return SRGPT_ERR_UNSUPPORTED;
+  }
+  const DecodeArgs a{reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(kv_pages), page_tables, pt_stride, page_size,
+                     n_kv_heads, n_heads / n_kv_heads, pos, scale * 1.4426950408889634f, off, n_prompt, T, n_cols, step, step_offset,
+                     reinterpret_cast<bf16*>(out), step_stride, row_stride, head_stride, reinterpret_cast<float2*>(ws)};
+  const dim3 grid(ceil_div(n_cols, DCHUNK), n_kv_heads, rows);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  decode_stats_kernel<<<grid, DTHREADS, 0, st>>>(a);
+  SRGPT_CHECK_LAUNCH();
+  decode_probs_kernel<<<grid, DTHREADS, 0, st>>>(a);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
 }  // namespace probs
 }  // namespace srgpt
 
@@ -260,4 +443,19 @@ extern "C" __attribute__((visibility("default"))) int srgpt_attention_probs_bf16
       scale * 1.4426950408889634f, reinterpret_cast<bf16*>(out), seq_stride, head_stride, ld, out_rows, row_off);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_attention_probs_decode_bf16(
+    const void* q, int q_ld, const void* kv_pages, const int* page_tables, int pt_stride, int page_size, const int* pos, int rows, int n_heads,
+    int n_kv_heads, int head_dim, float scale, const int* off, const int* n_prompt, int T, int n_cols, const int* step, int step_offset, void* out,
+    long long step_stride, long long row_stride, long long head_stride, float* ws, void* stream) {
+  return probs::decode_probs(q, q_ld, kv_pages, page_tables, pt_stride, page_size, pos, rows, n_heads, n_kv_heads, head_dim, scale, off, n_prompt,
+                             T, n_cols, step, step_offset, out, step_stride, row_stride, head_stride, ws, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_store_step_rows_bf16(const void* x, int rows, int H, const int* step, int step_offset,
+                                                                                 void* dst, long long step_stride, long long row_stride,
+                                                                                 void* stream) {
+  SRGPT_CHECK_ARG(step != nullptr);
+  return probs::store_rows(x, rows, H, 1, nullptr, dst, 0, row_stride, nullptr, stream, step, step_offset, step_stride);
 }

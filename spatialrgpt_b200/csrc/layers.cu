@@ -19,7 +19,7 @@ static inline char* mptr(void* p, size_t byte_off) { return reinterpret_cast<cha
 namespace srgpt {
 namespace probs {  // attention_probs.cu
 int store_rows(const void* x, int rows, int H, int n_seqs, const int* cu_seqlens, void* dst, long long seq_stride, long long ld, const int* row_off,
-               void* stream);
+               void* stream, const int* step = nullptr, int step_offset = 0, long long step_stride = 0);
 }
 }  // namespace srgpt
 
@@ -240,19 +240,33 @@ static int decode_step(void* h, const srgpt_llama_layer_weights* layers, const s
                        const srgpt_llama_layer_fp8* fp8, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads,
                        int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size,
                        const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
-                       float* logits_out, long long* out_ids, int* step, void* stream) {
+                       float* logits_out, long long* out_ids, int* step, void* stream, const srgpt_decode_probe* probe = nullptr) {
   SRGPT_CHECK_ARG(h && (layers || fp8) && q_buf && attn_buf && act_buf && pos && page_table && final_norm && lm_head && lm_workspace && out_ids && step);
+  SRGPT_CHECK_ARG(probe == nullptr || probe->hidden == nullptr || I >= H);  // act_buf holds the final norm row
   const int qd = n_heads * head_dim, nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
   const float scale = 1.0f / sqrtf((float)head_dim);
   for (int l = 0; l < n_layers; ++l) {
     const LayerRef w = layer_ref(l, layers, packed, nf4, fp8);
+    if (probe != nullptr && probe->hidden != nullptr)  // hidden_states[l] of this step: the row layer l reads
+      SRGPT_TRY(probs::store_rows(h, 1, H, 1, nullptr, mptr(probe->hidden, (size_t)l * probe->hidden_layer_stride * 2), 0, probe->hidden_row_stride,
+                                  nullptr, stream, step, probe->step_offset, probe->hidden_step_stride));
     SRGPT_TRY(gemv(w.m[0], h, q_buf, nqkv, H, w.in_norm, eps, nullptr, SRGPT_GEMV_QKV_ROPE, n_heads, n_kv_heads, head_dim, cos_tab, sin_tab, pos,
                    w.kv_pages, page_table, page_size, stream));
     SRGPT_TRY(srgpt_attention_decode_bf16(q_buf, attn_buf, w.kv_pages, page_table, page_size, pos, n_heads, n_kv_heads, head_dim, scale, stream));
+    if (probe != nullptr && probe->attn != nullptr)  // the rotated q of this step and the K pages the attention above just read
+      SRGPT_TRY(srgpt_attention_probs_decode_bf16(q_buf, qd, w.kv_pages, page_table, 0, page_size, pos, 1, n_heads, n_kv_heads, head_dim, scale,
+                                                  probe->off, probe->n_prompt, probe->T, probe->n_cols, step, probe->step_offset,
+                                                  mptr(probe->attn, (size_t)l * probe->attn_layer_stride * 2), probe->attn_step_stride,
+                                                  probe->attn_row_stride, probe->attn_head_stride, probe->ws, stream));
     SRGPT_TRY(gemv(w.m[1], attn_buf, h, H, qd, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, stream));
     SRGPT_TRY(gemv(w.m[2], h, act_buf, 2 * I, H, w.post_norm, eps, nullptr, SRGPT_GEMV_SWIGLU, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
                    stream));
     SRGPT_TRY(gemv(w.m[3], act_buf, h, H, I, nullptr, 0.f, h, SRGPT_GEMV_PLAIN, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, stream));
+  }
+  if (probe != nullptr && probe->hidden != nullptr) {  // hidden_states[L]: the final norm of the last residual row (LlamaDecoder.final_norm)
+    SRGPT_TRY(srgpt_rmsnorm_bf16(h, H, final_norm, act_buf, H, 1, H, eps, stream));
+    SRGPT_TRY(probs::store_rows(act_buf, 1, H, 1, nullptr, mptr(probe->hidden, (size_t)n_layers * probe->hidden_layer_stride * 2), 0,
+                                probe->hidden_row_stride, nullptr, stream, step, probe->step_offset, probe->hidden_step_stride));
   }
   if (packed_or_null(lm_packed) != nullptr)
     return srgpt_lm_head_argmax_packed_bf16(h, lm_packed, V, H, final_norm, eps, logits_out, lm_workspace, embed_table, h, out_ids, step, pos, stream);
@@ -296,6 +310,22 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_fp
     int* step, void* stream) {
   return decode_step(h, nullptr, nullptr, nullptr, layers, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab, pos,
                      page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids, step, stream);
+}
+
+// The decode step of any weight format (packed / nf4 / fp8 as the _packed / _nf4 / _fp8 entries take them; at most one given) with the
+// probes of `probe` recorded ahead of the lm_head that advances step and pos; h, the KV cache, the ids and the logits are those of the
+// unprobed entry.
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_step_probe_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4,
+    const srgpt_llama_layer_fp8* fp8, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int H, int n_heads, int n_kv_heads, int head_dim, int I,
+    float eps, const void* cos_tab, const void* sin_tab, int* pos, const int* page_table, int page_size, const void* final_norm, const void* lm_head,
+    const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_out, long long* out_ids, int* step,
+    const srgpt_decode_probe* probe, void* stream) {
+  SRGPT_CHECK_ARG(probe != nullptr && (probe->hidden != nullptr || probe->attn != nullptr));
+  SRGPT_CHECK_ARG((packed != nullptr) + (nf4 != nullptr) + (fp8 != nullptr) <= 1 && (fp8 != nullptr || layers != nullptr));
+  return decode_step(h, fp8 != nullptr ? nullptr : layers, packed, nf4, fp8, n_layers, q_buf, attn_buf, act_buf, H, n_heads, n_kv_heads, head_dim, I, eps,
+                     cos_tab, sin_tab, pos, page_table, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_out, out_ids,
+                     step, stream, probe);
 }
 
 // ---- T-row passes: T rows through the layer stack, every weight streamed once, each row with the arithmetic of a one-token step ------

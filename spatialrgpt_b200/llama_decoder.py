@@ -86,7 +86,8 @@ def decode_steps(launch, fetch, host, budgets: List[int], eos, stopping_fn) -> L
 class GraphKey(NamedTuple):
     """What a captured graph computes: its kind ("step", "batch", "rows", "beam", "verify" or "contrastive"), its rows (T for a verify
     pass), whether it samples, whether the logits processors run, the (address, step stride) of the score rows it writes (output_scores),
-    the n-gram size of a verify pass, and the candidates per prompt of a contrastive step (B * k rows)."""
+    the n-gram size of a verify pass, the candidates per prompt of a contrastive step (B * k rows), and the addresses and layout of the
+    hidden states / attentions it records (ops.StepProbe.key; generate(output_hidden_states=, output_attentions=))."""
     kind: str
     rows: int = 1
     sample: bool = False
@@ -94,6 +95,7 @@ class GraphKey(NamedTuple):
     scores: Optional[tuple] = None
     ngram: int = 0
     group: int = 0
+    probe: Optional[tuple] = None
 
 
 class BeamHypotheses:
@@ -341,6 +343,26 @@ class PrefillProbe:
     attn: Optional[torch.Tensor] = None
 
 
+@dataclass
+class GenerateProbe:
+    """What generate(output_hidden_states=, output_attentions=) records: ``prefill`` the prompt step (PrefillProbe over [B, T] padded rows),
+    ``final`` [B, T, H] the final norm of the prompt rows (None without hidden states), ``offs`` each prompt's first padded row, and
+    ``steps`` the decode steps (ops.StepProbe; None when there are none)."""
+    prefill: PrefillProbe
+    final: Optional[torch.Tensor]
+    offs: List[int]
+    steps: Optional[ops.StepProbe]
+
+    def record_final(self, llm: "LlamaDecoder", hidden: torch.Tensor, seq_lens: List[int]) -> None:
+        """final[b] at prompt b's rows: the final norm of the prefill's packed residual rows ``hidden`` (forward()'s hidden_states[L])."""
+        if self.final is None:
+            return
+        hn, o = llm.final_norm(hidden), 0
+        for b, n in enumerate(seq_lens):
+            self.final[b, self.offs[b]:self.offs[b] + n] = hn[o:o + n]
+            o += n
+
+
 class LlamaDecoder:
     def __init__(self, dims: LlamaDims, w: LlamaW, max_seq_len: int = 4096, max_new_tokens_cap: int = 4096, max_seqs: int = 1,
                  kv_pages: Optional[int] = None):
@@ -419,6 +441,7 @@ class LlamaDecoder:
     supports_batch_invariant = True  # generate(batch_invariant=True): generate_rows, each row bit-identical to batch 1
     supports_contrastive = True  # generate(penalty_alpha=, top_k=): generate_contrastive
     supports_forward_outputs = True  # forward(output_hidden_states=, output_attentions=): the probed prefill (PrefillProbe)
+    supports_generate_outputs = True  # generate(output_hidden_states=, output_attentions=): the probed prefill and decode steps
     packs_decode_weights = True
     _vstate = None  # buffers of the verify pass (prompt-lookup speculative decoding), allocated on first use
     _bstate = None  # buffers of the batched decode step, for the batch size of the last batched request
@@ -601,12 +624,13 @@ class LlamaDecoder:
 
     # ---------------------------------------------------------------------------------------------
     def _decode_step_launch(self, seq: int, logits_out: Optional[torch.Tensor] = None, sample: bool = False, proc: bool = False,
-                            scores: Optional[torch.Tensor] = None) -> None:
+                            scores: Optional[torch.Tensor] = None, probe: Optional[ops.StepProbe] = None) -> None:
         d, w = self.dims, self.w
         if (sample or proc or scores is not None) and logits_out is None:
             logits_out = self._sample_buffer()
         ops.llama_decode_step(self.h, self.stack, self.q_buf, self.attn_buf, self.act_buf, d, self.cos, self.sin, self.pos, self.active_pt, PAGE_SIZE,
-                              w.norm, w.lm_head, w.embed, self.lm_ws, self.out_ids, self.step, logits_out)
+                              w.norm, w.lm_head, w.embed, self.lm_ws, self.out_ids, self.step, logits_out,
+                              **({} if probe is None else dict(probe=probe)))
         self._choose(logits_out, sample, proc, scores)
 
     def _choose(self, raw: Optional[torch.Tensor], sample: bool, proc: bool, scores: Optional[torch.Tensor]) -> None:
@@ -690,6 +714,8 @@ class LlamaDecoder:
         replay launches (ops.LAUNCHES accounting)."""
         if key in self._graphs:
             return self._graphs[key][0]
+        if key.probe is not None:  # every request records into new tensors: keep one probed graph, not one per request
+            self._drop_graphs(lambda k: k.probe is not None)
         saved = [t.clone() for t in restore]
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream())  # after the clones are enqueued
@@ -720,13 +746,15 @@ class LlamaDecoder:
         entry = self._graphs.get(GraphKey("step"))
         return None if entry is None else entry[0]
 
-    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False, scores: Optional[torch.Tensor] = None) -> torch.cuda.CUDAGraph:
+    def _ensure_graph(self, seq: int, sample: bool = False, proc: bool = False, scores: Optional[torch.Tensor] = None,
+                      probe: Optional[ops.StepProbe] = None) -> torch.cuda.CUDAGraph:
         """The one-token step graph of this mode.  Sampling adds its kernel; processing adds 1 more when sampling, 3 when greedy
-        (processing, key unpack and pick); greedy score rows add their copy (the sampler writes its own)."""
+        (processing, key unpack and pick); greedy score rows add their copy (the sampler writes its own); a probe its launches."""
         kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0) + (
-            1 if scores is not None and not sample else 0)
-        return self._capture(GraphKey("step", 1, sample, proc, self._scores_key(scores)),
-                             lambda: self._decode_step_launch(seq, sample=sample, proc=proc, **self._scores_kw(scores)),
+            1 if scores is not None and not sample else 0) + (0 if probe is None else probe.kernels(self.dims.num_hidden_layers, final_norm=True))
+        return self._capture(GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key()),
+                             lambda: self._decode_step_launch(seq, sample=sample, proc=proc, **self._scores_kw(scores),
+                                                              **({} if probe is None else dict(probe=probe))),
                              (self.pos, self.step, self.h, self.out_ids), kernels)
 
     # ---- stop checks: generated ids reach the host through pinned memory while the next step runs --------------------------------
@@ -775,15 +803,19 @@ class LlamaDecoder:
         self.cache.reserve_many([n + max_new_tokens + slack for n in prompt_lens])
 
     def _prefill_first_token(self, embeds: torch.Tensor, seq: int, reuse_rows: int, logits_row: Optional[torch.Tensor], sample: bool,
-                             proc: bool, scores: Optional[torch.Tensor]) -> torch.Tensor:
+                             proc: bool, scores: Optional[torch.Tensor], probe: Optional[GenerateProbe] = None) -> torch.Tensor:
         """Batch 1's prefill of the prompt ``embeds`` [S, H] into sequence `seq` (its first reuse_rows rows are in the pages already)
         and its first token: final norm + lm_head + arg max on the last row, which writes out_ids[0], the token's embedding row (h)
         and pos = S, step = 1; then _choose.  The fp32 logits go to ``logits_row``, or to the sample buffer when the choice reads
         them.  generate_rows starts every row with it, so each row's first token is its batch-1 request's by construction.  Returns
-        the prefill's final residual stream of rows reuse_rows .. S - 1."""
+        the prefill's final residual stream of rows reuse_rows .. S - 1.  ``probe``: the prefill records the prompt step (whole prompts)."""
         d, w = self.dims, self.w
         S = embeds.shape[0]
-        hidden = self.prefill_hidden(embeds[reuse_rows:], seq, reuse_rows)
+        if probe is None:
+            hidden = self.prefill_hidden(embeds[reuse_rows:], seq, reuse_rows)
+        else:
+            hidden = self.prefill_hidden(embeds[reuse_rows:], seq, reuse_rows, probe=probe.prefill)
+            probe.record_final(self, hidden, [S])
         self.pos.fill_(S - 1)
         self.step.zero_()
         if logits_row is None and (sample or proc or scores is not None):
@@ -818,7 +850,7 @@ class LlamaDecoder:
     def generate_from_embeds(self, inputs_embeds: torch.Tensor, max_new_tokens: int, eos_token_ids=None, stopping_fn=None,
                              use_graph: bool = True, return_logits: bool = False, seq: int = 0, sampling=None, reuse_rows: int = 0,
                              lookup_ids: Optional[torch.Tensor] = None, lookup_k: int = 0, lookup_ngram: int = 2, processors=None,
-                             output_scores: bool = False):
+                             output_scores: bool = False, outputs: Optional[GenerateProbe] = None):
         """Greedy (or, with ``sampling=dict(temperature, top_p, seed)``, nucleus-sampled) decoding started from prompt
         embeddings [S, H].  Returns LongTensor [n_new] (and fp32 logits [n_new, V] when return_logits).
         ``stopping_fn(ids_so_far: LongTensor) -> bool``.
@@ -837,10 +869,14 @@ class LlamaDecoder:
         ``output_scores``: returns (what it returns without, {"scores": fp32 [n_new, 1, V]}), row t being the row token t was chosen from
         (HF's output_scores): the raw row when greedy, the processed row with processors, the warped row (logits / T, -inf where top-k /
         top-p removed the token) when sampled.  The decode graphs write them on the device; prompt-lookup decoding takes them from its
-        verify passes' logit rows (greedy without processors: the raw rows)."""
+        verify passes' logit rows (greedy without processors: the raw rows).
+        ``outputs`` (GenerateProbe of one row; not with reuse_rows or prompt lookup): the prefill records the prompt step and every
+        decode step records its hidden rows / attention probabilities at the device step; ids, scores and logits are unchanged."""
         d = self.dims
         S = inputs_embeds.shape[0]
         n_reuse = int(reuse_rows)
+        if outputs is not None and (n_reuse != 0 or lookup_k):
+            raise NotImplementedError("hidden states / attentions with a reused prompt prefix or prompt lookup")
         if n_reuse != 0 and (seq != 0 or n_reuse < 0 or n_reuse > self.prefix_rows or n_reuse > S - 1):
             raise ValueError(f"reuse_rows={n_reuse} is not a reusable prefix here: sequence {seq}, {self.prefix_rows} recorded prefill rows, "
                              f"{S} prompt rows (at most S - 1 may be reused)")
@@ -867,7 +903,8 @@ class LlamaDecoder:
         lookup_scores = output_scores and k > 0 and max_new_tokens > 1
         logits = torch.empty((n_rows, d.vocab_size), dtype=torch.float32, device=self.device) if return_logits or lookup_scores else None
         scores = self._scores_view(max_new_tokens, 1) if output_scores and not lookup_scores else None
-        self._prefill_first_token(inputs_embeds, seq, n_reuse, None if logits is None else logits[0], sample, proc, scores)
+        self._prefill_first_token(inputs_embeds, seq, n_reuse, None if logits is None else logits[0], sample, proc, scores,
+                                  **({} if outputs is None else dict(probe=outputs)))
         if seq == 0 and self.supports_prefix_reuse:
             self._record_prefix(S)
         if k > 0 and max_new_tokens > 1:
@@ -876,7 +913,8 @@ class LlamaDecoder:
                 return r
             out, lg = r
             return (r, {"scores": lg.unsqueeze(1).clone()}) if return_logits else (out, {"scores": lg.unsqueeze(1)})
-        r = self._decode_loop(seq, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, scores)
+        r = self._decode_loop(seq, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, scores,
+                              **({} if outputs is None or outputs.steps is None else dict(probe=outputs.steps)))
         if not output_scores:
             return r
         return r, {"scores": scores[:(r[0] if return_logits else r).numel()].clone()}
@@ -952,21 +990,22 @@ class LlamaDecoder:
         return out
 
     def _decode_loop(self, seq: int, max_new_tokens: int, eos, stopping_fn, use_graph: bool, logits, sample: bool = False,
-                     proc: bool = False, scores: Optional[torch.Tensor] = None):
+                     proc: bool = False, scores: Optional[torch.Tensor] = None, probe: Optional[ops.StepProbe] = None):
         """Steps 1..max_new_tokens-1 of sequence `seq` (greedy, or sampled; with the logits processors when proc); pos / step / h /
         out_ids[0] are already set.  ``scores`` ([T, 1, V] fp32): each step's score row goes to scores[step].  On a stop, the step in
         flight only touched this sequence's own KV slot and the step counters, which the next request resets."""
         self.active_pt.copy_(self.cache.page_tables[seq])
         graph = use_graph and logits is None
-        key = GraphKey("step", 1, sample, proc, self._scores_key(scores))
+        key = GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key())
+        probe_kw = {} if probe is None else dict(probe=probe)
         if graph:
-            self._ensure_graph(seq, sample, proc, scores)
+            self._ensure_graph(seq, sample, proc, scores, **probe_kw)
 
         def launch(n: int) -> None:
             if graph:
                 self._replay(key)
             else:
-                self._decode_step_launch(seq, None if logits is None else logits[n], sample, proc, **self._scores_kw(scores))
+                self._decode_step_launch(seq, None if logits is None else logits[n], sample, proc, **self._scores_kw(scores), **probe_kw)
 
         n = self._run_steps(launch, self.out_ids[:max_new_tokens].view(max_new_tokens, 1), [max_new_tokens], eos, stopping_fn)[0]
         out = self.out_ids[:n].clone()
@@ -993,12 +1032,13 @@ class LlamaDecoder:
         return st
 
     def _batch_step_launch(self, st, logits_only: bool = False, proc: bool = False, sample: bool = False,
-                           scores: Optional[torch.Tensor] = None) -> None:
+                           scores: Optional[torch.Tensor] = None, probe: Optional[ops.StepProbe] = None) -> None:
         """One decode step of all B sequences (llava_arch.py:549-611 + modeling_llama.py:540-562 semantics without padding): the
         projections are wgmma GEMMs over the B rows (tall stream-K configuration), RoPE / KV append and attention per sequence.
         ``sample``: row b draws its token with st["seeds"][b] at counter step (the counter the one-token loop uses for that token).
         ``scores`` ([T, B, V] fp32): the rows the tokens were chosen from go to scores[step] (the bf16 rows widened, the processed rows,
-        or the sampler's warped rows)."""
+        or the sampler's warped rows).  ``probe`` (ops.StepProbe of B rows): each layer's input rows and attention probabilities, and
+        the final norm rows, go to its outputs at the device step."""
         d, w, B = self.dims, self.w, st["B"]
         nh, nkv, hd, V = d.num_attention_heads, d.num_key_value_heads, d.head_dim, d.vocab_size
         qd = nh * hd
@@ -1009,15 +1049,22 @@ class LlamaDecoder:
             return ops.linear(x, wt, st.get("q8"), st.get("s8"), **kw)
         for l, lw in enumerate(w.layers):
             pages = self.cache.layer(l)
+            if probe is not None and probe.hidden is not None:
+                ops.store_step_rows(h, st["step"], probe.step_offset, probe.hidden[:, l])
             ops.rmsnorm(h, lw.in_norm, d.rms_norm_eps, out=xn)
             linear(xn, lw.qkv_w, out=qkv)
             ops.rope_kv_append_varlen(qkv, nh, nkv, hd, self.cos, self.sin, st["pos"], pages, pts, PAGE_SIZE, st["cu"])
             ops.attention_decode_batched(qkv[:, :qd], attn, pages, pts, PAGE_SIZE, st["pos"], nh, nkv, hd, self.scale)
+            if probe is not None and probe.attn is not None:
+                ops.attention_probs_decode(qkv[:, :qd], pages, pts, PAGE_SIZE, st["pos"], nh, nkv, hd, self.scale, probe.off, probe.n_prompt,
+                                           probe.T, st["step"], probe.step_offset, probe.attn[:, l], probe.ws)
             linear(attn, lw.o_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
             ops.rmsnorm(h, lw.post_norm, d.rms_norm_eps, out=xn)
             linear(xn, lw.gateup_w, epilogue=ops.EPI_SWIGLU, out=act)
             linear(act, lw.down_w, residual=h, epilogue=ops.EPI_BIAS_RESIDUAL, out=h)
         ops.rmsnorm(h, w.norm, d.rms_norm_eps, out=xn)
+        if probe is not None and probe.hidden is not None:  # hidden_states[L]: the rows the lm_head GEMM reads
+            ops.store_step_rows(xn, st["step"], probe.step_offset, probe.hidden[:, len(w.layers)])
         lg = st["logits"][:, :V]
         ops.gemm(xn, w.lm_head, out=lg)  # bf16 logits (modeling_llama.py:1044), arg max with the lowest index on ties
         if logits_only:  # beam search: the host picks the next tokens from the candidates of these logits
@@ -1039,7 +1086,7 @@ class LlamaDecoder:
 
     def _decode_batched(self, first: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos, stopping_fn, use_graph: bool,
                         proc: bool = False, sample_from: Optional[torch.Tensor] = None, seeds: Optional[List[int]] = None,
-                        scores: Optional[torch.Tensor] = None):
+                        scores: Optional[torch.Tensor] = None, probe: Optional[ops.StepProbe] = None):
         """Decode of B prefilled sequences together: greedy, or sampled when ``sample_from`` holds the B first-token rows to draw from
         ([B, V], the bf16 lm_head rows or the processed fp32 rows) and ``seeds`` the B row seeds.  Returns a list of LongTensor [n_b]
         (each cut at its own stop).  ``scores`` ([T, B, V] fp32; a greedy caller has written row 0): every step's rows go to scores[step].
@@ -1059,18 +1106,21 @@ class LlamaDecoder:
         st["h"].copy_(ops.splice_rows(self.w.embed, None, None, None, zero, first.to(torch.int32)))
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
-        key = GraphKey("batch", B, sample, proc, self._scores_key(scores))  # the graphs that write scores hold the buffer's address
+        # the graphs that write scores / probes hold the buffers' addresses
+        key = GraphKey("batch", B, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key())
+        probe_kw = {} if probe is None else dict(probe=probe)
         if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max (sampling: processing + draw)
-            self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample, scores=scores),
+            L = self.dims.num_hidden_layers
+            self._capture(key, lambda: self._batch_step_launch(st, proc=proc, sample=sample, scores=scores, **probe_kw),
                           (st["h"], st["pos"], st["step"], st["out"]),
-                          self._batch_kernels_per_layer * self.dims.num_hidden_layers + (5 if proc else 4) + (
-                              1 if scores is not None and not sample else 0))
+                          self._batch_kernels_per_layer * L + (5 if proc else 4) + (1 if scores is not None and not sample else 0) + (
+                              0 if probe is None else probe.kernels(L, final_norm=False)))
 
         def launch(n: int) -> None:
             if use_graph:
                 self._replay(key)
             else:
-                self._batch_step_launch(st, proc=proc, sample=sample, scores=scores)
+                self._batch_step_launch(st, proc=proc, sample=sample, scores=scores, **probe_kw)
 
         out2d = st["out"][: max_new_tokens * B].view(max_new_tokens, B)
         lens = self._run_steps(launch, out2d, [max_new_tokens] * B, eos, stopping_fn)
@@ -1483,7 +1533,7 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def generate_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], max_new_tokens: int, eos_token_ids=None,
                        stopping_fn=None, use_graph: bool = True, return_logits: bool = False, sampling=None, processors=None,
-                       num_return_sequences: int = 1, output_scores: bool = False):
+                       num_return_sequences: int = 1, output_scores: bool = False, outputs: Optional[GenerateProbe] = None):
         """Decoding of B prompts: ONE packed prefill pass (tensor-core bound, all prompts share every GEMM), one lm_head GEMM for the
         B first tokens, then BATCHED decode: every step advances all B sequences, each weight streamed once per step for the
         whole batch (_decode_batched), greedy or sampled (``sampling``: sequence b draws with sequence_seeds(seed, B)[b]).  With
@@ -1496,8 +1546,13 @@ class LlamaDecoder:
         ``output_scores``: returns (what it returns without, {"scores": fp32 [n_max, B * n, V]}), scores[t, r] being the row token t of
         row r was chosen from (generate_from_embeds) and n_max the longest row's length.  In the batched step a row that has stopped
         keeps its place, so its later steps hold what the step computed for it; the one-after-the-other path (return_logits) leaves
-        them 0."""
+        them 0.
+        ``outputs`` (GenerateProbe of B rows; B > 1, no return_logits, num_return_sequences 1): the packed prefill records the prompt step
+        and the batched step every decode step; ids and scores are unchanged."""
         n_ret = int(num_return_sequences)
+        if outputs is not None and (return_logits or n_ret != 1 or len(seq_lens) < 2):
+            raise NotImplementedError("hidden states / attentions of generate_batch need B > 1 prompts without output_logits or "
+                                      "num_return_sequences > 1")
         if n_ret < 1:
             raise ValueError(f"num_return_sequences must be >= 1, got {n_ret}")
         if n_ret > 1:
@@ -1516,7 +1571,10 @@ class LlamaDecoder:
         proc = self._set_processors(processors)
         row_lens = [int(n) for n in seq_lens for _ in range(n_ret)]  # row b * n_ret + j continues prompt b
         self._start_request(row_lens, max_new_tokens)
-        if n_ret == 1:
+        if outputs is not None:
+            hidden = self.prefill_packed(packed_embeds, seq_lens, probe=outputs.prefill)
+            outputs.record_final(self, hidden, [int(n) for n in seq_lens])
+        elif n_ret == 1:
             hidden = self.prefill_packed(packed_embeds, seq_lens)
         else:  # each prompt once, into the first of its rows; the other rows get copies of its prompt pages
             tables = [list(self.cache.owned[r]) for r in range(B)]
@@ -1540,7 +1598,8 @@ class LlamaDecoder:
         seeds = sequence_seeds(self.sample_seed, B) if sample else None
         if not return_logits and B > 1 and (not sample or self.supports_batch_sampling):
             outs = self._decode_batched(first, seq_lens, max_new_tokens, eos, stopping_fn, use_graph, proc,
-                                        sample_from=(first_rows if proc else lg) if sample else None, seeds=seeds, scores=scores)
+                                        sample_from=(first_rows if proc else lg) if sample else None, seeds=seeds, scores=scores,
+                                        **({} if outputs is None or outputs.steps is None else dict(probe=outputs.steps)))
             return (outs, {"scores": scores[:max(o.numel() for o in outs)].clone()}) if output_scores else outs
         if scores is not None and B > 1:  # one row after the other: a row's steps past its stop are never written
             scores.view(max_new_tokens, B * d.vocab_size)[1 if not sample else 0:].zero_()

@@ -15,7 +15,7 @@ import torch
 from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
-from .llama_decoder import LlamaDecoder, PrefillProbe, check_candidates, sequence_seeds
+from .llama_decoder import GenerateProbe, LlamaDecoder, PrefillProbe, check_candidates, sequence_seeds
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
@@ -136,6 +136,39 @@ def refuse_contrastive(top_k: int = 50, processors=None, lookup_k: int = 0, pref
         raise NotImplementedError("penalty_alpha with batch_invariant=True (the candidates run in the batched step)")
     if llm is not None and not getattr(llm, "supports_contrastive", False):
         raise NotImplementedError("penalty_alpha on the tensor-parallel decoder")
+
+
+def refuse_generate_outputs(num_beams: int = 1, contrastive: bool = False, guided: bool = False, batch_invariant: bool = False, lookup_k: int = 0,
+                            prefix_cache: bool = False, n_ret: int = 1, return_logits: bool = False, n_prompts: int = 1, llm=None) -> None:
+    """The generate() options output_hidden_states / output_attentions (with return_dict_in_generate=True) do not serve: raises
+    NotImplementedError before any GPU work.  They are recorded by the probed prefill and the probed batch-1 / batched decode steps."""
+    what = "output_hidden_states / output_attentions"
+    if num_beams != 1:
+        raise NotImplementedError(f"{what} with beam search")
+    if contrastive:
+        raise NotImplementedError(f"{what} with penalty_alpha (contrastive search)")
+    if guided:
+        raise NotImplementedError(f"{what} with guidance_scale != 1")
+    if batch_invariant:
+        raise NotImplementedError(f"{what} with batch_invariant=True")
+    if lookup_k:
+        raise NotImplementedError(f"{what} with prompt_lookup_num_tokens")
+    if prefix_cache:
+        raise NotImplementedError(f"{what} with prefix_cache=True")
+    if n_ret != 1:
+        raise NotImplementedError(f"{what} with num_return_sequences > 1")
+    if return_logits and n_prompts > 1:
+        raise NotImplementedError(f"{what} with output_logits over a batch (that path decodes the prompts one after another)")
+    if llm is not None and not getattr(llm, "supports_generate_outputs", False):
+        raise NotImplementedError(f"{what} on the tensor-parallel decoder: no rank holds every attention head")
+
+
+def generate_outputs_bytes(L: int, H: int, nh: int, B: int, T: int, N: int, hidden: bool, attentions: bool) -> int:
+    """Bytes of generate()'s hidden states / attentions for B prompts padded to T rows and N new tokens: the prompt step's (forward()'s
+    outputs), then the N - 1 decode steps' [N - 1, L + 1, B, H] and [N - 1, L, B, nh, T + N - 1] element-type tensors."""
+    N1 = max(int(N), 1) - 1
+    return (2 * ((L + 1) * B * T * H * hidden + L * B * nh * T * T * attentions)
+            + N1 * (L + 1) * B * H * 2 * hidden + N1 * L * B * nh * (T + N1) * 2 * attentions)
 
 
 def contrastive_alpha(penalty_alpha) -> float:
@@ -705,6 +738,10 @@ class LlavaLlamaModel:
         # dict, output_scores is ignored, as HF ignores it.
         return_dict = bool(generation_kwargs.pop("return_dict_in_generate", False))
         output_scores = bool(generation_kwargs.pop("output_scores", False)) and return_dict
+        # output_hidden_states / output_attentions (with the dict; ignored without it, as HF ignores them): HF's per-token tuples, entry 0
+        # the prompt step (forward()'s outputs, bit for bit), entry t >= 1 decode step t, recorded on the device by the probed steps
+        want_h = bool(generation_kwargs.pop("output_hidden_states", False)) and return_dict
+        want_a = bool(generation_kwargs.pop("output_attentions", False)) and return_dict
         use_graph = bool(generation_kwargs.pop("use_cuda_graph", True))
         # prefix_cache=True (batch 1, opt-in): keep the previous such request's encoder outputs and the K/V of its prompt rows, and
         # prefill only the rows after the longest unchanged prefix (a follow-up turn of a conversation).  The new rows run through
@@ -799,6 +836,13 @@ class LlavaLlamaModel:
         if output_scores and not getattr(self.llm, "supports_output_scores", False):
             raise NotImplementedError("output_scores on the tensor-parallel decoder (its logits are vocabulary-parallel: no rank holds a whole row)")
         n_prompts = 1 if input_ids is None else int(input_ids.shape[0])
+        if want_h or want_a:
+            refuse_generate_outputs(num_beams=num_beams, contrastive=contrastive, guided=guided, batch_invariant=batch_invariant, lookup_k=lookup_k,
+                                    prefix_cache=prefix_cache, n_ret=n_ret, return_logits=return_logits, n_prompts=n_prompts, llm=self.llm)
+            if images is None:  # the prompt rows and the token budget are known before any device work
+                B_, T_ = input_ids.shape
+                lens_ = [T_] * B_ if attention_mask is None else [int(n) for n in attention_mask.sum(-1).tolist()]
+                self._check_generate_outputs_fit(B_, T_, self._token_budget(max_new_tokens, max_length, lens_), want_h, want_a)
         if contrastive:
             refuse_contrastive(top_k=contrastive_k, processors=processors, lookup_k=lookup_k, prefix_cache=prefix_cache,
                                return_logits=return_logits, guided=guided, batch_invariant=batch_invariant, llm=self.llm)
@@ -852,10 +896,17 @@ class LlavaLlamaModel:
                 ids = input_ids[0].cpu() if attention_mask is None else input_ids[0].cpu()[attention_mask[0].cpu().bool()]
                 prefix.update(src_id=torch.full((ids.numel(),), SRC_TOKENS, dtype=torch.int32), src_row=ids.to(torch.int32), n_tok=1,
                               image_equal=[], mask_equal=[], encoders_skipped=False)
-        if max_new_tokens is None:
-            max_new_tokens = 20 if max_length is None else max(int(max_length) - max(lens), 1)  # HF default max_length=20
+        max_new_tokens = self._token_budget(max_new_tokens, max_length, lens)
 
         outs, all_logits = [], []
+        left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
+        gen_out, gp = None, None
+        if want_h or want_a:  # the prompts' padded layout: generate()'s inputs_embeds, or the spliced rows padded as forward() pads them
+            T_pad = int(inputs_embeds.shape[1]) if packed is None else max(int(n) for n in lens)
+            if packed is not None:
+                self._check_generate_outputs_fit(B, T_pad, int(max_new_tokens), want_h, want_a)
+            gen_out, gp = self._generate_probe([int(n) for n in lens], T_pad, int(max_new_tokens), left, want_h, want_a)
+        gp_kw = {} if gp is None else {"outputs": gp}
         extra = None  # the decoder's output_scores results
         sc_kw = {"output_scores": True} if output_scores else {}
         stop_fn = stopping_fn_of(stopping_criteria)
@@ -864,7 +915,6 @@ class LlavaLlamaModel:
         proc = {} if processors is None else {"processors": processors}
         if lookup_k and B != 1:
             raise NotImplementedError("prompt_lookup_num_tokens serves batch-1 requests")
-        left = getattr(self.config.llama, "tokenizer_padding_side", "right") == "left"
         if contrastive:  # any B: the prompts' unpadded rows, packed
             if packed is None:
                 T = inputs_embeds.shape[1]
@@ -897,7 +947,7 @@ class LlavaLlamaModel:
                             lookup_ngram=lookup_ngram)
             r = self.llm.generate_from_embeds(emb, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                               use_graph=use_graph, return_logits=return_logits, sampling=sampling, reuse_rows=reuse, **spec,
-                                              **proc, **sc_kw)
+                                              **proc, **sc_kw, **gp_kw)
             if output_scores:
                 r, extra = r
             if lookup_k:
@@ -925,14 +975,67 @@ class LlavaLlamaModel:
             else:
                 r = self.llm.generate_batch(packed, lens, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
                                             use_graph=use_graph, return_logits=return_logits, sampling=sampling, num_return_sequences=n_ret,
-                                            **proc, **sc_kw)
+                                            **proc, **sc_kw, **gp_kw)
                 if output_scores:
                     r, extra = r
                 if return_logits:
                     outs, all_logits = r
                 else:
                     outs = r
-        return self._generate_result(outs, pad_token_id, return_dict, all_logits if return_logits else None, extra, num_beams != 1)
+        res = self._generate_result(outs, pad_token_id, return_dict, all_logits if return_logits else None, extra, num_beams != 1)
+        if gen_out is not None:
+            res.hidden_states, res.attentions = self._generate_outputs(gen_out, max(o.numel() for o in outs))
+        return res
+
+    @staticmethod
+    def _token_budget(max_new_tokens, max_length, lens) -> int:
+        """generate()'s max_new_tokens: as given, else max_length less the longest prompt (at least 1), else HF's default max_length 20."""
+        if max_new_tokens is not None:
+            return max_new_tokens
+        return 20 if max_length is None else max(int(max_length) - max(lens), 1)
+
+    def _check_generate_outputs_fit(self, B: int, T: int, N: int, hidden: bool, attentions: bool) -> None:
+        """RuntimeError naming the bytes generate()'s hidden states / attentions need (generate_outputs_bytes) when they exceed the free
+        device memory."""
+        d = self.llm.dims
+        need = generate_outputs_bytes(d.num_hidden_layers, d.hidden_size, d.num_attention_heads, B, T, N, hidden, attentions)
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need > free:
+            raise RuntimeError(f"generate(output_hidden_states={hidden}, output_attentions={attentions}) over {B} x {T} prompt rows and {N} new "
+                               f"tokens needs {need} bytes ({need / 2 ** 30:.1f} GiB) for its outputs; {free} bytes are free on {self.device}")
+
+    def _generate_probe(self, lens: List[int], T: int, N: int, left: bool, hidden: bool, attentions: bool):
+        """The tensors generate()'s hidden states / attentions live in, and the GenerateProbe that has the decoder record into them:
+        the prompt step's [L + 1, B, T, H] / [L, B, nh, T, T] (forward()'s layout, 0 at padded rows) and the decode steps' [N - 1, L + 1,
+        B, H] / [N - 1, L, B, nh, T + N - 1]; prompt b occupies rows / columns off_b .. off_b + n_b - 1, off_b = T - n_b when left."""
+        d, dev, dt = self.llm.dims, self.device, self.dtype
+        L, H, nh, B = d.num_hidden_layers, d.hidden_size, d.num_attention_heads, len(lens)
+        offs = [T - n if left else 0 for n in lens]
+        hs0 = hsd = att0 = attd = None
+        if hidden:
+            hs0 = torch.zeros((L + 1, B, T, H), dtype=dt, device=dev)
+            hsd = torch.empty((N - 1, L + 1, B, H), dtype=dt, device=dev) if N > 1 else None
+        if attentions:  # every entry of these is written by the probability kernels, padding included
+            att0 = torch.empty((L, B, nh, T, T), dtype=dt, device=dev)
+            attd = torch.empty((N - 1, L, B, nh, T + N - 1), dtype=dt, device=dev) if N > 1 else None
+        off_dev = torch.tensor(offs, dtype=torch.int32).to(dev)
+        steps = None
+        if N > 1:
+            steps = ops.StepProbe(off_dev, torch.tensor(lens, dtype=torch.int32).to(dev), T, hidden=hsd, attn=attd, step_offset=-1)
+        gp = GenerateProbe(PrefillProbe(off_dev, None if hs0 is None else hs0[:L], att0), None if hs0 is None else hs0[L], offs, steps)
+        return (hs0, att0, hsd, attd, T), gp
+
+    @staticmethod
+    def _generate_outputs(gen_out, n_max: int):
+        """(hidden_states, attentions) of HF's generate(): one entry per token of the longest row, entry 0 the prompt step, entry t the
+        decode step that read token t - 1 ([B, 1, H] per slot, [B, nh, 1, T + t] per layer), as views of the tensors _generate_probe made."""
+        hs0, att0, hsd, attd, T = gen_out
+        hs = att = None
+        if hs0 is not None:
+            hs = (tuple(hs0.unbind(0)),) + tuple(tuple(x[:, None] for x in hsd[t - 1].unbind(0)) for t in range(1, n_max))
+        if att0 is not None:
+            att = (tuple(att0.unbind(0)),) + tuple(tuple(x[:, :, None, :T + t] for x in attd[t - 1].unbind(0)) for t in range(1, n_max))
+        return hs, att
 
     def _generate_batch_invariant(self, input_ids, images, depths, masks, attention_mask, max_new_tokens, max_length, eos_token_id, stopping_criteria,
                                   pad_token_id, use_graph: bool, return_logits: bool, return_dict: bool, sampling, seed, guidance=None):

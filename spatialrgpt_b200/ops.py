@@ -1396,6 +1396,104 @@ def attention_probs(q: torch.Tensor, k: torch.Tensor, n_heads: int, n_kv_heads: 
     return out
 
 
+DECODE_PROBS_CHUNK = 128  # output columns per CTA of srgpt_attention_probs_decode_bf16; its workspace holds a (max, sum) per chunk
+
+
+def attention_probs_decode_ws(rows: int, n_heads: int, n_cols: int, device) -> torch.Tensor:
+    """The fp32 workspace srgpt_attention_probs_decode_bf16 needs for `rows` rows of n_heads heads and n_cols output columns."""
+    return torch.empty(rows * n_heads * ((n_cols + DECODE_PROBS_CHUNK - 1) // DECODE_PROBS_CHUNK) * 2, dtype=torch.float32, device=device)
+
+
+def _check_decode_probs_out(out: torch.Tensor, R: int, n_heads: int, T: int, what: str) -> None:
+    _need(out, ELEM(), what)
+    if out.dim() != 4 or tuple(out.shape[1:3]) != (R, n_heads) or out.shape[3] < T or out.stride(3) != 1:
+        raise SrgptError(f"{what} must be [steps, {R}, {n_heads}, n_cols >= {T}] with unit inner stride, got {tuple(out.shape)}")
+
+
+def attention_probs_decode(q: torch.Tensor, kv_pages: torch.Tensor, page_tables: torch.Tensor, page_size: int, pos: torch.Tensor, n_heads: int,
+                           n_kv_heads: int, head_dim: int, scale: float, off: torch.Tensor, n_prompt: torch.Tensor, T: int, step: torch.Tensor,
+                           step_offset: int, out: torch.Tensor, ws: torch.Tensor) -> torch.Tensor:
+    """The attention probabilities of a one-token decode step of R rows over one layer's paged cache, in the element type: q [R, >=
+    n_heads * head_dim] (row-strided, e.g. the q columns of a fused qkv buffer; rotated), page_tables [>= R, cap] (or the one table of a
+    single row), pos int32 [R] each row's newest position.  Row r, head h goes to out[step + step_offset, r, h] (``out`` a [steps, R,
+    n_heads, n_cols] view with unit inner stride; ``step`` device int32 [1], read at run time) with prompt key p at column off[r] + p
+    (p < n_prompt[r]) and generated key n_prompt[r] + j at column T + j; every column of the row's [0, T + pos[r] + 1 - n_prompt[r]) is
+    written and nothing past it.  ``ws``: attention_probs_decode_ws(R, n_heads, n_cols)."""
+    _need(q, ELEM(), "attention_probs_decode.q")
+    for t, what in ((pos, "pos"), (off, "off"), (n_prompt, "n_prompt"), (step, "step"), (page_tables, "page_tables")):
+        _need(t, torch.int32, "attention_probs_decode." + what)
+    _need(ws, torch.float32, "attention_probs_decode.ws")
+    R = q.shape[0]
+    _check_decode_probs_out(out, R, n_heads, T, "attention_probs_decode.out")
+    n_cols = out.shape[3]
+    if pos.numel() < R or off.numel() < R or n_prompt.numel() < R or ws.numel() < attention_probs_decode_ws(R, n_heads, n_cols, "meta").numel():
+        raise SrgptError("attention_probs_decode: pos / off / n_prompt need one entry per row and ws attention_probs_decode_ws's size")
+    pt_stride = page_tables.stride(0) if page_tables.dim() == 2 else 0
+    if R > 1 and (page_tables.dim() != 2 or page_tables.shape[0] < R or page_tables.stride(1) != 1):
+        raise SrgptError("attention_probs_decode: R > 1 rows need page_tables [R, cap] with unit inner stride")
+    check(_lib.load().srgpt_attention_probs_decode_bf16(_p(q), _rowmajor2d(q, "attention_probs_decode.q"), _p(kv_pages), _p(page_tables), pt_stride,
+                                                        page_size, _p(pos), R, n_heads, n_kv_heads, head_dim, scale, _p(off), _p(n_prompt), T,
+                                                        n_cols, _p(step), step_offset, _p(out), out.stride(0), out.stride(1), out.stride(2),
+                                                        _p(ws), _stream()), "srgpt_attention_probs_decode_bf16")
+    _count(2)
+    return out
+
+
+def store_step_rows(x: torch.Tensor, step: torch.Tensor, step_offset: int, dst: torch.Tensor) -> None:
+    """Rows x [R, H] (contiguous, the element type) -> dst[step + step_offset] (``dst`` a [steps, R, H] view with unit inner stride;
+    ``step`` device int32 [1], read at run time)."""
+    _need(x, ELEM(), "store_step_rows.x"); _need(dst, ELEM(), "store_step_rows.dst"); _need(step, torch.int32, "store_step_rows.step")
+    x2 = x.view(1, -1) if x.dim() == 1 else x
+    if not x2.is_contiguous() or dst.dim() != 3 or tuple(dst.shape[1:]) != tuple(x2.shape) or dst.stride(2) != 1:
+        raise SrgptError(f"store_step_rows: dst must be [steps, {x2.shape[0]}, {x2.shape[1]}] with unit inner stride over contiguous rows")
+    check(_lib.load().srgpt_store_step_rows_bf16(_p(x2), x2.shape[0], x2.shape[1], _p(step), step_offset, _p(dst), dst.stride(0), dst.stride(1),
+                                                 _stream()), "srgpt_store_step_rows_bf16")
+    _count(1)
+
+
+class StepProbe:
+    """What the probed decode steps record (generate(output_hidden_states=, output_attentions=)): ``hidden`` [steps, L + 1, R, H] (slot l
+    the row layer l reads, slot L the final norm of the last layer's row) and ``attn`` [steps, L, R, n_heads, n_cols] (each layer's
+    probabilities in generate()'s padded columns: T prompt columns, row r's prompt at off[r], then the generated keys), either may be
+    None; a step writes slot step + step_offset.  off / n_prompt: device int32 [R]; ws: attention_probs_decode_ws(R, n_heads, n_cols)."""
+
+    def __init__(self, off: torch.Tensor, n_prompt: torch.Tensor, T: int, hidden: Optional[torch.Tensor] = None, attn: Optional[torch.Tensor] = None,
+                 step_offset: int = -1):
+        if hidden is None and attn is None:
+            raise SrgptError("StepProbe: nothing to record (hidden and attn are both None)")
+        for t, what in ((hidden, "hidden"), (attn, "attn")):
+            if t is not None and (t.stride(-1) != 1 or t.dtype != ELEM()):
+                raise SrgptError(f"StepProbe.{what} must be element-type with unit inner stride")
+        self.off, self.n_prompt, self.T, self.hidden, self.attn, self.step_offset = off, n_prompt, int(T), hidden, attn, int(step_offset)
+        self.ws = None if attn is None else attention_probs_decode_ws(attn.shape[2], attn.shape[3], attn.shape[4], attn.device)
+
+    def kernels(self, n_layers: int, final_norm: bool) -> int:
+        """Launches the probes add to a step of n_layers layers (the one-row step computes the final norm row itself)."""
+        return n_layers * ((self.hidden is not None) + 2 * (self.attn is not None)) + (self.hidden is not None) * (2 if final_norm else 1)
+
+    def key(self) -> tuple:
+        """GraphKey.probe: the addresses and strides a captured graph holds."""
+        return tuple((t.data_ptr(), tuple(t.shape), t.stride()) if t is not None else None
+                     for t in (self.hidden, self.attn, self.off, self.n_prompt, self.ws)) + (self.T, self.step_offset)
+
+    def desc(self, n_layers: int, n_heads: int):
+        """The srgpt_decode_probe of a one-row step."""
+        d = _lib.DecodeProbe()
+        if self.hidden is not None:
+            if self.hidden.dim() != 4 or self.hidden.shape[1] != n_layers + 1 or self.hidden.shape[2] != 1:
+                raise SrgptError(f"StepProbe.hidden must be [steps, {n_layers + 1}, 1, H], got {tuple(self.hidden.shape)}")
+            d.hidden, d.hidden_step_stride, d.hidden_layer_stride, d.hidden_row_stride = self.hidden.data_ptr(), *self.hidden.stride()[:3]
+        if self.attn is not None:
+            _check_decode_probs_out(self.attn[:, 0], 1, n_heads, self.T, "StepProbe.attn")
+            if self.attn.shape[1] != n_layers:
+                raise SrgptError(f"StepProbe.attn must hold {n_layers} layers, got {tuple(self.attn.shape)}")
+            a = self.attn.stride()
+            d.attn, d.attn_step_stride, d.attn_layer_stride, d.attn_row_stride, d.attn_head_stride = self.attn.data_ptr(), a[0], a[1], a[2], a[3]
+            d.n_cols = self.attn.shape[4]
+        d.step_offset, d.T, d.off, d.n_prompt, d.ws = self.step_offset, self.T, _p(self.off), _p(self.n_prompt), _p(self.ws)
+        return d
+
+
 def llama_prefill_chunk_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, sin, start_pos, page_tables, page_size: int, n_pages: int,
                                cu_seqlens: torch.Tensor, max_rows: int) -> torch.Tensor:
     """All decoder layers over x [S, H] in place: n_seqs chunks packed by cu_seqlens [n_seqs+1] that continue their sequences at
@@ -1410,9 +1508,22 @@ def llama_prefill_chunk_layers(x: torch.Tensor, stack: LlamaStack, dims, cos, si
 
 
 def llama_decode_step(h, stack: LlamaStack, q_buf, attn_buf, act_buf, dims, cos, sin, pos, page_table, page_size: int,
-                      final_norm, lm_head, embed, lm_ws, out_ids, step, logits_out=None) -> None:
-    """One whole decode step (5 kernels per layer, lm_head + arg max) streaming the stack's decode weights."""
+                      final_norm, lm_head, embed, lm_ws, out_ids, step, logits_out=None, probe: Optional["StepProbe"] = None) -> None:
+    """One whole decode step (5 kernels per layer, lm_head + arg max) streaming the stack's decode weights.  ``probe`` (a StepProbe of
+    one row): the step also records its hidden rows and attention probabilities (srgpt_llama_decode_step_probe_bf16); every other
+    output is bit-identical."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
+    if probe is not None:
+        fmt, arrays, lm = stack.formats("decode_step")
+        by = dict(zip({"": ("layers",), "fp8": ("fp8",)}.get(fmt, ("layers", fmt)), arrays))
+        desc = probe.desc(stack.n, nh)
+        check(_lib.load().srgpt_llama_decode_step_probe_bf16(
+            _p(h), by.get("layers"), by.get("packed"), by.get("nf4"), by.get("fp8"), stack.n, _p(q_buf), _p(attn_buf), _p(act_buf),
+            dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm),
+            _p(lm_head), lm[0] if lm else None, dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_out), _p(out_ids), _p(step), C.byref(desc),
+            _stream()), "srgpt_llama_decode_step_probe_bf16")
+        _count(stack.step_kernels + probe.kernels(stack.n, final_norm=True))
+        return
     name, arrays, lm = stack.entry("decode_step")
     check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), dims.hidden_size, nh, nkv, hd, I,
                                      dims.rms_norm_eps, _p(cos), _p(sin), _p(pos), _p(page_table), page_size, _p(final_norm), _p(lm_head), *lm,

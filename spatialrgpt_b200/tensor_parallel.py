@@ -71,6 +71,7 @@ class TPLlamaDecoder(LlamaDecoder):
     supports_batch_invariant = False  # the rows step (generate_rows) is a single-GPU kernel sequence
     supports_contrastive = False  # contrastive search runs the batched step and its choice on one GPU
     supports_forward_outputs = False  # forward()'s attentions need every head, and no rank holds them all
+    supports_generate_outputs = False  # generate()'s attentions likewise
 
     def score_candidates(self, *args, **kwargs):
         raise NotImplementedError("likelihood scoring (score()) on the tensor-parallel decoder")
