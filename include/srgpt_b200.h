@@ -357,6 +357,21 @@ int srgpt_sample_top_p_scores_f32(const float* logits, int V, const float* param
                                   long long step_stride, void* stream);
 int srgpt_sample_rows_scores(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
                              const int* step, int step_offset, long long* ids, float* scores, long long step_stride, void* stream);
+/* The four entry points above with HF's TypicalLogitsWarper, EpsilonLogitsWarper and EtaLogitsWarper after top-p, in HF's order, each on
+ * the set the earlier cuts kept (sampling.cu): params = device float[6] {temperature, top_p, top_k (0 = off), typical_p, epsilon_cutoff,
+ * eta_cutoff}.  Typical acts when typical_p < 1, epsilon when 0 < epsilon_cutoff < 1, eta when 0 < eta_cutoff < 1; epsilon and eta keep
+ * the tokens tied at the largest logit of what typical kept.  The draw uses the same counter stream, over the final kept set, and the
+ * warped row is -inf outside it.  With all three off, ids and rows equal those of the float[3] entry points. */
+int srgpt_sample_warped_f32(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step, int step_offset,
+                            long long* out_ids, const void* embed_table, void* next_x, int K, void* stream);
+int srgpt_sample_warped_scores_f32(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step,
+                                   int step_offset, long long* out_ids, const void* embed_table, void* next_x, int K, float* scores,
+                                   long long step_stride, void* stream);
+int srgpt_sample_rows_warped(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
+                             const int* step, int step_offset, long long* ids, void* stream);
+int srgpt_sample_rows_warped_scores(const void* logits, int logits_f32, int ld, int R, int V, const float* params,
+                                    const unsigned long long* seeds, const int* step, int step_offset, long long* ids, float* scores,
+                                    long long step_stride, void* stream);
 /* HF's logits processors on the device (logits_process.cu): replaces RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor,
  * NoBadWordsLogitsProcessor, MinLengthLogitsProcessor and MinNewTokensLengthLogitsProcessor (transformers generation/logits_process.py),
  * which HF runs on the host behind generate(repetition_penalty=, no_repeat_ngram_size=, bad_words_ids=, min_length=, min_new_tokens=)
@@ -749,6 +764,16 @@ int srgpt_llama_decode_rows_guided_bf16(void* h, const srgpt_llama_layer_weights
                                         int* pos_rows, const int* page_tables, int pt_stride, int page_size, const void* final_norm,
                                         const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
                                         float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids,
+                                        long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream);
+/* The sampled rows step, plain (guidance == NULL) or guided, drawing with srgpt_sample_rows_warped: warp_params = device float[6] as
+ * there, seeds needed.  Arguments otherwise as srgpt_llama_decode_rows_guided_bf16; the same kernels, the warped sampler in place of
+ * srgpt_sample_rows. */
+int srgpt_llama_decode_rows_warped_bf16(void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed,
+                                        const srgpt_llama_layer_nf4* nf4, int n_layers, void* q_buf, void* attn_buf, void* act_buf, int B, int H,
+                                        int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab, const void* sin_tab,
+                                        int* pos_rows, const int* page_tables, int pt_stride, int page_size, const void* final_norm,
+                                        const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
+                                        float* logits_rows, const float* warp_params, const unsigned long long* seeds, long long* ids,
                                         long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream);
 
 /* ---- contrastive search (contrastive.cu, beam.cu): replaces _ranking_fast and the candidate bookkeeping of HF

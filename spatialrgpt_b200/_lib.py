@@ -70,6 +70,10 @@ SIGNATURES = {
     "srgpt_sample_rows": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, ci, vp, vp]),
     "srgpt_sample_top_p_scores_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp, cll, vp]),
     "srgpt_sample_rows_scores": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, ci, vp, vp, cll, vp]),
+    "srgpt_sample_warped_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp]),
+    "srgpt_sample_rows_warped": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, ci, vp, vp]),
+    "srgpt_sample_warped_scores_f32": (ci, [vp, ci, vp, vp, vp, ci, vp, vp, vp, ci, vp, cll, vp]),
+    "srgpt_sample_rows_warped_scores": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, ci, vp, vp, cll, vp]),
     "srgpt_logits_process": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, ci, vp, ci, vp, vp, ci, vp, ci, vp, vp]),
     "srgpt_logits_pick_token": (ci, [vp, vp, ci, vp, vp, vp, ci, vp]),
     "srgpt_resample_u8": (ci, [vp, vp, ci, ci, ci, ci, ci, vp, vp, ci, vp]),
@@ -150,6 +154,8 @@ SIGNATURES = {
     "srgpt_guidance_rows": (ci, [vp, ci, ci, vp, vp, vp, vp, vp]),
     "srgpt_guidance_pair_ids": (ci, [vp, ci, vp]),
     "srgpt_llama_decode_rows_guided_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp,
+                                                 ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "srgpt_llama_decode_rows_warped_bf16": (ci, [vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, vp, vp, vp, vp, ci, ci, vp, vp, vp,
                                                  ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_contrastive_partial_floats": (cll, [ci, ci, ci]),
     "srgpt_contrastive_penalty_bf16": (ci, [vp, ci, vp, ci, ci, vp, ci, ci, vp, vp]),

@@ -446,7 +446,9 @@ static int decode_rows(void* h, const srgpt_llama_layer_weights* layers, const s
                        const void* cos_tab, const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size,
                        const void* final_norm, const void* lm_head, const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace,
                        float* logits_rows, const float* sample_params, const unsigned long long* seeds, long long* ids, long long* out_ids, int* step,
-                       const srgpt_guidance* guidance, void* stream) {
+                       const srgpt_guidance* guidance, void* stream, bool warped = false) {
+  // warped: sample_params is the float[6] of srgpt_sample_rows_warped (typical / epsilon / eta after top-p)
+  auto sample_rows = warped ? srgpt_sample_rows_warped : srgpt_sample_rows;
   SRGPT_CHECK_ARG(B >= 1 && B <= SRGPT_SPEC_T_MAX && pt_stride > 0);
   SRGPT_CHECK_ARG(guidance == nullptr || ((B % 2) == 0 && guidance->scale && guidance->guided_rows && ids && logits_rows));
   SRGPT_CHECK_ARG(h && layers && q_buf && attn_buf && act_buf && pos_rows && page_tables && final_norm && lm_head && embed_table && lm_workspace &&
@@ -459,12 +461,12 @@ static int decode_rows(void* h, const srgpt_llama_layer_weights* layers, const s
     const int P = B / 2;
     SRGPT_TRY(srgpt_guidance_rows(logits_rows, V, P, guidance->scale, guidance->guided_rows, nullptr, seeds == nullptr ? ids : nullptr, stream));
     if (seeds != nullptr) {
-      SRGPT_TRY(srgpt_sample_rows(guidance->guided_rows, 1, V, P, V, sample_params, seeds, step, 0, ids, stream));
+      SRGPT_TRY(sample_rows(guidance->guided_rows, 1, V, P, V, sample_params, seeds, step, 0, ids, stream));
       SRGPT_TRY(srgpt_guidance_pair_ids(ids, P, stream));
     }
     return srgpt_rows_advance(lm_workspace, V, ids, B, embed_table, h, H, out_ids, step, pos_rows, stream);
   }
-  if (seeds != nullptr) SRGPT_TRY(srgpt_sample_rows(logits_rows, 1, V, B, V, sample_params, seeds, step, 0, ids, stream));
+  if (seeds != nullptr) SRGPT_TRY(sample_rows(logits_rows, 1, V, B, V, sample_params, seeds, step, 0, ids, stream));
   return srgpt_rows_advance(lm_workspace, V, seeds != nullptr ? ids : nullptr, B, embed_table, h, H, out_ids, step, pos_rows, stream);
 }
 
@@ -514,4 +516,21 @@ extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_gu
   return decode_rows(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
                      pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
                      sample_params, seeds, ids, out_ids, step, guidance, stream);
+}
+
+// The sampled rows step, plain or guided (guidance may be NULL), drawing with srgpt_sample_rows_warped: warp_params = device float[6]
+// {temperature, top_p, top_k, typical_p, epsilon_cutoff, eta_cutoff}.  One entry point for every weight format of the step, as the
+// guided one; the same kernels as the sampled step of srgpt_llama_decode_rows_bf16 / _guided_bf16 with the warped sampler in place of
+// srgpt_sample_rows.
+extern "C" __attribute__((visibility("default"))) int srgpt_llama_decode_rows_warped_bf16(
+    void* h, const srgpt_llama_layer_weights* layers, const srgpt_llama_layer_packed* packed, const srgpt_llama_layer_nf4* nf4, int n_layers,
+    void* q_buf, void* attn_buf, void* act_buf, int B, int H, int n_heads, int n_kv_heads, int head_dim, int I, float eps, const void* cos_tab,
+    const void* sin_tab, int* pos_rows, const int* page_tables, int pt_stride, int page_size, const void* final_norm, const void* lm_head,
+    const srgpt_packed12* lm_packed, int V, const void* embed_table, void* lm_workspace, float* logits_rows, const float* warp_params,
+    const unsigned long long* seeds, long long* ids, long long* out_ids, int* step, const srgpt_guidance* guidance, void* stream) {
+  SRGPT_CHECK_ARG(packed == nullptr || nf4 == nullptr);
+  SRGPT_CHECK_ARG(warp_params != nullptr && seeds != nullptr);
+  return decode_rows(h, layers, packed, nf4, n_layers, q_buf, attn_buf, act_buf, B, H, n_heads, n_kv_heads, head_dim, I, eps, cos_tab, sin_tab,
+                     pos_rows, page_tables, pt_stride, page_size, final_norm, lm_head, lm_packed, V, embed_table, lm_workspace, logits_rows,
+                     warp_params, seeds, ids, out_ids, step, guidance, stream, true);
 }

@@ -13,6 +13,8 @@
 // the frequencies against the torch nucleus).  Greedy decoding (the graded mode) never runs this kernel.
 // A batch of sequences draws in one launch of sample_rows_kernel: one such CTA per row, the same arithmetic (sample_row) over fp32 rows or
 // the element-type rows of the batched lm_head, each row with its own seed.
+// The *_warped kernels add HF's TypicalLogitsWarper, EpsilonLogitsWarper and EtaLogitsWarper (transformers 5.5, same in 4.37.2) after
+// top-p, in HF's order, as sample_row<T, true>; sample_row<T, false> is the original arithmetic, which the original kernels keep.
 #include "common.cuh"
 #include "srgpt_b200.h"
 
@@ -50,9 +52,19 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
 __device__ __forceinline__ float logit(const float* __restrict__ x, int i) { return x[i]; }
 __device__ __forceinline__ float logit(const bf16* __restrict__ x, int i) { return e2f(x[i]); }  // exact: torch's .float() of the row
 
+// Whether the token of logit x and probability p is in the set the draw picks from: p >= t_keep (top-k and top-p), and with CUTS
+// the typical / epsilon / eta cuts of sample_row, whose state s_cut = {c, d*, top logit of K1, p cut} it computes.
+template <bool CUTS>
+__device__ __forceinline__ bool kept(float x, float p, float m, float inv_t, float t_keep, const float* s_cut) {
+  if constexpr (CUTS) return p >= t_keep && fabsf(s_cut[0] - (x - m) * inv_t) <= s_cut[1] && (x >= s_cut[2] || p >= s_cut[3]);
+  else return p >= t_keep;
+}
+
 // The draw of one row of V logits (fp32 or the element type) by the whole 1024-thread CTA; every thread returns the token.
 // params = {temperature, top_p, top_k (0 = off)} and the seed live in device memory, so one captured CUDA graph serves any request.
-template <typename T>
+// CUTS: params = {temperature, top_p, top_k, typical_p, epsilon, eta}; a warper acts where HF turns it on (typical_p < 1,
+// 0 < epsilon < 1, 0 < eta < 1) on the set the earlier cuts kept, and the draw and the warped row use the final set.
+template <typename T, bool CUTS = false>
 __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, const float* __restrict__ params,
                                           const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step, int step_offset,
                                           float* __restrict__ warped) {
@@ -116,13 +128,90 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
     mass = mass_lo;
   }
 
-  // the warped row (HF's output_scores of a sampled step): logits / T for the tokens the draw can pick (p >= t_keep, the set the top-k
-  // cut and the nucleus bisection kept), -inf for every other token.  A true fp32 division, as TemperatureLogitsWarper divides.
+  // Typical, epsilon and eta cuts (CUTS) over the kept set K0 = {p >= t_keep}, each on what the previous one left.  With s = the scaled
+  // logit (x - m) / T and q = p / mass(K0), -log q - H = E_q[s] - s, so typical's deviation is |c - s| with c = E_q[s]; the kept set is
+  // {|c - s| <= d*}, d* the smallest deviation whose set reaches typical_p of the mass (HF keeps every token up to the deviation at
+  // which the sorted cumulative mass first reaches typical_p, ties included), found by bisection on d.  Epsilon keeps
+  // p >= epsilon * mass(K1); eta keeps p >= min(eta, sqrt(eta) * exp(-H2)) * mass(K2), H2 the entropy of K2; both keep the tokens
+  // tied at the largest logit of K1 (HF's min_tokens_to_keep = 1).  All cuts together: kept<true>.
+  __shared__ float s_cut[4];  // c, d*, the top logit of K1 and the p cut, read by kept() (the kernel has no registers to spare)
+  if constexpr (CUTS) {  // the loops unroll by 8: the factor at which the three kernels fit 64 registers without local memory
+    float c_typ = 0.f, d_keep = INFINITY, x_top = -INFINITY, cut = 0.f;
+    const float typical_p = params[3], eps = params[4], eta = params[5];
+    const bool typ_on = typical_p < 1.0f, eps_on = eps > 0.f && eps < 1.0f, eta_on = eta > 0.f && eta < 1.0f;
+    if (typ_on) {
+      float a = 0.f, b = 0.f;
+      #pragma unroll 8
+      for (int i = lo; i < hi; ++i) {
+        const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
+        if (p >= t_keep && p > 0.f) { a += p; b += p * s; }
+      }
+      const float a0 = block_reduce_sum(a, red);
+      c_typ = block_reduce_sum(b, red) / a0;
+      float dm = 0.f;
+      #pragma unroll 8
+      for (int i = lo; i < hi; ++i) {
+        const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
+        if (p >= t_keep && p > 0.f) dm = fmaxf(dm, fabsf(c_typ - s));
+      }
+      float lo_d = 0.f, hi_d = block_reduce_max(dm, red);  // invariant: mass{|c - s| <= hi_d} >= typical_p * a0
+      const float target = typical_p * a0;
+      for (int it = 0; it < 26; ++it) {
+        const float mid = 0.5f * (lo_d + hi_d);
+        float sm = 0.f;
+        #pragma unroll 8
+        for (int i = lo; i < hi; ++i) {
+          const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
+          sm += (p >= t_keep && p > 0.f && fabsf(c_typ - s) <= mid) ? p : 0.f;
+        }
+        sm = block_reduce_sum(sm, red);
+        if (sm >= target) hi_d = mid; else lo_d = mid;
+      }
+      d_keep = hi_d;
+    }
+    if (eps_on || eta_on) {
+      float a = 0.f, xm = -INFINITY;
+      #pragma unroll 8
+      for (int i = lo; i < hi; ++i) {
+        const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+        if (p >= t_keep && fabsf(c_typ - s) <= d_keep) { a += p; xm = fmaxf(xm, x); }
+      }
+      const float a1 = block_reduce_sum(a, red);
+      x_top = block_reduce_max(xm, red);
+      if (eps_on) cut = eps * a1;
+      if (eta_on) {
+        float a2 = 0.f, b2 = 0.f;
+        #pragma unroll 8
+        for (int i = lo; i < hi; ++i) {
+          const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+          if (p >= t_keep && p > 0.f && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) { a2 += p; b2 += p * s; }
+        }
+        a2 = block_reduce_sum(a2, red);
+        b2 = block_reduce_sum(b2, red);
+        const float h2 = __logf(a2 / inv_z) - b2 / a2;  // entropy of K2: E_q[-log q], -log q = log(z * mass) - s
+        cut = fmaxf(cut, fminf(eta, sqrtf(eta) * __expf(-h2)) * a2);
+      }
+    }
+    if (typ_on || eps_on || eta_on) {
+      float sm = 0.f;
+      #pragma unroll 8
+      for (int i = lo; i < hi; ++i) {
+        const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+        sm += (p >= t_keep && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) ? p : 0.f;
+      }
+      mass = block_reduce_sum(sm, red);
+    }
+    if (tid == 0) { s_cut[0] = c_typ; s_cut[1] = d_keep; s_cut[2] = x_top; s_cut[3] = cut; }
+    __syncthreads();
+  }
+
+  // the warped row (HF's output_scores of a sampled step): logits / T for the tokens the draw can pick (the set the top-k cut, the
+  // nucleus bisection and the CUTS kept), -inf for every other token.  A true fp32 division, as TemperatureLogitsWarper divides.
   if (warped != nullptr) {
     const float t = params[0];
     for (int i = tid; i < V; i += THREADS) {
       const float x = logit(logits, i);
-      warped[i] = __expf((x - m) * inv_t) * inv_z >= t_keep ? __fdiv_rn(x, t) : -INFINITY;
+      warped[i] = kept<CUTS>(x, __expf((x - m) * inv_t) * inv_z, m, inv_t, t_keep, s_cut) ? __fdiv_rn(x, t) : -INFINITY;
     }
   }
 
@@ -132,8 +221,8 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   const float u = ((float)(r >> 40) + 0.5f) * (1.0f / 16777216.0f) * mass;  // (0, mass)
   float local = 0.f;
   for (int i = lo; i < hi; ++i) {
-    const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
-    local += (p >= t_keep) ? p : 0.f;
+    const float x = logit(logits, i), p = __expf((x - m) * inv_t) * inv_z;
+    local += kept<CUTS>(x, p, m, inv_t, t_keep, s_cut) ? p : 0.f;
   }
   s_scan[tid] = local;
   __syncthreads();
@@ -153,8 +242,8 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
     float acc = before;
     int pick = -1, last_kept = -1;
     for (int i = lo; i < hi; ++i) {
-      const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
-      if (p >= t_keep) {
+      const float x = logit(logits, i), p = __expf((x - m) * inv_t) * inv_z;
+      if (kept<CUTS>(x, p, m, inv_t, t_keep, s_cut)) {
         last_kept = i;
         acc += p;
         if (acc > uu) { pick = i; break; }
@@ -209,6 +298,30 @@ sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const floa
   if (threadIdx.x == 0) ids[r] = (long long)tok;
 }
 
+// sample_top_p_kernel and sample_rows_kernel with the typical / epsilon / eta cuts (params float[6]).
+__global__ void __launch_bounds__(THREADS)
+sample_top_p_warped_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr,
+                           const int* __restrict__ step, int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table,
+                           bf16* __restrict__ next_x, int K, float* __restrict__ scores, long long step_stride) {
+  float* warped = scores != nullptr ? scores + (long long)(*step + step_offset) * step_stride : nullptr;
+  const int tok = sample_row<float, true>(logits, V, params, seed_ptr, step, step_offset, warped);
+  if (threadIdx.x == 0) out_ids[*step + step_offset] = (long long)tok;
+  if (embed_table != nullptr && next_x != nullptr) {
+    const uint4* src = reinterpret_cast<const uint4*>(embed_table + (size_t)tok * K);
+    for (int c = threadIdx.x; c < (K >> 3); c += THREADS) reinterpret_cast<uint4*>(next_x)[c] = src[c];
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS)
+sample_rows_warped_kernel(const T* __restrict__ logits, long long ld, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seeds,
+                          const int* __restrict__ step, int step_offset, long long* __restrict__ ids, float* __restrict__ scores, long long step_stride) {
+  const int r = blockIdx.x;
+  float* warped = scores != nullptr ? scores + (long long)(*step + step_offset) * step_stride + (long long)r * V : nullptr;
+  const int tok = sample_row<T, true>(logits + (size_t)r * ld, V, params, seeds + r, step, step_offset, warped);
+  if (threadIdx.x == 0) ids[r] = (long long)tok;
+}
+
 }  // namespace sampling
 }  // namespace srgpt
 
@@ -216,13 +329,14 @@ using namespace srgpt;
 
 namespace {
 int launch_sample_top_p(const float* logits, int V, const float* params, const unsigned long long* seed, const int* step, int step_offset,
-                        long long* out_ids, const void* embed_table, void* next_x, int K, float* scores, long long step_stride, void* stream) {
+                        long long* out_ids, const void* embed_table, void* next_x, int K, float* scores, long long step_stride, void* stream,
+                        bool cuts = false) {
   SRGPT_CHECK_ARG(logits && params && seed && step && out_ids && V > 0);
   SRGPT_CHECK_ARG((embed_table == nullptr) == (next_x == nullptr));
   SRGPT_CHECK_ARG(embed_table == nullptr || ((K % 8) == 0 && K > 0 && (reinterpret_cast<uintptr_t>(embed_table) & 15) == 0 &&
                                              (reinterpret_cast<uintptr_t>(next_x) & 15) == 0));
   SRGPT_CHECK_ARG(scores == nullptr || step_stride >= V);
-  sampling::sample_top_p_kernel<<<1, sampling::THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  (cuts ? sampling::sample_top_p_warped_kernel : sampling::sample_top_p_kernel)<<<1, sampling::THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       logits, V, params, seed, step, step_offset, out_ids, reinterpret_cast<const bf16*>(embed_table), reinterpret_cast<bf16*>(next_x), K,
       scores, step_stride);
   SRGPT_CHECK_LAUNCH();
@@ -230,17 +344,17 @@ int launch_sample_top_p(const float* logits, int V, const float* params, const u
 }
 
 int launch_sample_rows(const void* logits, int logits_f32, int ld, int R, int V, const float* params, const unsigned long long* seeds,
-                       const int* step, int step_offset, long long* ids, float* scores, long long step_stride, void* stream) {
+                       const int* step, int step_offset, long long* ids, float* scores, long long step_stride, void* stream, bool cuts = false) {
   SRGPT_CHECK_ARG(logits && params && seeds && step && ids && R > 0 && R <= 65535 && V > 0 && ld >= V);
   SRGPT_CHECK_ARG(logits_f32 == 0 || logits_f32 == 1);
   SRGPT_CHECK_ARG(scores == nullptr || step_stride >= (long long)R * V);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (logits_f32)
-    sampling::sample_rows_kernel<float><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const float*>(logits), ld, V, params, seeds, step,
-                                                                         step_offset, ids, scores, step_stride);
+    (cuts ? sampling::sample_rows_warped_kernel<float> : sampling::sample_rows_kernel<float>)<<<R, sampling::THREADS, 0, st>>>(
+        reinterpret_cast<const float*>(logits), ld, V, params, seeds, step, step_offset, ids, scores, step_stride);
   else
-    sampling::sample_rows_kernel<bf16><<<R, sampling::THREADS, 0, st>>>(reinterpret_cast<const bf16*>(logits), ld, V, params, seeds, step,
-                                                                        step_offset, ids, scores, step_stride);
+    (cuts ? sampling::sample_rows_warped_kernel<bf16> : sampling::sample_rows_kernel<bf16>)<<<R, sampling::THREADS, 0, st>>>(
+        reinterpret_cast<const bf16*>(logits), ld, V, params, seeds, step, step_offset, ids, scores, step_stride);
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }
@@ -280,4 +394,35 @@ extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows_scores(c
                                                                                void* stream) {
   SRGPT_CHECK_ARG(scores != nullptr);
   return launch_sample_rows(logits, logits_f32, ld, R, V, params, seeds, step, step_offset, ids, scores, step_stride, stream);
+}
+
+// The same four entry points with HF's typical, epsilon and eta warpers after top-p: `params` = device float[6] {temperature, top_p,
+// top_k (0 = off), typical_p (>= 1 = off), epsilon_cutoff, eta_cutoff (each off outside (0, 1))}.  With all three off the draw and the
+// warped row are those of the float[3] entry points.
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_warped_f32(const float* logits, int V, const float* params, const unsigned long long* seed,
+                                                                              const int* step, int step_offset, long long* out_ids,
+                                                                              const void* embed_table, void* next_x, int K, void* stream) {
+  return launch_sample_top_p(logits, V, params, seed, step, step_offset, out_ids, embed_table, next_x, K, nullptr, 0, stream, true);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_warped_scores_f32(const float* logits, int V, const float* params,
+                                                                                     const unsigned long long* seed, const int* step, int step_offset,
+                                                                                     long long* out_ids, const void* embed_table, void* next_x, int K,
+                                                                                     float* scores, long long step_stride, void* stream) {
+  SRGPT_CHECK_ARG(scores != nullptr);
+  return launch_sample_top_p(logits, V, params, seed, step, step_offset, out_ids, embed_table, next_x, K, scores, step_stride, stream, true);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows_warped(const void* logits, int logits_f32, int ld, int R, int V,
+                                                                               const float* params, const unsigned long long* seeds, const int* step,
+                                                                               int step_offset, long long* ids, void* stream) {
+  return launch_sample_rows(logits, logits_f32, ld, R, V, params, seeds, step, step_offset, ids, nullptr, 0, stream, true);
+}
+
+extern "C" __attribute__((visibility("default"))) int srgpt_sample_rows_warped_scores(const void* logits, int logits_f32, int ld, int R, int V,
+                                                                                      const float* params, const unsigned long long* seeds,
+                                                                                      const int* step, int step_offset, long long* ids, float* scores,
+                                                                                      long long step_stride, void* stream) {
+  SRGPT_CHECK_ARG(scores != nullptr);
+  return launch_sample_rows(logits, logits_f32, ld, R, V, params, seeds, step, step_offset, ids, scores, step_stride, stream, true);
 }

@@ -86,8 +86,9 @@ def decode_steps(launch, fetch, host, budgets: List[int], eos, stopping_fn) -> L
 class GraphKey(NamedTuple):
     """What a captured graph computes: its kind ("step", "batch", "rows", "beam", "verify" or "contrastive"), its rows (T for a verify
     pass), whether it samples, whether the logits processors run, the (address, step stride) of the score rows it writes (output_scores),
-    the n-gram size of a verify pass, the candidates per prompt of a contrastive step (B * k rows), and the addresses and layout of the
-    hidden states / attentions it records (ops.StepProbe.key; generate(output_hidden_states=, output_attentions=))."""
+    the n-gram size of a verify pass, the candidates per prompt of a contrastive step (B * k rows), the addresses and layout of the
+    hidden states / attentions it records (ops.StepProbe.key; generate(output_hidden_states=, output_attentions=)), and whether its draw
+    runs the typical / epsilon / eta warpers (the warped sampler over LlamaDecoder.warp_params)."""
     kind: str
     rows: int = 1
     sample: bool = False
@@ -96,6 +97,20 @@ class GraphKey(NamedTuple):
     ngram: int = 0
     group: int = 0
     probe: Optional[tuple] = None
+    warp: bool = False
+
+
+def sampling_warpers(sampling) -> tuple:
+    """(typical_p, epsilon_cutoff, eta_cutoff) of a sampling dict, each at its neutral value (1, 0, 0) when absent or when HF leaves the
+    warper off: typical_p >= 1, a cutoff outside (0, 1) (transformers 5.5 _get_logits_processor; NaN included).  Raises ValueError where
+    HF's TypicalLogitsWarper does: typical_p <= 0."""
+    typ, eps, eta = (sampling.get(k) for k in ("typical_p", "epsilon_cutoff", "eta_cutoff"))
+    typ = 1.0 if typ is None else float(typ)
+    eps = 0.0 if eps is None else float(eps)
+    eta = 0.0 if eta is None else float(eta)
+    if typ < 1.0 and not typ > 0.0:
+        raise ValueError(f"`typical_p` has to be a float > 0 and < 1, but is {typ}")
+    return (typ if typ < 1.0 else 1.0, eps if 0.0 < eps < 1.0 else 0.0, eta if 0.0 < eta < 1.0 else 0.0)
 
 
 class BeamHypotheses:
@@ -406,6 +421,10 @@ class LlamaDecoder:
         self._graphs = {}
         # sampling mode (do_sample=True): temperature / top_p live in device memory so one captured graph serves any setting
         self.sample_params = torch.tensor([1.0, 1.0, 0.0], dtype=torch.float32, device=dev)
+        # with typical_p / epsilon_cutoff / eta_cutoff on, the draws read these 6 floats {T, top_p, top_k, typical_p, epsilon, eta}
+        # instead (the warped sampler, its own graphs: GraphKey.warp); with all three off they run exactly as before
+        self.warp_params = torch.tensor([1.0, 1.0, 0.0, 1.0, 0.0, 0.0], dtype=torch.float32, device=dev)
+        self.warp = False
         self.sample_logits: Optional[torch.Tensor] = None
         self.sample_seed = 0
         self.sample_seed_dev = torch.zeros(1, dtype=torch.int64, device=dev)  # device copy: the captured graph reads the seed at run time
@@ -640,7 +659,7 @@ class LlamaDecoder:
         if proc:
             self._process_row(raw, sample, scores)
         elif sample:  # replaces the greedy id / next embedding row the finalize kernel just wrote (step already advanced)
-            ops.sample_top_p(raw, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, self.w.embed, self.h,
+            ops.sample_top_p(raw, self._draw_params, self.sample_seed_dev, self.step, -1, self.out_ids, self.w.embed, self.h,
                              **self._scores_kw(scores, True))
         elif scores is not None:
             ops.step_scores(raw, self.step, -1, scores)
@@ -653,7 +672,7 @@ class LlamaDecoder:
             self.proc_logits = torch.empty(self.dims.vocab_size, dtype=torch.float32, device=self.device)
         if sample:
             ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, out=self.proc_logits)
-            ops.sample_top_p(self.proc_logits, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
+            ops.sample_top_p(self.proc_logits, self._draw_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
                              **self._scores_kw(scores, True))
         else:
             ops.logits_process(raw, self.out_ids, 0, 1, self.step, -1, self.proc_fparams, self.proc_spec, ids=self.proc_ids,
@@ -752,7 +771,8 @@ class LlamaDecoder:
         (processing, key unpack and pick); greedy score rows add their copy (the sampler writes its own); a probe its launches."""
         kernels = self.kernels_per_decode_step + (1 if sample else 0) + ((1 if sample else 3) if proc else 0) + (
             1 if scores is not None and not sample else 0) + (0 if probe is None else probe.kernels(self.dims.num_hidden_layers, final_norm=True))
-        return self._capture(GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key()),
+        return self._capture(GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key(),
+                                      warp=sample and self.warp),
                              lambda: self._decode_step_launch(seq, sample=sample, proc=proc, **self._scores_kw(scores),
                                                               **({} if probe is None else dict(probe=probe))),
                              (self.pos, self.step, self.h, self.out_ids), kernels)
@@ -826,7 +846,9 @@ class LlamaDecoder:
         return hidden
 
     def _set_sampling(self, sampling) -> bool:
-        """sampling = None (greedy) or dict(temperature=, top_p=, top_k=, seed=).  Returns True when tokens are sampled."""
+        """sampling = None (greedy) or dict(temperature=, top_p=, top_k=, seed=, and optionally typical_p=, epsilon_cutoff=, eta_cutoff=).
+        Returns True when tokens are sampled; self.warp tells whether a typical / epsilon / eta warper is on."""
+        self.warp = False
         if not sampling:
             return False
         t = float(sampling.get("temperature") or 1.0)
@@ -836,10 +858,19 @@ class LlamaDecoder:
         k = 50 if k is None else int(k)  # GenerationConfig's default top_k, applied by HF whenever do_sample=True
         if t <= 0.0 or not (0.0 < p <= 1.0) or k < 0:
             raise ValueError(f"sampling needs temperature > 0, 0 < top_p <= 1 and top_k >= 0, got temperature={t}, top_p={p}, top_k={k}")
+        warpers = sampling_warpers(sampling)
         self.sample_params.copy_(torch.tensor([t, p, float(k)], dtype=torch.float32))
+        self.warp = warpers != (1.0, 0.0, 0.0)
+        if self.warp:
+            self.warp_params.copy_(torch.tensor([t, p, float(k), *warpers], dtype=torch.float32))
         seed = sampling.get("seed")
         self._set_seed(int(torch.initial_seed() if seed is None else seed))
         return True
+
+    @property
+    def _draw_params(self) -> torch.Tensor:
+        """The params the draws read: warp_params (the warped sampler) when a warper is on, else sample_params."""
+        return self.warp_params if self.warp else self.sample_params
 
     def _set_seed(self, seed: int) -> None:
         self.sample_seed = seed & 0x7FFFFFFFFFFFFFFF
@@ -996,7 +1027,7 @@ class LlamaDecoder:
         flight only touched this sequence's own KV slot and the step counters, which the next request resets."""
         self.active_pt.copy_(self.cache.page_tables[seq])
         graph = use_graph and logits is None
-        key = GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key())
+        key = GraphKey("step", 1, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key(), warp=sample and self.warp)
         probe_kw = {} if probe is None else dict(probe=probe)
         if graph:
             self._ensure_graph(seq, sample, proc, scores, **probe_kw)
@@ -1072,7 +1103,7 @@ class LlamaDecoder:
         if sample:  # from the bf16 rows, or from the processed fp32 rows
             if proc:
                 ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, out=st["proc_rows"])
-            ops.sample_rows(st["proc_rows"] if proc else lg, self.sample_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
+            ops.sample_rows(st["proc_rows"] if proc else lg, self._draw_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
         elif proc:  # the processors over each sequence's bf16 row and its history st["out"][t * B + b], t < step; then the arg max
             ops.logits_process(lg, st["out"], 1, B, st["step"], 0, self.proc_fparams, self.proc_spec, ids=st["ids"],
                                **({} if scores is None else {"out": st["proc_rows"]}))
@@ -1099,7 +1130,7 @@ class LlamaDecoder:
         if sample:  # the first tokens in one launch, at counter 0
             st["seeds"].copy_(torch.tensor(seeds, dtype=torch.int64))
             st["step"].zero_()
-            ops.sample_rows(sample_from, self.sample_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
+            ops.sample_rows(sample_from, self._draw_params, st["seeds"], st["step"], 0, st["ids"], **self._scores_kw(scores))
             first = st["ids"]
         zero = torch.zeros(B, dtype=torch.int32, device=self.device)
         st["out"][:B].copy_(first)
@@ -1107,7 +1138,8 @@ class LlamaDecoder:
         st["pos"].copy_(torch.tensor(seq_lens, dtype=torch.int32))
         st["step"].fill_(1)
         # the graphs that write scores / probes hold the buffers' addresses
-        key = GraphKey("batch", B, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key())
+        key = GraphKey("batch", B, sample, proc, self._scores_key(scores), probe=None if probe is None else probe.key(),
+                       warp=sample and self.warp)
         probe_kw = {} if probe is None else dict(probe=probe)
         if use_graph:  # with processing on, the processing kernel + key unpack replace the arg max (sampling: processing + draw)
             L = self.dims.num_hidden_layers
@@ -1154,7 +1186,7 @@ class LlamaDecoder:
     def _rows_step_launch(self, B: int, sample: bool, guided: bool = False) -> None:
         """The rows step over B rows; ``guided``: B = 2P rows, row P + b the unconditional branch of row b (llama_decode_rows' guidance)."""
         d, w, st = self.dims, self.w, self._rstate
-        kw = dict(sample_params=self.sample_params, seeds=st["seeds"], ids=st["ids"]) if sample else {}
+        kw = dict(sample_params=self._draw_params, seeds=st["seeds"], ids=st["ids"]) if sample else {}
         if guided:
             kw.update(ids=st["ids"], guidance=(st["scale"], st["guided"]))
         ops.llama_decode_rows(st["h"][:B], self.stack, st["q"][:B], st["attn"][:B], st["act"][:B], B, d, self.cos, self.sin, st["pos"],
@@ -1213,7 +1245,7 @@ class LlamaDecoder:
             ids = st["ids"][:R]
             ops.guidance_rows(st["logits"][:R], st["scale"], st["guided"][:B], ids=None if sample else ids)
             if sample:
-                ops.sample_rows(st["guided"][:B], self.sample_params, st["seeds"][:B], st["step"], 0, st["ids"][:B])
+                ops.sample_rows(st["guided"][:B], self._draw_params, st["seeds"][:B], st["step"], 0, st["ids"][:B])
                 ops.guidance_pair_ids(ids, B)
             st["out"][:R].copy_(ids)
             st["h"][:R].copy_(ops.splice_rows(self.w.embed, None, None, None, torch.zeros(R, dtype=torch.int32, device=self.device),
@@ -1230,7 +1262,7 @@ class LlamaDecoder:
         st["step"].fill_(1)
         if sample and not guided:
             st["seeds"][:B].copy_(torch.tensor([int(s) & SEED_MASK for s in seeds], dtype=torch.int64))
-        key = GraphKey("guided" if guided else "rows", B, sample)
+        key = GraphKey("guided" if guided else "rows", B, sample, warp=sample and self.warp)
         graph = use_graph and logits is None
         if graph:
             self._capture(key, lambda: self._rows_step_launch(R, sample, guided), (st["h"], st["pos"], st["step"], st["out"]),
@@ -1617,7 +1649,7 @@ class LlamaDecoder:
             if sample:  # re-draw the first token of this sequence from its logits row (a different draw per sequence: the seed moves)
                 self._set_seed(seeds[b])
                 row = first_rows[b] if proc else lg[b].float().contiguous()
-                ops.sample_top_p(row, self.sample_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
+                ops.sample_top_p(row, self._draw_params, self.sample_seed_dev, self.step, -1, self.out_ids, w.embed, self.h,
                                  **self._scores_kw(col, True))
             r = self._decode_loop(b, max_new_tokens, eos, stopping_fn, use_graph, logits, sample, proc, col)
             if return_logits:

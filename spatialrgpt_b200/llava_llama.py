@@ -15,7 +15,7 @@ import torch
 from . import logits_processors, ops
 from .config import LlavaConfig
 from .constants import IGNORE_INDEX, IMAGE_TOKEN_INDEX
-from .llama_decoder import GenerateProbe, LlamaDecoder, PrefillProbe, check_candidates, sequence_seeds
+from .llama_decoder import GenerateProbe, LlamaDecoder, PrefillProbe, check_candidates, sampling_warpers, sequence_seeds
 from .multimodal_encoder import VisionTower
 from .multimodal_projector import MultimodalProjector
 from .region_extractor import RegionExtractor
@@ -758,9 +758,14 @@ class LlavaLlamaModel:
         lookup_ngram = int(generation_kwargs.pop("max_matching_ngram_size", 2) or 2)
         # do_sample=True -> HF's TemperatureLogitsWarper + TopPLogitsWarper + multinomial, here one kernel per token
         # (eval_spatial.py:231-236 passes do_sample = temperature > 0, so temperature 0 stays greedy)
+        # typical_p / epsilon_cutoff / eta_cutoff (HF's TypicalLogitsWarper, EpsilonLogitsWarper, EtaLogitsWarper after top-p, in that
+        # order): applied by the same kernel when sampling; greedy decoding ignores them, as HF does.  typical_p <= 0 raises as HF's
+        # warper does; typical_p >= 1 and cutoffs outside (0, 1) leave a warper off.
+        warpers = {k: generation_kwargs.pop(k, None) for k in ("typical_p", "epsilon_cutoff", "eta_cutoff")}
         sampling = None
         if do_sample and temperature not in (0, 0.0):
-            sampling = dict(temperature=1.0 if temperature is None else float(temperature), top_p=top_p, top_k=top_k, seed=seed)
+            sampling = dict(temperature=1.0 if temperature is None else float(temperature), top_p=top_p, top_k=top_k, seed=seed, **warpers)
+            sampling_warpers(sampling)  # the ValueError, before any device work
         # num_return_sequences=n (sampling): n answers per prompt, rows b * n .. b * n + n - 1 of the result (HF's repeat_interleave
         # order); each prompt is prefilled once and its n rows decode together in the batched sampled step
         n_ret = generation_kwargs.pop("num_return_sequences", None)

@@ -836,6 +836,8 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
     """One token from softmax(logits / T) restricted to its top-p nucleus -> out_ids[step + step_offset] (and next_x = embed row).
     ``params`` = device float32 [temperature, top_p, top_k (0 = off)]; ``step`` = device int32 [1]; ``seed`` = device int64 [1]
     (read by the kernel at run time - graph-capturable), or a Python int for one-off eager calls.
+    ``params`` of 6 floats [temperature, top_p, top_k, typical_p, epsilon_cutoff, eta_cutoff] adds HF's typical, epsilon and eta
+    warpers after top-p (srgpt_sample_warped_f32; off at typical_p >= 1 and cutoffs outside (0, 1)).
     ``scores`` (fp32, optional): the warped row the draw picked from (logits / T where kept, -inf elsewhere) goes to
     scores.view(-1)[(step + step_offset) * step_stride:][:V]."""
     if not isinstance(seed, torch.Tensor):
@@ -846,6 +848,8 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
     if logits.dim() != 1 or not logits.is_contiguous() or params.numel() < 3:
         raise SrgptError("sample_top_p: logits must be a contiguous fp32 vector [V] and params [temperature, top_p, top_k]")
     K = 0 if embed_table is None else embed_table.shape[1]
+    if params.numel() == 6:
+        return _sample_warped(logits, params, seed, step, step_offset, out_ids, embed_table, next_x, K, scores, step_stride)
     if scores is not None:
         _need(scores, torch.float32, "sample_top_p.scores")
         check(_lib.load().srgpt_sample_top_p_scores_f32(_p(logits), logits.numel(), _p(params), _p(seed), _p(step), step_offset, _p(out_ids),
@@ -856,11 +860,22 @@ def sample_top_p(logits: torch.Tensor, params: torch.Tensor, seed, step: torch.T
                                              _p(out_ids), _p(embed_table), _p(next_x), K, _stream()), "srgpt_sample_top_p_f32")
 
 
+def _sample_warped(logits, params, seed, step, step_offset: int, out_ids, embed_table, next_x, K: int, scores, step_stride: int) -> None:
+    if scores is not None:
+        _need(scores, torch.float32, "sample_top_p.scores")
+        check(_lib.load().srgpt_sample_warped_scores_f32(_p(logits), logits.numel(), _p(params), _p(seed), _p(step), step_offset, _p(out_ids),
+                                                         _p(embed_table), _p(next_x), K, _p(scores), int(step_stride), _stream()),
+              "srgpt_sample_warped_scores_f32")
+        return
+    check(_lib.load().srgpt_sample_warped_f32(_p(logits), logits.numel(), _p(params), _p(seed), _p(step), step_offset, _p(out_ids),
+                                              _p(embed_table), _p(next_x), K, _stream()), "srgpt_sample_warped_f32")
+
+
 def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor, step: torch.Tensor, step_offset: int,
                 ids: torch.Tensor, scores: Optional[torch.Tensor] = None) -> None:
     """One token per row of ``logits`` ([R, V] fp32 or the element type, unit inner stride, e.g. the batched lm_head's rows) in one
     launch -> ids int64 [R].  Row r draws with seeds[r] (device int64 [R]) at counter step + step_offset, the token sample_top_p draws
-    from that row in fp32 with that seed and counter.  ``params`` and ``step`` as for sample_top_p.
+    from that row in fp32 with that seed and counter.  ``params`` and ``step`` as for sample_top_p (6 params: srgpt_sample_rows_warped).
     ``scores`` (contiguous fp32 [T, R, V], optional): row r's warped row goes to scores[step + step_offset, r]."""
     _need(params, torch.float32, "sample_rows.params"); _need(seeds, torch.int64, "sample_rows.seeds")
     _need(step, torch.int32, "sample_rows.step"); _need(ids, torch.int64, "sample_rows.ids")
@@ -882,11 +897,12 @@ def sample_rows(logits: torch.Tensor, params: torch.Tensor, seeds: torch.Tensor,
         _need(scores, torch.float32, "sample_rows.scores")
         if scores.dim() != 3 or scores.shape[1:] != (R, V) or not scores.is_contiguous():
             raise SrgptError(f"sample_rows: scores must be contiguous fp32 [T, {R}, {V}], got shape {tuple(scores.shape)}")
-        check(_lib.load().srgpt_sample_rows_scores(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids),
-                                                   _p(scores), R * V, _stream()), "srgpt_sample_rows_scores")
+        name = "srgpt_sample_rows_warped_scores" if params.numel() == 6 else "srgpt_sample_rows_scores"
+        check(getattr(_lib.load(), name)(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids), _p(scores),
+                                         R * V, _stream()), name)
         return
-    check(_lib.load().srgpt_sample_rows(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids), _stream()),
-          "srgpt_sample_rows")
+    name = "srgpt_sample_rows_warped" if params.numel() == 6 else "srgpt_sample_rows"
+    check(getattr(_lib.load(), name)(_p(logits), int(f32), ld, R, V, _p(params), _p(seeds), _p(step), step_offset, _p(ids), _stream()), name)
 
 
 def step_scores(rows: torch.Tensor, step: torch.Tensor, step_offset: int, scores: torch.Tensor) -> None:
@@ -1714,21 +1730,24 @@ def llama_decode_rows(h, stack: LlamaStack, q_buf, attn_buf, act_buf, B: int, di
     [>= B, cap] row-major view; row b of h / pos_rows / page_tables is sequence b.
     ``guidance`` = (scale, guided): classifier-free guidance over B = 2P rows, row P + b the unconditional branch of row b
     (srgpt_llama_decode_rows_guided_bf16): both rows of a pair take the arg max of guided row b, or with ``seeds`` ([P]) the draw from
-    it.  scale is the device fp32 g, guided the fp32 [P, V] rows; ids [B] and logits_rows are needed."""
+    it.  scale is the device fp32 g, guided the fp32 [P, V] rows; ids [B] and logits_rows are needed.
+    ``sample_params`` of 6 floats (with ``seeds``): the draws run HF's typical / epsilon / eta warpers after top-p
+    (srgpt_llama_decode_rows_warped_bf16, guided or not; sample_top_p's params)."""
     nh, nkv, hd, I = dims.num_attention_heads, dims.num_key_value_heads, dims.head_dim, dims.intermediate_size
-    if guidance is not None:  # one entry point for every format of the rows step: the format's array goes to its own argument
+    warped = seeds is not None and sample_params is not None and sample_params.numel() == 6
+    if guidance is not None or warped:  # one entry point for every format of the rows step: the format's array goes to its own argument
         fmt, arrays, lm = stack.formats("decode_rows")
-        scale, guided = guidance
-        desc = _lib.Guidance(_p(scale), _p(guided))
+        desc = None if guidance is None else _lib.Guidance(_p(guidance[0]), _p(guidance[1]))
         layers = arrays[0]
         packed = arrays[1] if fmt == "packed" else None
         nf4 = arrays[1] if fmt == "nf4" else None
-        check(_lib.load().srgpt_llama_decode_rows_guided_bf16(
+        name = "srgpt_llama_decode_rows_warped_bf16" if warped else "srgpt_llama_decode_rows_guided_bf16"
+        check(getattr(_lib.load(), name)(
             _p(h), layers, packed, nf4, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), B, dims.hidden_size, nh, nkv, hd, I, dims.rms_norm_eps,
             _p(cos), _p(sin), _p(pos_rows), _p(page_tables), _rowmajor2d(page_tables, "llama_decode_rows.page_tables"), page_size, _p(final_norm),
             _p(lm_head), lm[0] if lm else None, dims.vocab_size, _p(embed), _p(lm_ws), _p(logits_rows), _p(sample_params), _p(seeds), _p(ids),
-            _p(out_ids), _p(step), C.byref(desc), _stream()), "srgpt_llama_decode_rows_guided_bf16")
-        _count(stack.rows_kernels + (3 if seeds is not None else 1))
+            _p(out_ids), _p(step), None if desc is None else C.byref(desc), _stream()), name)
+        _count(stack.rows_kernels + ((3 if seeds is not None else 1) if guidance is not None else 1))
         return
     name, arrays, lm = stack.entry("decode_rows")
     check(getattr(_lib.load(), name)(_p(h), *arrays, stack.n, _p(q_buf), _p(attn_buf), _p(act_buf), B, dims.hidden_size, nh, nkv, hd, I,
