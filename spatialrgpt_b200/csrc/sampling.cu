@@ -6,8 +6,8 @@
 //   scores = logits / T;  keep the top_k scores (GenerationConfig default 50);  p = softmax over them;  keep the smallest set of
 //   highest-probability tokens whose mass reaches top_p (at least one token);  renormalise;  draw one token.
 // HF sorts the whole vocabulary every step; here ONE 1024-thread CTA makes a few passes over the 128 K logits (L2 resident):
-//   max -> normaliser -> the nucleus threshold by bisection on the probability value (S(t) = mass of {p_i >= t} is monotone)
-//   -> a draw u * S(t*) located with a block prefix sum over index-ordered chunks.
+//   max -> normaliser -> the top-k and nucleus cuts by exact searches over the logits' 32-bit keys (sample_row)
+//   -> a draw u * mass(kept set) located with a block prefix sum over index-ordered chunks.
 // The draw uses a counter-based generator (splitmix64 of seed and step), so a request is reproducible given its seed; it is
 // NOT torch's Philox stream, so sampled ids are comparable with the reference in distribution only (tests check the support and
 // the frequencies against the torch nucleus).  Greedy decoding (the graded mode) never runs this kernel.
@@ -52,12 +52,32 @@ __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
 __device__ __forceinline__ float logit(const float* __restrict__ x, int i) { return x[i]; }
 __device__ __forceinline__ float logit(const bf16* __restrict__ x, int i) { return e2f(x[i]); }  // exact: torch's .float() of the row
 
-// Whether the token of logit x and probability p is in the set the draw picks from: p >= t_keep (top-k and top-p), and with CUTS
+// Order-preserving 32-bit key of a float (a <= b iff key(a) <= key(b) for non-NaN a, b; -0 folded into +0, which compare equal).
+__device__ __forceinline__ unsigned key_of(float x) {
+  const unsigned u = __float_as_uint(__fadd_rn(x, 0.f));
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float of_key(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+// The smallest logit whose fl(x / t) reaches fl(xc / t): the cut at logit xc widened over every token HF's x / T ties with it
+// (x -> fl(x / t) is monotone for t > 0 but not one-to-one, so distinct logits can share a scaled value).
+template <typename T>
+__device__ __forceinline__ float widen_cut(const T* __restrict__ logits, int V, float xc, float t, float* red) {
+  const float sc = __fdiv_rn(xc, t);
+  float lo = xc;
+  for (int i = threadIdx.x; i < V; i += THREADS) {
+    const float x = logit(logits, i);
+    if (x < lo && __fdiv_rn(x, t) >= sc) lo = x;
+  }
+  return -block_reduce_max(-lo, red);
+}
+
+// Whether the token of logit x and probability p is in the set the draw picks from: x >= x_keep (top-k and top-p), and with CUTS
 // the typical / epsilon / eta cuts of sample_row, whose state s_cut = {c, d*, top logit of K1, p cut} it computes.
 template <bool CUTS>
-__device__ __forceinline__ bool kept(float x, float p, float m, float inv_t, float t_keep, const float* s_cut) {
-  if constexpr (CUTS) return p >= t_keep && fabsf(s_cut[0] - (x - m) * inv_t) <= s_cut[1] && (x >= s_cut[2] || p >= s_cut[3]);
-  else return p >= t_keep;
+__device__ __forceinline__ bool kept(float x, float p, float m, float inv_t, float x_keep, const float* s_cut) {
+  if constexpr (CUTS) return x >= x_keep && fabsf(s_cut[0] - (x - m) * inv_t) <= s_cut[1] && (x >= s_cut[2] || p >= s_cut[3]);
+  else return x >= x_keep;
 }
 
 // The draw of one row of V logits (fp32 or the element type) by the whole 1024-thread CTA; every thread returns the token.
@@ -87,48 +107,61 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   z = block_reduce_sum(z, red);
   const float inv_z = 1.0f / z;
 
-  // top-k first (HF's warper order: temperature, top_k, top_p; GenerationConfig's default top_k is 50): t_floor = the largest t
-  // with count{p >= t} >= k, found by bisection on the count (monotone in t); ties at the threshold stay in.
-  float t_floor = 0.f, mass_floor = 1.f;
+  // The cuts select on logit keys, exactly: HF compares fl(x / T), which is monotone in x, so the k-th largest x / T is fl(x_k / T) of
+  // the k-th largest logit x_k, and a cut at logit xc keeps {fl(x / T) >= fl(xc / T)} = {x >= widen_cut(xc)}.  (A cut on the probability
+  // value cannot tell apart probabilities below its resolution, nor the probabilities that underflow to 0 where HF keeps finite scores.)
+  // The key searches count in index-strided order (integer counts do not depend on it); the masses the draw uses are summed per chunk.
+  // top-k first (HF's warper order: temperature, top_k, top_p; GenerationConfig's default top_k is 50): the k-th largest key, found bit
+  // by bit from the top (the largest c with count{key >= c} >= k); every token tied with it in x / T stays in.
+  const float t = params[0];
+  float x_floor = -INFINITY, mass_floor = 1.f;
   if (top_k > 0 && top_k < V) {
-    float lo_t = 0.f, hi_t = inv_z;
-    for (int it = 0; it < 26; ++it) {
-      const float mid = 0.5f * (lo_t + hi_t);
-      float c = 0.f;
-      for (int i = lo; i < hi; ++i) c += (__expf((logit(logits, i) - m) * inv_t) * inv_z >= mid) ? 1.f : 0.f;
-      c = block_reduce_sum(c, red);
-      if (c >= (float)top_k) lo_t = mid; else hi_t = mid;
+    unsigned c = 0u;
+    for (int b = 31; b >= 0; --b) {
+      const unsigned cand = c | (1u << b);
+      float n = 0.f;
+      for (int i = tid; i < V; i += THREADS) n += key_of(logit(logits, i)) >= cand ? 1.f : 0.f;
+      if (block_reduce_sum(n, red) >= (float)top_k) c = cand;
     }
-    t_floor = lo_t;
+    x_floor = widen_cut(logits, V, of_key(c), t, red);
     float s = 0.f;
     for (int i = lo; i < hi; ++i) {
-      const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
-      s += (p >= t_floor) ? p : 0.f;
+      const float x = logit(logits, i);
+      s += (x >= x_floor) ? __expf((x - m) * inv_t) * inv_z : 0.f;
     }
     mass_floor = block_reduce_sum(s, red);
   }
-  // nucleus threshold inside the top-k set: the largest t >= t_floor with mass{p >= t} >= top_p * mass(top-k set).
-  // p_max = exp(0) / z is always kept (>= 1 token).
-  float t_keep = t_floor, mass = mass_floor;
+  // nucleus inside the top-k set: the largest key c with mass{key >= c} >= top_p * mass(top-k set), searched over the bits below the
+  // common prefix of the top-k cut's key and the top logit's key (c lies between them); the top logit is always kept (>= 1 token).
+  float x_keep = x_floor, mass = mass_floor;
   if (top_p < 1.0f) {
     const float target = top_p * mass_floor;
-    float lo_t = t_floor, hi_t = inv_z;  // invariant: mass(lo_t) >= target
-    float mass_lo = mass_floor;
-    for (int it = 0; it < 26; ++it) {
-      const float mid = 0.5f * (lo_t + hi_t);
-      float s = 0.f;
-      for (int i = lo; i < hi; ++i) {
-        const float p = __expf((logit(logits, i) - m) * inv_t) * inv_z;
-        s += (p >= mid) ? p : 0.f;
+    const unsigned kf = key_of(x_floor), km = key_of(m);
+    unsigned c = kf;
+    if (kf != km) {
+      const int hb = 31 - __clz(kf ^ km);
+      c = kf & ~((2u << hb) - 1u);  // the common prefix (hb = 31: none)
+      for (int b = hb; b >= 0; --b) {
+        const unsigned cand = c | (1u << b), cut = max(cand, kf);
+        float s = 0.f;
+        for (int i = tid; i < V; i += THREADS) {
+          const float x = logit(logits, i);
+          s += key_of(x) >= cut ? __expf((x - m) * inv_t) * inv_z : 0.f;
+        }
+        if (block_reduce_sum(s, red) >= target) c = cand;
       }
-      s = block_reduce_sum(s, red);
-      if (s >= target) { lo_t = mid; mass_lo = s; } else { hi_t = mid; }
+      c = min(max(c, kf), km);
     }
-    t_keep = lo_t;
-    mass = mass_lo;
+    x_keep = widen_cut(logits, V, of_key(c), t, red);
+    float s = 0.f;
+    for (int i = lo; i < hi; ++i) {
+      const float x = logit(logits, i);
+      s += (x >= x_keep) ? __expf((x - m) * inv_t) * inv_z : 0.f;
+    }
+    mass = block_reduce_sum(s, red);
   }
 
-  // Typical, epsilon and eta cuts (CUTS) over the kept set K0 = {p >= t_keep}, each on what the previous one left.  With s = the scaled
+  // Typical, epsilon and eta cuts (CUTS) over the kept set K0 = {x >= x_keep}, each on what the previous one left.  With s = the scaled
   // logit (x - m) / T and q = p / mass(K0), -log q - H = E_q[s] - s, so typical's deviation is |c - s| with c = E_q[s]; the kept set is
   // {|c - s| <= d*}, d* the smallest deviation whose set reaches typical_p of the mass (HF keeps every token up to the deviation at
   // which the sorted cumulative mass first reaches typical_p, ties included), found by bisection on d.  Epsilon keeps
@@ -143,16 +176,16 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
       float a = 0.f, b = 0.f;
       #pragma unroll 8
       for (int i = lo; i < hi; ++i) {
-        const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
-        if (p >= t_keep && p > 0.f) { a += p; b += p * s; }
+        const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+        if (x >= x_keep && p > 0.f) { a += p; b += p * s; }
       }
       const float a0 = block_reduce_sum(a, red);
       c_typ = block_reduce_sum(b, red) / a0;
       float dm = 0.f;
       #pragma unroll 8
       for (int i = lo; i < hi; ++i) {
-        const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
-        if (p >= t_keep && p > 0.f) dm = fmaxf(dm, fabsf(c_typ - s));
+        const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+        if (x >= x_keep && p > 0.f) dm = fmaxf(dm, fabsf(c_typ - s));
       }
       float lo_d = 0.f, hi_d = block_reduce_max(dm, red);  // invariant: mass{|c - s| <= hi_d} >= typical_p * a0
       const float target = typical_p * a0;
@@ -161,8 +194,8 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
         float sm = 0.f;
         #pragma unroll 8
         for (int i = lo; i < hi; ++i) {
-          const float s = (logit(logits, i) - m) * inv_t, p = __expf(s) * inv_z;
-          sm += (p >= t_keep && p > 0.f && fabsf(c_typ - s) <= mid) ? p : 0.f;
+          const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
+          sm += (x >= x_keep && p > 0.f && fabsf(c_typ - s) <= mid) ? p : 0.f;
         }
         sm = block_reduce_sum(sm, red);
         if (sm >= target) hi_d = mid; else lo_d = mid;
@@ -174,7 +207,7 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
       #pragma unroll 8
       for (int i = lo; i < hi; ++i) {
         const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
-        if (p >= t_keep && fabsf(c_typ - s) <= d_keep) { a += p; xm = fmaxf(xm, x); }
+        if (x >= x_keep && fabsf(c_typ - s) <= d_keep) { a += p; xm = fmaxf(xm, x); }
       }
       const float a1 = block_reduce_sum(a, red);
       x_top = block_reduce_max(xm, red);
@@ -184,7 +217,7 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
         #pragma unroll 8
         for (int i = lo; i < hi; ++i) {
           const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
-          if (p >= t_keep && p > 0.f && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) { a2 += p; b2 += p * s; }
+          if (x >= x_keep && p > 0.f && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) { a2 += p; b2 += p * s; }
         }
         a2 = block_reduce_sum(a2, red);
         b2 = block_reduce_sum(b2, red);
@@ -197,7 +230,7 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
       #pragma unroll 8
       for (int i = lo; i < hi; ++i) {
         const float x = logit(logits, i), s = (x - m) * inv_t, p = __expf(s) * inv_z;
-        sm += (p >= t_keep && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) ? p : 0.f;
+        sm += (x >= x_keep && fabsf(c_typ - s) <= d_keep && (x >= x_top || p >= cut)) ? p : 0.f;
       }
       mass = block_reduce_sum(sm, red);
     }
@@ -206,12 +239,11 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   }
 
   // the warped row (HF's output_scores of a sampled step): logits / T for the tokens the draw can pick (the set the top-k cut, the
-  // nucleus bisection and the CUTS kept), -inf for every other token.  A true fp32 division, as TemperatureLogitsWarper divides.
+  // nucleus and the CUTS kept), -inf for every other token.  A true fp32 division, as TemperatureLogitsWarper divides.
   if (warped != nullptr) {
-    const float t = params[0];
     for (int i = tid; i < V; i += THREADS) {
       const float x = logit(logits, i);
-      warped[i] = kept<CUTS>(x, __expf((x - m) * inv_t) * inv_z, m, inv_t, t_keep, s_cut) ? __fdiv_rn(x, t) : -INFINITY;
+      warped[i] = kept<CUTS>(x, __expf((x - m) * inv_t) * inv_z, m, inv_t, x_keep, s_cut) ? __fdiv_rn(x, t) : -INFINITY;
     }
   }
 
@@ -222,7 +254,7 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   float local = 0.f;
   for (int i = lo; i < hi; ++i) {
     const float x = logit(logits, i), p = __expf((x - m) * inv_t) * inv_z;
-    local += kept<CUTS>(x, p, m, inv_t, t_keep, s_cut) ? p : 0.f;
+    local += kept<CUTS>(x, p, m, inv_t, x_keep, s_cut) ? p : 0.f;
   }
   s_scan[tid] = local;
   __syncthreads();
@@ -237,13 +269,13 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   __syncthreads();
   const float before = tid == 0 ? 0.f : s_scan[tid - 1];
   const float total = s_scan[THREADS - 1];
-  const float uu = fminf(u, total * 0.99999994f);  // rounding of the bisection mass vs the scan total
+  const float uu = fminf(u, total * 0.99999994f);  // rounding of the chunk-summed mass vs the scan total
   if (uu >= before && uu < s_scan[tid] && hi > lo) {
     float acc = before;
     int pick = -1, last_kept = -1;
     for (int i = lo; i < hi; ++i) {
       const float x = logit(logits, i), p = __expf((x - m) * inv_t) * inv_z;
-      if (kept<CUTS>(x, p, m, inv_t, t_keep, s_cut)) {
+      if (p > 0.f && kept<CUTS>(x, p, m, inv_t, x_keep, s_cut)) {  // a kept token of p = 0 (exp underflow, -inf) is never drawn
         last_kept = i;
         acc += p;
         if (acc > uu) { pick = i; break; }
@@ -273,7 +305,7 @@ __device__ __forceinline__ int sample_row(const T* __restrict__ logits, int V, c
   return tok;
 }
 
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr, const int* __restrict__ step,
                     int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table, bf16* __restrict__ next_x, int K,
                     float* __restrict__ scores, long long step_stride) {
@@ -289,7 +321,7 @@ sample_top_p_kernel(const float* __restrict__ logits, int V, const float* __rest
 // R rows at once, one CTA per row: row r = logits + r * ld draws with seeds[r] at counter *step + step_offset -> ids[r].
 // Each row's token is the one sample_top_p_kernel draws from that row in fp32 with the same seed and counter.
 template <typename T>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seeds,
                    const int* __restrict__ step, int step_offset, long long* __restrict__ ids, float* __restrict__ scores, long long step_stride) {
   const int r = blockIdx.x;
@@ -299,7 +331,7 @@ sample_rows_kernel(const T* __restrict__ logits, long long ld, int V, const floa
 }
 
 // sample_top_p_kernel and sample_rows_kernel with the typical / epsilon / eta cuts (params float[6]).
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 sample_top_p_warped_kernel(const float* __restrict__ logits, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seed_ptr,
                            const int* __restrict__ step, int step_offset, long long* __restrict__ out_ids, const bf16* __restrict__ embed_table,
                            bf16* __restrict__ next_x, int K, float* __restrict__ scores, long long step_stride) {
@@ -313,7 +345,7 @@ sample_top_p_warped_kernel(const float* __restrict__ logits, int V, const float*
 }
 
 template <typename T>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 sample_rows_warped_kernel(const T* __restrict__ logits, long long ld, int V, const float* __restrict__ params, const unsigned long long* __restrict__ seeds,
                           const int* __restrict__ step, int step_offset, long long* __restrict__ ids, float* __restrict__ scores, long long step_stride) {
   const int r = blockIdx.x;

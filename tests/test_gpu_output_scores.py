@@ -95,8 +95,9 @@ def test_batch1_processors_prefix_cache_and_prompt_lookup(dtype):
 
 
 def hf_warp(rows: torch.Tensor, temperature: float, top_k: int, top_p: float):
-    """transformers' TemperatureLogitsWarper, TopKLogitsWarper and TopPLogitsWarper on fp32 CPU rows [R, V], and per row whether a
-    near-tie at the top-k or top-p cut makes the kept set depend on rounding."""
+    """transformers' TemperatureLogitsWarper, TopKLogitsWarper and TopPLogitsWarper on fp32 CPU rows [R, V], and per row whether the
+    kept set may differ from the kernel's as DESIGN.md §7 allows: a cumulative mass within 1e-4 of top_p, or tokens of equal score that
+    HF's sort splits at the nucleus cut (the kernel keeps every tied token).  The top-k set is exact: no exemption."""
     from transformers.generation import logits_process as lp
     x = rows.float().cpu()
     x = lp.TemperatureLogitsWarper(temperature)(None, x)
@@ -104,14 +105,13 @@ def hf_warp(rows: torch.Tensor, temperature: float, top_k: int, top_p: float):
     x = lp.TopPLogitsWarper(top_p)(None, x)
     t = rows.float().cpu() / temperature
     srt = t.sort(-1, descending=True).values
-    near_k = (srt[:, top_k - 1] - srt[:, top_k]).abs() < 1e-4
     p = torch.softmax(srt[:, :top_k], -1)
     cum = p.cumsum(-1)
     near_p = ((cum - top_p).abs() < 1e-4).any(-1)
-    # a tie (equal logits, frequent in 16-bit rows) across the cut HF's sort made: the kernel keeps every tied token
+    # a tie (equal scores, frequent in 16-bit rows) across the cut HF's sort made: the kernel keeps every tied token
     n = torch.isfinite(x).sum(-1).clamp(max=srt.shape[-1] - 1)
-    at = srt.gather(-1, (n - 1)[:, None])[:, 0] - srt.gather(-1, n[:, None])[:, 0]
-    return x, near_k | near_p | (at.abs() < 1e-4)
+    split = srt.gather(-1, (n - 1)[:, None])[:, 0] == srt.gather(-1, n[:, None])[:, 0]
+    return x, near_p | split
 
 
 def _check_warped(sc, raw_rows, seqs, lens=None):
@@ -129,15 +129,8 @@ def _check_warped(sc, raw_rows, seqs, lens=None):
                 continue
             checked += 1
             fin, gfin = torch.isfinite(ref[r]), torch.isfinite(got[r])
-            both = fin & gfin
-            assert torch.equal(got[r][both], ref[r][both]), (t, r)
-            # the kernel's cuts bisect on the probability over [0, p_max] in 26 steps: a token below that resolution may fall on
-            # either side of the cut; any other difference in the kept set (on a row without a tie at the cut) is an error
-            z = raw_rows[t][r].float().cpu() / SMP["temperature"]
-            rel = torch.exp(z - z.max())
-            diff = fin ^ gfin
-            assert bool((rel[diff] < 2.0 ** -20).all()), (t, r, diff.nonzero().flatten().tolist(), rel[diff].tolist(), int(fin.sum()),
-                                                          int(gfin.sum()))
+            assert torch.equal(fin, gfin), (t, r, (fin ^ gfin).nonzero().flatten().tolist(), int(fin.sum()), int(gfin.sum()))
+            assert torch.equal(got[r][fin], ref[r][fin]), (t, r)
     assert checked >= total // 2, (checked, total)
 
 
