@@ -305,6 +305,12 @@ int srgpt_beam_candidates_bf16(const void* logits, int ldx, int n_beams, int V, 
  * [n_beams, ldo], ldo >= V: HF's output_scores of a beam step (next_token_scores_processed). */
 int srgpt_beam_candidates_scores_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
                                       float* cand_scores, int* cand_tokens, float* logprobs, long long ldo, void* stream);
+/* Diverse beam search's candidates (rowops.cu): per row the n_cand best (log_softmax(logits.float())[token] + beam_scores[row], token) in
+ * (score desc, token asc) order of that fp32 score, which the rounding of + beam_scores can make differ from the logit order ->
+ * cand_scores / cand_tokens [n_beams, n_cand], and the row's (max, log-sum-exp) of the rounded logits -> stats [n_beams][2] (8-byte
+ * aligned), from which log_softmax[token] = (logit - max) - lse. */
+int srgpt_beam_candidates_scored_bf16(const void* logits, int ldx, int n_beams, int V, const float* beam_scores, int n_cand,
+                                      float* cand_scores, int* cand_tokens, float* stats, void* stream);
 /* Score rows of a decode step (rowops.cu): HF's output_scores of a greedy step.  Row r of rows [R, ld] (fp32 when rows_f32, else the
  * element type widened exactly, as .float()) -> scores + (*step + step_offset) * step_stride + r * row_stride, for r < R.  The index is
  * read at run time, so one captured decode graph writes every step's rows.  R <= 65535, ld >= V, row_stride >= V. */
@@ -316,6 +322,20 @@ int srgpt_step_scores(const void* rows, int rows_f32, long long ld, int R, int V
  * prompt has fewer valid candidates).  One CTA per prompt; k * n_cand <= 4096. */
 int srgpt_beam_select(const float* cand_scores, const int* cand_tokens, int n_groups, int k, int n_cand, float* out_scores, int* out_beams,
                       int* out_tokens, void* stream);
+/* Diverse beam search over a batch of prompts (beam.cu; HF group_beam_search with HammingDiversityLogitsProcessor, transformers 4.37.2):
+ * prompt p owns rows p*k .. p*k+k-1, group g of it the gs = k / n_groups rows p*k + g*gs ..  One CTA per prompt takes the groups in
+ * order.  Each token of group g's rows scores fl(fl(logp - fl(diversity_penalty * c)) + beam_scores[row]), c = how often groups 0 .. g-1
+ * of the prompt chose it in this step and logp = (logit - max) - lse from stats; the candidates are the L tokens per row that
+ * srgpt_beam_candidates_scored_bf16 wrote (cand_tokens [rows, L]) and the earlier groups' choices, which is exact for L >= n_cand + k - gs.
+ * The group's n_cand best (score, beam within the group, token) in (score desc, beam asc, token asc) order -> out_* [n_prompts,
+ * n_groups, n_cand] (-inf / -1 / -1 past the valid ones); BeamSearchScorer.process's choice (EOS candidates closing no beam here) ->
+ * next_beams (the parent, a beam within the prompt) and next_tokens [n_prompts * k], -1 where a group runs out of non-EOS candidates.  A
+ * group with done[p * n_groups + g] != 0 writes no candidates and gives each of its beams parent g*gs and token pad_id.  Chosen and pad
+ * tokens both count for the later groups.  k <= 64, n_cand <= 512, V <= 2^26, gs * (L + k - gs) <= 4096. */
+int srgpt_beam_group_select(const void* logits, int ldx, int V, const float* stats, const float* beam_scores, const int* cand_tokens, int L,
+                            int n_prompts, int k, int n_groups, int n_cand, const int* eos, int n_eos, int pad_id, float diversity_penalty,
+                            const int* done, float* out_scores, int* out_beams, int* out_tokens, int* next_beams, int* next_tokens,
+                            void* stream);
 /* Bytes of the workspace srgpt_kv_copy_pages needs for n_staged pairs (-1 on invalid arguments). */
 long long srgpt_kv_copy_workspace_bytes(int n_staged, int n_layers, int page_rows, int row_bytes);
 /* Copies rows of KV pages for K and V of every layer (beam.cu).  pages: [n_layers, n_pages, 2 (K, V), page_rows, row_bytes] bytes, the

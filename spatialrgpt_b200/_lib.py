@@ -61,8 +61,10 @@ SIGNATURES = {
     "srgpt_argmax_bf16": (ci, [vp, ci, ci, ci, vp, vp]),
     "srgpt_beam_candidates_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp, vp]),
     "srgpt_beam_candidates_scores_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp, vp, cll, vp]),
+    "srgpt_beam_candidates_scored_bf16": (ci, [vp, ci, ci, ci, vp, ci, vp, vp, vp, vp]),
     "srgpt_step_scores": (ci, [vp, ci, cll, ci, ci, vp, ci, vp, cll, cll, vp]),
     "srgpt_beam_select": (ci, [vp, vp, ci, ci, ci, vp, vp, vp, vp]),
+    "srgpt_beam_group_select": (ci, [vp, ci, ci, vp, vp, vp, ci, ci, ci, ci, ci, vp, ci, ci, cf, vp, vp, vp, vp, vp, vp, vp]),
     "srgpt_kv_copy_workspace_bytes": (cll, [ci, ci, ci, ci]),
     "srgpt_kv_copy_pages": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, vp, cll, vp]),
     "srgpt_token_logprobs": (ci, [vp, cll, ci, ci, vp, vp, ci, vp, cll, vp, vp, vp, vp]),

@@ -329,9 +329,13 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
   }
   return t;
 }
-__global__ void __launch_bounds__(BEAM_THREADS)
-beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const float* __restrict__ beam_scores, int n_cand, float* __restrict__ cand_scores,
-                       int* __restrict__ cand_tokens, float* __restrict__ logprobs, long long ldo) {
+// SCORED (diverse beam search, beam.cu group_select_kernel): the candidates are ranked by their fp32 score ((v - m) - lse) + bs, token
+// asc on ties, rather than by the logit, so a row's list is exactly its top n_cand in the order the group merge uses even where the
+// rounding of + bs ties different logits; and the row's (m, lse) go to stats[row], so the merge can score any other token of the row.
+template <bool SCORED>
+__device__ __forceinline__ void beam_candidates_row(const bf16* __restrict__ logits, int ldx, int V, const float* __restrict__ beam_scores, int n_cand,
+                                                    float* __restrict__ cand_scores, int* __restrict__ cand_tokens, float* __restrict__ logprobs,
+                                                    long long ldo, float2* __restrict__ stats) {
   __shared__ unsigned long long sk[32];
   __shared__ float sred[32];
   const bf16* row = logits + (size_t)blockIdx.x * ldx;
@@ -358,14 +362,16 @@ beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const fl
     for (int c = tid; c < V; c += BEAM_THREADS) orow[c] = (e2f(row[c]) - m) - lse;
   }
   const float bs = beam_scores[blockIdx.x];
-  // key = (order-preserving bits of the logit, ~token): the maximum key below the previous one is the next candidate
+  if (SCORED && tid == 0) stats[blockIdx.x] = make_float2(m, lse);
+  // key = (order-preserving bits of the logit (SCORED: of the score), ~token): the maximum key below the previous one is the next candidate
   unsigned long long prev = ~0ull;
   for (int j = 0; j < n_cand; ++j) {
     unsigned long long best = 0ull;
     for (int c = tid; c < V; c += BEAM_THREADS) {
       const float v = e2f(row[c]);
       if (v == v) {
-        const unsigned long long k = ((unsigned long long)float_order_bits(v) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned int)c);
+        const unsigned long long k = ((unsigned long long)float_order_bits(SCORED ? ((v - m) - lse) + bs : v) << 32) |
+                                     (unsigned long long)(0xFFFFFFFFu - (unsigned int)c);
         if (k < prev && k > best) best = k;
       }
     }
@@ -383,6 +389,16 @@ beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const fl
     }
     prev = best == 0ull ? 0ull : best;
   }
+}
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_candidates_kernel(const bf16* __restrict__ logits, int ldx, int V, const float* __restrict__ beam_scores, int n_cand, float* __restrict__ cand_scores,
+                       int* __restrict__ cand_tokens, float* __restrict__ logprobs, long long ldo) {
+  beam_candidates_row<false>(logits, ldx, V, beam_scores, n_cand, cand_scores, cand_tokens, logprobs, ldo, nullptr);
+}
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_candidates_scored_kernel(const bf16* __restrict__ logits, int ldx, int V, const float* __restrict__ beam_scores, int n_cand,
+                              float* __restrict__ cand_scores, int* __restrict__ cand_tokens, float2* __restrict__ stats) {
+  beam_candidates_row<true>(logits, ldx, V, beam_scores, n_cand, cand_scores, cand_tokens, nullptr, 0, stats);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -544,6 +560,19 @@ extern "C" __attribute__((visibility("default"))) int srgpt_beam_candidates_scor
   SRGPT_CHECK_ARG(logprobs == nullptr || ldo >= V);
   beam_candidates_kernel<<<n_beams, BEAM_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const bf16*>(logits), ldx, V, beam_scores, n_cand,
                                                                                              cand_scores, cand_tokens, logprobs, ldo);
+  SRGPT_CHECK_LAUNCH();
+  return SRGPT_OK;
+}
+
+// Diverse beam search's candidates (llama_decoder.generate_beam_batch with num_beam_groups > 1): per row the n_cand best (score, token) in
+// (score desc, token asc) order of the score itself, and the row's (max, log-sum-exp) -> stats [n_beams] float2.
+extern "C" __attribute__((visibility("default"))) int srgpt_beam_candidates_scored_bf16(const void* logits, int ldx, int n_beams, int V,
+                                                                                         const float* beam_scores, int n_cand, float* cand_scores,
+                                                                                         int* cand_tokens, float* stats, void* stream) {
+  SRGPT_CHECK_ARG(logits && beam_scores && cand_scores && cand_tokens && stats && n_beams > 0 && V > 0 && ldx >= V && n_cand > 0 && n_cand <= V);
+  SRGPT_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 7) == 0);
+  beam_candidates_scored_kernel<<<n_beams, BEAM_THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const bf16*>(logits), ldx, V, beam_scores, n_cand, cand_scores, cand_tokens, reinterpret_cast<float2*>(stats));
   SRGPT_CHECK_LAUNCH();
   return SRGPT_OK;
 }

@@ -160,18 +160,34 @@ class BeamHypotheses:
         self.scores = [sc for sc, _, _ in nxt]
         return [b for _, b, _ in nxt]
 
-    def best(self, max_new_tokens: int) -> List[int]:
-        """finalize (beam_search.py): unless done, the running beams become hypotheses over their generated length; the best one, with the
-        first EOS appended when it is shorter than max_new_tokens."""
+    def close(self) -> None:
+        """finalize (beam_search.py): unless done, the running beams become hypotheses over their generated length."""
         if not self.done:
             for i in range(self.k):
                 self.keep(self.scores[i] / (len(self.seqs[i]) ** self.length_penalty), list(self.seqs[i]), list(self.beams[i]))
+
+    def best(self, max_new_tokens: int) -> List[int]:
+        """finalize (beam_search.py): close, then the best hypothesis, with the first EOS appended when it is shorter than max_new_tokens."""
+        self.close()
         i = max(range(len(self.hyps)), key=lambda j: self.hyps[j][0])
         self.best_score, self.best_beams = self.hyps[i][0], list(self.hyp_beams[i])
         best = list(self.hyps[i][1])
         if len(best) < max_new_tokens and self.eos:
             best.append(self.eos[0])
         return best
+
+
+def group_best(groups: List[BeamHypotheses], max_new_tokens: int) -> List[int]:
+    """The answer of one prompt of diverse beam search (BeamSearchScorer.finalize with num_beam_groups, transformers 4.37.2): every group
+    closes, and of all groups' hypotheses, in group order, a stable sort by score and pop() take the last best one (a tie goes to the
+    later group); the first EOS is appended when it is shorter than max_new_tokens."""
+    for grp in groups:
+        grp.close()
+    best = list(sorted((h for grp in groups for h in grp.hyps), key=lambda h: h[0])[-1][1])
+    eos = groups[0].eos
+    if len(best) < max_new_tokens and eos:
+        best.append(eos[0])
+    return best
 
 
 def beam_page_pairs(tables: List[List[int]], parents: List[int], starts: List[int], n_gen: int, page_size: int = PAGE_SIZE):
@@ -1483,7 +1499,8 @@ class LlamaDecoder:
     @ops.in_own_dtype
     def generate_beam_batch(self, packed_embeds: torch.Tensor, seq_lens: List[int], num_beams: int, max_new_tokens: int, eos_token_ids=None,
                             stopping_fn=None, length_penalty: float = 1.0, early_stopping: bool = False, use_graph: bool = True,
-                            output_scores: bool = False):
+                            output_scores: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
+                            pad_token_id: Optional[int] = None):
         """Beam search over B prompts packed back to back ([sum S_b, H]) at once (HF beam_search + BeamSearchScorer with batch_size = B).
         Row g * k + i of every step is beam i of prompt g, so one batched decode step serves all B * k beams.  Device side: ONE packed
         prefill of the B prompts, their pages copied into the other k - 1 beams of each (kv_copy_pages), then per step the candidates
@@ -1493,19 +1510,34 @@ class LlamaDecoder:
         prompt is done, at max_new_tokens, or when ``stopping_fn`` holds for every beam of the prompts still running.  Returns a list
         of B LongTensors of NEW ids, each prompt's best hypothesis.  ``output_scores``: returns (ids, extra) as generate_beam, the score
         rows [steps, B * k, V] in the step's row order (row g * k + i = beam i of prompt g).  A prompt that is done keeps its rows in the
-        step, so its rows of the later steps hold what the step computed for them."""
+        step, so its rows of the later steps hold what the step computed for them.
+        ``num_beam_groups`` G > 1 with ``diversity_penalty`` > 0: diverse beam search (HF group_beam_search, transformers 4.37.2), B = 1
+        included.  Beam i of a prompt belongs to group i // (k / G); each (prompt, group) has its own BeamHypotheses, and one kernel
+        per step (beam_group_select) takes every prompt's groups in order, each penalised by diversity_penalty per earlier choice of a
+        token in this step, and makes HF's choice on the device; the host replays it from the ranked candidates.  A done group emits
+        ``pad_token_id`` (default: the first EOS id), which still counts for the later groups; the answer is the best hypothesis over all
+        groups (group_best).  Not with output_scores."""
         d, w, k, B = self.dims, self.w, int(num_beams), len(seq_lens)
         V, R, dev = d.vocab_size, B * int(num_beams), self.device
         seq_lens = [int(n) for n in seq_lens]
+        G = int(num_beam_groups)
         if k < 2:
             raise ValueError("generate_beam_batch needs num_beams >= 2")
+        if G != 1:
+            if G < 1 or G > k or k % G:
+                raise ValueError(f"num_beams ({k}) must be divisible by num_beam_groups ({G}), and num_beam_groups at most num_beams")
+            if not float(diversity_penalty) > 0.0:
+                raise ValueError(f"diverse beam search needs diversity_penalty > 0, got {diversity_penalty}")
+            if output_scores:
+                raise NotImplementedError("output_scores with num_beam_groups > 1")
         if B < 1 or packed_embeds.shape[0] != sum(seq_lens) or min(seq_lens) < 1:
             raise RuntimeError("generate_beam_batch: rows do not match seq_lens")
         if max_new_tokens < 1:
             empty = [torch.empty(0, dtype=torch.int64, device=dev) for _ in range(B)]
             return (empty, self._beam_extra(None, 0, [])) if output_scores else empty
         eos = eos_list(eos_token_ids)
-        n_cand = max(2, 1 + len(eos)) * k
+        gs = k // G  # the beams of a group
+        n_cand = max(2, 1 + len(eos)) * gs
         starts = [n for n in seq_lens for _ in range(k)]  # row r = g * k + i: the first generated position of its prompt
         self._start_request(starts, max_new_tokens, writes_ids=False)
         tables = [list(self.cache.owned[r]) for r in range(R)]
@@ -1518,30 +1550,53 @@ class LlamaDecoder:
         rows = ops.splice_rows(hidden, None, None, None, torch.zeros_like(last), last)
         ops.rmsnorm(rows, w.norm, d.rms_norm_eps, out=st["xn"])
         ops.gemm(st["xn"], w.lm_head, out=st["logits"][:, :V])
-        groups = [BeamHypotheses(k, eos, length_penalty, early_stopping, row0=g * k) for g in range(B)]
+        # group q = prompt * G + its group owns rows q * gs .. q * gs + gs - 1; G = 1: one per prompt
+        groups = [BeamHypotheses(gs, eos, length_penalty, early_stopping, row0=q * gs) for q in range(B * G)]
         rows_out = self._scores_view(max_new_tokens, R) if output_scores else None
         d_scores = torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32).to(dev)
-        cand_s = torch.empty((R, n_cand), dtype=torch.float32, device=dev)
-        cand_t = torch.empty((R, n_cand), dtype=torch.int32, device=dev)
-        sel = torch.empty((3, B, n_cand), dtype=torch.int32, device=dev)  # the merge's scores (as bits), beams, tokens: one copy to the host
-        h_sel = torch.empty((3, B, n_cand), dtype=torch.int32, pin_memory=True)
+        # G > 1: each row's list must outlast the k - gs tokens the earlier groups may penalise (srgpt_beam_group_select)
+        n_list = n_cand if G == 1 else min(n_cand + k - gs, V)
+        cand_s = torch.empty((R, n_list), dtype=torch.float32, device=dev)
+        cand_t = torch.empty((R, n_list), dtype=torch.int32, device=dev)
+        n_sel = 3 * B * G * n_cand
+        # the merge's scores (as bits), beams, tokens (G > 1: then each beam's parent and token): one copy to the host
+        sel_all = torch.empty(n_sel + (2 * R if G > 1 else 0), dtype=torch.int32, device=dev)
+        sel = sel_all[:n_sel].view(3, B * G, n_cand)
+        h_all = torch.empty(sel_all.shape, dtype=torch.int32, pin_memory=True)
+        h_sel = h_all[:n_sel].view(3, B * G, n_cand)
         h_scores = h_sel[0].view(torch.float32)
+        if G > 1:
+            stats = torch.empty((R, 2), dtype=torch.float32, device=dev)
+            d_eos = torch.tensor(eos, dtype=torch.int32).to(dev)
+            d_done = torch.zeros((B, G), dtype=torch.int32, device=dev)
+            pad = pad_token_id if pad_token_id is not None else (eos[0] if eos else 0)
+            nxt = sel_all[n_sel:].view(2, R)
         zero = torch.zeros(R, dtype=torch.int32, device=dev)
         tokens = [0] * R  # the token each row feeds to the next step (a done prompt's rows repeat theirs)
         for step in range(max_new_tokens):
-            ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t, **self._logprobs_kw(rows_out, step))
-            ops.beam_select(cand_s, cand_t, k, sel[0].view(torch.float32), sel[1], sel[2])
-            h_sel.copy_(sel, non_blocking=True)
+            if G == 1:
+                ops.beam_candidates(st["logits"][:, :V], d_scores, cand_s, cand_t, **self._logprobs_kw(rows_out, step))
+                ops.beam_select(cand_s, cand_t, k, sel[0].view(torch.float32), sel[1], sel[2])
+            else:
+                ops.beam_candidates_scored(st["logits"][:, :V], d_scores, cand_s, cand_t, stats)
+                ops.beam_group_select(st["logits"][:, :V], stats, d_scores, cand_t, k, G, d_eos, pad, diversity_penalty, d_done,
+                                      sel[0].view(torch.float32).view(B, G, n_cand), sel[1].view(B, G, n_cand), sel[2].view(B, G, n_cand),
+                                      nxt[0], nxt[1])
+            h_all.copy_(sel_all, non_blocking=True)
             torch.cuda.current_stream().synchronize()
             scores, beams, toks = h_scores.tolist(), h_sel[1].tolist(), h_sel[2].tolist()
+            chosen = h_all[n_sel:].view(2, R).tolist() if G > 1 else None
             parents = list(range(R))
-            for g, grp in enumerate(groups):
+            for q, grp in enumerate(groups):
                 if grp.done:
                     continue
-                ranked = [(scores[g][j], beams[g][j], toks[g][j]) for j in range(n_cand) if toks[g][j] >= 0]
+                ranked = [(scores[q][j], beams[q][j], toks[q][j]) for j in range(n_cand) if toks[q][j] >= 0]
                 for i, b in enumerate(grp.advance(ranked, step + 1)):
-                    parents[g * k + i] = g * k + b
-                    tokens[g * k + i] = grp.seqs[i][-1]
+                    parents[q * gs + i] = q * gs + b
+                    tokens[q * gs + i] = grp.seqs[i][-1]
+                    if G > 1 and (chosen[0][q * gs + i] + q // G * k, chosen[1][q * gs + i]) != (q * gs + b, tokens[q * gs + i]):
+                        raise RuntimeError(f"beam_group_select chose beam {chosen[0][q * gs + i]} / token {chosen[1][q * gs + i]} where "
+                                           f"BeamSearchScorer.process takes {q * gs + b - q // G * k} / {tokens[q * gs + i]}")
             if all(grp.done for grp in groups) or step == max_new_tokens - 1:
                 break
             if stopping_fn is not None and all(stopping_fn(torch.tensor(q, dtype=torch.int64)) for grp in groups if not grp.done for q in grp.seqs):
@@ -1552,13 +1607,18 @@ class LlamaDecoder:
             st["h"].copy_(ops.splice_rows(w.embed, None, None, None, zero, torch.tensor(tokens, dtype=torch.int32).to(dev)))
             st["pos"].copy_(torch.tensor([n + step for n in starts], dtype=torch.int32))
             d_scores.copy_(torch.tensor([s for grp in groups for s in grp.scores], dtype=torch.float32))
+            if G > 1:
+                d_done.copy_(torch.tensor([grp.done for grp in groups], dtype=torch.int32).view(B, G))
             if use_graph:  # keyed by the row count, as generate_beam's graph: the same launch over the same buffers
                 self._capture(GraphKey("beam", R), lambda: self._batch_step_launch(st, logits_only=True), (st["h"],),
                               self._batch_kernels_per_layer * d.num_hidden_layers + 2)
                 self._replay(GraphKey("beam", R))
             else:
                 self._batch_step_launch(st, logits_only=True)
-        outs = [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
+        if G == 1:
+            outs = [torch.tensor(grp.best(max_new_tokens), dtype=torch.int64, device=dev) for grp in groups]
+        else:
+            outs = [torch.tensor(group_best(groups[b * G:(b + 1) * G], max_new_tokens), dtype=torch.int64, device=dev) for b in range(B)]
         return (outs, self._beam_extra(rows_out, step + 1, groups)) if output_scores else outs
 
     @torch.no_grad()

@@ -138,6 +138,48 @@ def refuse_contrastive(top_k: int = 50, processors=None, lookup_k: int = 0, pref
         raise NotImplementedError("penalty_alpha on the tensor-parallel decoder")
 
 
+def group_beam_args(num_beams: int, num_beam_groups, diversity_penalty, do_sample: bool) -> Tuple[int, float]:
+    """generate()'s num_beam_groups / diversity_penalty as (G, lambda), raising ValueError where transformers 4.37.2 does
+    (GenerationConfig.validate, BeamSearchScorer, HammingDiversityLogitsProcessor): num_beams not a multiple of G or G > num_beams,
+    do_sample with G > 1, lambda <= 0 with G > 1, lambda > 0 without groups.  G = 1 and lambda = 0 are plain beam search."""
+    G = 1 if num_beam_groups is None else int(num_beam_groups)
+    lam = 0.0 if diversity_penalty is None else float(diversity_penalty)
+    if G < 1 or G > num_beams or num_beams % G:
+        raise ValueError(f"num_beams ({num_beams}) has to be divisible by num_beam_groups ({G}), and num_beam_groups at most num_beams")
+    if G > 1 and do_sample:
+        raise ValueError("diverse beam search (num_beam_groups > 1) needs do_sample=False")
+    if G > 1 and not lam > 0.0:
+        raise ValueError(f"diverse beam search (num_beam_groups > 1) needs diversity_penalty > 0, got {diversity_penalty}")
+    if G == 1 and lam > 0.0:
+        raise ValueError("diversity_penalty > 0 needs num_beam_groups > 1 (HF's HammingDiversityLogitsProcessor)")
+    return G, lam
+
+
+def refuse_group_beams(processors=None, return_logits: bool = False, output_scores: bool = False, generate_outputs: bool = False,
+                       prefix_cache: bool = False, lookup_k: int = 0, guided: bool = False, batch_invariant: bool = False, n_ret: int = 1,
+                       llm=None) -> None:
+    """The generate() options diverse beam search (num_beam_groups > 1) does not serve: raises NotImplementedError before any GPU work.
+    Its groups run as the beams of the batched beam step (LlamaDecoder.generate_beam_batch with num_beam_groups)."""
+    if processors is not None:
+        raise NotImplementedError("num_beam_groups with logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length)")
+    if return_logits or output_scores:
+        raise NotImplementedError("num_beam_groups with output_logits / output_scores")
+    if generate_outputs:
+        raise NotImplementedError("num_beam_groups with output_hidden_states / output_attentions")
+    if prefix_cache:
+        raise NotImplementedError("num_beam_groups with prefix_cache=True")
+    if lookup_k:
+        raise NotImplementedError("num_beam_groups with prompt_lookup_num_tokens")
+    if guided:
+        raise NotImplementedError("num_beam_groups with guidance_scale != 1")
+    if batch_invariant:
+        raise NotImplementedError("num_beam_groups with batch_invariant=True")
+    if n_ret != 1:
+        raise NotImplementedError("num_beam_groups with num_return_sequences > 1")
+    if llm is not None and (not hasattr(llm, "generate_beam_batch") or type(llm).__name__ == "TPLlamaDecoder"):
+        raise NotImplementedError("num_beam_groups on the tensor-parallel decoder")
+
+
 def refuse_generate_outputs(num_beams: int = 1, contrastive: bool = False, guided: bool = False, batch_invariant: bool = False, lookup_k: int = 0,
                             prefix_cache: bool = False, n_ret: int = 1, return_logits: bool = False, n_prompts: int = 1, llm=None) -> None:
     """The generate() options output_hidden_states / output_attentions (with return_dict_in_generate=True) do not serve: raises
@@ -808,6 +850,12 @@ class LlavaLlamaModel:
                        and not do_sample)
         length_penalty = float(generation_kwargs.pop("length_penalty", 1.0))
         early_stopping = bool(generation_kwargs.pop("early_stopping", False))
+        # num_beam_groups=G with diversity_penalty=lambda (HF's group (diverse) beam search, transformers 4.37.2): the num_beams beams
+        # form G groups chosen one after the other in every step, each token's log-prob lowered by lambda for every time an earlier
+        # group of the prompt chose it in that step.  G = 1 with lambda = 0 is plain beam search.
+        group_kw = {k: generation_kwargs.pop(k) for k in ("num_beam_groups", "diversity_penalty") if k in generation_kwargs}
+        n_groups, diversity = group_beam_args(num_beams, group_kw.get("num_beam_groups"), group_kw.get("diversity_penalty"), do_sample) \
+            if group_kw else (1, 0.0)
         # HF's logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_new_tokens / min_length), applied on the
         # device inside the decode step before the greedy choice or the sampling warpers (logits_processors.py, csrc/logits_process.cu).
         # The history is the generated tokens, as HF's given only inputs_embeds.  Neutral values leave generate() unchanged.
@@ -818,6 +866,10 @@ class LlavaLlamaModel:
         if generation_kwargs:
             raise TypeError(f"unsupported generation kwargs: {sorted(generation_kwargs)}")
         processors = logits_processors.parse(**proc_kw, eos_token_id=eos_token_id, vocab_size=getattr(self.config.llama, "vocab_size", None))
+        if n_groups > 1:
+            refuse_group_beams(processors=processors, return_logits=return_logits, output_scores=output_scores, generate_outputs=want_h or want_a,
+                               prefix_cache=prefix_cache, lookup_k=lookup_k, guided=guided, batch_invariant=batch_invariant, n_ret=n_ret,
+                               llm=self.llm)
         if processors is not None:
             if num_beams != 1:
                 raise NotImplementedError("logits processors (repetition_penalty, no_repeat_ngram_size, bad_words_ids, min_length) with beam search")
@@ -928,7 +980,7 @@ class LlavaLlamaModel:
                                                  eos_token_ids=eos_token_id, stopping_fn=stop_fn, use_graph=use_graph, **sc_kw)
             if output_scores:
                 outs, extra = outs
-        elif B == 1 and num_beams != 1:
+        elif B == 1 and num_beams != 1 and n_groups == 1:
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
             r = self.llm.generate_beam(emb, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
@@ -936,7 +988,7 @@ class LlavaLlamaModel:
             if output_scores:
                 r, extra = r
             outs.append(r)
-        elif B == 1 and n_ret == 1:
+        elif B == 1 and n_ret == 1 and n_groups == 1:  # diverse beams of one prompt run the batched beam step below
             n = lens[0]
             emb = packed if packed is not None else (inputs_embeds[0, inputs_embeds.shape[1] - n:] if left else inputs_embeds[0, :n])
             reuse = 0
@@ -973,8 +1025,10 @@ class LlavaLlamaModel:
                 T = inputs_embeds.shape[1]
                 packed = torch.cat([inputs_embeds[b, T - lens[b]:] if left else inputs_embeds[b, :lens[b]] for b in range(B)], 0)
             if num_beams != 1:
+                grp_kw = {} if n_groups == 1 else dict(num_beam_groups=n_groups, diversity_penalty=diversity, pad_token_id=pad_token_id)
                 outs = self.llm.generate_beam_batch(packed, lens, num_beams, int(max_new_tokens), eos_token_ids=eos_token_id, stopping_fn=stop_fn,
-                                                    length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph, **sc_kw)
+                                                    length_penalty=length_penalty, early_stopping=early_stopping, use_graph=use_graph, **sc_kw,
+                                                    **grp_kw)
                 if output_scores:
                     outs, extra = outs
             else:

@@ -1019,6 +1019,57 @@ def beam_candidates(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores
                                                  _p(cand_scores), _p(cand_tokens), _stream()), "srgpt_beam_candidates_bf16")
 
 
+def beam_candidates_scored(logits: torch.Tensor, beam_scores: torch.Tensor, cand_scores: torch.Tensor, cand_tokens: torch.Tensor,
+                           stats: torch.Tensor) -> None:
+    """Per beam row: the n_cand best (log_softmax(logits)[token] + beam_scores[row], token) in (score desc, token asc) order of the fp32
+    score -> cand_scores / cand_tokens [k, n_cand], and the row's (max, log-sum-exp) -> stats fp32 [k, 2] (diverse beam search)."""
+    _need(logits, ELEM(), "beam_candidates_scored.logits"); _need(beam_scores, torch.float32, "beam_candidates_scored.beam_scores")
+    _need(cand_scores, torch.float32, "beam_candidates_scored.cand_scores"); _need(cand_tokens, torch.int32, "beam_candidates_scored.cand_tokens")
+    _need(stats, torch.float32, "beam_candidates_scored.stats")
+    k, V = logits.shape
+    if cand_scores.shape != cand_tokens.shape or cand_scores.shape[0] != k or not cand_scores.is_contiguous() or not cand_tokens.is_contiguous():
+        raise SrgptError("beam_candidates_scored: cand_scores / cand_tokens must be contiguous [n_beams, n_cand]")
+    if tuple(stats.shape) != (k, 2) or not stats.is_contiguous():
+        raise SrgptError(f"beam_candidates_scored: stats must be contiguous fp32 [{k}, 2]")
+    check(_lib.load().srgpt_beam_candidates_scored_bf16(_p(logits), _rowmajor2d(logits, "beam_candidates_scored.logits"), k, V, _p(beam_scores),
+                                                        cand_scores.shape[1], _p(cand_scores), _p(cand_tokens), _p(stats), _stream()),
+          "srgpt_beam_candidates_scored_bf16")
+
+
+def beam_group_select(logits: torch.Tensor, stats: torch.Tensor, beam_scores: torch.Tensor, cand_tokens: torch.Tensor, k: int, n_groups: int,
+                      eos: torch.Tensor, pad_id: int, diversity_penalty: float, done: torch.Tensor, out_scores: torch.Tensor,
+                      out_beams: torch.Tensor, out_tokens: torch.Tensor, next_beams: torch.Tensor, next_tokens: torch.Tensor) -> None:
+    """Diverse beam search's choice for the P = rows / k prompts of the [P * k, V] logits, group by group (srgpt_beam_group_select):
+    stats / cand_tokens [P * k, L] from beam_candidates_scored over the same logits and beam_scores; eos int32 [n_eos]; done int32
+    [P, n_groups].  -> out_scores / out_beams / out_tokens [P, n_groups, n_cand] (each group's ranked candidates, beams within the group)
+    and next_beams / next_tokens int32 [P * k] (each beam's parent within its prompt, and its token)."""
+    _need(logits, ELEM(), "beam_group_select.logits"); _need(stats, torch.float32, "beam_group_select.stats")
+    _need(beam_scores, torch.float32, "beam_group_select.beam_scores"); _need(cand_tokens, torch.int32, "beam_group_select.cand_tokens")
+    _need(eos, torch.int32, "beam_group_select.eos"); _need(done, torch.int32, "beam_group_select.done")
+    _need(out_scores, torch.float32, "beam_group_select.out_scores")
+    for t, name in ((out_beams, "out_beams"), (out_tokens, "out_tokens"), (next_beams, "next_beams"), (next_tokens, "next_tokens")):
+        _need(t, torch.int32, f"beam_group_select.{name}")
+    R, V = logits.shape
+    if k < 1 or n_groups < 1 or R % k:
+        raise SrgptError(f"beam_group_select: {R} rows are not prompts of k = {k} beams")
+    P, L, n_cand = R // k, cand_tokens.shape[1], out_scores.shape[-1]
+    if cand_tokens.shape[0] != R or not cand_tokens.is_contiguous() or tuple(stats.shape) != (R, 2) or not stats.is_contiguous():
+        raise SrgptError(f"beam_group_select: cand_tokens must be contiguous [{R}, L] and stats [{R}, 2]")
+    if beam_scores.numel() != R or tuple(done.shape) != (P, n_groups) or not done.is_contiguous() or not eos.is_contiguous():
+        raise SrgptError(f"beam_group_select: beam_scores must hold {R} scores and done be [{P}, {n_groups}]")
+    for o in (out_scores, out_beams, out_tokens):
+        if tuple(o.shape) != (P, n_groups, n_cand) or not o.is_contiguous():
+            raise SrgptError(f"beam_group_select: ranked outputs must be contiguous [{P}, {n_groups}, {n_cand}]")
+    for o in (next_beams, next_tokens):
+        if o.numel() != R or not o.is_contiguous():
+            raise SrgptError(f"beam_group_select: next_beams / next_tokens must hold {R} entries")
+    check(_lib.load().srgpt_beam_group_select(_p(logits), _rowmajor2d(logits, "beam_group_select.logits"), V, _p(stats), _p(beam_scores),
+                                              _p(cand_tokens), L, P, k, n_groups, n_cand, _p(eos) if eos.numel() else None, eos.numel(),
+                                              int(pad_id), float(diversity_penalty), _p(done), _p(out_scores), _p(out_beams), _p(out_tokens),
+                                              _p(next_beams), _p(next_tokens), _stream()),
+          "srgpt_beam_group_select")
+
+
 def beam_select(cand_scores: torch.Tensor, cand_tokens: torch.Tensor, k: int, out_scores: torch.Tensor, out_beams: torch.Tensor,
                 out_tokens: torch.Tensor) -> None:
     """Per prompt (k consecutive rows of the [G * k, n_cand] candidates of beam_candidates): its n_cand best (score, beam in the prompt,
